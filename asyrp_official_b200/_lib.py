@@ -54,10 +54,7 @@ SIGNATURES = {
     "asyrp_conv_stats_tiles": (c_int, [c_int, c_int, c_int, c_int]),
     "asyrp_conv_stats_tiles_up2": (c_int, [c_int, c_int, c_int]),
     "asyrp_conv_tile_config": (c_int, [c_int, c_int, c_int, c_int]),
-    "asyrp_set_cta2": (c_int, [c_int]),
-    "asyrp_set_pair128": (c_int, [c_int]),
     "asyrp_set_silu_tanh": (c_int, [c_int]),
-    "asyrp_conv_is_cta2": (c_int, [c_void_p]),
     "asyrp_conv_create": (c_int, [C.POINTER(AsyrpConvDesc), C.POINTER(c_void_p)]),
     "asyrp_conv_launch": (c_int, [c_void_p, c_void_p]),
     "asyrp_conv_set_scales": (c_int, [c_void_p, c_float, c_float]),

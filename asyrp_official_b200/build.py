@@ -1,4 +1,4 @@
-"""Build libasyrp_b200.so in-tree with nvcc for sm_100a.
+"""Build libasyrp_b200.so in-tree with nvcc for sm_90a (H100).
 
 The shared library is the C-ABI boundary (include/asyrp_b200.h).  It is built into the package directory
 so that it travels with the repository snapshot to the GPU box; nothing is JIT-compiled at import time.
@@ -14,7 +14,7 @@ SUFFIX = os.environ.get("ASYRP_LIB_SUFFIX", "")
 LIB = os.path.join(HERE, f"libasyrp_b200{SUFFIX}.so")
 SOURCES = ["common.cu", "conv_gemm.cu", "pointwise.cu", "attention.cu"]
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+    "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
     "-Xcompiler", "-fPIC", "-Xcompiler", "-fvisibility=hidden", "-cudart", "static",
 ]
 
@@ -42,7 +42,7 @@ def build_library(force=False, verbose=False):
             (["-Xptxas", "-v"] if verbose else [])
         subprocess.run(cmd, check=True)
         objs.append(obj)
-    subprocess.run([nvcc, "-shared", "-cudart", "static", "-o", LIB, *objs], check=True)
+    subprocess.run([nvcc, "-shared", *NVCC_FLAGS[:2], "-cudart", "static", "-o", LIB, *objs], check=True)
     return LIB
 
 

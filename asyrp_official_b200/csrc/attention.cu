@@ -1,7 +1,7 @@
 // Self-attention over the spatial positions of one feature map (softmax(q k^T / sqrt(d)) v), fp16 in/out,
 // fp32 logits / softmax / accumulation.  Reference: AttnBlock.forward (ddpm/diffusion.py:200-225, one head,
 // d = C) and QKVAttentionLegacy.forward (improved_ddpm/unet.py:379-396, heads of 64 channels, q and k each
-// scaled by d^-1/4, softmax in fp32).  The q/k/v projections and proj_out run on the tcgen05 GEMM kernel
+// scaled by d^-1/4, softmax in fp32).  The q/k/v projections and proj_out run on the wgmma GEMM kernel
 // (conv_gemm.cu); this kernel is the T x T part with a warp-level online softmax.
 //
 // Layout: qkv [N][T][3*C] with C = heads*D: q at [0,C), k at [C,2C), v at [2C,3C), head h at h*D.

@@ -16,7 +16,7 @@ enum : int {
   ASYRP_OK = 0,
   ASYRP_ERR_INVALID = -1,   // bad argument / unsupported shape
   ASYRP_ERR_CUDA = -2,      // CUDA runtime / driver error
-  ASYRP_ERR_NO_DEVICE = -3, // no sm_100 device available
+  ASYRP_ERR_NO_DEVICE = -3, // no sm_90 device available
 };
 
 void set_error(const char* fmt, ...);
@@ -60,12 +60,11 @@ int sm_count();
 
 // Programmatic dependent launch (PDL).  Every kernel of the library starts with `griddepcontrol.launch_dependents`
 // and executes `griddepcontrol.wait` before its first global-memory access; launched with the
-// programmaticStreamSerialization attribute, kernel i+1 is scheduled (and runs its prologue: barrier init, TMEM
-// allocation, descriptor prefetch) while kernel i drains, instead of after it — inside a captured graph too.
-// Measured on the 40-step trajectory graph (round 2, B200): 443.0 ms without vs 448.7 ms with PDL — inside a CUDA graph
-// the launch gaps are already hidden and a 227 KB / 608-thread CTA cannot become resident before its predecessor on
-// the same SM has exited, so there is nothing to overlap.  Hence OFF by default; asyrp_set_pdl(1) / ASYRP_PDL=1
-// enables it (eager, launch-bound callers of the C ABI benefit).
+// programmaticStreamSerialization attribute, kernel i+1 is scheduled (and runs its prologue: barrier init,
+// descriptor prefetch) while kernel i drains, instead of after it — inside a captured graph too.  Inside a CUDA graph
+// the launch gaps are already hidden and a conv CTA with ~227 KB of shared memory cannot become resident before its
+// predecessor on the same SM has exited, so there is little to overlap.  Hence OFF by default; asyrp_set_pdl(1) /
+// ASYRP_PDL=1 enables it (eager, launch-bound callers of the C ABI benefit).
 int pdl_enabled();
 
 template <typename... Exp, typename... Act>

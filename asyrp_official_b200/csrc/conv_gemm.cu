@@ -1,4 +1,4 @@
-// Implicit-GEMM convolution / batched GEMM on tcgen05 tensor cores (sm_100a), TMA-fed.
+// Implicit-GEMM convolution / batched GEMM on Hopper tensor cores (wgmma, sm_90a), TMA-fed.
 //
 // One kernel serves every dense contraction of the Asyrp UNet path:
 //   * 3x3 stride-1 pad-1 convs        (ResnetBlock.conv1/conv2, Upsample.conv; ddpm/diffusion.py:122-133,77-81)
@@ -8,35 +8,33 @@
 //   * plain GEMMs (rows = "pixels" of an H=1 image)
 //
 // Data layout: activations NHWC fp16, weights [Cout][K] fp16 with K = sum over segments of taps*C_seg
-// (tap-major, channel-minor), accumulation fp32 in TMEM, epilogue fp32.
+// (tap-major, channel-minor), accumulation fp32 in registers, epilogue fp32.
 //
 // The K loop walks "segments": each segment is one source tensor (so a channel-concat input is two
 // segments and never materialised; a fused 1x1 shortcut is one more segment accumulated into the same
-// TMEM tile).  For a 3x3/s1 segment the producer loads, per 64-channel chunk, ONE (TH+2) x (8+2)-pixel halo tile
+// accumulators).  For a 3x3/s1 segment the producer loads, per 64-channel chunk, ONE (TH+2) x (8+2)-pixel halo tile
 // and the nine taps are start-address offsets into it (the 128B swizzle is a function of the shared-memory
 // address, the descriptor's stride-byte-offset is the halo pitch); layers narrower than 8x16 pixels use three
 // dx-shifted copies whose dy taps are 1024B-aligned row offsets.  TMA's out-of-bounds zero fill is the padding.
 //
-// Warp roles (608 threads): warp 0 = activation TMA producer, warp 18 = weight TMA producer, warp 1 = TMEM allocator
-// + MMA issuer (all three: whole-warp uniform control flow, one elected lane issues), warps 2..9 = epilogue
-// (TMEM -> registers -> bias/residual -> fp16 NHWC store + GroupNorm partial sums), warps 10..17 = in-place operand
-// transform (fused GroupNorm-apply + SiLU).  Persistent: each CTA loops over output tiles; two TMEM accumulators
-// so the epilogue of tile i overlaps the MMAs of tile i+1.
+// Warp roles (576 threads): warps 0..7 = two consumer warpgroups (wgmma into register accumulators, then the
+// epilogue: accumulators -> shared-memory staging tile -> bias/residual -> fp16 NHWC store + GroupNorm partial sums),
+// warps 8..15 = in-place operand transform (fused GroupNorm-apply + SiLU), warp 16 = activation TMA producer,
+// warp 17 = weight TMA producer (whole-warp uniform control flow, one elected lane issues).  Persistent: each CTA
+// loops over output tiles; the producers run ahead across tile boundaries, so the loads of tile i+1 overlap the
+// epilogue of tile i.
 #include "common.h"
 #include "ptx.cuh"
 #include <cstring>
 
 namespace asyrp {
 
-#ifndef ASYRP_PAIR128_DEFAULT
-#define ASYRP_PAIR128_DEFAULT 0
-#endif
 static constexpr int kMaxSeg = 3;
-static constexpr int kNumEpilogueWarps = 8;   // two warps per TMEM lane quarter, alternating 32-column chunks
+static constexpr int kNumConsumerWarps = 8;   // two warpgroups
 static constexpr int kNumTransformWarps = 8;
-static constexpr int kWarpT = 2 + kNumEpilogueWarps;            // first transform warp
-static constexpr int kWarpB = kWarpT + kNumTransformWarps;      // weight (B operand) producer warp
-// warps: 0 A-producer, 1 MMA issuer, 2..9 epilogue, 10..17 operand transform, 18 B-producer
+static constexpr int kWarpT = kNumConsumerWarps;                // first transform warp
+static constexpr int kWarpA = kWarpT + kNumTransformWarps;      // activation (A operand) producer warp
+static constexpr int kWarpB = kWarpA + 1;                       // weight (B operand) producer warp
 static constexpr int kNumThreads = 32 * (kWarpB + 1);
 
 struct ConvSegDev {
@@ -304,118 +302,28 @@ __device__ __forceinline__ void stat_atomic_add(long long* dst, float v) {
   atomicAdd(reinterpret_cast<unsigned long long*>(dst), static_cast<unsigned long long>(__float2ll_rn(v * kStatScale)));
 }
 
-// Residual values of one 32-pixel chunk (rows row0 .. of the tile, this lane's channel) read through the resample index
-// map: mode 1 nearest-x2 (tile pixel (dy, dx) <- source pixel (dy >> 1, dx >> 1) of the half-resolution tensor; tile
-// origins are even), mode 2 2x2 average pool of the double-resolution tensor in fp32 like F.avg_pool2d.
-// rp: source tensor at the tile's origin and this lane's channel; rrow / cout: elements per source row / pixel.
-template <int TWS>
-__device__ __noinline__ void load_resampled_residual(__half2 (&rv)[16], const __half* rp, int mode, int row0, int rrow,
-                                                     int cout) {
-  constexpr int TW = 1 << TWS;
-  if (mode == 1) {
-    rp += static_cast<size_t>(row0 >> 1) * rrow;
+template <int BN>
+__device__ __forceinline__ void wgmma_bn(float (&d)[BN / 2], uint64_t desc_a, uint64_t desc_b, uint32_t accumulate) {
+  static_assert(BN == 16 || BN == 64 || BN == 128, "wgmma tile widths of this kernel");
+  if constexpr (BN == 16) wgmma_f16_n16(d, desc_a, desc_b, accumulate);
+  else if constexpr (BN == 64) wgmma_f16_n64(d, desc_a, desc_b, accumulate);
+  else wgmma_f16_n128(d, desc_a, desc_b, accumulate);
+}
+
+// NV consecutive fp32 values of the staging tile at shared address `addr` (16-byte aligned)
+template <int NV>
+__device__ __forceinline__ void ld_staged(uint32_t addr, uint32_t (&r)[NV]) {
 #pragma unroll
-    for (int i = 0; i < 32; i += 2) {
-      const __half v0 = rp[((i >> TWS) >> 1) * rrow + ((i & (TW - 1)) >> 1) * cout];
-      rv[i >> 1] = __halves2half2(v0, v0);  // pixels i, i+1 share their source pixel (i even)
-    }
-  } else {
-    rp += static_cast<size_t>(row0 * 2) * rrow;
-#pragma unroll 4
-    for (int i = 0; i < 32; i += 2) {
-      float a2[2];
-#pragma unroll
-      for (int k = 0; k < 2; ++k) {
-        const __half* q = rp + ((i + k) >> TWS) * 2 * rrow + ((i + k) & (TW - 1)) * 2 * cout;
-        a2[k] = 0.25f * ((__half2float(q[0]) + __half2float(q[cout])) + (__half2float(q[rrow]) + __half2float(q[rrow + cout])));
-      }
-      rv[i >> 1] = __floats2half2_rn(a2[0], a2[1]);
-    }
+  for (int i = 0; i < NV / 4; ++i) {
+    const uint4 v = lds128(addr + 16 * i);
+    r[4 * i] = v.x; r[4 * i + 1] = v.y; r[4 * i + 2] = v.z; r[4 * i + 3] = v.w;
   }
 }
 
-// Swapped-operand epilogue of one warp: TMEM lane = output channel c, columns = the tile's pixels (row-major in the
-// TW x (MT*128/TW) tile); this warp drains the 32-pixel column chunks half, half+2, ...  TWS = log2(TW).
-// RES: the residual is read through a resample index map (ADM up / down blocks); a separate instantiation so that the
-// common one (the hot loop of 55 % of the conv time, instruction-issue bound) carries no extra live registers
-// RESM: 0 no residual (every DDPM layer on this tile: identity skips and shortcuts are K columns), 1 residual with the
-// output's geometry, 2 resampled residual.  Separate instantiations: the residual prefetch registers and its address
-// arithmetic pushed the common no-residual loop over the 96-register budget of a 608-thread CTA (spills to local memory,
-// with an L1 of ~28 KB next to 227 KB of shared memory).
-template <int TWS, int MT, int RESM>
-__device__ __forceinline__ void swap_epilogue(const ConvParams& p, uint32_t taddr, int half, size_t obase,
-                                              int row_stride, int cout, int lane_off, uint32_t sel, float eb,
-                                              size_t rbase, int rrow, float& s1, float& s2) {
-  const float scale = p.acc_scale, rs = p.res_scale;  // constant-bank operands (device-side scales: generic tile only)
-  // obase: element offset of the tile's first pixel at this lane's channel; row_stride / cout: elements between
-  // vertically / horizontally adjacent tile pixels in the output (doubled for the sub-pixel phases of an up2 conv)
-  constexpr int TW = 1 << TWS;
-  constexpr int kRows = 32 / TW;  // image rows per 32-pixel chunk
-  const __half* __restrict__ resp = p.res;
-  __half* __restrict__ outp = p.out;
-#pragma unroll 1
-  for (int cc = half; cc < (MT * 128) / 32; cc += 2) {
-    uint32_t r[32];
-    tmem_ld_32x32(taddr + cc * 32, r);
-    // element offset of the chunk's first pixel
-    const size_t o0 = obase + static_cast<size_t>(cc * kRows) * row_stride;
-    [[maybe_unused]] __half2 rv[RESM != 0 ? 16 : 1];
-    if constexpr (RESM == 1) {  // all residual loads first: independent of the stores below
-      const __half* rp = resp + o0;
-#pragma unroll
-      for (int i = 0; i < 32; i += 2)
-        rv[i >> 1] = __halves2half2(rp[(i >> TWS) * row_stride + (i & (TW - 1)) * cout],
-                                    rp[((i + 1) >> TWS) * row_stride + ((i + 1) & (TW - 1)) * cout]);
-    } else if constexpr (RESM == 2) {
-      // ADM up / down blocks only: kept out of line so that the common path's register allocation is untouched
-      load_resampled_residual<TWS>(rv, resp + rbase, p.res_mode, cc * kRows, rrow, cout);
-    }
-    tmem_ld_wait();
-    float v[32];
-#pragma unroll
-    for (int i = 0; i < 32; ++i) v[i] = fmaf(__uint_as_float(r[i]), scale, eb);
-    if constexpr (RESM != 0) {
-#pragma unroll
-      for (int i = 0; i < 32; i += 2) {
-        const float2 f = __half22float2(rv[i >> 1]);
-        v[i] = fmaf(rs, f.x, v[i]);
-        v[i + 1] = fmaf(rs, f.y, v[i + 1]);
-      }
-    }
-    __half* lp = outp + o0 + lane_off;
-#pragma unroll
-    for (int dy = 0; dy < kRows; ++dy) {
-      __half* rowp = lp + dy * row_stride;
-#pragma unroll
-      for (int dx = 0; dx < TW; dx += 2) {
-        const int i = dy * TW + dx;
-        const __half2 mine = __floats2half2_rn(v[i], v[i + 1]);  // (pixel i, pixel i+1) of this lane's channel
-        const uint32_t x = *reinterpret_cast<const uint32_t*>(&mine);
-        const uint32_t y = __shfl_xor_sync(0xffffffffu, x, 1);
-        // even lane: (own, partner) at pixel i; odd lane: (partner, own) at pixel i+1
-        *reinterpret_cast<uint32_t*>(rowp + dx * cout) = __byte_perm(x, y, sel);
-        s1 += v[i] + v[i + 1];
-        s2 = fmaf(v[i], v[i], s2);
-        s2 = fmaf(v[i + 1], v[i + 1], s2);
-      }
-    }
-  }
-}
-
-// SWAP: operand roles exchanged — the weight tile (128 output channels) is the M side and the MT*128 pixels are the
-// N side of ONE N=256 MMA per K step, so D is [channel lane][pixel column].  Per MMA the tensor core then reads
-// 4 KB (weights) + 8 KB (pixels) of shared memory per 128 cycles instead of 4 + 4 KB per 64 cycles: the Cout=128
-// layers (70% of the FLOPs) stop being shared-memory-bandwidth bound.
-//
-// CTA2: the kernel runs as clusters of two CTAs (one TPC) that share every weight tile.  Each CTA keeps its own
-// 128-pixel tile (A operand, loaded and transformed locally) and HALF of the 256 weight rows (B operand) in its shared
-// memory; the leader (cluster rank 0) issues `tcgen05.mma.cta_group::2` with M = 256: per K step each SM reads
-// 4 + 4 KB of operands instead of 4 + 8 KB and ingests 16 instead of 32 KB of weights per stage (the 128 px x 256 ch
-// tile of one CTA is bound by exactly that ingest, 64 of the ~66 B/clk one SM takes).  Synchronisation: TMA bytes of
-// both weight halves are counted on the leader's fullB barrier; transform warps of both CTAs arrive on the leader's
-// readyA; MMA completion is committed to both CTAs' empty / tmem-full barriers (multicast); both epilogues arrive on
-// the leader's tmem-empty barrier.  Numerically identical to the one-CTA kernel (same K order per tile).
-template <int BN, int MT, bool SWAP = false, bool CTA2 = false>
+// BN output channels x MT sub-tiles of 128 pixels per CTA tile; each consumer warpgroup accumulates MT x BN/2 fp32
+// registers per thread.  MT * BN <= 128 bounds them to 64: ptxas allocates 96 registers per thread to every
+// instantiation at 576 threads, and the 64- and 128-channel ones still spill ~100 bytes outside the wgmma chain.
+template <int BN, int MT>
 __global__ void __launch_bounds__(kNumThreads, 1) conv_gemm_kernel(const __grid_constant__ ConvParams p) {
   pdl_trigger();  // the next kernel of the stream may be scheduled as soon as every CTA of this grid is running
   extern __shared__ uint8_t smem_raw[];
@@ -424,293 +332,127 @@ __global__ void __launch_bounds__(kNumThreads, 1) conv_gemm_kernel(const __grid_
 
   const int warp = uniform_warp_id();
   const int lane = threadIdx.x & 31;
-  constexpr uint32_t kBStage = (CTA2 ? BN / 2 : BN) * 128;
-  static_assert(!SWAP || (BN == 128 && MT == 2), "swapped-operand variant: 128 channels x 256 pixels");
-  static_assert(!CTA2 || (((BN == 256 && MT == 1) || (BN == 128 && MT == 2)) && !SWAP),
-                "CTA-pair variants: 2 x 128 pixels x 256 channels, 2 x 256 pixels x 128 channels");
-  const uint32_t cta_rank = CTA2 ? cluster_ctarank() : 0u;
-  constexpr uint32_t kAccCols = SWAP ? MT * 128 : MT * BN;  // fp32 columns of one accumulator set
-  constexpr uint32_t kTmemCols = 2 * kAccCols;                // two sets (epilogue / MMA overlap)
-  static_assert(kTmemCols <= 512 && kTmemCols >= 32, "TMEM budget");
+  constexpr uint32_t kBStage = BN * 128;
+  constexpr int kCPitch = MT * BN + 4;  // staging row pitch in floats: +16 B per row keeps the row reads conflict-free
+  static_assert(MT * BN <= 128, "accumulator registers per consumer thread");
 
   uint8_t* sA = smem;
   uint8_t* sL = sA + p.a_stages * p.a_stage_bytes;  // light ring (may be empty)
   uint8_t* sB = sL + p.l_stages * p.l_stage_bytes;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(sB + p.b_stages * kBStage);
+  float* sC = reinterpret_cast<float*>(sB + p.b_stages * kBStage);  // [128][kCPitch] accumulator staging tile
+  uint64_t* bars = reinterpret_cast<uint64_t*>(sC + 128 * kCPitch);
   const int n_aslots = p.a_stages + p.l_stages;     // barrier index: heavy slots first, then light slots
   uint64_t* fullA = bars;
   uint64_t* emptyA = fullA + n_aslots;
   uint64_t* readyA = emptyA + n_aslots;
   uint64_t* fullB = readyA + n_aslots;
   uint64_t* emptyB = fullB + p.b_stages;
-  uint64_t* tfull = emptyB + p.b_stages;
-  uint64_t* tempty = tfull + 2;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tempty + 2);
-  float* s_stats = reinterpret_cast<float*>(tmem_slot + 4);  // [2][4][BN/32][32]
+  float* s_stats = reinterpret_cast<float*>(emptyB + p.b_stages);     // [2][4][BN/32][32]
   float2* s_gstat = reinterpret_cast<float2*>(s_stats + 2 * 4 * BN);  // [2][kMaxSeg][32] (mean, rstd), see gn_affine8
   const int THT = MT * p.TH;  // rows of the CTA tile
 
   if (threadIdx.x == 0) {
     for (int i = 0; i < n_aslots; ++i) {
       mbar_init(&fullA[i], 1);
-      mbar_init(&emptyA[i], 1);
-      mbar_init(&readyA[i], (CTA2 ? 2 : 1) * kNumTransformWarps);
+      mbar_init(&emptyA[i], kNumConsumerWarps);
+      mbar_init(&readyA[i], kNumTransformWarps);
     }
     for (int i = 0; i < p.b_stages; ++i) {
       mbar_init(&fullB[i], 1);
-      mbar_init(&emptyB[i], 1);
-    }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&tfull[i], 1);
-      mbar_init(&tempty[i], (CTA2 ? 2 : 1) * kNumEpilogueWarps);
+      mbar_init(&emptyB[i], kNumConsumerWarps);
     }
     fence_mbar_init();
   }
-  if (warp == 0 && lane == 0) {
+  if (warp == kWarpA && lane == 0) {
     for (int s = 0; s < p.nseg; ++s) tma_prefetch_desc(&p.tmA[s]);
     tma_prefetch_desc(&p.tmB);
   }
-  if (warp == 1) {
-    if constexpr (CTA2) {
-      tmem_alloc_2cta(tmem_slot, kTmemCols);
-      tmem_relinquish_2cta();
-    } else {
-      tmem_alloc(tmem_slot, kTmemCols);
-      tmem_relinquish();
-    }
-  }
-  tc_fence_before();
   __syncthreads();
-  if constexpr (CTA2) cluster_sync_all();  // the peer's barriers are initialised before anything arrives on them
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-  // everything above (barrier init, TMEM allocation, descriptor prefetch) overlapped the previous kernel's tail; from
-  // here on global memory written by it is read (and buffers it may still read are written)
+  // everything above (barrier init, descriptor prefetch) overlapped the previous kernel's tail; from here on global
+  // memory written by it is read (and buffers it may still read are written)
   pdl_wait();
 
   const int total_tiles = p.m_tiles * p.n_tiles;
-  // work items: output tiles, or (CTA2) pairs of horizontally adjacent pixel tiles sharing one weight tile; a CTA of a
-  // pair processes tile 2*pm + rank of channel tile nt
-  const int n_workers = CTA2 ? gridDim.x / 2 : gridDim.x;
-  const int worker0 = CTA2 ? blockIdx.x / 2 : blockIdx.x;
-  const int n_work = CTA2 ? total_tiles / 2 : total_tiles;
-  auto own_tile = [&](int w) -> int {
-    if constexpr (!CTA2) return w;
-    const int half_m = p.m_tiles >> 1;
-    const int nt_ = w / half_m;
-    return nt_ * p.m_tiles + 2 * (w - nt_ * half_m) + static_cast<int>(cta_rank);
-  };
 
-  if (warp == 0) {
+  if (warp == kWarpA) {
     // ======================================================== TMA producer, A operand (activations)
     // A and B have independent rings and independent producer threads, so the activation prefetch (which the
     // transform warps must also touch) runs a full A-ring ahead regardless of the weight ring's depth.
     // Whole warp, uniform control flow; one elected lane issues (see elect_one()).
-    {
-      int sa = 0, sl = 0;      // heavy / light ring cursors
-      uint32_t pa = 0, pl = 0;
-      [[maybe_unused]] int tr_n = 0;
-      for (int w = worker0; w < n_work; w += n_workers) {
-        const int tile = own_tile(w);
-        const TileCoord tc = tile_coord(p, tile);
-        const int x0 = tc.tx * p.TW, y0 = tc.ty * THT, n0 = tc.tn * p.NB;
-        for (int e = 0; e < p.n_sched; ++e) {
-          const int s = p.sched[e] >> 6, ch = p.sched[e] & 63;
-          const ConvSegDev sg = p.seg[s];
-          const bool lt = p.l_stages != 0 && sg.mode == 0;
-          const int ncopies = (sg.mode == 0 || sg.mode == 3) ? 1 : (sg.mode == 1 ? 3 : 9);
-          const uint32_t a_bytes = sg.mode == 3 ? (THT + 2) * (p.TW + 2) * 128u
-                                                : (sg.mode == 1 ? (THT + 2) : THT) * p.row_bytes;
-          {
-            for (int cp = 0; cp < ncopies; ++cp) {
-              const int slot = lt ? p.a_stages + sl : sa;
-              mbar_wait_suspend(&emptyA[slot], (lt ? pl : pa) ^ 1);
-              ASYRP_TRACE_STAMP(0, tr_n);
-              ++tr_n;
-              uint8_t* dst = lt ? sL + sl * p.l_stage_bytes : sA + sa * p.a_stage_bytes;
-              int c0 = ch * 64, c1, c2 = n0, c3 = 0, c4;
-              if (sg.mode == 3) {
-                c1 = x0 - 1; c4 = y0 - 1;
-              } else if (sg.mode == 0) {
-                c1 = x0; c2 = n0 / p.a_heads; c3 = n0 % p.a_heads; c4 = y0;
-              } else if (sg.mode == 1) {
-                c1 = x0 + cp - 1; c4 = y0 - 1;
-              } else {
-                const int ky = cp / 3, kx = cp % 3;
-                c0 += (kx & 1) * sg.C; c1 = x0 + (kx >> 1); c3 = ky & 1; c4 = y0 + (ky >> 1);
-              }
-              if (elect_one()) {
-                mbar_arrive_expect_tx(&fullA[slot], a_bytes);
-                tma_load_5d(dst, &p.tmA[s], &fullA[slot], c0, c1, c2, c3, c4);
-              }
-              if (lt) {
-                if (++sl == p.l_stages) { sl = 0; pl ^= 1; }
-              } else {
-                if (++sa == p.a_stages) { sa = 0; pa ^= 1; }
-              }
-            }
+    int sa = 0, sl = 0;      // heavy / light ring cursors
+    uint32_t pa = 0, pl = 0;
+    [[maybe_unused]] int tr_n = 0;
+    for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
+      const TileCoord tc = tile_coord(p, tile);
+      const int x0 = tc.tx * p.TW, y0 = tc.ty * THT, n0 = tc.tn * p.NB;
+      for (int e = 0; e < p.n_sched; ++e) {
+        const int s = p.sched[e] >> 6, ch = p.sched[e] & 63;
+        const ConvSegDev sg = p.seg[s];
+        const bool lt = p.l_stages != 0 && sg.mode == 0;
+        const int ncopies = (sg.mode == 0 || sg.mode == 3) ? 1 : (sg.mode == 1 ? 3 : 9);
+        const uint32_t a_bytes = sg.mode == 3 ? (THT + 2) * (p.TW + 2) * 128u
+                                              : (sg.mode == 1 ? (THT + 2) : THT) * p.row_bytes;
+        for (int cp = 0; cp < ncopies; ++cp) {
+          const int slot = lt ? p.a_stages + sl : sa;
+          mbar_wait_suspend(&emptyA[slot], (lt ? pl : pa) ^ 1);
+          ASYRP_TRACE_STAMP(0, tr_n);
+          ++tr_n;
+          uint8_t* dst = lt ? sL + sl * p.l_stage_bytes : sA + sa * p.a_stage_bytes;
+          int c0 = ch * 64, c1, c2 = n0, c3 = 0, c4;
+          if (sg.mode == 3) {
+            c1 = x0 - 1; c4 = y0 - 1;
+          } else if (sg.mode == 0) {
+            c1 = x0; c2 = n0 / p.a_heads; c3 = n0 % p.a_heads; c4 = y0;
+          } else if (sg.mode == 1) {
+            c1 = x0 + cp - 1; c4 = y0 - 1;
+          } else {
+            const int ky = cp / 3, kx = cp % 3;
+            c0 += (kx & 1) * sg.C; c1 = x0 + (kx >> 1); c3 = ky & 1; c4 = y0 + (ky >> 1);
+          }
+          if (elect_one()) {
+            mbar_arrive_expect_tx(&fullA[slot], a_bytes);
+            tma_load_5d(dst, &p.tmA[s], &fullA[slot], c0, c1, c2, c3, c4);
+          }
+          if (lt) {
+            if (++sl == p.l_stages) { sl = 0; pl ^= 1; }
+          } else {
+            if (++sa == p.a_stages) { sa = 0; pa ^= 1; }
           }
         }
       }
     }
   } else if (warp == kWarpB) {
     // ======================================================== TMA producer, B operand (weights)
-    {
-      int sb = 0;
-      uint32_t pb = 0;
-      for (int w = worker0; w < n_work; w += n_workers) {
-        const int tile = own_tile(w);
-        const TileCoord tc = tile_coord(p, tile);
-        const int nt = tc.nt, tn = tc.tn;
-        const int bz = p.b_batched ? tn * p.NB : 0;
-        const int b_n = bz / p.b_heads, b_h = bz % p.b_heads;
-        for (int e = 0; e < p.n_sched; ++e) {
-          const int s = p.sched[e] >> 6, ch = p.sched[e] & 63;
-          const ConvSegDev sg = p.seg[s];
-          const int ncopies = (sg.mode == 0 || sg.mode == 3) ? 1 : (sg.mode == 1 ? 3 : 9);
-          const int ntaps = sg.mode == 1 ? 3 : (sg.mode == 3 ? (p.up2 ? 4 : 9) : 1);
-          {
-            for (int cp = 0; cp < ncopies; ++cp) {
-              for (int tp = 0; tp < ntaps; ++tp) {
-                // tap index in the weight matrix: ky*3+kx (up2: dy*2+dx of the phase's 2x2 kernel; the weight rows
-                // nt*BN already select the phase)
-                const int tap = sg.mode == 0 ? 0 : (sg.mode == 1 ? tp * 3 + cp : (sg.mode == 3 ? tp : cp));
-                mbar_wait_suspend(&emptyB[sb], pb ^ 1);
-                if constexpr (CTA2) {
-                  // this CTA's half of the weight rows; the bytes of both halves are counted on the leader's barrier
-                  // the leader's copy of fullB[sb]: shared-window addresses carry the CTA's rank within the pair in bit
-                  // 24; clearing it is plain ALU work on a warp-uniform value (a `mapa` result lives in a vector
-                  // register and would put the TMA instruction into a vote / R2UR waterfall loop)
-                  const uint32_t bar = smem_u32(&fullB[sb]) & 0xFEFFFFFFu;
-                  if (elect_one()) {
-                    if (cta_rank == 0) mbar_arrive_expect_tx(&fullB[sb], 2 * kBStage);
-                    tma_load_4d_2cta(sB + sb * kBStage, &p.tmB, bar, sg.kbase + tap * sg.C + ch * 64,
-                                     nt * BN + static_cast<int>(cta_rank) * (BN / 2), b_h, b_n);
-                  }
-                } else if (elect_one()) {
-                  mbar_arrive_expect_tx(&fullB[sb], kBStage);
-                  tma_load_4d(sB + sb * kBStage, &p.tmB, &fullB[sb], sg.kbase + tap * sg.C + ch * 64, nt * BN, b_h,
-                              b_n);
-                }
-                if (++sb == p.b_stages) { sb = 0; pb ^= 1; }
-              }
+    int sb = 0;
+    uint32_t pb = 0;
+    for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
+      const TileCoord tc = tile_coord(p, tile);
+      const int nt = tc.nt, tn = tc.tn;
+      const int bz = p.b_batched ? tn * p.NB : 0;
+      const int b_n = bz / p.b_heads, b_h = bz % p.b_heads;
+      for (int e = 0; e < p.n_sched; ++e) {
+        const int s = p.sched[e] >> 6, ch = p.sched[e] & 63;
+        const ConvSegDev sg = p.seg[s];
+        const int ncopies = (sg.mode == 0 || sg.mode == 3) ? 1 : (sg.mode == 1 ? 3 : 9);
+        const int ntaps = sg.mode == 1 ? 3 : (sg.mode == 3 ? (p.up2 ? 4 : 9) : 1);
+        for (int cp = 0; cp < ncopies; ++cp) {
+          for (int tp = 0; tp < ntaps; ++tp) {
+            // tap index in the weight matrix: ky*3+kx (up2: dy*2+dx of the phase's 2x2 kernel; the weight rows
+            // nt*BN already select the phase)
+            const int tap = sg.mode == 0 ? 0 : (sg.mode == 1 ? tp * 3 + cp : (sg.mode == 3 ? tp : cp));
+            mbar_wait_suspend(&emptyB[sb], pb ^ 1);
+            if (elect_one()) {
+              mbar_arrive_expect_tx(&fullB[sb], kBStage);
+              tma_load_4d(sB + sb * kBStage, &p.tmB, &fullB[sb], sg.kbase + tap * sg.C + ch * 64, nt * BN, b_h, b_n);
             }
+            if (++sb == p.b_stages) { sb = 0; pb ^= 1; }
           }
         }
       }
     }
-  } else if (warp == 1) {
-    // ======================================================== MMA issuer (whole warp, elected lane issues)
-    if (!CTA2 || cta_rank == 0) {  // CTA pair: the leader issues for both SMs
-      constexpr uint32_t idesc = CTA2 ? umma_idesc_f16_m256(BN) : umma_idesc_f16_m128(SWAP ? MT * 128 : BN);
-      const uint32_t b_lo0 = umma_desc_lo(smem_u32(sB));
-      int sa = 0, sl = 0, sb = 0;
-      uint32_t pa = 0, pl = 0, pb = 0;
-      int it = 0;
-      [[maybe_unused]] int tr_n = 0;
-      for (int w = worker0; w < n_work; w += n_workers, ++it) {
-        const int tile = own_tile(w);
-        const int acc = it & 1;
-        const uint32_t acc_phase = (it >> 1) & 1;
-        ASYRP_TRACE_STAMP(5, it);
-        mbar_wait_suspend(&tempty[acc], acc_phase ^ 1);
-        ASYRP_TRACE_STAMP(6, it);
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + acc * kAccCols;
-        int up_a = 0, up_b = 0;  // up2: sub-pixel phase of this tile = first tap (ky, kx) of its 2x2 kernel
-        if (p.up2) {
-          const int ph = fast_div(tile, p.mul_m, p.m_tiles) / (p.Cout / BN);
-          up_a = ph >> 1;
-          up_b = ph & 1;
-        }
-        uint32_t accumulate = 0;
-        for (int e = 0; e < p.n_sched; ++e) {
-          const int s = p.sched[e] >> 6;
-          const ConvSegDev sg = p.seg[s];
-          const bool lt = p.l_stages != 0 && sg.mode == 0;
-          const int ncopies = (sg.mode == 0 || sg.mode == 3) ? 1 : (sg.mode == 1 ? 3 : 9);
-          const int ntaps = sg.mode == 1 ? 3 : (sg.mode == 3 ? (p.up2 ? 4 : 9) : 1);
-          // byte strides inside the A stage: between 8-row groups, between sub-tiles, per ky / kx tap step
-          const uint32_t halo_pitch = (p.TW + 2) * 128u;
-          const uint32_t sbo = sg.mode == 3 ? halo_pitch : 1024u;
-          const uint32_t sub_stride = sg.mode == 3 ? p.TH * halo_pitch : p.TH * p.row_bytes;
-          // descriptors as (lo, hi) words: only the start-address field (16-byte units) changes inside the loop
-          const uint32_t a_hi = umma_desc_hi(sbo), b_hi = umma_desc_hi(1024u);
-          const uint32_t sub16 = sub_stride >> 4;
-          // tap step in 16-byte units.  mode 1: dy tap = row shift inside the dx copy; mode 3: (ky, kx) = pixel
-          // offset inside the halo tile: +128 B per kx, and from kx=2 to the next ky row +halo_pitch-256 B
-          // (up2: 2x2 taps starting at (up_a, up_b): +128 B per kx, +halo_pitch-128 B to the next ky row)
-          const uint32_t step16 = sg.mode == 3 ? 8u : (p.row_bytes >> 4);
-          const int kxn = p.up2 ? 2 : 3;
-          const uint32_t wrap16 = sg.mode == 3 ? ((halo_pitch - 128u * (kxn - 1)) >> 4) : step16;
-          const uint32_t first16 = (sg.mode == 3 && p.up2) ? ((up_a * halo_pitch + up_b * 128u) >> 4) : 0u;
-          {
-            for (int cp = 0; cp < ncopies; ++cp) {
-              const int slot = lt ? p.a_stages + sl : sa;
-              ASYRP_TRACE_STAMP(3, tr_n);
-              mbar_wait((p.any_transform || CTA2) ? &readyA[slot] : &fullA[slot], lt ? pl : pa);
-              ASYRP_TRACE_STAMP(4, tr_n);
-              ++tr_n;
-              tc_fence_after();
-              uint32_t a_lo =
-                  umma_desc_lo(smem_u32(lt ? sL + sl * p.l_stage_bytes : sA + sa * p.a_stage_bytes)) + first16;
-              int kx = 0;
-              for (int tp = 0; tp < ntaps; ++tp) {
-                mbar_wait(&fullB[sb], pb);
-                tc_fence_after();
-                const uint32_t b_lo = b_lo0 + sb * (kBStage >> 4);
-                if (elect_one()) {
-                  if constexpr (CTA2) {
-                    // M = 256: the 128 pixel rows of sub-tile `sub` of BOTH CTAs; N = BN channels, half of the weight
-                    // rows in each CTA's shared memory
-#pragma unroll
-                    for (int sub = 0; sub < MT; ++sub) {
-#pragma unroll
-                      for (int k = 0; k < 4; ++k)
-                        umma_f16_w_2cta(d_tmem + sub * BN, a_lo + sub * sub16 + 2 * k, a_hi, b_lo + 2 * k, b_hi, idesc,
-                                        (accumulate | k) ? 1u : 0u);
-                    }
-                  } else if constexpr (SWAP) {
-                    // M = 128 weight rows, N = all MT*128 pixel rows (uniform 8-row-group pitch across sub-tiles)
-#pragma unroll
-                    for (int k = 0; k < 4; ++k)
-                      umma_f16_w(d_tmem, b_lo + 2 * k, b_hi, a_lo + 2 * k, a_hi, idesc, (accumulate | k) ? 1u : 0u);
-                  } else {
-#pragma unroll
-                    for (int sub = 0; sub < MT; ++sub) {
-#pragma unroll
-                      for (int k = 0; k < 4; ++k)
-                        umma_f16_w(d_tmem + sub * BN, a_lo + sub * sub16 + 2 * k, a_hi, b_lo + 2 * k, b_hi, idesc,
-                                   (accumulate | k) ? 1u : 0u);
-                    }
-                  }
-                  if constexpr (CTA2) umma_commit_2cta(&emptyB[sb]); else umma_commit(&emptyB[sb]);
-                }
-                accumulate = 1;
-                if (++sb == p.b_stages) { sb = 0; pb ^= 1; }
-                if (++kx == kxn) { kx = 0; a_lo += wrap16; } else { a_lo += step16; }
-              }
-              if (elect_one()) {
-                if constexpr (CTA2) umma_commit_2cta(&emptyA[slot]); else umma_commit(&emptyA[slot]);
-              }
-              ASYRP_TRACE_STAMP(9, tr_n - 1);
-              if (lt) {
-                if (++sl == p.l_stages) { sl = 0; pl ^= 1; }
-              } else {
-                if (++sa == p.a_stages) { sa = 0; pa ^= 1; }
-              }
-            }
-          }
-        }
-        if (elect_one()) {
-          if constexpr (CTA2) umma_commit_2cta(&tfull[acc]); else umma_commit(&tfull[acc]);
-        }
-      }
-    }
-    __syncwarp();
   } else if (warp >= kWarpT) {
     // ======================================================== operand transform warps, in place
-    if (p.any_transform || CTA2) {  // CTA pair: these warps also relay "A stage landed" to the leader's barrier
+    if (p.any_transform) {
       constexpr int kLanes = kNumTransformWarps * 4;  // pixels handled concurrently (8 threads per pixel)
       const int tt = threadIdx.x - kWarpT * 32;
       const int jl = tt & 7;                  // logical 16B chunk = channels [jl*8, jl*8+8) of the 64-channel slab
@@ -740,11 +482,11 @@ __global__ void __launch_bounds__(kNumThreads, 1) conv_gemm_kernel(const __grid_
       // In-kernel GroupNorm: lane g of transform warp s computes (mean, rstd) of group g of segment s for the sample of a
       // tile, ONE tile ahead (the buffer of tile i+1 is written while tile i is transformed; the named barrier at the
       // top of tile i+1 publishes it).  fp64 like gn_finalize_kernel; 32 x nseg threads per tile, not every thread.
-      auto group_stats = [&](int w_next, int buf) {
+      auto group_stats = [&](int tile_next, int buf) {
         const int s = tt >> 5;
         if (s < p.nseg && p.seg[s].gn_gamma != nullptr) {
           const ConvSegDev& sg = p.seg[s];
-          const TileCoord tcn = tile_coord(p, own_tile(w_next));
+          const TileCoord tcn = tile_coord(p, tile_next);
           const int n = tcn.tn < p.N ? tcn.tn : 0;  // NB == 1
           const int cpg = (sg.gn_C[0] + sg.gn_C[1]) >> 5;
           float m, r;
@@ -753,15 +495,14 @@ __global__ void __launch_bounds__(kNumThreads, 1) conv_gemm_kernel(const __grid_
           s_gstat[(buf * kMaxSeg + s) * 32 + (tt & 31)] = make_float2(m, r);
         }
       };
-      if (p.any_gn && worker0 < n_work) group_stats(worker0, 0);
+      if (p.any_gn && static_cast<int>(blockIdx.x) < total_tiles) group_stats(blockIdx.x, 0);
       int git = 0;
-      for (int w = worker0; w < n_work; w += n_workers, ++git) {
-        const int tile = own_tile(w);
+      for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x, ++git) {
         const TileCoord tc = tile_coord(p, tile);
         const int x0 = tc.tx * p.TW, y0 = tc.ty * THT, n0 = tc.tn * p.NB;
         if (p.any_gn) {
           named_bar_sync(2, kNumTransformWarps * 32);
-          if (w + n_workers < n_work) group_stats(w + n_workers, (git + 1) & 1);
+          if (tile + static_cast<int>(gridDim.x) < total_tiles) group_stats(tile + gridDim.x, (git + 1) & 1);
         }
         for (int e = 0; e < p.n_sched; ++e) {
           const int s = p.sched[e] >> 6, ch = p.sched[e] & 63;
@@ -877,10 +618,7 @@ __global__ void __launch_bounds__(kNumThreads, 1) conv_gemm_kernel(const __grid_
               __syncwarp();
               if (warp == kWarpT) ASYRP_TRACE_STAMP(2, tr_n);
               ++tr_n;
-              if (lane == 0) {
-                if constexpr (CTA2) mbar_arrive_remote(mapa_shared(smem_u32(&readyA[slot]), 0u));
-                else mbar_arrive(&readyA[slot]);
-              }
+              if (lane == 0) mbar_arrive(&readyA[slot]);
               if (lt) {
                 if (++sl == p.l_stages) { sl = 0; plt ^= 1; }
               } else {
@@ -892,25 +630,134 @@ __global__ void __launch_bounds__(kNumThreads, 1) conv_gemm_kernel(const __grid_
       }
     }
   } else {
-    // ======================================================== epilogue (warps 2..9)
-    // Warp (q, half): TMEM lanes [32q, 32q+32) = 32 pixels of every sub-tile, column chunks cc = half, half+2, ...
-    const int q = warp & 3;            // TMEM lane quarter this warp may access
-    const int half = (warp - 2) >> 2;  // which alternate 32-column chunks this warp drains
-    const int ep_tid = (warp - 2) * 32 + lane;
+    // ======================================================== consumers (warps 0..7): wgmma, then the epilogue
+    // Warpgroup wg accumulates rows [64 wg, 64 wg + 64) of every 128-pixel sub-tile in registers.  The epilogue works
+    // on the staging tile in shared memory (row = pixel of the sub-tile, column = sub * BN + channel): warp (q, half)
+    // owns pixel rows [32q, 32q+32) and drains the 32-channel column chunks half, half+2, ...
+    const int wg = warp >> 2;
+    const uint32_t b_lo0 = gmma_desc_lo(smem_u32(sB));
+    const uint32_t sC_addr = smem_u32(sC);
+    const int q = warp & 3;
+    const int half = warp >> 2;
+    const int ep_tid = warp * 32 + lane;
     const int row = q * 32 + lane;
     const int xx = row % p.TW, nn = (row / p.TW) % p.NB, yy = row / (p.TW * p.NB);
     const int tiles_per_sample = p.tiles_x * p.tiles_y * (p.up2 ? 4 : 1);  // statistics slots per sample
-    constexpr int kEpThreads = kNumEpilogueWarps * 32;
+    constexpr int kEpThreads = kNumConsumerWarps * 32;
     float acc_scale = p.acc_scale, res_scale = p.res_scale;
     if (p.scales != nullptr) {
       acc_scale = __ldg(p.scales);
       res_scale = __ldg(p.scales + 1);
     }
+    // ring slots whose last reader is a wgmma group: handed back to the producers once that group has completed
+    auto release = [&](int b, int a) {
+      __syncwarp();
+      if (lane == 0) {
+        if (b >= 0) mbar_arrive(&emptyB[b]);
+        if (a >= 0) mbar_arrive(&emptyA[a]);
+      }
+    };
+    int sa = 0, sl = 0, sb = 0;
+    uint32_t pa = 0, pl = 0, pb = 0;
     int it = 0;
-    for (int w = worker0; w < n_work; w += n_workers, ++it) {
-      const int tile = own_tile(w);
-      const int acc = it & 1;
-      const uint32_t acc_phase = (it >> 1) & 1;
+    [[maybe_unused]] int tr_n = 0;
+    for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x, ++it) {
+      ASYRP_TRACE_STAMP(5, it);
+      float acc[MT][BN / 2];
+#pragma unroll
+      for (int sub = 0; sub < MT; ++sub)
+#pragma unroll
+        for (int i = 0; i < BN / 2; ++i) acc[sub][i] = 0.f;
+      int up_a = 0, up_b = 0;  // up2: sub-pixel phase of this tile = first tap (ky, kx) of its 2x2 kernel
+      if (p.up2) {
+        const int ph = fast_div(tile, p.mul_m, p.m_tiles) / (p.Cout / BN);
+        up_a = ph >> 1;
+        up_b = ph & 1;
+      }
+      uint32_t accumulate = 0;
+      int rel_b = -1, rel_a = -1;  // slots read by the wgmma group in flight
+      for (int e = 0; e < p.n_sched; ++e) {
+        const int s = p.sched[e] >> 6;
+        const ConvSegDev sg = p.seg[s];
+        const bool lt = p.l_stages != 0 && sg.mode == 0;
+        const int ncopies = (sg.mode == 0 || sg.mode == 3) ? 1 : (sg.mode == 1 ? 3 : 9);
+        const int ntaps = sg.mode == 1 ? 3 : (sg.mode == 3 ? (p.up2 ? 4 : 9) : 1);
+        // byte strides inside the A stage: between 8-row groups, between sub-tiles, per ky / kx tap step
+        const uint32_t halo_pitch = (p.TW + 2) * 128u;
+        const uint32_t sbo = sg.mode == 3 ? halo_pitch : 1024u;
+        const uint32_t sub_stride = sg.mode == 3 ? p.TH * halo_pitch : p.TH * p.row_bytes;
+        // descriptors as (lo, hi) words: only the start-address field (16-byte units) changes inside the loop
+        const uint32_t a_hi = gmma_desc_hi(sbo), b_hi = gmma_desc_hi(1024u);
+        const uint32_t sub16 = sub_stride >> 4;
+        // this warpgroup's 64 rows start 8 row groups into the sub-tile
+        const uint32_t wg16 = (8u * wg * sbo) >> 4;
+        // tap step in 16-byte units.  mode 1: dy tap = row shift inside the dx copy; mode 3: (ky, kx) = pixel
+        // offset inside the halo tile: +128 B per kx, and from kx=2 to the next ky row +halo_pitch-256 B
+        // (up2: 2x2 taps starting at (up_a, up_b): +128 B per kx, +halo_pitch-128 B to the next ky row)
+        const uint32_t step16 = sg.mode == 3 ? 8u : (p.row_bytes >> 4);
+        const int kxn = p.up2 ? 2 : 3;
+        const uint32_t wrap16 = sg.mode == 3 ? ((halo_pitch - 128u * (kxn - 1)) >> 4) : step16;
+        const uint32_t first16 = (sg.mode == 3 && p.up2) ? ((up_a * halo_pitch + up_b * 128u) >> 4) : 0u;
+        for (int cp = 0; cp < ncopies; ++cp) {
+          const int slot = lt ? p.a_stages + sl : sa;
+          ASYRP_TRACE_STAMP(3, tr_n);
+          mbar_wait(p.any_transform ? &readyA[slot] : &fullA[slot], lt ? pl : pa);
+          ASYRP_TRACE_STAMP(4, tr_n);
+          ++tr_n;
+          uint32_t a_lo =
+              gmma_desc_lo(smem_u32(lt ? sL + sl * p.l_stage_bytes : sA + sa * p.a_stage_bytes)) + first16 + wg16;
+          int kx = 0;
+          for (int tp = 0; tp < ntaps; ++tp) {
+            mbar_wait(&fullB[sb], pb);
+            const uint32_t b_lo = b_lo0 + sb * (kBStage >> 4);
+            wgmma_fence();
+#pragma unroll
+            for (int sub = 0; sub < MT; ++sub) {
+#pragma unroll
+              for (int k = 0; k < 4; ++k)
+                wgmma_bn<BN>(acc[sub], gmma_desc(a_lo + sub * sub16 + 2 * k, a_hi), gmma_desc(b_lo + 2 * k, b_hi),
+                             (accumulate | k) ? 1u : 0u);
+            }
+            wgmma_commit();
+            // the group before this one has completed: its weight stage (and the activation stage it finished) go back
+            wgmma_wait<1>();
+            release(rel_b, rel_a);
+            rel_b = sb;
+            rel_a = tp == ntaps - 1 ? slot : -1;
+            accumulate = 1;
+            if (++sb == p.b_stages) { sb = 0; pb ^= 1; }
+            if (++kx == kxn) { kx = 0; a_lo += wrap16; } else { a_lo += step16; }
+          }
+          ASYRP_TRACE_STAMP(9, tr_n - 1);
+          if (lt) {
+            if (++sl == p.l_stages) { sl = 0; pl ^= 1; }
+          } else {
+            if (++sa == p.a_stages) { sa = 0; pa ^= 1; }
+          }
+        }
+      }
+      wgmma_wait<0>();
+      release(rel_b, rel_a);
+#pragma unroll
+      for (int sub = 0; sub < MT; ++sub) wgmma_fence_operands(acc[sub]);
+
+      // accumulators -> staging tile; the barrier before makes sure every consumer has drained the previous tile
+      named_bar_sync(3, kEpThreads);
+      if (warp == 0) ASYRP_TRACE_STAMP(7, it);
+      {
+        const int r0 = 64 * wg + 16 * q + (lane >> 2);
+#pragma unroll
+        for (int sub = 0; sub < MT; ++sub)
+#pragma unroll
+          for (int j = 0; j < BN / 8; ++j)
+#pragma unroll
+            for (int h = 0; h < 2; ++h)
+              *reinterpret_cast<float2*>(sC + (r0 + 8 * h) * kCPitch + sub * BN + 8 * j + 2 * (lane & 3)) =
+                  make_float2(acc[sub][4 * j + 2 * h], acc[sub][4 * j + 2 * h + 1]);
+      }
+      named_bar_sync(3, kEpThreads);
+      const uint32_t c_row = sC_addr + static_cast<uint32_t>(row * kCPitch) * 4u;
+
       const TileCoord tc = tile_coord(p, tile);
       const int tx = tc.tx, ty = tc.ty, tn = tc.tn;
       // up2: the channel-tile index carries the sub-pixel phase (a, b); outputs land on the (2H, 2W) grid
@@ -920,74 +767,11 @@ __global__ void __launch_bounds__(kNumThreads, 1) conv_gemm_kernel(const __grid_
         ph = nt / cts;
         nt -= ph * cts;
       }
-      const int ps = p.up2 ? 2 : 1, OH = p.H * ps, OW = p.W * ps, pa = ph >> 1, pb = ph & 1;
+      const int ps = p.up2 ? 2 : 1, OH = p.H * ps, OW = p.W * ps, pa_ = ph >> 1, pb_ = ph & 1;
       const int x = tx * p.TW + xx, n = tn * p.NB + nn;
       const int tile_in_sample = (ty * p.tiles_x + tx) * (p.up2 ? 4 : 1) + ph;
-      float* st = s_stats + acc * (4 * BN);
-      // swapped variant: this thread's bias (+temb) value, fetched before the wait (a global-load latency per tile)
-      float eb_swap = 0.f;
-      if constexpr (SWAP) {
-        if (p.ebias != nullptr)
-          eb_swap = p.ebias[static_cast<size_t>(tn) * p.ebias_stride + nt * 128 + q * 32 + lane];
-      }
-
-      mbar_wait_suspend(&tfull[acc], acc_phase);
-      if (warp == 2) ASYRP_TRACE_STAMP(7, it);
-      tc_fence_after();
-      if constexpr (SWAP) {
-        // thread = output channel (TMEM lane), registers = 32 consecutive pixels of the 8(16)-wide x 32(16)-tall
-        // tile.  The swapped tile is only selected when it lies fully inside the image (conv_config), so there are
-        // no bounds predicates here: this epilogue is instruction-issue bound (it set a ~9 us floor per tile).
-        const int c = nt * 128 + q * 32 + lane;
-        const float eb = eb_swap * p.acc_scale;
-        const bool odd = (lane & 1) != 0;
-        // lanes (2j, 2j+1) hold adjacent channels: the even lane stores pixel i, the odd lane pixel i+1, each as one
-        // half2 (channel pair) -> a warp store covers two pixels x 64 B
-        const uint32_t sel = odd ? 0x3276u : 0x5410u;
-        const int pix_stride = p.Cout * ps, row_stride = OW * pix_stride;
-        const int lane_off = odd ? pix_stride - 1 : 0;
-        const size_t obase = ((static_cast<size_t>(tn) * OH + ty * THT * ps + pa) * OW + tx * p.TW * ps + pb) * p.Cout + c;
-        float s1 = 0.f, s2 = 0.f;
-        const uint32_t tq = tmem_base + (static_cast<uint32_t>(q * 32) << 16) + acc * kAccCols;
-        if (p.res == nullptr) {
-          if (p.TW == 8)
-            swap_epilogue<3, MT, 0>(p, tq, half, obase, row_stride, pix_stride, lane_off, sel, eb, 0, 0, s1, s2);
-          else
-            swap_epilogue<4, MT, 0>(p, tq, half, obase, row_stride, pix_stride, lane_off, sel, eb, 0, 0, s1, s2);
-        } else if (p.res_mode == 0) {
-          if (p.TW == 8)
-            swap_epilogue<3, MT, 1>(p, tq, half, obase, row_stride, pix_stride, lane_off, sel, eb, 0, 0, s1, s2);
-          else
-            swap_epilogue<4, MT, 1>(p, tq, half, obase, row_stride, pix_stride, lane_off, sel, eb, 0, 0, s1, s2);
-        } else {
-          // residual source geometry for res_mode 1 (half resolution) / 2 (double resolution)
-          const int rW = p.res_mode == 1 ? (p.W >> 1) : (p.W << 1), rH = p.res_mode == 1 ? (p.H >> 1) : (p.H << 1);
-          const int rrow = rW * p.Cout;
-          const size_t rbase =
-              p.res_mode == 1
-                  ? ((static_cast<size_t>(tn) * rH + ((ty * THT) >> 1)) * rW + ((tx * p.TW) >> 1)) * p.Cout + c
-                  : ((static_cast<size_t>(tn) * rH + ty * THT * 2) * rW + tx * p.TW * 2) * p.Cout + c;
-          if (p.TW == 8)
-            swap_epilogue<3, MT, 2>(p, tq, half, obase, row_stride, pix_stride, lane_off, sel, eb, rbase, rrow, s1, s2);
-          else
-            swap_epilogue<4, MT, 2>(p, tq, half, obase, row_stride, pix_stride, lane_off, sel, eb, rbase, rrow, s1, s2);
-        }
-        if (p.stats != nullptr) {
-          // channel pair = lanes (2j, 2j+1); each (tile, half) owns one slot: nothing to reduce across warps
-          s1 += __shfl_xor_sync(0xffffffffu, s1, 1);
-          s2 += __shfl_xor_sync(0xffffffffu, s2, 1);
-          if ((lane & 1) == 0) {
-            *reinterpret_cast<float2*>(p.stats + ((static_cast<size_t>(tn) * tiles_per_sample * 2 +
-                                                    tile_in_sample * 2 + half) * (p.Cout / 2) + (c >> 1)) * 2) =
-                make_float2(s1, s2);
-            if (p.sums_out != nullptr) {
-              long long* q = p.sums_out + (static_cast<size_t>(tn) * (p.Cout / 2) + (c >> 1)) * 2;
-              stat_atomic_add(q, s1);
-              stat_atomic_add(q + 1, s2);
-            }
-          }
-        }
-      } else if constexpr (BN == 16) {
+      float* st = s_stats + (it & 1) * (4 * BN);
+      if constexpr (BN == 16) {
         // narrow-N tile of conv_out (3 / 6 real output channels, fp32 planar store): one 16-column load per sub-tile,
         // warps of the second half have nothing to drain
         if (half == 0) {
@@ -996,8 +780,7 @@ __global__ void __launch_bounds__(kNumThreads, 1) conv_gemm_kernel(const __grid_
             const int y = ty * THT + sub * p.TH + yy;
             const bool valid = (x < p.W) && (y < p.H) && (n < p.N);
             uint32_t r[16];
-            tmem_ld_32x16(tmem_base + (static_cast<uint32_t>(q * 32) << 16) + acc * (MT * BN) + sub * BN, r);
-            tmem_ld_wait();
+            ld_staged<16>(c_row + sub * BN * 4, r);
             if (valid) {
               const float* eb = p.ebias != nullptr ? p.ebias + static_cast<size_t>(n) * p.ebias_stride : nullptr;
               const size_t hw = static_cast<size_t>(p.H) * p.W;
@@ -1014,7 +797,7 @@ __global__ void __launch_bounds__(kNumThreads, 1) conv_gemm_kernel(const __grid_
         const int c0 = nt * BN + cc * 32;
         // statistics of this chunk: slot `lane` (see below) summed over the sub-tiles.  Reduced across the lanes once per
         // sub-tile: per-lane partial sums kept alive across the sub-tile loop (32 more registers next to r[] and v[])
-        // spill, and with 227 KB of shared memory carved out the L1 that would catch the spills is ~28 KB
+        // would spill
         float wtot = 0.f;
 #pragma unroll 1
         for (int sub = 0; sub < MT; ++sub) {
@@ -1024,11 +807,10 @@ __global__ void __launch_bounds__(kNumThreads, 1) conv_gemm_kernel(const __grid_
           const int y = ty * THT + sub * p.TH + yy;
           const bool valid = (x < p.W) && (y < p.H) && (n < p.N);
           // output row of this pixel: batch entry n may be a (sample, head) pair writing a channel slice
-          const size_t pix = ((static_cast<size_t>(n / p.out_heads) * OH + y * ps + pa) * OW + x * ps + pb) * p.out_ld +
+          const size_t pix = ((static_cast<size_t>(n / p.out_heads) * OH + y * ps + pa_) * OW + x * ps + pb_) * p.out_ld +
                              static_cast<size_t>(n % p.out_heads) * p.Cout;
           uint32_t r[32];
-          tmem_ld_32x32(tmem_base + (static_cast<uint32_t>(q * 32) << 16) + acc * (MT * BN) + sub * BN + cc * 32, r);
-          tmem_ld_wait();
+          ld_staged<32>(c_row + (sub * BN + cc * 32) * 4, r);
           float v[32];
 #pragma unroll
           for (int i = 0; i < 32; ++i) v[i] = __uint_as_float(r[i]);
@@ -1167,17 +949,10 @@ __global__ void __launch_bounds__(kNumThreads, 1) conv_gemm_kernel(const __grid_
         }  // sub
         if (p.stats != nullptr && p.NB == 1) st[(q * (BN / 32) + cc) * 32 + lane] = wtot;
       }  // cc
-      }  // !SWAP
-      // accumulator fully drained into registers/global: release it to the MMA warp
-      tc_fence_before();
-      __syncwarp();
-      if (warp == 2) ASYRP_TRACE_STAMP(8, it);
-      if (lane == 0) {
-        if constexpr (CTA2) mbar_arrive_remote(mapa_shared(smem_u32(&tempty[acc]), 0u));
-        else mbar_arrive(&tempty[acc]);
       }
+      if (warp == 0) ASYRP_TRACE_STAMP(8, it);
 
-      if (!SWAP && BN >= 32 && p.stats != nullptr && p.NB == 1) {
+      if (BN >= 32 && p.stats != nullptr && p.NB == 1) {
         named_bar_sync(1, kEpThreads);
         for (int e = ep_tid; e < BN; e += kEpThreads) {
           const int cc = e >> 5, j = e & 31;
@@ -1194,13 +969,6 @@ __global__ void __launch_bounds__(kNumThreads, 1) conv_gemm_kernel(const __grid_
       }
     }
   }
-
-  __syncthreads();
-  if constexpr (CTA2) cluster_sync_all();  // the peer may still read this CTA's shared memory / arrive on its barriers
-  if (warp == 1) {
-    tc_fence_after();
-    if constexpr (CTA2) tmem_dealloc_2cta(tmem_base, kTmemCols); else tmem_dealloc(tmem_base, kTmemCols);
-  }
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -1210,7 +978,6 @@ struct ConvOp {
   ConvParams p;
   int BN;
   int MT;
-  int cta2;  // launched as clusters of two CTAs sharing each weight tile (tcgen05 cta_group::2)
   int grid;
   size_t smem_bytes;
 };
@@ -1219,14 +986,10 @@ struct ConvOp {
 
 using namespace asyrp;
 
-static const void* conv_kernel_ptr(int BN, int MT, int cta2 = 0) {
-  if (cta2) return BN == 256 ? reinterpret_cast<const void*>(&conv_gemm_kernel<256, 1, false, true>)
-                             : reinterpret_cast<const void*>(&conv_gemm_kernel<128, 2, false, true>);
+static const void* conv_kernel_ptr(int BN, int MT) {
   if (BN == 16) return MT == 2 ? reinterpret_cast<const void*>(&conv_gemm_kernel<16, 2>)
                                : reinterpret_cast<const void*>(&conv_gemm_kernel<16, 1>);
-  if (BN == 256) return reinterpret_cast<const void*>(&conv_gemm_kernel<256, 1>);
-  if (BN == 128) return MT == 2 ? reinterpret_cast<const void*>(&conv_gemm_kernel<128, 2, true>)
-                                : reinterpret_cast<const void*>(&conv_gemm_kernel<128, 1>);
+  if (BN == 128) return reinterpret_cast<const void*>(&conv_gemm_kernel<128, 1>);
   return MT == 2 ? reinterpret_cast<const void*>(&conv_gemm_kernel<64, 2>)
                  : reinterpret_cast<const void*>(&conv_gemm_kernel<64, 1>);
 }
@@ -1285,32 +1048,10 @@ struct AsyrpConvDesc {
 
 static void conv_tile_shape(int H, int W, int halo, int* TW, int* TH, int* NB);
 
-static int g_cta2 = -1;
-static int cta2_enabled() {  // ASYRP_CTA2=0 / asyrp_set_cta2(0): never use the CTA-pair kernel (A/B measurements)
-  if (g_cta2 < 0) {
-    const char* e = getenv("ASYRP_CTA2");
-    g_cta2 = (e != nullptr && e[0] == '0') ? 0 : 1;
-  }
-  return g_cta2;
-}
-
-// CTA pairs for the 256 px x 128 ch tile too (instead of the one-CTA swapped-operand tile): each CTA of a pair keeps 64
-// of the 128 weight rows, so a CTA ingests (and writes to shared memory) half the weight bytes per tile.
-// ASYRP_PAIR128=0/1 / asyrp_set_pair128().
-static int g_pair128 = -1;
-static int pair128_enabled() {
-  if (g_pair128 < 0) {
-    const char* e = getenv("ASYRP_PAIR128");
-    g_pair128 = (e != nullptr) ? (e[0] != '0') : ASYRP_PAIR128_DEFAULT;
-  }
-  return g_pair128;
-}
 // The fused operand transform evaluates SiLU with ONE special-function op (tanh.approx.f32, 11 bits: absolute error
-// <= 2^-12 |x|, the size of the fp16 rounding the operand receives anyway) instead of ex2 + rcp.  The pipeline timeline
-// (scripts/conv_trace.py, profiles/r2_conv_pipeline_trace.md) shows the transform of a 3x3 stage taking as long as its 36
-// MMAs (4.5-5.0k vs 4.6k cycles), the tensor pipe waiting for "stage ready" 10-15 % of the time; with one MUFU and 4
-// instead of 7.5 instructions per element it takes 3.0k and the wait halves: +4.3 % images/s, end-to-end error
-// 3.4e-4 -> 4.0e-4 of max|x_0| on the bench fixture.  ASYRP_SILU_TANH=0 / asyrp_set_silu_tanh(0): the 2-MUFU form.
+// <= 2^-12 |x|, the size of the fp16 rounding the operand receives anyway) instead of ex2 + rcp: 4 instead of 7.5
+// instructions per element on the transform warps, whose work per 3x3 stage is comparable to that stage's MMAs.
+// ASYRP_SILU_TANH=0 / asyrp_set_silu_tanh(0): the 2-MUFU form.
 static int g_silu_tanh = -1;
 static int silu_tanh_enabled() {
   if (g_silu_tanh < 0) {
@@ -1319,25 +1060,14 @@ static int silu_tanh_enabled() {
   }
   return g_silu_tanh;
 }
-// Does a conv with this tile configuration run as CTA pairs?  Two horizontally adjacent pixel tiles share each weight
-// tile: needs an even number of pixel tiles per sample (so that the pairing does not depend on the batch) and, at the
-// nominal batch of 16, enough pairs to occupy the 74 TPCs.  The arithmetic per tile is that of the one-CTA kernel.
-// txy: pixel tiles per sample, n_tiles: channel tiles (x sub-pixel phases).
-static int conv_pairs(int bn, int mt, int NB, int txy, int n_tiles) {
-  if (!cta2_enabled() || NB != 1 || txy % 2 != 0 || (txy / 2) * 16 * n_tiles < 64) return 0;
-  if (bn == 256 && mt == 1) return 1;
-  if (bn == 128 && mt == 2) return pair128_enabled();
-  return 0;
-}
-
 // A 3x3/s1 conv whose output is at least 8 wide and 16 tall uses 8x16-pixel sub-tiles fed from one halo tile per
 // 64-channel chunk ("halo" geometry, segment mode 3); otherwise three dx-shifted copies (mode 1).
 static int conv_halo_ok(int H, int W) { return H % 16 == 0 && W % 8 == 0; }
 
 // Tile configuration: BN output channels x MT sub-tiles of 128 pixels per CTA tile.  Larger tiles re-use operands
-// better (BN=256, or the swapped-operand 128x256 variant for BN=128/MT=2: TMEM holds 2*MT*BN <= 512 fp32 columns);
-// small layers instead need enough tiles to occupy the 148 SMs.  Pick the most efficient configuration that still
-// yields ~a full wave of tiles at a NOMINAL batch of 16, else the one with the most tiles.  The choice must not
+// better (the accumulators of a consumer warpgroup, MT*BN/2 fp32 registers per thread, bound MT*BN <= 128); small
+// layers instead need enough tiles to occupy the 132 SMs of an H100 SXM.  Pick the most efficient configuration that
+// still yields ~a full wave of tiles (0.8 x 132) at a NOMINAL batch of 16, else the one with the most tiles.  The choice must not
 // depend on the actual batch: the tile partition fixes the summation order of the GroupNorm partial sums, and a
 // sample's result has to be bit-identical whatever batch (or batch shard on another GPU) it is part of.
 static void conv_config(int H, int W, int Cout, int halo, int* BN, int* MT, int phases = 1) {
@@ -1350,15 +1080,15 @@ static void conv_config(int H, int W, int Cout, int halo, int* BN, int* MT, int 
     return;
   }
   const int tiles_x = (W + TW - 1) / TW, tiles_n = (kNominalBatch + NB - 1) / NB;
-  const int cand[5][2] = {{256, 1}, {128, 2}, {128, 1}, {64, 2}, {64, 1}};  // by decreasing operand re-use
+  const int cand[3][2] = {{128, 1}, {64, 2}, {64, 1}};  // by decreasing operand re-use
   int best = -1, best_tiles = -1;
-  for (int i = 0; i < 5; ++i) {
+  for (int i = 0; i < 3; ++i) {
     const int bn = cand[i][0], mt = cand[i][1];
     if (Cout % bn != 0) continue;
-    // two stacked sub-tiles: whole tiles only (the swapped-operand epilogue has no bounds predicates)
+    // two stacked sub-tiles: whole tiles only
     if (mt == 2 && !(NB == 1 && H > 1 && H % (2 * TH) == 0 && W % TW == 0)) continue;
     const int tiles = tiles_x * ((H + TH * mt - 1) / (TH * mt)) * tiles_n * (Cout / bn) * phases;
-    if (tiles >= 120) { best = i; break; }
+    if (tiles >= 106) { best = i; break; }
     if (tiles > best_tiles) { best = i; best_tiles = tiles; }
   }
   *BN = cand[best][0];
@@ -1397,22 +1127,15 @@ ASYRP_API int asyrp_conv_stats_tiles(int H, int W, int Cout, int has_3x3) {
   conv_config(H, W, Cout, halo, &bn, &mt);
   const int tht = TH * mt;
   const int tiles = ((W + TW - 1) / TW) * ((H + tht - 1) / tht);
-  // swapped-operand kernel: one slot per (tile, warp half)
-  if (bn == 128 && mt == 2 && !conv_pairs(bn, mt, NB, tiles, Cout / bn)) return tiles * 2;
   return NB == 1 ? tiles : tiles * 4;
 }
 
-// tile configuration of a conv with this output geometry: BN * 16 + MT (e.g. 128 * 16 + 2 = the swapped-operand
-// 128-channel x 256-pixel tile).  Lets the caller route work that the swapped tile's epilogue handles badly (a
-// residual read through a resample index map: scattered 2-byte loads per lane) to another formulation.
+// tile configuration of a conv with this output geometry: BN * 16 + MT (e.g. 128 * 16 + 1 = 128 channels x 128 pixels)
 ASYRP_API int asyrp_conv_tile_config(int H, int W, int Cout, int has_3x3) {
-  int bn, mt, TW, TH, NB;
+  int bn, mt;
   const int halo = has_3x3 && conv_halo_ok(H, W);
   conv_config(H, W, Cout, halo, &bn, &mt);
-  conv_tile_shape(H, W, halo, &TW, &TH, &NB);
-  const int txy = ((W + TW - 1) / TW) * ((H + TH * mt - 1) / (TH * mt));
-  // bit 16: runs as CTA pairs (generic epilogue) — for 128 x 2 that means "not the swapped-operand tile"
-  return bn * 16 + mt + (conv_pairs(bn, mt, NB, txy, Cout / bn) ? (1 << 16) : 0);
+  return bn * 16 + mt;
 }
 
 // statistics slots per sample written by an up2 conv over an H x W SOURCE image (output 2H x 2W)
@@ -1422,9 +1145,7 @@ ASYRP_API int asyrp_conv_stats_tiles_up2(int H, int W, int Cout) {
   conv_tile_shape(H, W, 1, &TW, &TH, &NB);
   conv_config(H, W, Cout, 1, &bn, &mt, 4);
   const int tht = TH * mt;
-  const int txy = ((W + TW - 1) / TW) * ((H + tht - 1) / tht);
-  const int tiles = txy * 4;
-  return (bn == 128 && mt == 2 && !conv_pairs(bn, mt, NB, txy, 4 * (Cout / bn))) ? tiles * 2 : tiles;
+  return ((W + TW - 1) / TW) * ((H + tht - 1) / tht) * 4;
 }
 
 ASYRP_API int asyrp_conv_create(const AsyrpConvDesc* d, void** out_op) {
@@ -1457,9 +1178,6 @@ ASYRP_API int asyrp_conv_create(const AsyrpConvDesc* d, void** out_op) {
   p.tiles_n = (d->N + p.NB - 1) / p.NB;
   p.m_tiles = p.tiles_x * p.tiles_y * p.tiles_n;
   p.n_tiles = (d->Cout / op->BN) * (p.up2 ? 4 : 1);
-  op->cta2 = !d->weight_batched && d->a_heads <= 1 && d->out_heads <= 1 && !d->out_f32 &&
-             conv_pairs(op->BN, op->MT, p.NB, p.tiles_x * p.tiles_y, p.n_tiles);
-  const bool swapped = op->BN == 128 && op->MT == 2 && !op->cta2;  // the one-CTA swapped-operand tile
   {
     // x / dv == umulhi(x, 2^32/dv + 1) for all x with x*dv < 2^32; the largest dividend is the tile count
     const unsigned long long xmax = static_cast<unsigned long long>(p.m_tiles) * p.n_tiles;
@@ -1549,7 +1267,7 @@ ASYRP_API int asyrp_conv_create(const AsyrpConvDesc* d, void** out_op) {
     ASYRP_REQUIRE(bh == 1 || wld >= bh * static_cast<uint64_t>(ktot), "asyrp_conv_create: b_heads needs weight_ld >= heads*K");
     // dim 2 = head (column slices of width K inside a row of weight_ld elements), dim 3 = sample
     uint64_t strides[3] = {wld * 2, (bh > 1 ? static_cast<uint64_t>(ktot) : wbs) * 2, wbs * 2};
-    uint32_t box[4] = {64, static_cast<uint32_t>(op->cta2 ? op->BN / 2 : op->BN), 1, 1};
+    uint32_t box[4] = {64, static_cast<uint32_t>(op->BN), 1, 1};
     int rc = encode_tensor_map(&p.tmB, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 4, d->weight, dims, strides, box,
                                CU_TENSOR_MAP_SWIZZLE_128B);
     if (rc != ASYRP_OK) { delete op; return rc; }
@@ -1581,19 +1299,20 @@ ASYRP_API int asyrp_conv_create(const AsyrpConvDesc* d, void** out_op) {
   p.out_heads = d->out_heads > 1 ? d->out_heads : 1;
   p.out_ld = d->Cout * p.out_heads;
   p.out_f32 = d->out_f32;
-  ASYRP_REQUIRE(!d->out_f32 || (d->residual == nullptr && d->stats == nullptr && d->out_planar == nullptr && !swapped),
-                "asyrp_conv_create: out_f32 excludes residual / stats / planar output and the swapped-operand tile");
-  ASYRP_REQUIRE(p.out_heads == 1 || (d->N % p.out_heads == 0 && d->stats == nullptr && d->out_planar == nullptr &&
-                                     !swapped),
-                "asyrp_conv_create: out_heads needs N %% heads == 0, no stats / planar output, Cout != 128*odd");
+  ASYRP_REQUIRE(!d->out_f32 || (d->residual == nullptr && d->stats == nullptr && d->out_planar == nullptr),
+                "asyrp_conv_create: out_f32 excludes residual / stats / planar output");
+  ASYRP_REQUIRE(p.out_heads == 1 || (d->N % p.out_heads == 0 && d->stats == nullptr && d->out_planar == nullptr),
+                "asyrp_conv_create: out_heads needs N %% heads == 0, no stats / planar output");
   p.a_stage_bytes = halo ? (((THT + 2) * (p.TW + 2) * 128u + 1023u) / 1024u) * 1024u
                          : (any3 ? THT + 2 : THT) * p.row_bytes;
-  const uint32_t b_stage = (op->cta2 ? op->BN / 2 : op->BN) * 128;
-  // operand rings: everything the 227 KB of shared memory leaves after barriers and the statistics scratch.
-  // Activations: 3-4 stages; weights: as deep as fits (<= 16 stages) — small-N tiles issue an MMA group every ~100
-  // cycles, so the weight prefetch must run many K steps ahead of the ~1 us TMA latency.
+  const uint32_t b_stage = op->BN * 128;
+  // accumulator staging tile of the epilogue: 128 pixel rows x (MT*BN + 4) fp32
+  const uint32_t staging = 128u * (op->MT * op->BN + 4) * 4u;
+  // operand rings: everything the 227 KB of shared memory leaves after the staging tile, barriers and the statistics
+  // scratch.  Activations: 3-4 stages; weights: as deep as fits (<= 16 stages) — small-N tiles issue an MMA group
+  // every ~100 cycles, so the weight prefetch must run many K steps ahead of the ~1 us TMA latency.
   const uint32_t ring_budget = 227 * 1024 - 1024 /*alignment*/ - 1024 /*barriers*/ - 2 * 4 * op->BN * 4 /*stats*/ -
-                               2048 /*per-tile GroupNorm group statistics: 2 x 3 x 32 float2*/;
+                               2048 /*per-tile GroupNorm group statistics: 2 x 3 x 32 float2*/ - staging;
   bool has_light = false;
   for (int s = 0; s < d->nseg; ++s) has_light = has_light || d->seg[s].mode == 0;
   p.l_stages = 0;
@@ -1608,7 +1327,7 @@ ASYRP_API int asyrp_conv_create(const AsyrpConvDesc* d, void** out_op) {
 #ifdef ASYRP_TRACE
   if (const char* e = getenv("ASYRP_A_STAGES")) {  // diagnostic build: ring depths from the environment
     const int v = atoi(e);
-    if (v >= 2 && !(op->BN == 128 && op->MT == 2)) p.a_stages = v;
+    if (v >= 2) p.a_stages = v;
   }
   if (const char* e = getenv("ASYRP_L_STAGES")) {
     const int v = atoi(e);
@@ -1631,14 +1350,10 @@ ASYRP_API int asyrp_conv_create(const AsyrpConvDesc* d, void** out_op) {
   p.planar_c = d->planar_c;
   ASYRP_REQUIRE(d->out_planar == nullptr || (d->planar_c >= 1 && d->planar_c <= 8),
                 "asyrp_conv_create: planar_c=%d out of range", d->planar_c);
-  ASYRP_REQUIRE(!(d->out_planar != nullptr && swapped),
-                "asyrp_conv_create: planar output needs Cout == 64 (padded conv_out)");
   p.res = static_cast<const __half*>(d->residual);
   p.res_scale = d->res_scale;
   p.acc_scale = d->acc_scale;
   p.scales = d->scales;
-  ASYRP_REQUIRE(d->scales == nullptr || !swapped,
-                "asyrp_conv_create: device-side scales are not supported by the swapped-operand tile");
   p.res_mode = d->residual != nullptr ? d->res_mode : 0;
   ASYRP_REQUIRE(p.res_mode >= 0 && p.res_mode <= 2, "asyrp_conv_create: res_mode %d", d->res_mode);
   ASYRP_REQUIRE(p.res_mode == 0 || (!p.up2 && p.out_heads == 1 && !d->out_f32 && d->out_planar == nullptr &&
@@ -1651,18 +1366,14 @@ ASYRP_API int asyrp_conv_create(const AsyrpConvDesc* d, void** out_op) {
                 "asyrp_conv_create: sums_out needs stats and tiles inside one sample");
   op->smem_bytes = 1024 + static_cast<size_t>(p.a_stages) * p.a_stage_bytes +
                    static_cast<size_t>(p.l_stages) * p.l_stage_bytes + static_cast<size_t>(p.b_stages) * b_stage +
-                   (3 * (p.a_stages + p.l_stages) + 2 * p.b_stages + 4) * 8 + 16 + 2 * 4 * op->BN * 4 +
+                   staging + (3 * (p.a_stages + p.l_stages) + 2 * p.b_stages) * 8 + 2 * 4 * op->BN * 4 +
                    2 * kMaxSeg * 32 * sizeof(float2);
   ASYRP_REQUIRE(op->smem_bytes <= 227 * 1024, "asyrp_conv_create: smem %zu too large", op->smem_bytes);
   const int sms = sm_count();
   if (sms <= 0) { delete op; return ASYRP_ERR_NO_DEVICE; }
   const int total = p.m_tiles * p.n_tiles;
   op->grid = total < sms ? total : sms;
-  if (op->cta2) {
-    const int pairs = total / 2, clusters = sms / 2;
-    op->grid = 2 * (pairs < clusters ? pairs : clusters);
-  }
-  cudaError_t e = cudaFuncSetAttribute(conv_kernel_ptr(op->BN, op->MT, op->cta2),
+  cudaError_t e = cudaFuncSetAttribute(conv_kernel_ptr(op->BN, op->MT),
                                        cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
   if (e != cudaSuccess) {
     set_error("asyrp_conv_create: cudaFuncSetAttribute: %s", cudaGetErrorString(e));
@@ -1679,7 +1390,7 @@ ASYRP_API int asyrp_conv_launch(void* handle, void* stream) {
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   void* args[] = {&op->p};
   cudaLaunchConfig_t cfg = {};
-  cudaLaunchAttribute attr[2];
+  cudaLaunchAttribute attr[1];
   cfg.gridDim = dim3(op->grid);
   cfg.blockDim = dim3(kNumThreads);
   cfg.dynamicSmemBytes = op->smem_bytes;
@@ -1690,14 +1401,7 @@ ASYRP_API int asyrp_conv_launch(void* handle, void* stream) {
     attr[cfg.numAttrs].val.programmaticStreamSerializationAllowed = 1;
     ++cfg.numAttrs;
   }
-  if (op->cta2) {
-    attr[cfg.numAttrs].id = cudaLaunchAttributeClusterDimension;
-    attr[cfg.numAttrs].val.clusterDim.x = 2;
-    attr[cfg.numAttrs].val.clusterDim.y = 1;
-    attr[cfg.numAttrs].val.clusterDim.z = 1;
-    ++cfg.numAttrs;
-  }
-  ASYRP_CHECK_CUDA(cudaLaunchKernelExC(&cfg, conv_kernel_ptr(op->BN, op->MT, op->cta2), args));
+  ASYRP_CHECK_CUDA(cudaLaunchKernelExC(&cfg, conv_kernel_ptr(op->BN, op->MT), args));
   return ASYRP_OK;
 }
 
@@ -1713,11 +1417,6 @@ ASYRP_API int asyrp_conv_set_scales(void* handle, float acc_scale, float res_sca
 
 ASYRP_API void asyrp_conv_destroy(void* handle) { delete static_cast<ConvOp*>(handle); }
 
-// CTA-pair (tcgen05 cta_group::2) variant of the 128 px x 256 ch tile: on by default; affects ops created afterwards
-ASYRP_API int asyrp_set_cta2(int enabled) {
-  g_cta2 = enabled ? 1 : 0;
-  return ASYRP_OK;
-}
 #ifdef ASYRP_TRACE
 // diagnostic build only: device buffer [grid][kTraceRoles][kTraceLen] int64 receiving the pipeline timeline
 ASYRP_API int asyrp_conv_set_trace(void* handle, long long* buf) {
@@ -1726,19 +1425,11 @@ ASYRP_API int asyrp_conv_set_trace(void* handle, long long* buf) {
   return static_cast<ConvOp*>(handle)->grid;
 }
 #endif
-// CTA pairs for the 256 px x 128 ch tile (instead of the swapped-operand tile); affects ops created afterwards AND the
-// statistics-slot counts asyrp_conv_stats_tiles*() report — set it before building a plan
-ASYRP_API int asyrp_set_pair128(int enabled) {
-  g_pair128 = enabled < 0 ? -1 : (enabled ? 1 : 0);  // negative: back to the default (ASYRP_PAIR128, else built-in)
-  return ASYRP_OK;
-}
 // SiLU of the fused operand transform: 1 = one tanh.approx (default), 0 = ex2 + rcp; negative: back to the default
 // (ASYRP_SILU_TANH).  Affects ops created afterwards.
 ASYRP_API int asyrp_set_silu_tanh(int enabled) {
   g_silu_tanh = enabled < 0 ? -1 : (enabled ? 1 : 0);
   return ASYRP_OK;
 }
-// 1 if `op` runs as CTA pairs
-ASYRP_API int asyrp_conv_is_cta2(void* handle) { return handle ? static_cast<ConvOp*>(handle)->cta2 : 0; }
 
 }  // extern "C"

@@ -469,7 +469,7 @@ using namespace asyrp;
 
 static inline int grid_for(size_t total, int block, int cap_mult = 8) {
   size_t g = (total + block - 1) / block;
-  const size_t cap = static_cast<size_t>(sm_count() > 0 ? sm_count() : 148) * cap_mult;
+  const size_t cap = static_cast<size_t>(sm_count() > 0 ? sm_count() : 132) * cap_mult;
   if (g > cap) g = cap;
   if (g < 1) g = 1;
   return static_cast<int>(g);
@@ -508,7 +508,7 @@ ASYRP_API int asyrp_apply(const void* src_a, int Ca, const void* src_b, int Cb, 
   const int threads = lanes * octs;
   const int npix = p.Ho * p.Wo;
   int gx = (npix + lanes * 4 - 1) / (lanes * 4);
-  const int cap = (sm_count() > 0 ? sm_count() : 148) * 8;
+  const int cap = (sm_count() > 0 ? sm_count() : 132) * 8;
   const int max_gx = cap / N > 0 ? cap / N : 1;
   if (gx > max_gx) gx = max_gx;
   if (gx < 1) gx = 1;

@@ -1,5 +1,5 @@
-// Thin inline-PTX wrappers for the sm_100a features the Asyrp kernels use:
-// mbarrier, TMA (cp.async.bulk.tensor), tcgen05 (alloc / mma / commit / ld), proxy fences.
+// Thin inline-PTX wrappers for the sm_90a features the Asyrp kernels use:
+// mbarrier, TMA (cp.async.bulk.tensor), wgmma (fence / mma_async / commit / wait), proxy fences.
 // Only what the kernels in this directory need; everything is __device__ __forceinline__.
 #pragma once
 #include <cstdint>
@@ -17,10 +17,10 @@ __device__ __forceinline__ int lane_id() { return threadIdx.x & 31; }
 // computed inside them from uniform inputs lives in uniform registers).
 __device__ __forceinline__ int uniform_warp_id() { return __shfl_sync(0xffffffffu, threadIdx.x >> 5, 0); }
 
-// elect.sync: true in exactly one lane of a converged warp.  The single-thread instructions (tcgen05.mma / commit,
-// TMA) take uniform-register operands: issued from warp-uniform control flow under this predicate they compile to
-// a plain predicated instruction; issued from an `if (lane == 0)` branch the compiler wraps every one of them in
-// a vote / R2UR / BRA.U.ANY "waterfall" loop (~140 cycles per MMA: the K loop of the N<=128 tiles was bound by it).
+// elect.sync: true in exactly one lane of a converged warp.  The single-thread TMA instructions take uniform-register
+// operands: issued from warp-uniform control flow under this predicate they compile to a plain predicated
+// instruction; issued from an `if (lane == 0)` branch the compiler wraps every one of them in a vote / R2UR /
+// BRA.U.ANY "waterfall" loop.
 __device__ __forceinline__ bool elect_one() {
   uint32_t pred;
   asm volatile(
@@ -91,7 +91,7 @@ __device__ __forceinline__ void mbar_wait_suspend(uint64_t* bar, uint32_t parity
 }
 
 // ---------------------------------------------------------------- proxy fences
-// generic-proxy smem writes -> visible to the async proxy (TMA / tcgen05 operand reads)
+// generic-proxy smem writes -> visible to the async proxy (TMA / wgmma operand reads)
 __device__ __forceinline__ void fence_proxy_async_smem() {
   asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
 }
@@ -125,171 +125,73 @@ __device__ __forceinline__ void tma_load_5d(void* smem_dst, const void* tmap, ui
       : "memory");
 }
 
-// ---------------------------------------------------------------- tcgen05 / TMEM
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_dst, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_dst)),
-               "r"(ncols)
-               : "memory");
+// ---------------------------------------------------------------- wgmma (warpgroup MMA, sm_90a)
+// D[64 x N registers of the warpgroup] (+)= A[smem desc, 64 x 16] * B[smem desc, N x 16]^T, fp16 operands (both
+// K-major), fp32 accumulators.  Accumulator fragment of thread t (warp w = t/32 of the warpgroup, lane l):
+// d[4j + 2h + e] = D[16w + l/4 + 8h][8j + 2(l%4) + e].
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() {
+  asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory");
 }
-__device__ __forceinline__ void tmem_relinquish() {
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
+// keeps the compiler from moving accesses of accumulator registers across wgmma_fence / wgmma_wait
+template <int R>
+__device__ __forceinline__ void wgmma_fence_operands(float (&d)[R]) {
+#pragma unroll
+  for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() {
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-}
-__device__ __forceinline__ void tc_fence_after() {
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-}
-// D[tmem] (+)= A[smem desc] * B[smem desc], kind::f16 (fp16/bf16 operands, fp32 accumulate)
-__device__ __forceinline__ void umma_f16(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc,
-                                         uint32_t accumulate) {
+__device__ __forceinline__ void wgmma_f16_n16(float (&d)[8], uint64_t desc_a, uint64_t desc_b,
+                                                uint32_t accumulate) {
   asm volatile(
       "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}" ::"r"(tmem_d),
-      "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
+      "setp.ne.b32 p, %10, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n16k16.f32.f16.f16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7}, "
+      "%8, %9, p, 1, 1, 0, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+      : "l"(desc_a), "l"(desc_b), "r"(accumulate)
       : "memory");
 }
-// same, descriptors given as (lo, hi) words: the K-loop only ever changes the 14-bit start-address field (lo)
-__device__ __forceinline__ void umma_f16_w(uint32_t tmem_d, uint32_t a_lo, uint32_t a_hi, uint32_t b_lo,
-                                           uint32_t b_hi, uint32_t idesc, uint32_t accumulate) {
+__device__ __forceinline__ void wgmma_f16_n64(float (&d)[32], uint64_t desc_a, uint64_t desc_b,
+                                                uint32_t accumulate) {
   asm volatile(
-      "{\n\t.reg .pred p;\n\t.reg .b64 da, db;\n\t"
-      "mov.b64 da, {%1, %2};\n\t"
-      "mov.b64 db, {%3, %4};\n\t"
-      "setp.ne.b32 p, %6, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], da, db, %5, p;\n\t}" ::"r"(tmem_d),
-      "r"(a_lo), "r"(a_hi), "r"(b_lo), "r"(b_hi), "r"(idesc), "r"(accumulate)
+      "{\n\t.reg .pred p;\n\t"
+      "setp.ne.b32 p, %34, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, "
+      "%32, %33, p, 1, 1, 0, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "l"(desc_a), "l"(desc_b), "r"(accumulate)
       : "memory");
 }
-// arrive on an mbarrier when all previously issued tcgen05 async ops of this thread complete
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(
-                   smem_u32(bar))
-               : "memory");
-}
-// 32 lanes x 32 columns of fp32: thread i of the warp gets lane (base_lane + i), columns [col, col+32)
-__device__ __forceinline__ void tmem_ld_32x32(uint32_t taddr, uint32_t (&r)[32]) {
+__device__ __forceinline__ void wgmma_f16_n128(float (&d)[64], uint64_t desc_a, uint64_t desc_b,
+                                                uint32_t accumulate) {
   asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-        "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]),
-        "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]),
-        "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]),
-        "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
+      "{\n\t.reg .pred p;\n\t"
+      "setp.ne.b32 p, %66, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, "
+      "%64, %65, p, 1, 1, 0, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "l"(desc_a), "l"(desc_b), "r"(accumulate)
       : "memory");
 }
-// 32 lanes x 16 columns (narrow-N accumulators: the 3/6-channel conv_out tile)
-__device__ __forceinline__ void tmem_ld_32x16(uint32_t taddr, uint32_t (&r)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-        "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
 
-// K-major, SWIZZLE_128B shared-memory matrix descriptor (rows of 128 B, 8-row atoms of 1024 B).
-// Field layout follows the PTX ISA "tcgen05 shared memory descriptor": start>>4 [0,14), LBO>>4 [16,30),
-// SBO>>4 [32,46), version=1 [46,48), base_offset [49,52), layout_type [61,64) (2 = SWIZZLE_128B).
+// K-major, SWIZZLE_128B shared-memory matrix descriptor of wgmma (rows of 128 B, 8-row atoms).
+// Field layout follows the PTX ISA "matrix descriptor format": start>>4 [0,14), LBO>>4 [16,30), SBO>>4 [32,46),
+// base_offset [49,52) (0: every operand stage is 1024B-aligned), layout_type [62,64) (1 = SWIZZLE_128B).
 // sbo_bytes: distance between consecutive 8-row groups (1024 for a dense tile; (TW+2)*128 when the rows are the
 // pixels of a halo tile whose image rows are TW+2 pixels apart).  The 128B swizzle is a function of the shared
 // memory ADDRESS bits (chunk ^= (addr >> 7) & 7), so start addresses need only be 16B-aligned as long as the data
 // was written with the same address-based pattern (TMA does, given a 1024B-aligned box base).
-__device__ __forceinline__ uint64_t umma_desc_k128(uint32_t smem_addr, uint32_t sbo_bytes = 1024) {
-  uint64_t d = 0;
-  d |= static_cast<uint64_t>((smem_addr & 0x3FFFF) >> 4);
-  d |= static_cast<uint64_t>(1) << 16;            // LBO (unused for swizzled K-major)
-  d |= static_cast<uint64_t>(sbo_bytes >> 4) << 32;  // SBO: bytes between 8-row groups
-  d |= static_cast<uint64_t>(1) << 46;            // descriptor version (Blackwell)
-  d |= static_cast<uint64_t>(2) << 61;            // SWIZZLE_128B
-  return d;
-}
-// the two 32-bit words of umma_desc_k128(): lo = start address field (+ LBO), hi = SBO / version / swizzle mode
-__device__ __forceinline__ uint32_t umma_desc_lo(uint32_t smem_addr) {
+// lo word = start address field (+ LBO), hi word = SBO / swizzle mode: the K loop only ever changes lo.
+__device__ __forceinline__ uint32_t gmma_desc_lo(uint32_t smem_addr) {
   return ((smem_addr & 0x3FFFF) >> 4) | (1u << 16);
 }
-__device__ __forceinline__ uint32_t umma_desc_hi(uint32_t sbo_bytes) {
-  return (sbo_bytes >> 4) | (1u << 14) | (2u << 29);
-}
-// Instruction descriptor for kind::f16: fp16 A/B (K-major), fp32 D, M=128, N=n.
-__host__ __device__ constexpr uint32_t umma_idesc_f16_m128(uint32_t n) {
-  return (1u << 4) | (0u << 7) | (0u << 10) | ((n >> 3) << 17) | ((128u >> 4) << 24);
-}
-
-// ---------------------------------------------------------------- CTA pairs (cta_group::2)
-// Two CTAs of a cluster (the two SMs of a TPC) execute one M=256 MMA: each holds its own 128 A rows and half of the
-// B columns in its shared memory, the leader (cluster rank 0) issues, accumulators land in both CTAs' TMEM.
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-  return r;
-}
-__device__ __forceinline__ void cluster_sync_all() {
-  asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-// shared::cluster address of the same shared-memory offset in CTA `rank` of the cluster
-__device__ __forceinline__ uint32_t mapa_shared(uint32_t addr, uint32_t rank) {
-  uint32_t r;
-  asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(addr), "r"(rank));
-  return r;
-}
-// arrive on an mbarrier of another CTA of the cluster (release at cluster scope: this thread's prior writes,
-// including fenced generic-proxy writes to its own shared memory, are ordered before the arrival)
-__device__ __forceinline__ void mbar_arrive_remote(uint32_t cluster_addr) {
-  asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(cluster_addr) : "memory");
-}
-__device__ __forceinline__ void tmem_alloc_2cta(uint32_t* smem_dst, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_dst)),
-               "r"(ncols)
-               : "memory");
-}
-__device__ __forceinline__ void tmem_relinquish_2cta() {
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc_2cta(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-// M=256 MMA of the CTA pair; descriptors are shared-memory offsets valid in BOTH CTAs
-__device__ __forceinline__ void umma_f16_w_2cta(uint32_t tmem_d, uint32_t a_lo, uint32_t a_hi, uint32_t b_lo,
-                                                uint32_t b_hi, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t.reg .b64 da, db;\n\t"
-      "mov.b64 da, {%1, %2};\n\t"
-      "mov.b64 db, {%3, %4};\n\t"
-      "setp.ne.b32 p, %6, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], da, db, %5, p;\n\t}" ::"r"(tmem_d),
-      "r"(a_lo), "r"(a_hi), "r"(b_lo), "r"(b_hi), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// completion of all prior MMAs of the pair -> arrive on the mbarrier at this offset in both CTAs
-__device__ __forceinline__ void umma_commit_2cta(uint64_t* bar) {
-  asm volatile(
-      "tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(
-          smem_u32(bar)),
-      "h"(static_cast<uint16_t>(3))
-      : "memory");
-}
-// TMA load into this CTA's shared memory whose completion bytes are counted on an mbarrier that may live in the
-// peer CTA (cluster address)
-__device__ __forceinline__ void tma_load_4d_2cta(void* smem_dst, const void* tmap, uint32_t bar_cluster_addr, int c0,
-                                                 int c1, int c2, int c3) {
-  asm volatile(
-      "cp.async.bulk.tensor.4d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes"
-      " [%0], [%1, {%3, %4, %5, %6}], [%2];" ::"r"(smem_u32(smem_dst)),
-      "l"(reinterpret_cast<uint64_t>(tmap)), "r"(bar_cluster_addr), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
-      : "memory");
-}
-__host__ __device__ constexpr uint32_t umma_idesc_f16_m256(uint32_t n) {
-  return (1u << 4) | (0u << 7) | (0u << 10) | ((n >> 3) << 17) | ((256u >> 4) << 24);
+__device__ __forceinline__ uint32_t gmma_desc_hi(uint32_t sbo_bytes) { return (sbo_bytes >> 4) | (1u << 30); }
+__device__ __forceinline__ uint64_t gmma_desc(uint32_t lo, uint32_t hi) {
+  return (static_cast<uint64_t>(hi) << 32) | lo;
 }
 
 // ---------------------------------------------------------------- programmatic dependent launch

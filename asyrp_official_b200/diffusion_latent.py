@@ -1,4 +1,4 @@
-"""`Asyrp` runner — inference/editing half of the reference's diffusion_latent.py on the B200 engine.
+"""`Asyrp` runner — inference/editing half of the reference's diffusion_latent.py on the CUDA engine.
 
 Mirrors, with the same attribute / flag names:
   Asyrp.__init__               diffusion_latent.py:32-73    betas, logvar tables

@@ -29,17 +29,13 @@ DUAL_STREAM = os.environ.get("ASYRP_DUAL_STREAM", "1") != "0"
 FUSE_MIN_H = int(os.environ.get("ASYRP_FUSE_MIN_H", "16"))
 # ASYRP_GN_FOLD=1: GroupNorm finalised inside the consuming conv kernel from integer-atomic per-sample sums the
 # producers' epilogues accumulate (no gn_finalize launch, no affine table) for every layer of at least 16x16: 226 instead
-# of 315 launches per edit evaluation, non-conv time 1.04 -> 0.68 ms — but the conv kernels pay more than that back
-# (per-tile group statistics on the transform warps' critical path, 64-bit atomics in every epilogue): measured
-# 34.2 -> 32.0 img/s (DDPM b16), 35.8 -> 33.7 (AFHQ b8), 5.45 -> 5.17 (ImageNet b4).  Off by default; the path is
-# complete and covered by tests (test_groupnorm_finalised_inside_the_consumer_conv, and the whole GPU suite passes
-# with it on).
+# of 315 launches per edit evaluation — at the price of per-tile group statistics on the transform warps' critical
+# path and 64-bit atomics in every epilogue.  Off by default; the path is complete and covered by tests
+# (test_groupnorm_finalised_inside_the_consumer_conv).
 GN_FOLD = os.environ.get("ASYRP_GN_FOLD", "0") in ("1", "2")
 GN_FOLD_PRODUCERS_ONLY = os.environ.get("ASYRP_GN_FOLD", "0") == "2"  # diagnostic: atomics on, consumers use tables
 # ResBlock identity skips x + h ride conv2's K loop as an identity weight block (C extra MACs per output, exact: fp16 x
-# times 1.0 into the fp32 accumulator).  ASYRP_SKIP_AS_K=0 reads x in the epilogue instead.  A/B on one B200 (round 2,
-# ABAB order): 35.57 / 35.51 img/s with the K columns vs 34.39 / 34.30 with the epilogue read — the scattered fp16
-# residual loads of the swapped-operand epilogue cost more than 11 % extra MMAs on those convs.
+# times 1.0 into the fp32 accumulator).  ASYRP_SKIP_AS_K=0 reads x in the epilogue instead.
 SKIP_AS_K = os.environ.get("ASYRP_SKIP_AS_K", "1") != "0"
 
 
@@ -387,7 +383,7 @@ class Plan:
         eoff = eng.emb_off[p]
         mode = {"none": RESAMPLE_NONE, "up": RESAMPLE_UP2, "down": RESAMPLE_AVGPOOL2}[layer.resample]
         aff1 = self._gn(srcs, W[p + ".g1"], W[p + ".be1"])
-        xr, a1, res_mode, up_fused = None, None, 0, False
+        a1, res_mode, up_fused = None, 0, False
         if mode != RESAMPLE_NONE:
             # ADM up/down block: the resample sits between SiLU and the conv, and the skip branch is resampled too
             # (unet.py:279-284).  The skip branch is never materialised: conv2's epilogue reads x through the resample
@@ -396,13 +392,6 @@ class Plan:
             # materialised (a quarter of the input's size).
             src = srcs[0]
             res_mode = 1 if mode == RESAMPLE_UP2 else 2
-            Ho = src.H * 2 if mode == RESAMPLE_UP2 else src.H // 2
-            if ops.conv_tile_config(Ho, Ho * src.W // src.H, layer.cout, True) == (128, 2):
-                # swapped-operand tile: its epilogue owns one channel per lane, a resampled residual is 32 scattered
-                # 2-byte loads per chunk (measured 260 vs 121 us at 256^2) -> materialise x_upd(x) and add it as
-                # identity K columns like every other skip
-                res_mode = 0
-                xr = self._apply(srcs, None, 0, mode)
             up_fused = mode == RESAMPLE_UP2 and src.H >= 16 and ops.conv_stats_tiles_up2(src.H, src.W, layer.cout) > 0
             if up_fused:
                 H, Wd = 2 * src.H, 2 * src.W
@@ -435,16 +424,14 @@ class Plan:
         elif layer.cin != layer.cout:
             out, _ = self._conv(segs2 + [(s_, MODE_1x1) for s_ in srcs], W[p + ".w2"], layer.cout, H, Wd,
                                 ebias=W[p + ".b2"])
-        elif SKIP_AS_K or xr is not None:
-            out, _ = self._conv(segs2 + [(xr if xr is not None else srcs[0], MODE_1x1)], W[p + ".w2"], layer.cout, H, Wd,
+        elif SKIP_AS_K:
+            out, _ = self._conv(segs2 + [(srcs[0], MODE_1x1)], W[p + ".w2"], layer.cout, H, Wd,
                                 ebias=W[p + ".b2"],
                                 algo_flops=2.0 * self.N * H * Wd * layer.cout * 9 * layer.cout)
         else:
             out, _ = self._conv(segs2, W[p + ".w2r"], layer.cout, H, Wd, ebias=W[p + ".b2"], residual=srcs[0])
         aff2.release()
         self._free(h)
-        if xr is not None:
-            self._free(xr)
         self._drop_temps()
         return out
 
@@ -590,8 +577,8 @@ class Plan:
                                        st["use_mask"]), "slerp")
         # ---- decoders: (h2 -> et_mod) and (h -> et); same weights, same skip tensors.  The second pass allocates from
         # its own pool: in an edit step the two passes are independent and run CONCURRENTLY on two streams
-        # (run_edit_and_decoder) — a persistent conv kernel leaves SMs idle in its last wave (512 tiles on 148 SMs =
-        # 3.46 rounds), and the other pass's kernel fills them
+        # (run_edit_and_decoder) — a persistent conv kernel leaves SMs idle in its last wave (512 tiles on 132 SMs =
+        # 3.88 rounds), and the other pass's kernel fills them
         self._cur = self.dec_mod_ops
         self._decoder(self.h2, self.et_mod)
         self._cur = self.dec_ops
@@ -748,7 +735,7 @@ class UNetEngine:
 
     def __init__(self, arch: Arch, state_dict, device, n_delta=0):
         if not torch.cuda.is_available():
-            raise ops._lib.AsyrpError("UNetEngine needs a CUDA device (sm_100a); there is no CPU path")
+            raise ops._lib.AsyrpError("UNetEngine needs a CUDA device (sm_90a); there is no CPU path")
         ops._lib.load()
         self.arch, self.device, self.n_delta = arch, torch.device(device), n_delta
         self.state = {"ignore_timestep": False, "slerp_t": 0.0, "use_mask": False}

@@ -1,4 +1,4 @@
-"""Drop-in nn.Module mirrors of the reference's UNet classes, backed by the B200 engine.
+"""Drop-in nn.Module mirrors of the reference's UNet classes, backed by the CUDA engine.
 
 Same constructors, state-dict keys, `setattr_layers`, `layer_i` attributes and forward signature / return tuple as
   models/ddpm/diffusion.py          DDPM            (:327-580)
@@ -6,7 +6,7 @@ Same constructors, state-dict keys, `setattr_layers`, `layer_i` attributes and f
   models/guided_diffusion/unet.py   UNetModel       (:437-776)   + script_util.guided_Diffusion (:173-178)
 
 The modules hold parameters only (so `load_state_dict`, `.to(device)`, `state_dict()` and the Δh checkpoint format
-work unchanged); `forward` runs the hand-written sm_100a kernels through UNetEngine — there is no PyTorch compute
+work unchanged); `forward` runs the hand-written sm_90a kernels through UNetEngine — there is no PyTorch compute
 path, and calling forward without a CUDA device raises.
 """
 import math

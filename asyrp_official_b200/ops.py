@@ -66,11 +66,9 @@ def conv_stats_tiles(H, W, C, has_3x3):
 
 
 def conv_tile_config(H, W, C, has_3x3):
-    """(BN, MT) of the tile the library uses for this output geometry; (128, 2) is the swapped-operand tile, unless the
-    conv runs as CTA pairs with the generic epilogue — then (128, 2, "pair")"""
+    """(BN, MT) of the tile the library uses for this output geometry: BN output channels x MT * 128 pixels"""
     v = _lib.load().asyrp_conv_tile_config(H, W, C, int(has_3x3))
-    cfg = ((v & 0xFFFF) // 16, v % 16)
-    return cfg + ("pair",) if (v >> 16) & 1 and cfg == (128, 2) else cfg
+    return v // 16, v % 16
 
 
 def conv_stats_tiles_up2(H, W, C):
@@ -199,11 +197,6 @@ class ConvOp:
         check(self._lib.asyrp_conv_launch(self._h, _stream()), "asyrp_conv_launch")
 
     __call__ = launch
-
-    @property
-    def cta2(self):
-        """runs as CTA pairs (tcgen05 cta_group::2)"""
-        return bool(self._lib.asyrp_conv_is_cta2(self._h))
 
     def set_scales(self, acc_scale, res_scale):
         check(self._lib.asyrp_conv_set_scales(self._h, acc_scale, res_scale), "asyrp_conv_set_scales")

@@ -1,5 +1,5 @@
 """Drop-in for the reference's utils/diffusion_utils.py (get_beta_schedule :5-9, extract :12-20,
-denoising_step :24-109) on the B200 engine: same names, argument meaning and return values.
+denoising_step :24-109) on the CUDA engine: same names, argument meaning and return values.
 
 `denoising_step` keeps the reference's per-call semantics (one UNet forward + one update, new tensors returned).
 The fast path for whole trajectories is UNetEngine.sample() (engine.py), which `Asyrp.run_test` uses.

@@ -14,22 +14,20 @@ broadcast).
 Prints ONE JSON line (rank 0):
   value          device-timed (CUDA events, inputs resident in HBM), whole job
   e2e            through Asyrp.edit_batch with pinned host buffers (H2D of x_T, D2H of x_0 inside the timed region)
-  roofline       the tcgen05 conv kernel: algorithmic conv FLOPs of one edit-step UNet evaluation / (device time of the
+  roofline       the wgmma conv kernel: algorithmic conv FLOPs of one edit-step UNet evaluation / (device time of the
                  captured evaluation minus that of its non-conv launches; CUDA graphs, CUDA events), vs the measured
-                 sustained bf16 cuBLAS peak; `traffic` is read from the committed ncu capture under profiles/
+                 tensor-core peak of the H100 data sheet (or MEASURED_PEAKS.json where present)
   parity         engine vs the REFERENCE's own output (tests/golden/, written by tests/golden/make_golden.py) on the
                  same weights / x_T / noise, for this workload
-  cpu_baseline   the reference's own CPU code (baseline/_ref, staged by scripts/stage_reference.py; falls back to the
+  cpu_baseline   the reference's own CPU code (oracle/_ref, staged by oracle/stage_reference.py; falls back to the
                  restatement oracle/ = kind "port") on a bounded sample, on the host's cores
-  eager_gpu_baseline  the reference's own modules + denoising_step in eager PyTorch (TF32 default) on the same B200
+  eager_gpu_baseline  the reference's own modules + denoising_step in eager PyTorch (TF32 default) on the same GPU
 
 `--impl reference` times the reference's CPU implementation: a "step" there is a bounded sample (one edit reverse step
 + one non-edit reverse step at B=1, scaled x n_edit / x n_plain to a trajectory), `ms_per_step` is the measured time of
 that sample, and one full B=1 trajectory is run in the warm-up to validate the scaling.
 """
 import argparse
-import csv
-import glob
 import json
 import os
 import sys
@@ -40,7 +38,7 @@ import torch
 
 ROOT = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, ROOT)
-REF_DIR = os.path.join(ROOT, "baseline", "_ref")
+REF_DIR = os.path.join(ROOT, "oracle", "_ref")
 GOLD = os.path.join(ROOT, "tests", "golden")
 
 METRIC = "256x256 images/sec, 40-step Asyrp edit"
@@ -64,7 +62,7 @@ def peaks():
         d = json.load(open(p))
         return d["bf16_tflops_sustained"], d["hbm_gbs"], d.get("bf16_tflops"), \
             "measured (MEASURED_PEAKS.json: sustained bf16 cuBLAS for a kernel timed inside a long step)"
-    return 1400.0, 6650.0, 1590.0, "fallback (B200_PROFILING.md)"
+    return 989.0, 3350.0, None, "fallback (H100 SXM data sheet: 989 TFLOP/s dense fp16/bf16, 3.35 TB/s HBM3)"
 
 
 class ClockSampler(threading.Thread):
@@ -130,11 +128,11 @@ def f_img(key, steps, n_edit):
 
 
 # ---------------------------------------------------------------------------------------------------------------
-# the reference itself (baseline/_ref): CPU arm, CPU baseline, eager-GPU baseline
+# the reference itself (oracle/_ref): CPU arm, CPU baseline, eager-GPU baseline
 # ---------------------------------------------------------------------------------------------------------------
 def reference_model(family, key, state_dict, device):
     """the reference's own UNet class (models/ddpm/diffusion.py:327, improved_ddpm/script_util.py:102) holding
-    `state_dict`; None when baseline/_ref has not been staged"""
+    `state_dict`; None when oracle/_ref has not been staged"""
     if not os.path.isdir(os.path.join(REF_DIR, "models")):
         return None, None
     if REF_DIR not in sys.path:
@@ -194,7 +192,7 @@ def cpu_setup(family, key, ckpt, traj_steps):
         def run(only):
             return reference_trajectory(ref, du, x, seq, seq_next, betas, logvar, family == "adm", only=only)[1]
         kind = "reference"
-    else:  # baseline/_ref not staged: the restatement (oracle/) — the one other place bench.py may execute oracle/
+    else:  # oracle/_ref not staged: the restatement (oracle/) — the one other place bench.py may execute oracle/
         from oracle import adm as oa, ddpm as od, sampler as osmp
         if family == "ddpm":
             fwd = lambda *a, **k: od.ddpm_forward(sd, od.CELEBA_CFG, *a, **k)  # noqa: E731
@@ -243,7 +241,7 @@ def cpu_sample(run, kind, seq, traj_steps, reps=1):
         if te + tp < sum(best):
             best = (te, tp)
     traj_s = n_edit * best[0] + (traj_steps - n_edit) * best[1]
-    what = "the reference's own denoising_step + UNet (baseline/_ref)" if kind == "reference" else \
+    what = "the reference's own denoising_step + UNet (oracle/_ref)" if kind == "reference" else \
         "fp32 torch CPU restatement of the reference (oracle/)"
     return {"value": 1.0 / traj_s, "unit": "img/s", "cores": torch.get_num_threads(), "kind": kind,
             "sample": f"B=1: 1 edit reverse step ({best[0]:.2f}s) + 1 non-edit reverse step ({best[1]:.2f}s) of the "
@@ -252,7 +250,7 @@ def cpu_sample(run, kind, seq, traj_steps, reps=1):
 
 
 def eager_gpu(family, key, ckpt, batch, traj_steps, dev, reps=2, golden=None):
-    """the reference's modules + denoising_step, eager PyTorch on the B200 (cuDNN/cuBLAS, TF32 convs as torch's
+    """the reference's modules + denoising_step, eager PyTorch on the GPU (cuDNN/cuBLAS, TF32 convs as torch's
     default): full trajectories at the bench batch"""
     mirror, _ = build_model(family, key, "cpu", ckpt)
     sd = {k: v.float() for k, v in mirror.state_dict().items()}
@@ -305,28 +303,32 @@ def eager_gpu(family, key, ckpt, batch, traj_steps, dev, reps=2, golden=None):
     torch.cuda.empty_cache()
     return {"value": round(batch / best, 3), "unit": "img/s", "batch": batch, "s_per_trajectory": round(best, 3),
             "parity_vs_cpu_reference": ref_parity,
-            "how": "baseline/_ref modules + utils.diffusion_utils.denoising_step in the save_image loop "
+            "how": "oracle/_ref modules + utils.diffusion_utils.denoising_step in the save_image loop "
                    "(diffusion_latent.py:499-520), eager PyTorch on cuda:0, fp32 tensors, "
                    f"cudnn.allow_tf32={torch.backends.cudnn.allow_tf32}, matmul.allow_tf32="
                    f"{torch.backends.cuda.matmul.allow_tf32}; the reference always runs both decoders (34.4 vs the "
                    "27.1 TFLOP/img the engine executes)"}
 
 
-def ncu_traffic():
-    """dram__bytes_read.sum + dram__bytes_write.sum per launch of the dominant conv instantiation, from the newest
-    committed ncu --set full summary under profiles/ (bytes), or None"""
-    files = sorted(glob.glob(os.path.join(ROOT, "profiles", "r*_conv_ncu_full.csv")))
-    for f in reversed(files):
-        try:
-            rows = list(csv.reader(open(f)))
-            hdr, units = rows[0], rows[1]
-            ir, iw = hdr.index("dram__bytes_read.sum"), hdr.index("dram__bytes_write.sum")
-            mult = {"Mbyte": 1e6, "Gbyte": 1e9, "Kbyte": 1e3, "byte": 1.0}[units[ir]]
-            r = rows[2]
-            return (float(r[ir]) + float(r[iw])) * mult, os.path.relpath(f, ROOT), r[0]
-        except Exception:  # noqa: BLE001
-            continue
-    return None, None, None
+DUMP_CAP_BYTES = 64 << 20
+
+
+def dump_outputs(x0, out_dir, cap=DUMP_CAP_BYTES, seed=1234):
+    """Write the x_0 batch the timed path returned as out_dir/x0.npy (float32).  A batch larger than `cap` bytes is
+    reduced to a fixed, seeded sample of whole images (sorted indices, also written as out_dir/x0_indices.npy), so two
+    builds run with the same arguments write the same samples."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    x0 = x0.detach().float().cpu()
+    per = x0[0].numel() * 4
+    keep = max(1, min(x0.shape[0], cap // per))
+    if keep < x0.shape[0]:
+        g = torch.Generator().manual_seed(seed)
+        idx = torch.randperm(x0.shape[0], generator=g)[:keep].sort().values
+        x0 = x0[idx]
+        np.save(os.path.join(out_dir, "x0_indices.npy"), idx.numpy().astype(np.int64))
+    np.save(os.path.join(out_dir, "x0.npy"), x0.numpy())
+    return x0.shape[0]
 
 
 def parity_check(model, runner, sch_kw, golden, dev):
@@ -366,7 +368,16 @@ def main():
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-eager-baseline", action="store_true")
     ap.add_argument("--no-parity", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the x_0 batch of the last timed step to DIR/x0.npy (float32; at most 64 MB: a larger "
+                         "batch is reduced to a seeded sample of images, indices in DIR/x0_indices.npy); with --gpus N "
+                         "only rank 0's shard is written")
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be at least 1")
+    if args.dump_outputs and args.impl == "reference":
+        # the reference arm times a sample of single reverse steps; it computes no x_0 batch to write
+        ap.error("--dump-outputs applies to the engine arm only, not to --impl reference")
     family, key, batch, traj_steps, ckpt, golden = WORKLOADS[args.workload]
     batch = args.batch or batch
     rank, world = int(os.environ.get("RANK", "0")), int(os.environ.get("WORLD_SIZE", "1"))
@@ -385,7 +396,7 @@ def main():
                           f"({ckpt or 'seeded random'}), hs_coeff (1,1)",
               "per_gpu_batch": batch, "global_batch": batch * args.gpus, "trajectory_steps": traj_steps,
               "parallelism": f"batch-sharded x{args.gpus} (one process per GPU, no per-step collective)",
-              "cache": "per-step working set (GBs of activations) exceeds the 126 MB L2; no explicit flush needed"}
+              "cache": "per-step working set (GBs of activations) exceeds the 50 MB L2 of an H100; no explicit flush needed"}
 
     # ------------------------------------------------------------------ reference arm (CPU)
     if args.impl == "reference":
@@ -412,7 +423,7 @@ def main():
         cb = {"value": value, "unit": "img/s", "cores": torch.get_num_threads(), "kind": kind,
               "sample": f"each step = 1 edit reverse step ({te:.2f}s) + 1 non-edit reverse step ({tp:.2f}s) at B=1, "
                         f"scaled x{n_edit}/x{traj_steps - n_edit} to the {traj_steps}-step trajectory; "
-                        f"{'the reference own code from baseline/_ref' if kind == 'reference' else 'oracle/ port'}, "
+                        f"{'the reference own code from oracle/_ref' if kind == 'reference' else 'oracle/ port'}, "
                         f"{torch.get_num_threads()} threads"}
         line = {"impl": "reference", "metric": METRIC, "value": value, "unit": "img/s", "n_gpus": args.gpus,
                 "steps": args.steps, "warmup": args.warmup, "ms_per_step": 1000.0 * timed / args.steps,
@@ -429,9 +440,9 @@ def main():
         print(json.dumps(line))
         return
 
-    # ------------------------------------------------------------------ B200 arm
+    # ------------------------------------------------------------------ engine arm (GPU)
     if not torch.cuda.is_available():
-        raise SystemExit("bench.py: no CUDA device — the B200 arm has no CPU fallback (use --impl reference)")
+        raise SystemExit("bench.py: no CUDA device — the engine arm has no CPU fallback (use --impl reference)")
     dev = torch.device("cuda", local)
     torch.cuda.set_device(dev)
     dist = None
@@ -452,7 +463,8 @@ def main():
     x_host = torch.randn(batch, 3, 256, 256, generator=g).pin_memory()
     out_host = torch.empty_like(x_host).pin_memory()
     x_dev = x_host.to(dev)
-    noise = torch.randn(sch.n_stochastic, batch, 3, 256, 256, device=dev)
+    # seeded like x_T, so that the same arguments give the same inputs on every run
+    noise = torch.randn(sch.n_stochastic, batch, 3, 256, 256, generator=g).to(dev)
 
     def barrier():
         if dist is not None:
@@ -477,6 +489,8 @@ def main():
     if dist is not None:
         dist.all_reduce(ms, op=dist.ReduceOp.MAX)
     ms_per_step = ms.item() / args.steps
+    if args.dump_outputs and rank == 0:
+        dump_outputs(out_dev, args.dump_outputs)
     value = batch * args.gpus / (ms_per_step / 1000.0)
     launches = eng.last_launches * args.steps
 
@@ -500,14 +514,14 @@ def main():
             dist.barrier()
             dist.destroy_process_group()
         return
-    # ---- roofline of the dominant kernel (tcgen05 implicit-GEMM conv), timed inside the captured evaluation:
+    # ---- roofline of the dominant kernel (wgmma implicit-GEMM conv), timed inside the captured evaluation:
     # eval_ms   = device time of a CUDA graph holding ALL launches of one edit-step UNet evaluation (valid data flow,
     #             the clocks / power state of the real trajectory), replayed back to back, CUDA events around the replays
     # other_ms  = the same for a graph holding every NON-conv launch of that evaluation
     # conv_ms   = eval_ms - other_ms (launch gaps are charged to the conv kernel)
     # A graph of the conv launches alone is NOT used: without the GroupNorm finalise launches between them the
-    # activations degenerate to NaN within a few replays, the board draws less power, clocks rise from ~1.57 to
-    # 1.97 GHz and the kernel reads 25-30 % faster than it runs on real data (measured: 10.1 vs 13.1 ms).
+    # activations degenerate to NaN within a few replays, the board draws less power, clocks rise and the kernel reads
+    # faster than it runs on real data.
     peak_tf, peak_gbs, burst_tf, peak_src = peaks()
     P = eng.plan(batch)
     seq_l = P.launches(True, temb=False)
@@ -529,12 +543,8 @@ def main():
         nb = sum(L.nbytes for L in ls)
         kern[k] = {"ms": round(ms_k, 3), "launches": len(ls), "gbs": round(nb / (ms_k * 1e-3) / 1e9, 1) if nb else None}
     P.graph_time(seq_l, reps=1, warm=0)  # leave valid activations behind
-    traffic, traffic_src, traffic_kernel = ncu_traffic()
-    roofline = {"bound": "tensor", "kernel": "conv_gemm_kernel (tcgen05 implicit GEMM, fp16 operands, fp32 accumulate)",
+    roofline = {"bound": "tensor", "kernel": "conv_gemm_kernel (wgmma implicit GEMM, fp16 operands, fp32 accumulate)",
                 "achieved": round(conv_tf, 1), "peak": peak_tf, "unit": "TFLOP/s", "frac": round(conv_tf / peak_tf, 4),
-                "traffic": traffic,
-                "traffic_note": None if traffic is None else
-                f"dram read+write bytes per launch of {traffic_kernel} from {traffic_src} (ncu --set full)",
                 "peak_source": peak_src,
                 "frac_of_burst_peak": (round(conv_tf / burst_tf, 4) if burst_tf else None),
                 "executed_tflops": round(conv_exec_tf, 1),

@@ -1,4 +1,4 @@
-/* libasyrp_b200.so — C ABI of the B200-native Asyrp sampling engine (sm_100a).
+/* libasyrp_b200.so — C ABI of the Asyrp sampling engine (hand-written CUDA for the H100, sm_90a).
  *
  * The reference (kwonminki/Asyrp_official) has no FFI: its seam for this path is Python call signatures
  * (utils/diffusion_utils.py:24 denoising_step, models/ddpm/diffusion.py:473 DDPM.forward,
@@ -37,7 +37,7 @@ const char* asyrp_last_error(void);
 int asyrp_set_pdl(int enabled);
 int asyrp_get_pdl(void);
 
-/* ---- implicit-GEMM convolution on tcgen05 tensor cores ------------------------------------------------
+/* ---- implicit-GEMM convolution on wgmma tensor cores ---------------------------------------------------
  * Replaces torch.nn.Conv2d / Conv1d(k=1) / bmm call sites of the UNets:
  *   ResnetBlock.conv1/conv2/nin_shortcut  models/ddpm/diffusion.py:122-149     (3x3 s1 p1, 1x1)
  *   Downsample.conv (pad (0,1,0,1), s2)   models/ddpm/diffusion.py:96-108
@@ -135,20 +135,10 @@ typedef struct AsyrpConvDesc {
  * ASYRP_CONV_3x3 segment (selects the 8x16 halo tile geometry when H%16==0 and W%8==0) */
 int asyrp_conv_stats_tiles(int H, int W, int Cout, int has_3x3);
 /* tile configuration the library picks for this output geometry: BN * 16 + MT (BN output channels x MT * 128 pixels per
- * CTA tile; 128 * 16 + 2 is the swapped-operand tile;
- * bit 16 is set when the conv runs as CTA pairs with the generic epilogue instead) */
+ * CTA tile) */
 int asyrp_conv_tile_config(int H, int W, int Cout, int has_3x3);
 /* the same for an up2 conv over an H x W source image (0 if the geometry is unsupported) */
 int asyrp_conv_stats_tiles_up2(int H, int W, int Cout);
-/* CTA pairs: convs whose tile is 128 pixels x 256 channels run as clusters of two CTAs (the two SMs of a TPC) that share
- * every weight tile through `tcgen05.mma.cta_group::2` (M = 256): each SM loads half of the weight rows.  Bit-identical
- * to the one-CTA kernel.  On by default (ASYRP_CTA2=0 or asyrp_set_cta2(0) disables it for ops created afterwards). */
-int asyrp_set_cta2(int enabled);
-/* CTA pairs for the 256 pixel x 128 channel tile as well (each SM keeps 64 of the 128 weight rows) instead of the one-CTA
- * swapped-operand tile; changes the statistics-slot counts asyrp_conv_stats_tiles*() report, so set it before building
- * a plan (ASYRP_PAIR128=0/1) */
-int asyrp_set_pair128(int enabled);
-int asyrp_conv_is_cta2(void* op);
 /* SiLU inside the fused GroupNorm-apply + SiLU operand transform: 1 (default) = h + h * tanh.approx(h), h = x / 2 (one
  * special-function op, 11-bit tanh), 0 = x * rcp.approx(1 + ex2.approx(-x log2 e)); negative = default (ASYRP_SILU_TANH).
  * Affects ops created afterwards. */

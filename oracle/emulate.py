@@ -1,7 +1,7 @@
 """CPU emulation of the ENGINE'S numerics on the DDPM family — TEST / ANALYSIS INFRASTRUCTURE ONLY.
 
 The same network as oracle/ddpm.py (which restates models/ddpm/diffusion.py), evaluated in fp32 on the CPU but with
-the roundings the B200 engine performs, each behind a switch, so that the engine-vs-reference error of a trajectory
+the roundings the CUDA engine performs, each behind a switch, so that the engine-vs-reference error of a trajectory
 can be attributed to its sources without GPU time (scripts/attribute_error.py):
 
   w16      conv weights rounded to fp16                         (asyrp_official_b200/ops.py pack_conv_weight)

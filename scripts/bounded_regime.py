@@ -9,7 +9,7 @@ small gamma keeps the whole pipeline the reference runs — DDIM inversion of an
 The UNet itself is unchanged up to its last conv (GroupNorm re-normalises whatever magnitude it is fed), so every
 kernel runs on ordinary O(1) activations; only the amplitude with which its output enters the sampler is calibrated.
 This script measures, on the CPU, the fp32 oracle (bit-identical to the reference) against the emulation of the
-engine's roundings (oracle/emulate.py): the prediction for the max-ABSOLUTE error of the B200 engine on an O(1) image.
+engine's roundings (oracle/emulate.py): the prediction for the max-ABSOLUTE error of the CUDA engine on an O(1) image.
 Analysis tool: nothing here is a product path."""
 import argparse
 import os

@@ -22,4 +22,4 @@ for fused in (0, 1):
         ms = e0.elapsed_time(e1) / 5
         fl = 2.0 * N * H * W * Cout * 9 * Cin
         tiles = N * H * W / 256
-        print(f"fused={fused} Cin={Cin:4d} stages/tile={Cin//64:2d}  {ms*1e3:8.1f} us  {fl/ms/1e9:7.1f} TF/s   per-tile {ms*1e3*148/tiles:6.2f} us")
+        print(f"fused={fused} Cin={Cin:4d} stages/tile={Cin//64:2d}  {ms*1e3:8.1f} us  {fl/ms/1e9:7.1f} TF/s   per-tile {ms*1e3*132/tiles:6.2f} us")

@@ -38,7 +38,7 @@ out = torch.empty(N, H, H, Cout, device=dev, dtype=torch.float16)
 op = ops.ConvOp(segs, w, out=out, stats=ops.new_stats(N, H, H, Cout, dev, True))
 lib = _lib.load()
 ROLES, LEN = 10, 128
-buf = torch.zeros(148 * ROLES * LEN, dtype=torch.int64, device=dev)
+buf = torch.zeros(132 * ROLES * LEN, dtype=torch.int64, device=dev)
 lib.asyrp_conv_set_trace.restype = C.c_int
 lib.asyrp_conv_set_trace.argtypes = [C.c_void_p, C.c_void_p]
 for _ in range(3):
@@ -48,7 +48,7 @@ grid = lib.asyrp_conv_set_trace(op._h, buf.data_ptr())
 e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
 e0.record(); op.launch(); e1.record(); torch.cuda.synchronize()
 us = e0.elapsed_time(e1) * 1e3
-t = buf.cpu().numpy().reshape(148, ROLES, LEN)[:grid]
+t = buf.cpu().numpy().reshape(132, ROLES, LEN)[:grid]
 os.makedirs(os.path.dirname(a.out) or ".", exist_ok=True)
 np.savez_compressed(a.out, t=t, spec=a.spec, us=us, grid=grid)
 print(f"{a.spec}: {us:.1f} us, grid {grid}, {2.0 * N * H * H * Cout * K / us / 1e6:.0f} TF/s")

@@ -1,6 +1,6 @@
 // Micro-benchmark: TMA ingest rate per SM (bytes/clk) for (a) all CTAs streaming the same matrix (weights),
 // (b) every CTA its own rows (activations, L2-resident), (c) as (a) with cluster-of-2 multicast halves.
-// Build + run: nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o /tmp/probe_tma scripts/probe_tma.cu && /tmp/probe_tma
+// Build + run: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o /tmp/probe_tma scripts/probe_tma.cu && /tmp/probe_tma
 #include <cuda.h>
 #include <cuda_runtime.h>
 #include <cuda_fp16.h>
@@ -93,9 +93,9 @@ int main() {
   void* fp = nullptr; cudaDriverEntryPointQueryResult q;
   CK(cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &fp, cudaEnableDefault, &q));
   PFN_enc enc = (PFN_enc)fp;
-  const int K = 2304, rows = 148 * 128;
+  const int K = 2304, rows = 132 * 128;
   __half* w; CK(cudaMalloc(&w, (size_t)rows * K * 2)); CK(cudaMemset(w, 0, (size_t)rows * K * 2));
-  long long* cyc; CK(cudaMalloc(&cyc, 148 * 8));
+  long long* cyc; CK(cudaMalloc(&cyc, 132 * 8));
   auto make = [&](int boxrows, CUtensorMap* tm) {
     cuuint64_t gd[2] = {(cuuint64_t)K, (cuuint64_t)rows}; cuuint64_t gs[1] = {(cuuint64_t)K * 2};
     cuuint32_t bx[2] = {64, (cuuint32_t)boxrows}, es[2] = {1, 1};
@@ -111,7 +111,7 @@ int main() {
   cudaEvent_t e0, e1; cudaEventCreate(&e0); cudaEventCreate(&e1);
   for (int mc = 0; mc < 2; ++mc)
     for (int mode = 0; mode < 2; ++mode)
-      for (int grid : {148, 74, 36}) {
+      for (int grid : {132, 66, 33}) {
         if (mc && mode == 1) continue;
         for (int it = 0; it < 2; ++it) {  // second run timed (L2 warm)
           cudaEventRecord(e0);

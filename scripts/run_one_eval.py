@@ -1,5 +1,5 @@
-"""One eager UNet evaluation (edit step: encoder + DeltaBlock + two decoders) at the bench workload — the short
-command ncu wraps (profiles/README.md)."""
+"""One eager UNet evaluation (edit step: encoder + DeltaBlock + two decoders) at the bench workload — a short
+command to wrap in a profiler."""
 import argparse
 import os
 import sys

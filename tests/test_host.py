@@ -24,14 +24,10 @@ def test_library_exports_every_declared_symbol():
     assert declared == set(_lib.SIGNATURES), declared ^ set(_lib.SIGNATURES)
     assert lib.asyrp_last_error() is not None
     # pure host helper (no device): tile bookkeeping for the GroupNorm partial sums
-    assert lib.asyrp_conv_stats_tiles(256, 256, 256, 0) == 512  # 128x256 tiles
-    lib.asyrp_set_pair128(0)
-    assert lib.asyrp_conv_stats_tiles(256, 256, 128, 1) == 512  # swapped 128x256 tiles, two slots each
-    assert lib.asyrp_conv_tile_config(256, 256, 128, 1) == 128 * 16 + 2
-    lib.asyrp_set_pair128(1)
-    assert lib.asyrp_conv_stats_tiles(256, 256, 128, 1) == 256  # CTA pairs, 256 px x 128 ch per CTA: one slot per tile
-    assert lib.asyrp_conv_tile_config(256, 256, 128, 1) == 128 * 16 + 2 + (1 << 16)
-    lib.asyrp_set_pair128(-1)
+    assert lib.asyrp_conv_stats_tiles(256, 256, 256, 0) == 512  # 16x8-pixel tiles, 128 channels each
+    assert lib.asyrp_conv_stats_tiles(256, 256, 128, 1) == 512  # 8x16-pixel halo tiles, one slot each
+    assert lib.asyrp_conv_tile_config(256, 256, 128, 1) == 128 * 16 + 1
+    assert lib.asyrp_conv_tile_config(16, 16, 128, 1) == 64 * 16 + 1   # small layer: more, narrower tiles
     assert lib.asyrp_conv_stats_tiles(8, 8, 512, 1) == 4        # 2 samples per tile, one slot per lane quarter
 
 
@@ -62,7 +58,7 @@ def test_param_inventory_matches_oracle_inventory():
 
 def test_module_state_dict_and_delta_checkpoint_format():
     """same keys as the reference modules; a Δh checkpoint {"0": layer_0.state_dict()} loads with all keys matched
-    (diffusion_latent.py:674-676).  Uses a shipped checkpoint when the reference tree is present."""
+    (diffusion_latent.py:674-676), on the reference's shipped 'smiling' checkpoint (tests/golden/checkpoint/)."""
     from asyrp_official_b200 import modules, synthetic
     from asyrp_official_b200.configs import load_config
     m = modules.DDPM(load_config("celeba.yml"))
@@ -71,14 +67,11 @@ def test_module_state_dict_and_delta_checkpoint_format():
     assert keys == {"conv1.weight", "conv1.bias", "temb_proj.weight", "temb_proj.bias", "norm2.weight", "norm2.bias",
                     "conv2.weight", "conv2.bias"}
     v0 = m._version
-    ck = "/root/reference/checkpoint/smiling_LC_CelebA_HQ_t999_ninv40_ngen40_0.pth"
-    if os.path.exists(ck):
-        sd = torch.load(ck, map_location="cpu", weights_only=True)["0"]
-        res = m.layer_0.load_state_dict(sd)
-        assert not res.missing_keys and not res.unexpected_keys
-        assert torch.equal(m.layer_0.conv1.weight, sd["conv1.weight"])
-    else:
-        m.layer_0.load_state_dict({k: torch.zeros_like(v) for k, v in m.layer_0.state_dict().items()})
+    ck = os.path.join(ROOT, "tests", "golden", "checkpoint", "smiling_LC_CelebA_HQ_t999_ninv40_ngen40_0.pth")
+    sd = torch.load(ck, map_location="cpu", weights_only=True)["0"]
+    res = m.layer_0.load_state_dict(sd)
+    assert not res.missing_keys and not res.unexpected_keys
+    assert torch.equal(m.layer_0.conv1.weight, sd["conv1.weight"])
     assert m._version > v0  # engine weights are re-packed after any load_state_dict
     a = modules.i_DDPM("AFHQ")
     a.setattr_layers(1)
@@ -142,16 +135,16 @@ def test_config_and_cli_surface(tmp_path, monkeypatch):
 
 
 def test_runner_host_logic():
-    """sequences, hs_coeff scaling (diffusion_latent.py:626,654,659) and LPIPS-table t_edit lookup"""
+    """sequences, hs_coeff scaling (diffusion_latent.py:626,654,659) and LPIPS-table t_edit lookup (the reference's
+    CelebA tables, tests/golden/lpips/)"""
     from asyrp_official_b200.configs import load_config
     from asyrp_official_b200.diffusion_latent import Asyrp
     a = argparse.Namespace(user_defined_t_edit=None, user_defined_t_addnoise=None, clip_cosine=0.8, config="celeba.yml",
-                           lpips_table_dir="/root/reference/utils", add_noise_from_xt=True)
+                           lpips_table_dir=os.path.join(ROOT, "tests", "golden", "lpips"), add_noise_from_xt=True)
     r = Asyrp(a, load_config("celeba"), device="cpu")
     assert r.betas.dtype == torch.float32 and r.logvar.shape == (1000,)
-    if os.path.isdir(a.lpips_table_dir):
-        r.set_t_edit_t_addnoise(LPIPS_th=0.33, LPIPS_addnoise_th=1.2)
-        assert 400 <= r.t_edit <= 560 and r.t_addnoise == 167  # SURVEY.md Appendix D
+    r.set_t_edit_t_addnoise(LPIPS_th=0.33, LPIPS_addnoise_th=1.2)
+    assert 400 <= r.t_edit <= 560 and r.t_addnoise == 167  # SURVEY.md Appendix D
     a2 = argparse.Namespace(user_defined_t_edit=500, user_defined_t_addnoise=200)
     r2 = Asyrp(a2, load_config("celeba"), device="cpu")
     r2.set_t_edit_t_addnoise()
@@ -262,22 +255,24 @@ def test_schedule_sample_type_dt_lambda_and_key(mode):
 
 
 def test_reference_staging_script(tmp_path):
-    """scripts/stage_reference.py copies the reference's hot-path sources verbatim into a git-ignored directory
-    (only where /root/reference exists, i.e. in the build container)"""
-    import importlib.util
-    spec = importlib.util.spec_from_file_location("stage_reference", os.path.join(ROOT, "scripts", "stage_reference.py"))
-    mod = importlib.util.module_from_spec(spec)
-    spec.loader.exec_module(mod)
-    assert "baseline/_ref/" in open(os.path.join(ROOT, ".gitignore")).read()
-    if not os.path.isdir("/root/reference"):
-        assert mod.stage("/root/reference", str(tmp_path / "x"), quiet=True) is False
-        return
-    assert mod.stage("/root/reference", str(tmp_path / "ref"), quiet=True)
-    for rel in ("utils/diffusion_utils.py", "models/ddpm/diffusion.py", "models/improved_ddpm/unet.py",
-                "models/guided_diffusion/unet.py", "configs/celeba.yml",
-                "checkpoint/smiling_LC_CelebA_HQ_t999_ninv40_ngen40_0.pth"):
-        a, b = os.path.join("/root/reference", rel), os.path.join(str(tmp_path / "ref"), rel)
-        assert open(a, "rb").read() == open(b, "rb").read(), rel
+    """oracle/stage_reference.py copies the reference's hot-path sources verbatim into a git-ignored directory, and
+    does nothing where no reference tree exists.  Runs on a stand-in tree with the reference's layout."""
+    from oracle import stage_reference as mod
+    assert os.path.relpath(mod.DST, ROOT) == os.path.join("oracle", "_ref")
+    assert "oracle/_ref/" in open(os.path.join(ROOT, ".gitignore")).read()
+    src = tmp_path / "reference"
+    assert mod.stage(str(src), str(tmp_path / "x"), quiet=True) is False
+    rels = ["utils/diffusion_utils.py", "models/ddpm/diffusion.py", "models/improved_ddpm/unet.py",
+            "models/guided_diffusion/unet.py", "configs/celeba.yml"] + ["checkpoint/" + c for c in mod.CKPTS]
+    for i, rel in enumerate(rels):
+        (src / rel).parent.mkdir(parents=True, exist_ok=True)
+        (src / rel).write_bytes(bytes([i]) * (100 + i))
+    (src / "utils" / "__pycache__").mkdir()
+    (src / "utils" / "__pycache__" / "x.pyc").write_bytes(b"0")
+    assert mod.stage(str(src), str(tmp_path / "ref"), quiet=True)
+    for rel in rels:
+        assert (src / rel).read_bytes() == (tmp_path / "ref" / rel).read_bytes(), rel
+    assert not (tmp_path / "ref" / "utils" / "__pycache__").exists()
 
 
 def test_engine_numerics_emulation_switches():
@@ -311,3 +306,28 @@ def test_shipped_delta_block_fixtures_load():
     ck = torch.load(os.path.join(d, "dog_happy_LC_dog_t999_ninv40_ngen40_0.pth"), map_location="cpu", weights_only=True)
     res = a.layer_0.load_state_dict(ck["0"])
     assert not res.missing_keys and not res.unexpected_keys
+
+
+def test_bench_dump_outputs_is_capped_and_seeded(tmp_path):
+    """bench.py --dump-outputs: a batch over 64 MB becomes a fixed, seeded sample of whole images (indices written next
+    to it), the same on every run; a smaller batch is written whole; --steps below 1, and a dump of the reference arm
+    (which computes no x_0 batch), are rejected"""
+    import subprocess
+    import sys
+    import numpy as np
+    import bench
+    x = torch.randn(100, 3, 256, 256, generator=torch.Generator().manual_seed(0))  # 78.6 MB of float32
+    n = bench.dump_outputs(x, str(tmp_path / "a"))
+    a, idx = np.load(tmp_path / "a" / "x0.npy"), np.load(tmp_path / "a" / "x0_indices.npy")
+    assert a.dtype == np.float32 and a.nbytes <= 64 << 20 and a.shape == (n, 3, 256, 256) and n == 85
+    assert len(set(idx.tolist())) == n and np.array_equal(a, x.numpy()[idx])
+    bench.dump_outputs(x, str(tmp_path / "b"))
+    assert np.array_equal(np.load(tmp_path / "b" / "x0_indices.npy"), idx)
+    assert bench.dump_outputs(x[:4], str(tmp_path / "c")) == 4
+    assert np.array_equal(np.load(tmp_path / "c" / "x0.npy"), x[:4].numpy())
+    assert not (tmp_path / "c" / "x0_indices.npy").exists()
+    r = subprocess.run([sys.executable, os.path.join(ROOT, "bench.py"), "--steps", "0"], capture_output=True, text=True)
+    assert r.returncode == 2 and "--steps must be at least 1" in r.stderr
+    r = subprocess.run([sys.executable, os.path.join(ROOT, "bench.py"), "--impl", "reference", "--dump-outputs",
+                        str(tmp_path / "d")], capture_output=True, text=True)
+    assert r.returncode == 2 and "engine arm only" in r.stderr and not (tmp_path / "d").exists()

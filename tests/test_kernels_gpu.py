@@ -86,7 +86,7 @@ def test_conv1x1_concat_two_sources(cuda_device):
 
 
 def test_conv3x3_with_fused_1x1_shortcut(cuda_device):
-    """conv2(a2) + nin_shortcut(cat(x1, x2)) accumulated in one TMEM tile (ddpm/diffusion.py:159-170)."""
+    """conv2(a2) + nin_shortcut(cat(x1, x2)) accumulated in one accumulator tile (ddpm/diffusion.py:159-170)."""
     ops = _ops()
     g = torch.Generator().manual_seed(3)
     N, H, W, C1, C2, Cout = 2, 32, 32, 128, 64, 128
@@ -445,149 +445,6 @@ def test_upsample_conv_subpixel(cuda_device, N, H, W, C):
     assert (st - sref).abs().max().item() <= 3e-3 * sref.abs().max().item() + 1e-3
 
 
-@pytest.mark.parametrize("case", ["plain", "fused_shortcut", "stride2", "cout512", "up2"])
-def test_cta_pair_kernel_matches_reference_and_one_cta_kernel(cuda_device, case):
-    """tcgen05 cta_group::2 variant of the 128 px x 256 ch tile (two CTAs of a cluster share every weight tile): against
-    the fp64 formula AND bit-for-bit against the one-CTA kernel on the same operands"""
-    ops = _ops()
-    lib = ops._lib.load()
-    g = torch.Generator().manual_seed(31)
-    N = 3
-    kw, ref, shape = {}, None, None
-    if case == "plain":
-        H = W = 32
-        x, w = _rand((N, 256, H, W), g), _rand((256, 256, 3, 3), g, 1.0 / math.sqrt(9 * 256))
-        eb, res = _rand((N, 256), g), _rand((N, 256, H, W), g)
-        ref = 0.75 * (F.conv2d(_h(x), _h(w), padding=1) + eb.double()[:, :, None, None]) + 1.5 * _h(res)
-        segs = [(_nhwc_half(x, cuda_device), ops.MODE_3x3)]
-        wp = ops.pack_conv_weight(w)
-        kw = dict(ebias=eb.to(cuda_device), ebias_stride=256, residual=_nhwc_half(res, cuda_device), res_scale=1.5,
-                  acc_scale=0.75)
-        shape = (N, H, W, 256)
-    elif case == "fused_shortcut":
-        H = W = 32
-        h, x1, x2 = _rand((N, 256, H, W), g), _rand((N, 256, H, W), g), _rand((N, 128, H, W), g)
-        aff = torch.stack([_rand((N, 256), g) * 0.5 + 1.0, _rand((N, 256), g) * 0.5], dim=-1).contiguous()
-        w3 = _rand((256, 256, 3, 3), g, 1.0 / math.sqrt(9 * 256))
-        w1 = _rand((256, 384, 1, 1), g, 1.0 / math.sqrt(384))
-        y = _h(h) * aff[..., 0].double()[:, :, None, None] + aff[..., 1].double()[:, :, None, None]
-        y = _h((y * torch.sigmoid(y)).float())
-        ref = F.conv2d(y, _h(w3), padding=1) + F.conv2d(torch.cat([_h(x1), _h(x2)], 1), _h(w1))
-        segs = [(_nhwc_half(h, cuda_device), ops.MODE_3x3, aff.to(cuda_device), 0, 1),
-                (_nhwc_half(x1, cuda_device), ops.MODE_1x1), (_nhwc_half(x2, cuda_device), ops.MODE_1x1)]
-        wp = torch.cat([ops.pack_conv_weight(w3), ops.pack_conv_weight(w1[:, :256]), ops.pack_conv_weight(w1[:, 256:])], 1)
-        shape = (N, H, W, 256)
-    elif case == "stride2":
-        x, w = _rand((N, 256, 64, 64), g), _rand((256, 256, 3, 3), g, 1.0 / math.sqrt(9 * 256))
-        ref = F.conv2d(F.pad(_h(x), (0, 1, 0, 1)), _h(w), stride=2)
-        segs = [(_nhwc_half(x, cuda_device), ops.MODE_3x3_S2)]
-        wp = ops.pack_conv_weight(w)
-        shape = (N, 32, 32, 256)
-    elif case == "cout512":
-        H = W = 32
-        x, w = _rand((N, 128, H, W), g), _rand((512, 128, 3, 3), g, 1.0 / math.sqrt(9 * 128))
-        ref = F.conv2d(_h(x), _h(w), padding=1)
-        segs = [(_nhwc_half(x, cuda_device), ops.MODE_3x3)]
-        wp = ops.pack_conv_weight(w)
-        shape = (N, H, W, 512)
-    else:
-        H = W = 16
-        x, w = _rand((N, 256, H, W), g), _rand((256, 256, 3, 3), g, 1.0 / math.sqrt(9 * 256))
-        ref = F.conv2d(F.interpolate(_h(x), scale_factor=2.0, mode="nearest"), w.double(), padding=1)
-        segs = [(_nhwc_half(x, cuda_device), ops.MODE_3x3)]
-        wp = ops.pack_upconv_weight(w)
-        kw = dict(up2=True)
-        shape = (N, 2 * H, 2 * W, 256)
-    outs = []
-    try:
-        for on in (1, 0):
-            lib.asyrp_set_cta2(on)
-            out = torch.zeros(shape, dtype=torch.float16, device=cuda_device)
-            tiles = ops.conv_stats_tiles_up2(16, 16, 256) if case == "up2" else \
-                ops.conv_stats_tiles(shape[1], shape[2], shape[3], int(case in ("plain", "fused_shortcut", "cout512")))
-            stats = torch.zeros(N, tiles, shape[3] // 2, 2, dtype=torch.float32, device=cuda_device)
-            op = ops.ConvOp(segs, wp.contiguous().to(cuda_device), out=out, stats=stats, **kw)
-            assert op.cta2 == bool(on), f"{case}: CTA-pair selection {op.cta2} with cta2={on}"
-            op.launch()
-            op.launch()
-            torch.cuda.synchronize()
-            outs.append((out, stats))
-    finally:
-        lib.asyrp_set_cta2(1)
-    _check(_from_nhwc(outs[0][0]), ref, 2.5e-3, f"cta pair {case}")
-    assert torch.equal(outs[0][0], outs[1][0]) and torch.equal(outs[0][1], outs[1][1]), "CTA-pair kernel != one-CTA kernel"
-
-
-@pytest.mark.parametrize("case", ["plain", "fused_shortcut", "up2"])
-def test_pair128_kernel_matches_reference_and_swapped_kernel(cuda_device, case):
-    """CTA-pair variant of the 256 px x 128 ch tile (cta_group::2, M = 2 x 128 pixels, 64 weight rows per CTA, generic
-    epilogue) against the fp64 formula and against the one-CTA swapped-operand kernel it replaces (same K order per
-    tile; the GroupNorm partial sums use one slot per tile instead of two)"""
-    ops = _ops()
-    lib = ops._lib.load()
-    g = torch.Generator().manual_seed(37)
-    N, C = 3, 128
-    kw = {}
-    if case == "plain":
-        H = W = 64
-        x, w = _rand((N, C, H, W), g), _rand((C, C, 3, 3), g, 1.0 / math.sqrt(9 * C))
-        eb, res = _rand((N, C), g), _rand((N, C, H, W), g)
-        ref = 0.75 * (F.conv2d(_h(x), _h(w), padding=1) + eb.double()[:, :, None, None]) + 1.5 * _h(res)
-        segs = [(_nhwc_half(x, cuda_device), ops.MODE_3x3)]
-        wp = ops.pack_conv_weight(w)
-        kw = dict(ebias=eb.to(cuda_device), ebias_stride=C, residual=_nhwc_half(res, cuda_device), res_scale=1.5,
-                  acc_scale=0.75)
-        shape = (N, H, W, C)
-    elif case == "fused_shortcut":
-        H = W = 64
-        h, x1, x2 = _rand((N, C, H, W), g), _rand((N, C, H, W), g), _rand((N, C, H, W), g)
-        aff = torch.stack([_rand((N, C), g) * 0.5 + 1.0, _rand((N, C), g) * 0.5], dim=-1).contiguous()
-        w3 = _rand((C, C, 3, 3), g, 1.0 / math.sqrt(9 * C))
-        w1 = _rand((C, 2 * C, 1, 1), g, 1.0 / math.sqrt(2 * C))
-        y = _h(h) * aff[..., 0].double()[:, :, None, None] + aff[..., 1].double()[:, :, None, None]
-        y = _h((y * torch.sigmoid(y)).float())
-        ref = F.conv2d(y, _h(w3), padding=1) + F.conv2d(torch.cat([_h(x1), _h(x2)], 1), _h(w1))
-        segs = [(_nhwc_half(h, cuda_device), ops.MODE_3x3, aff.to(cuda_device), 0, 1),
-                (_nhwc_half(x1, cuda_device), ops.MODE_1x1), (_nhwc_half(x2, cuda_device), ops.MODE_1x1)]
-        wp = torch.cat([ops.pack_conv_weight(w3), ops.pack_conv_weight(w1[:, :C]), ops.pack_conv_weight(w1[:, C:])], 1)
-        shape = (N, H, W, C)
-    else:
-        H = W = 32
-        x, w = _rand((N, C, H, W), g), _rand((C, C, 3, 3), g, 1.0 / math.sqrt(9 * C))
-        ref = F.conv2d(F.interpolate(_h(x), scale_factor=2.0, mode="nearest"), w.double(), padding=1)
-        segs = [(_nhwc_half(x, cuda_device), ops.MODE_3x3)]
-        wp = ops.pack_upconv_weight(w)
-        kw = dict(up2=True)
-        shape = (N, 2 * H, 2 * W, C)
-    outs = []
-    try:
-        for on in (1, 0):
-            lib.asyrp_set_pair128(on)
-            cfg = ops.conv_tile_config(64, 64, C, True) if case != "up2" else None
-            assert cfg is None or cfg == ((128, 2, "pair") if on else (128, 2)), cfg
-            out = torch.zeros(shape, dtype=torch.float16, device=cuda_device)
-            tiles = ops.conv_stats_tiles_up2(32, 32, C) if case == "up2" else ops.conv_stats_tiles(64, 64, C, 1)
-            stats = torch.zeros(N, tiles, C // 2, 2, dtype=torch.float32, device=cuda_device)
-            op = ops.ConvOp(segs, wp.contiguous().to(cuda_device), out=out, stats=stats, **kw)
-            assert op.cta2 == bool(on), f"{case}: CTA-pair selection {op.cta2} with pair128={on}"
-            op.launch()
-            op.launch()
-            torch.cuda.synchronize()
-            outs.append((out, stats))
-    finally:
-        lib.asyrp_set_pair128(-1)
-    tol = 2.5e-3
-    for out, stats in outs:
-        _check(_from_nhwc(out), ref, tol, f"pair128 {case}")
-        st = stats.sum(dim=1).cpu().double()
-        sref = _stats_ref(ref)
-        assert (st - sref).abs().max().item() <= 3e-3 * sref.abs().max().item() + 1e-3
-    assert outs[0][1].shape[1] * 2 == outs[1][1].shape[1], "one statistics slot per tile (pair) vs two (swapped)"
-    # the same products are accumulated in the same K order by both kernels
-    d = (outs[0][0].float() - outs[1][0].float()).abs().max().item()
-    assert d <= 2.0 ** -9 * ref.abs().max().item(), f"pair128 vs swapped kernel: {d}"
-
-
 def test_fused_silu_one_mufu_vs_two_mufu(cuda_device):
     """SiLU inside the operand transform: h + h*tanh.approx(h) (default, one special-function op) against
     x*rcp(1 + ex2(-x log2 e)) and against the fp64 formula.  Stated bound: the element-wise error of the tanh form is
@@ -649,8 +506,8 @@ def test_conv_out_narrow_tile(cuda_device, Co, fused):
                                       (128, 16, "up"), (128, 64, "up")])
 def test_resampled_residual_in_the_epilogue(cuda_device, C, H, mode):
     """skip branch of the ADM ResBlock(up / down) (improved_ddpm/unet.py:279-284,297): out = conv3x3(a) + resample(x),
-    x read by the epilogue through the nearest-x2 / 2x2-average index map (AsyrpConvDesc.res_mode), both epilogues
-    (swapped 128-channel tile and generic / CTA-pair tile)"""
+    x read by the epilogue through the nearest-x2 / 2x2-average index map (AsyrpConvDesc.res_mode), on 64- and
+    128-channel tiles"""
     ops = _ops()
     g = torch.Generator().manual_seed(51)
     N = 2

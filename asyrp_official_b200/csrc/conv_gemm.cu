@@ -26,6 +26,7 @@
 #include "common.h"
 #include "ptx.cuh"
 #include <cstring>
+#include <memory>
 
 namespace asyrp {
 
@@ -1031,7 +1032,7 @@ struct AsyrpConvDesc {
   int a_heads;         // >1: segment 0 is [N/a_heads][H][W][ld] and head h reads channels [h*C, (h+1)*C)
   int b_heads;         // >1: the weights are [N/b_heads][Cout][weight_ld] and head h reads columns [h*K, (h+1)*K)
   int out_heads;       // >1: out is [N/out_heads][H][W][out_heads*Cout], head h writes channels [h*Cout, ...)
-  int out_f32;         // 1: `out` is fp32 NHWC instead of fp16 (no residual / stats; not with Cout == 128*odd)
+  int out_f32;         // 1: `out` is fp32 NHWC instead of fp16 (no residual / stats)
   const float* ebias;  // fp32, row n at ebias + n*ebias_stride (stride 0: shared row), or null
   int ebias_stride;
   const void* residual;  // fp16 NHWC [N][H][W][Cout] or null
@@ -1073,6 +1074,11 @@ static int conv_halo_ok(int H, int W) { return H % 16 == 0 && W % 8 == 0; }
 static void conv_config(int H, int W, int Cout, int halo, int* BN, int* MT, int phases = 1) {
   int TW, TH, NB;
   conv_tile_shape(H, W, halo, &TW, &TH, &NB);
+  if (NB == 0) {  // no 128-pixel tile fits this geometry
+    *BN = 0;
+    *MT = 0;
+    return;
+  }
   constexpr int kNominalBatch = 16;
   if (Cout == 16) {  // conv_out: 3 / 6 real channels in one 16-wide N tile (an N=64 tile spends 4x the operand reads)
     *BN = 16;
@@ -1095,10 +1101,16 @@ static void conv_config(int H, int W, int Cout, int halo, int* BN, int* MT, int 
   *MT = cand[best][1];
 }
 
+// TW x TH pixels of NB samples, TW * TH * NB == 128; NB == 0 (and TH == 0) when no such tile exists: a width that is
+// not a power of two below the tile width (e.g. W = 12, or W = 96 for H = 1), or an empty image
 static void conv_tile_shape(int H, int W, int halo, int* TW, int* TH, int* NB) {
   int tw, th;
   if (halo) {
     *TW = 8; *TH = 16; *NB = 1;
+    return;
+  }
+  if (H < 1 || W < 1) {
+    *TW = 0; *TH = 0; *NB = 0;
     return;
   }
   if (H == 1) {
@@ -1111,26 +1123,29 @@ static void conv_tile_shape(int H, int W, int halo, int* TW, int* TH, int* NB) {
     if (th > H) th = H;
   }
   // largest power-of-two tile that divides 128
-  while (128 % (tw * th) != 0) --th;
+  while (th > 0 && 128 % (tw * th) != 0) --th;
   *TW = tw;
   *TH = th;
-  *NB = 128 / (tw * th);
+  *NB = th > 0 ? 128 / (tw * th) : 0;
 }
 
 // number of pixel tiles per sample the stats buffer must hold: stats is [N][tiles][Cout/2][2] floats.
 // For layers whose tile spans several samples (NB>1) the kernel writes one slot per epilogue warp (4).
-// has_3x3: the conv producing the statistics contains a 3x3 stride-1 segment (tile geometry depends on it)
+// has_3x3: the conv producing the statistics contains a 3x3 stride-1 segment (tile geometry depends on it).
+// 0: the geometry cannot be tiled (asyrp_conv_create rejects it)
 ASYRP_API int asyrp_conv_stats_tiles(int H, int W, int Cout, int has_3x3) {
   int TW, TH, NB, bn, mt;
   const int halo = has_3x3 && conv_halo_ok(H, W);
   conv_tile_shape(H, W, halo, &TW, &TH, &NB);
+  if (NB == 0) return 0;
   conv_config(H, W, Cout, halo, &bn, &mt);
   const int tht = TH * mt;
   const int tiles = ((W + TW - 1) / TW) * ((H + tht - 1) / tht);
   return NB == 1 ? tiles : tiles * 4;
 }
 
-// tile configuration of a conv with this output geometry: BN * 16 + MT (e.g. 128 * 16 + 1 = 128 channels x 128 pixels)
+// tile configuration of a conv with this output geometry: BN * 16 + MT (e.g. 128 * 16 + 1 = 128 channels x 128 pixels);
+// 0: the geometry cannot be tiled
 ASYRP_API int asyrp_conv_tile_config(int H, int W, int Cout, int has_3x3) {
   int bn, mt;
   const int halo = has_3x3 && conv_halo_ok(H, W);
@@ -1154,7 +1169,8 @@ ASYRP_API int asyrp_conv_create(const AsyrpConvDesc* d, void** out_op) {
   ASYRP_REQUIRE(d->Cout % 64 == 0 || (d->Cout == 16 && d->out_planar != nullptr && d->stats == nullptr &&
                                       d->residual == nullptr && !d->up2 && !d->weight_batched),
                 "asyrp_conv_create: Cout=%d must be a multiple of 64 (or 16 with a planar fp32 output)", d->Cout);
-  ConvOp* op = new ConvOp();
+  // owned here until it is handed out, so that every rejection below frees it
+  std::unique_ptr<ConvOp> op(new ConvOp());
   ConvParams& p = op->p;
   memset(&p, 0, sizeof(p));
   p.N = d->N; p.H = d->H; p.W = d->W; p.Cout = d->Cout;
@@ -1254,7 +1270,7 @@ ASYRP_API int asyrp_conv_create(const AsyrpConvDesc* d, void** out_op) {
     }
     int rc = encode_tensor_map(&p.tmA[s], CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 5, sg.src, dims, strides, box,
                                CU_TENSOR_MAP_SWIZZLE_128B);
-    if (rc != ASYRP_OK) { delete op; return rc; }
+    if (rc != ASYRP_OK) return rc;
   }
   {
     const uint64_t bh = (d->weight_batched && d->b_heads > 1) ? d->b_heads : 1;
@@ -1270,7 +1286,7 @@ ASYRP_API int asyrp_conv_create(const AsyrpConvDesc* d, void** out_op) {
     uint32_t box[4] = {64, static_cast<uint32_t>(op->BN), 1, 1};
     int rc = encode_tensor_map(&p.tmB, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 4, d->weight, dims, strides, box,
                                CU_TENSOR_MAP_SWIZZLE_128B);
-    if (rc != ASYRP_OK) { delete op; return rc; }
+    if (rc != ASYRP_OK) return rc;
   }
   {
     // K-loop schedule.  Single activation ring: heavy chunks (3x3 taps) in order, then the light chunks (1x1
@@ -1370,17 +1386,16 @@ ASYRP_API int asyrp_conv_create(const AsyrpConvDesc* d, void** out_op) {
                    2 * kMaxSeg * 32 * sizeof(float2);
   ASYRP_REQUIRE(op->smem_bytes <= 227 * 1024, "asyrp_conv_create: smem %zu too large", op->smem_bytes);
   const int sms = sm_count();
-  if (sms <= 0) { delete op; return ASYRP_ERR_NO_DEVICE; }
+  if (sms <= 0) return ASYRP_ERR_NO_DEVICE;
   const int total = p.m_tiles * p.n_tiles;
   op->grid = total < sms ? total : sms;
   cudaError_t e = cudaFuncSetAttribute(conv_kernel_ptr(op->BN, op->MT),
                                        cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
   if (e != cudaSuccess) {
     set_error("asyrp_conv_create: cudaFuncSetAttribute: %s", cudaGetErrorString(e));
-    delete op;
     return ASYRP_ERR_CUDA;
   }
-  *out_op = op;
+  *out_op = op.release();
   return ASYRP_OK;
 }
 

@@ -132,10 +132,11 @@ typedef struct AsyrpConvDesc {
 } AsyrpConvDesc;
 
 /* number of tile slots of the stats buffer of a conv with this output geometry; has_3x3: the conv has an
- * ASYRP_CONV_3x3 segment (selects the 8x16 halo tile geometry when H%16==0 and W%8==0) */
+ * ASYRP_CONV_3x3 segment (selects the 8x16 halo tile geometry when H%16==0 and W%8==0).  0 if the geometry is
+ * unsupported (no 128-pixel tile fits it, e.g. W = 12; asyrp_conv_create rejects it with ASYRP_ERR_INVALID) */
 int asyrp_conv_stats_tiles(int H, int W, int Cout, int has_3x3);
 /* tile configuration the library picks for this output geometry: BN * 16 + MT (BN output channels x MT * 128 pixels per
- * CTA tile) */
+ * CTA tile); 0 if the geometry is unsupported */
 int asyrp_conv_tile_config(int H, int W, int Cout, int has_3x3);
 /* the same for an up2 conv over an H x W source image (0 if the geometry is unsupported) */
 int asyrp_conv_stats_tiles_up2(int H, int W, int Cout);

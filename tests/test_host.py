@@ -31,6 +31,53 @@ def test_library_exports_every_declared_symbol():
     assert lib.asyrp_conv_stats_tiles(8, 8, 512, 1) == 4        # 2 samples per tile, one slot per lane quarter
 
 
+_UNTILEABLE_PROBE = r"""
+import ctypes as C, sys
+sys.path.insert(0, sys.argv[1])
+from asyrp_official_b200 import _lib
+lib = _lib.load()
+for H, W in ((4, 12), (3, 3), (1, 96)):
+    for has3 in (0, 1):
+        print("stats_tiles", H, W, has3, lib.asyrp_conv_stats_tiles(H, W, 64, has3), flush=True)
+        print("tile_config", H, W, has3, lib.asyrp_conv_tile_config(H, W, 64, has3), flush=True)
+        d = _lib.AsyrpConvDesc()
+        d.N, d.H, d.W, d.Cout, d.nseg = 2, H, W, 64, 1
+        d.seg[0].src, d.seg[0].C, d.seg[0].mode = None, 64, has3
+        h = C.c_void_p()
+        rc = lib.asyrp_conv_create(C.byref(d), C.byref(h))
+        print("create", H, W, has3, rc, bool(h.value), lib.asyrp_last_error().decode(), flush=True)
+for H, W in ((2, 0), (0, 0)):  # empty images
+    print("stats_tiles", H, W, 0, lib.asyrp_conv_stats_tiles(H, W, 64, 0), flush=True)
+    print("tile_config", H, W, 0, lib.asyrp_conv_tile_config(H, W, 64, 0), flush=True)
+"""
+
+
+def test_untileable_conv_geometry_is_reported_not_fatal():
+    """A width that no 128-pixel tile fits (W = 12 for H = 4, 3x3 images, a T = 96 GEMM row) or an empty image is
+    unsupported: the tile queries return 0 and asyrp_conv_create returns ASYRP_ERR_INVALID before touching a device,
+    instead of dividing by zero in the tiler.  Run in a subprocess so that a crash is reported as a failure of this
+    test."""
+    import subprocess
+    import sys
+    from asyrp_official_b200.build import build_library
+    build_library()
+    r = subprocess.run([sys.executable, "-c", _UNTILEABLE_PROBE, ROOT], capture_output=True, text=True, timeout=120)
+    assert r.returncode == 0, f"probe exited with {r.returncode}\n{r.stdout}\n{r.stderr}"
+    lines = [ln.split(" ", 4) for ln in r.stdout.splitlines()]
+    assert len(lines) == 22, r.stdout
+    for ln in lines:
+        if ln[0] == "create":
+            rc, made, msg = ln[4].split(" ", 2)
+            assert rc == "-1" and made == "False" and "cannot tile" in msg, ln
+        else:
+            assert ln[4] == "0", ln
+    # geometries that tile still do
+    from asyrp_official_b200 import _lib
+    lib = _lib.load()
+    for H, W in ((16, 16), (24, 24), (1, 200)):
+        assert lib.asyrp_conv_stats_tiles(H, W, 64, 0) > 0 and lib.asyrp_conv_tile_config(H, W, 64, 0) > 0
+
+
 def test_no_cpu_fallback():
     from asyrp_official_b200 import modules
     from asyrp_official_b200._lib import AsyrpError

@@ -43,6 +43,7 @@ class AsyrpConvDesc(C.Structure):
         ("scales", c_void_p),
         ("res_mode", c_int),
         ("sums_out", c_void_p),
+        ("scales_stride", c_int),
     ]
 
 

@@ -95,6 +95,9 @@ struct ConvParams {
   // optional device-side copy of (acc_scale, res_scale): when set it overrides the two by-value fields, so that one
   // captured CUDA graph serves every hs_coeff tuple (the DeltaBlock coefficients are per-call arguments of forward())
   const float* scales;
+  // 0: `scales` is one pair for every sample; > 0: batch entry n reads the pair at scales + n*scales_stride (per-sample
+  // hs_coeff rows: one batch mixes edit strengths / attributes)
+  int scales_stride;
   __half* out;             // [N][H][W][Cout] fp16, or nullptr when out_planar is used
   float* out_planar;       // optional fp32 planar [N][planar_c][H][W] holding output channels [0, planar_c)
   int planar_c;
@@ -138,6 +141,14 @@ static constexpr int kTraceRoles = 10, kTraceLen = 128;
 __device__ __forceinline__ int fast_div(int x, uint32_t mul, int d) {
   // mul == 0: d == 1; mul == 1: range too large for the 32-bit multiply-high (huge batches) -> hardware division
   return mul > 1u ? static_cast<int>(__umulhi(static_cast<uint32_t>(x), mul)) : (mul == 0u ? x : x / d);
+}
+// epilogue coefficient `which` (0: acc_scale, 1: res_scale) of batch entry n: the by-value field, the device pair, or
+// (scales_stride > 0) entry n's row of the device table.  Read where it is used rather than held in registers across
+// the tile loop; a tile of NB > 1 samples (8x8 DeltaBlock convs) mixes rows.  Entries past the batch store nothing and
+// read row 0 instead of running off the table.
+__device__ __forceinline__ float conv_scale(const ConvParams& p, int n, int which) {
+  if (p.scales == nullptr) return which ? p.res_scale : p.acc_scale;
+  return __ldg(p.scales + (p.scales_stride > 0 && n < p.N ? static_cast<size_t>(n) * p.scales_stride : 0) + which);
 }
 // tile index -> (pixel tile column, row, sample-group, channel tile); a runtime integer division costs ~20
 // dependent instructions and every role needs these five at each tile start
@@ -645,11 +656,6 @@ __global__ void __launch_bounds__(kNumThreads, 1) conv_gemm_kernel(const __grid_
     const int xx = row % p.TW, nn = (row / p.TW) % p.NB, yy = row / (p.TW * p.NB);
     const int tiles_per_sample = p.tiles_x * p.tiles_y * (p.up2 ? 4 : 1);  // statistics slots per sample
     constexpr int kEpThreads = kNumConsumerWarps * 32;
-    float acc_scale = p.acc_scale, res_scale = p.res_scale;
-    if (p.scales != nullptr) {
-      acc_scale = __ldg(p.scales);
-      res_scale = __ldg(p.scales + 1);
-    }
     // ring slots whose last reader is a wgmma group: handed back to the producers once that group has completed
     auto release = [&](int b, int a) {
       __syncwarp();
@@ -786,6 +792,7 @@ __global__ void __launch_bounds__(kNumThreads, 1) conv_gemm_kernel(const __grid_
               const float* eb = p.ebias != nullptr ? p.ebias + static_cast<size_t>(n) * p.ebias_stride : nullptr;
               const size_t hw = static_cast<size_t>(p.H) * p.W;
               float* pp = p.out_planar + static_cast<size_t>(n) * p.planar_c * hw + static_cast<size_t>(y) * p.W + x;
+              const float acc_scale = conv_scale(p, n, 0);
 #pragma unroll
               for (int i = 0; i < 8; ++i)
                 if (i < p.planar_c) pp[i * hw] = (__uint_as_float(r[i]) + (eb != nullptr ? eb[i] : 0.f)) * acc_scale;
@@ -823,11 +830,13 @@ __global__ void __launch_bounds__(kNumThreads, 1) conv_gemm_kernel(const __grid_
               v[i] += b4.x; v[i + 1] += b4.y; v[i + 2] += b4.z; v[i + 3] += b4.w;
             }
           }
-          if (acc_scale != 1.0f) {
+          const float acc_scale = conv_scale(p, n, 0);
+          if (acc_scale != 1.0f) {  // exact skip: multiplying by 1 changes nothing
 #pragma unroll
             for (int i = 0; i < 32; ++i) v[i] *= acc_scale;
           }
           if (p.res != nullptr && valid) {
+            const float res_scale = conv_scale(p, n, 1);
             if (p.res_mode == 2) {
               // skip branch of a down ResBlock: 2x2 average of the double-resolution tensor, fp32
               const size_t rW = static_cast<size_t>(p.W) * 2;
@@ -1045,6 +1054,7 @@ struct AsyrpConvDesc {
   const float* scales;  // optional DEVICE pointer to (acc_scale, res_scale); overrides the two fields above at run time
   int res_mode;         // 0: residual has the output geometry; 1: [N][H/2][W/2][Cout], nearest-x2; 2: [N][2H][2W][Cout], avg-pool 2x2
   long long* sums_out;  // optional [N][Cout/2][2] int64: (sum, sumsq) * 2^18 of the output, accumulated atomically
+  int scales_stride;    // 0: `scales` is one pair for all samples; > 0: sample n's pair is at scales + n*scales_stride
 };
 
 static void conv_tile_shape(int H, int W, int halo, int* TW, int* TH, int* NB);
@@ -1370,6 +1380,10 @@ ASYRP_API int asyrp_conv_create(const AsyrpConvDesc* d, void** out_op) {
   p.res_scale = d->res_scale;
   p.acc_scale = d->acc_scale;
   p.scales = d->scales;
+  ASYRP_REQUIRE(d->scales_stride >= 0, "asyrp_conv_create: scales_stride=%d is negative", d->scales_stride);
+  ASYRP_REQUIRE(d->scales_stride == 0 || d->scales != nullptr,
+                "asyrp_conv_create: scales_stride=%d needs a scales table", d->scales_stride);
+  p.scales_stride = d->scales_stride;
   p.res_mode = d->residual != nullptr ? d->res_mode : 0;
   ASYRP_REQUIRE(p.res_mode >= 0 && p.res_mode <= 2, "asyrp_conv_create: res_mode %d", d->res_mode);
   ASYRP_REQUIRE(p.res_mode == 0 || (!p.up2 && p.out_heads == 1 && !d->out_f32 && d->out_planar == nullptr &&

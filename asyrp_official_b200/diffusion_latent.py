@@ -224,8 +224,9 @@ class Asyrp(object):
         """x_T (host or device, [B,3,S,S]) -> edited x_0 on the host.  One graph replay; the H2D copy of x_T and the
         D2H copy of x_0 are the only transfers.  The N(0,1) draws of the stochastic steps are made on the device
         up-front, as the reference's torch.randn_like does per step (utils/diffusion_utils.py:79,97), unless `noise`
-        ([n_stochastic, B, 3, S, S]) is given.  sample_kw: delta_hs / use_mask / record_dh / record_process of
-        UNetEngine.sample()."""
+        ([n_stochastic, B, 3, S, S]) is given.  sample_kw: delta_hs / use_mask / record_dh / record_process / hs_coeffs
+        of UNetEngine.sample(); hs_coeffs ([B][1 + n_delta] fp32) gives every row its own hs_coeff tuple, so one batch
+        can mix attributes or edit strengths."""
         eng = model.engine
         dev = eng.device
         if schedule.n_stochastic and noise is None:
@@ -238,13 +239,14 @@ class Asyrp(object):
             return out
         return x0.cpu()
 
-    def _write_process(self, eng, schedule, folder, prefix, bs):
-        """per-step grids of [x_t ; x0_t] (save_process_origin / save_process_delta_h, :485-491,523-527)"""
+    def _write_process(self, eng, schedule, folder, prefix, bs, rows=slice(None)):
+        """per-step grids of [x_t ; x0_t] (save_process_origin / save_process_delta_h, :485-491,523-527) of the batch
+        rows `rows` of the last replay"""
         import torchvision.utils as tvu
         rec = eng.last_records
         os.makedirs(folder, exist_ok=True)
         for k, st in enumerate(schedule.steps):
-            out = (torch.cat([rec["x"][k], rec["x0_t"][k]], dim=0).cpu() + 1) * 0.5
+            out = (torch.cat([rec["x"][k][rows], rec["x0_t"][k][rows]], dim=0).cpu() + 1) * 0.5
             tvu.save_image(tvu.make_grid(out, nrow=bs, padding=1), os.path.join(folder, f'{prefix}_{int(st.t)}.png'))
 
     @torch.no_grad()
@@ -272,32 +274,61 @@ class Asyrp(object):
                 self._write_process(eng, sch, os.path.join(folder_dir, file_name), "origin", bs)
         if not getattr(a, "pass_editing", False):
             coeffs = hs_coeff if isinstance(hs_coeff, list) else [hs_coeff]
-            for tup in coeffs:
-                sch = self.make_schedule(seq_inv, seq_inv_next, tup)
-                edit_ts = [st.t for st in sch.steps if st.edit and st.kind == "ddim"]
-                explicit = (not get_delta_hs) and delta_h_dict is not None and any(
-                    torch.is_tensor(v) for v in delta_h_dict.values())
-                kw = {}
-                if explicit:  # :517: dict[0] with --ignore_timesteps --train_delta_h, else dict[t] for t >= t_edit
-                    glob = bool(getattr(a, "ignore_timesteps", False) and getattr(a, "train_delta_h", False))
-                    rows = []
-                    for t in edit_ts:
-                        dh = delta_h_dict[0] if glob else delta_h_dict[int(t)]
-                        if dh is None:
-                            raise KeyError(f"no Δh for edit timestep {t} in the checkpoint")
-                        dh = dh.detach().float()
-                        rows.append(dh[0] if dh.dim() == 4 and dh.shape[0] == 1 else dh)
-                    if rows:
-                        kw["delta_hs"] = torch.stack(rows)
-                elif get_delta_hs:
-                    kw["record_dh"] = True
-                x_list.append(self.edit_batch(model, x_lat_tensor, sch, record_process=save_process_delta_h, **kw))
-                if save_process_delta_h:
-                    self._write_process(eng, sch, os.path.join(folder_dir, file_name), "delta_h", bs)
-                if get_delta_hs:
+            # the reference replays the trajectory once per tuple (:495-532); the tuples share x_T and the schedule, so
+            # they run as rows of one batch (tuples x images), each row with its own hs_coeff, in chunks of whole tuples
+            # of at most --max_rows_per_replay rows.  A sample's result does not depend on its batch neighbours, so
+            # every row equals the per-tuple replay bit for bit.
+            sch = self.make_schedule(seq_inv, seq_inv_next, coeffs[0])
+            edit_ts = [st.t for st in sch.steps if st.edit and st.kind == "ddim"]  # the same for every tuple
+            explicit = (not get_delta_hs) and delta_h_dict is not None and any(
+                torch.is_tensor(v) for v in delta_h_dict.values())
+            kw = {}
+            if explicit:  # :517: dict[0] with --ignore_timesteps --train_delta_h, else dict[t] for t >= t_edit
+                glob = bool(getattr(a, "ignore_timesteps", False) and getattr(a, "train_delta_h", False))
+                rows = []
+                for t in edit_ts:
+                    dh = delta_h_dict[0] if glob else delta_h_dict[int(t)]
+                    if dh is None:
+                        raise KeyError(f"no Δh for edit timestep {t} in the checkpoint")
+                    dh = dh.detach().float()
+                    rows.append(dh[0] if dh.dim() == 4 and dh.shape[0] == 1 else dh)
+                if rows:
+                    kw["delta_hs"] = torch.stack(rows)
+            elif get_delta_hs:
+                kw["record_dh"] = True
+            max_rows = getattr(a, "max_rows_per_replay", 16)
+            if "delta_hs" in kw and len({float(tup[0]) for tup in coeffs}) > 1:
+                max_rows = 0  # explicit Δh takes one slerp weight 1 - c0 per replay: one tuple per chunk
+            tpc, chunks = plan_sweep(len(coeffs), bs, max_rows)
+            n = eng.n_delta
+            # explicit Δh reads only c0, which the chunk's schedule carries; DeltaBlocks read one tuple per row
+            per_row = "delta_hs" not in kw and n > 0 and all(len(tup) >= n + 1 for tup in coeffs)
+            if "delta_hs" in kw and kw["delta_hs"].dim() == 5:  # per-image Δh rows: repeat them for every tuple row
+                kw["delta_hs"] = kw["delta_hs"].repeat(1, tpc, 1, 1, 1)
+            for chunk in chunks:
+                sch = self.make_schedule(seq_inv, seq_inv_next, coeffs[chunk[0]])
+                rows_x = pad_rows(x_lat_tensor.repeat(len(chunk), 1, 1, 1), tpc * bs)
+                noise = None
+                if sch.n_stochastic:  # the per-tuple draws of the sequential loop, in tuple order
+                    noise = chunk_noise(len(chunk), tpc, bs, lambda: torch.randn(
+                        (sch.n_stochastic, *x_lat_tensor.shape), device=eng.device))
+                if per_row:
+                    table = torch.tensor([[float(c) for c in coeffs[i][:n + 1]] for i in chunk for _ in range(bs)],
+                                         dtype=torch.float32)
+                    kw["hs_coeffs"] = pad_rows(table, tpc * bs)
+                x0 = self.edit_batch(model, rows_x, sch, noise=noise, record_process=save_process_delta_h, **kw)
+                for j in range(len(chunk)):
+                    x_list.append(x0[j * bs:(j + 1) * bs].clone())
+                if save_process_delta_h and chunk is chunks[-1]:  # each tuple rewrote these files: the last one stays
+                    j = len(chunk) - 1
+                    self._write_process(eng, sch, os.path.join(folder_dir, file_name), "delta_h", bs,
+                                        rows=slice(j * bs, (j + 1) * bs))
+                if get_delta_hs:  # accumulated tuple by tuple, as the per-tuple loop adds them
                     rec = eng.last_records["delta_h"].cpu()
-                    for ei, t in enumerate(edit_ts):
-                        delta_h_dict[int(t)] = rec[ei] if delta_h_dict.get(int(t)) is None else delta_h_dict[int(t)] + rec[ei]
+                    for j in range(len(chunk)):
+                        for ei, t in enumerate(edit_ts):
+                            r = rec[ei][j * bs:(j + 1) * bs]
+                            delta_h_dict[int(t)] = r if delta_h_dict.get(int(t)) is None else delta_h_dict[int(t)] + r
         x = (torch.cat(x_list, dim=0) + 1) * 0.5
         grid = tvu.make_grid(x, nrow=a.bs_train, padding=1)
         os.makedirs(folder_dir, exist_ok=True)
@@ -476,6 +507,32 @@ class Asyrp(object):
             a.train_delta_h = a_train_delta_h_prev
         self.last_delta_h_dict = delta_h_dict
         return results
+
+
+def plan_sweep(n_tuples, bs, max_rows):
+    """Chunks of an hs_coeff sweep run as rows of one batch: (tuples per chunk, [tuple indices of each chunk]).
+    A chunk holds whole tuples, at most max_rows // bs of them (at least one); every chunk runs as tuples-per-chunk * bs
+    rows, the last one padded (pad_rows), so that one plan and one captured graph serve them all."""
+    tpc = min(n_tuples, max(1, max_rows // bs))
+    return tpc, [list(range(k, min(k + tpc, n_tuples))) for k in range(0, n_tuples, tpc)]
+
+
+def pad_rows(t, n):
+    """t with its last row repeated up to n rows (padding rows of a sweep chunk; their results are discarded)"""
+    if t.shape[0] >= n:
+        return t
+    return torch.cat([t, t[-1:].expand(n - t.shape[0], *t.shape[1:])], dim=0)
+
+
+def chunk_noise(n_tuples, tpc, bs, draw):
+    """Noise of one sweep chunk, [n_stochastic][tpc * bs][...]: draw() ([n_stochastic][bs][...]) once per tuple, in tuple
+    order, concatenated along the batch axis, so the random stream is consumed exactly as by one replay per tuple.
+    Padding rows copy the last real row and draw nothing."""
+    z = torch.cat([draw() for _ in range(n_tuples)], dim=1)
+    if n_tuples < tpc:
+        pad = (tpc - n_tuples) * bs
+        z = torch.cat([z, z[:, -1:].expand(z.shape[0], pad, *z.shape[2:])], dim=1)
+    return z
 
 
 def _atomic_save(obj, path):

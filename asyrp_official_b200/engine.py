@@ -255,6 +255,34 @@ def pack_weights(arch: Arch, sd, device, n_delta):
     return W, emb_off, off
 
 
+def coef_pairs(table, n_delta):
+    """hs_coeff rows [N][1 + n_delta] -> the DeltaBlock epilogue pairs [N][n_delta][2]: block i of sample n computes
+    c_{i+1}*(conv + bias) + (c0 if i == 0 else 1)*prev, i.e. (acc_scale, res_scale) = (c_{i+1}, c0 | 1)"""
+    t = torch.as_tensor(table, dtype=torch.float32)
+    out = torch.ones(t.shape[0], n_delta, 2, dtype=torch.float32, device=t.device)
+    out[:, :, 0] = t[:, 1:n_delta + 1]
+    out[:, 0, 1] = t[:, 0]
+    return out
+
+
+def coeff_table(hs_coeffs, N, n_delta):
+    """validate a per-sample hs_coeff table: fp32 [N][1 + n_delta] (host or device), returned as an fp32 tensor"""
+    t = torch.as_tensor(hs_coeffs)
+    if t.dim() != 2 or tuple(t.shape) != (N, 1 + n_delta) or not (t.is_floating_point()):
+        raise ops._lib.AsyrpError(f"hs_coeffs must be a float [{N}][{1 + n_delta}] table (batch x (1 + DeltaBlocks)), "
+                                  f"got {t.dtype} {tuple(t.shape)}")
+    return t.to(torch.float32)
+
+
+def shared_c0(table):
+    """c0 of a per-sample table used with explicit Δh: the slerp weight 1 - c0 is one value for the whole batch"""
+    c0 = table[:, 0].cpu()
+    if not bool((c0 == c0[0]).all()):
+        raise ops._lib.AsyrpError("explicit delta_h takes one c0 for the batch (slerp_t = 1 - c0); the hs_coeffs "
+                                  f"table has c0 values {sorted(set(c0.tolist()))}")
+    return float(c0[0])
+
+
 class Plan:
     """Static launch sequence for one batch size"""
 
@@ -269,8 +297,9 @@ class Plan:
         self.et_mod = torch.zeros(N, a.out_ch, S, S, dtype=torch.float32, device=dev)
         self.temb_ops, self.enc_ops, self.delta_ops, self.dec_ops, self.dec_mod_ops = [], [], [], [], []
         # DeltaBlock coefficients (acc_scale, res_scale) of the h2 = c0*h + sum_i c_{i+1}*delta_h_i epilogues live in
-        # device memory: one captured graph serves every hs_coeff tuple
-        self.coef = torch.ones(max(eng.n_delta, 1), 2, dtype=torch.float32, device=dev)
+        # device memory, one [n_delta][2] block per sample: one captured graph serves every hs_coeff tuple, and one
+        # batch can mix tuples (an edit-strength sweep as rows of one batch)
+        self.coef = torch.ones(N, max(eng.n_delta, 1), 2, dtype=torch.float32, device=dev)
         # int64 (sum, sum of squares) accumulators of every >= 16x16 conv output, one arena zeroed by ONE memset at the
         # start of an evaluation (a buffer is never reused: two producers must not add into the same sums)
         self.sums_arena = torch.zeros(max(1 << 20, N * 98304), dtype=torch.int64, device=dev) if GN_FOLD else None
@@ -329,7 +358,8 @@ class Plan:
         return out
 
     def _conv(self, segs, weight, Cout, H, W, ebias=None, ebias_stride=0, residual=None, res_scale=1.0,
-              acc_scale=1.0, stats=True, planar=None, algo_flops=None, up2=False, scales=None, res_mode=0):
+              acc_scale=1.0, stats=True, planar=None, algo_flops=None, up2=False, scales=None, res_mode=0,
+              scales_stride=0):
         """H, W: output geometry (for up2 = twice the source's)"""
         out = None
         if planar is None:
@@ -340,7 +370,7 @@ class Plan:
                         ebias_stride=ebias_stride, residual=residual.t if residual is not None else None,
                         res_scale=res_scale, acc_scale=acc_scale, stats=out.stats if out else None,
                         out_planar=planar, out_shape=(self.N, H, W, Cout), up2=up2, scales=scales, res_mode=res_mode,
-                        sums_out=out.sums if out else None)
+                        sums_out=out.sums if out else None, scales_stride=scales_stride)
         ktot = weight.shape[-1]
         flops = algo_flops if algo_flops is not None else 2.0 * self.N * H * W * Cout * ktot
         nbytes = 2.0 * (sum(sg[0].t.numel() for sg in segs) + weight.numel() + self.N * H * W * Cout
@@ -614,9 +644,10 @@ class Plan:
         if last:  # API-visible delta_h = output of the last DeltaBlock
             dh, _ = self._conv(seg2, W[p + ".w2"], C, h.H, h.W, ebias=W[p + ".b2"], stats=False)
             self.delta_h = dh
-        # h2 = c_{i+1} * (conv2(a2) + b2) + (c0*h | 1*h2_prev), with GroupNorm partial sums for the decoder
+        # h2 = c_{i+1} * (conv2(a2) + b2) + (c0*h | 1*h2_prev), with GroupNorm partial sums for the decoder; sample n
+        # reads its own pair coef[n][i]
         h2, op = self._conv(seg2, W[p + ".w2"], C, h.H, h.W, ebias=W[p + ".b2"], residual=h2_prev,
-                            scales=self.coef[i])
+                            scales=self.coef[0, i], scales_stride=self.coef.stride(0))
         aff.release()
         self._free(d1)
         self._drop_temps()
@@ -640,14 +671,20 @@ class Plan:
 
     # ------------------------------------------------------------------ execution
     def set_coeffs(self, hs_coeff):
-        """hs_coeff = (c0, c1, ..): DeltaBlock i's epilogue computes c_{i+1}*(conv + bias) + (c0 if i == 0 else 1)*prev;
-        written to device memory (stream-ordered), so it also takes effect for an already captured graph"""
+        """hs_coeff = (c0, c1, ..) for every sample: DeltaBlock i's epilogue computes
+        c_{i+1}*(conv + bias) + (c0 if i == 0 else 1)*prev; written to device memory (stream-ordered), so it also takes
+        effect for an already captured graph"""
         n = self.eng.n_delta
         if n == 0 or len(hs_coeff) < n + 1:
             return  # schedules without edit steps (origin pass, inversion) carry no DeltaBlock coefficients
-        host = torch.tensor([[float(hs_coeff[i + 1]), float(hs_coeff[0]) if i == 0 else 1.0] for i in range(n)],
-                            dtype=torch.float32)
-        self.coef.copy_(host, non_blocking=False)
+        row = torch.tensor([[float(c) for c in hs_coeff[:n + 1]]], dtype=torch.float32)
+        self.coef.copy_(coef_pairs(row, n).expand_as(self.coef), non_blocking=False)
+
+    def set_coeff_rows(self, table):
+        """per-sample hs_coeff: table [N][1 + n_delta] fp32 (host or device), row n = sample n's (c0, c1, ..)"""
+        n = self.eng.n_delta
+        if n:
+            self.coef.copy_(coef_pairs(table, n), non_blocking=False)
 
     def launches(self, edit, temb=True):
         """kernel launches of one UNet evaluation"""
@@ -754,9 +791,14 @@ class UNetEngine:
     def forward(self, x, t, index=None, t_edit=400, hs_coeff=(1.0, 1.0), ignore_timestep=False, delta_h=None,
                 use_mask=False):
         """(et, et_modified | None, delta_h | None, middle_h) as fp32 NCHW tensors (new tensors, like the reference).
-        delta_h given: the explicit-Δh branch, h2 = slerp(1 - hs_coeff[0], h, |h| Δh / |Δh|) (ddpm/diffusion.py:518-539)."""
+        delta_h given: the explicit-Δh branch, h2 = slerp(1 - hs_coeff[0], h, |h| Δh / |Δh|) (ddpm/diffusion.py:518-539).
+        hs_coeff may also be a per-sample table, fp32 [N][1 + n_delta] (host or device): row n is sample n's tuple.  With
+        delta_h its c0 column must be constant."""
         N = x.shape[0]
         P = self.plan(N)
+        table = None
+        if torch.is_tensor(hs_coeff) and hs_coeff.dim() == 2:
+            table = coeff_table(hs_coeff, N, self.n_delta)
         with torch.cuda.device(self.device):
             P.x.copy_(x)
             P.t.copy_(t.to(torch.float32))
@@ -771,13 +813,17 @@ class UNetEngine:
             if edit and explicit:
                 dh = delta_h.detach().to(self.device, torch.float32)
                 P.dh_user.copy_(dh if dh.dim() == 4 else dh[None].expand_as(P.dh_user))
-                self.state["slerp_t"], self.state["use_mask"] = 1.0 - float(hs_coeff[0]), bool(use_mask)
+                c0 = shared_c0(table) if table is not None else float(hs_coeff[0])
+                self.state["slerp_t"], self.state["use_mask"] = 1.0 - c0, bool(use_mask)
                 P.run_edit(explicit=True)
                 delta = delta_h  # the reference returns the tensor it was given
             elif edit:
                 if index + 1 != self.n_delta:
                     raise ops._lib.AsyrpError("forward(index=i) requires i+1 == number of packed DeltaBlocks")
-                P.set_coeffs(hs_coeff)
+                if table is not None:
+                    P.set_coeff_rows(table)
+                else:
+                    P.set_coeffs(hs_coeff)
                 P.run_edit()
                 ops.unpack_nchw(P.delta_h.t, P.delta_f32)
                 delta = P.delta_f32.clone()
@@ -875,7 +921,7 @@ class UNetEngine:
         return g
 
     def sample(self, x_T, schedule, noise=None, use_graph=True, out=None, delta_hs=None, use_mask=False,
-               record_dh=False, record_process=False):
+               record_dh=False, record_process=False, hs_coeffs=None):
         """Run the reverse trajectory of `schedule` (sampler.Schedule) from x_T; returns x_0 (fp32 NCHW).
 
         The step list, the edit/plain/stochastic phase of every step and all sampler coefficients are host-side
@@ -887,11 +933,20 @@ class UNetEngine:
         delta_hs: explicit Δh for the edit steps, [n_edit][C][h][w] (or [n_edit][N][C][h][w]) — the reference's
         forward(delta_h=...) branch: h2 = slerp(1 - hs_coeff[0], h, |h| Δh/|Δh|) (ddpm/diffusion.py:518-539).
         record_dh / record_process: keep the DeltaBlock output of every edit step / (x_t, x0_t) of every step in
-        `self.last_records` (device tensors owned by the cached trajectory; clone before the next call)."""
+        `self.last_records` (device tensors owned by the cached trajectory; clone before the next call).
+
+        hs_coeffs: per-sample coefficients, fp32 [N][1 + n_delta] (host or device), overriding schedule.hs_coeff row by
+        row.  Like the tuple they are graph inputs: every table replays the same captured graph, and sample n's result
+        is bit-identical to a batch-1 run with row n as schedule.hs_coeff.  With delta_hs the c0 column must be constant
+        (one slerp weight for the batch)."""
         N = x_T.shape[0]
         P = self.plan(N)
         explicit = delta_hs is not None
-        slerp_t = 1.0 - float(schedule.hs_coeff[0]) if explicit else 0.0
+        table = coeff_table(hs_coeffs, N, self.n_delta) if hs_coeffs is not None else None
+        if explicit:
+            slerp_t = 1.0 - (shared_c0(table) if table is not None else float(schedule.hs_coeff[0]))
+        else:
+            slerp_t = 0.0
         key = (N, bool(use_graph), schedule.key(), explicit, slerp_t, bool(use_mask) if explicit else False,
                bool(record_dh), bool(record_process))
         with torch.cuda.device(self.device):
@@ -911,7 +966,10 @@ class UNetEngine:
             self.graphs[key] = g  # most recently used last
             self.last_launches = g["launches"]
             self.last_records = g["rec"]
-            P.set_coeffs(schedule.hs_coeff)
+            if table is not None:
+                P.set_coeff_rows(table)
+            else:
+                P.set_coeffs(schedule.hs_coeff)
             if explicit and g["n_edit"]:
                 dh = delta_hs.to(self.device, torch.float32)
                 assert dh.shape[0] == g["n_edit"], f"delta_hs has {dh.shape[0]} rows, schedule has {g['n_edit']} edit steps"

@@ -86,6 +86,9 @@ def build_parser():
     p.add_argument('--clip_cosine', type=float, help='text-direction cosine CLIP would give (no CLIP offline)')
     p.add_argument('--lpips_table_dir', type=str, help='directory with <category>_LPIPS_distance_{x,x0_t}.tsv')
     p.add_argument('--checkpoint_dir', type=str, default='checkpoint')
+    p.add_argument('--max_rows_per_replay', type=int, default=16,
+                   help='rows (hs_coeff tuples x images) of one batched trajectory in save_image; bounds the memory of '
+                        'the per-batch plan (DDPM 256x256: about 4.3 GB at 16 rows); 1 = one replay per tuple')
     return p
 
 

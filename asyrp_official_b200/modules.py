@@ -108,8 +108,8 @@ class _EngineUNet(nn.Module):
 
     def _forward(self, x, t, index, t_edit, hs_coeff, delta_h, ignore_timestep, use_mask):
         eng = self.engine
-        if not isinstance(hs_coeff, (tuple, list)):
-            hs_coeff = (hs_coeff,)
+        if not isinstance(hs_coeff, (tuple, list)) and not (torch.is_tensor(hs_coeff) and hs_coeff.dim() == 2):
+            hs_coeff = (hs_coeff,)  # a 2-D tensor is a per-sample [N][1 + n_delta] table (UNetEngine.forward)
         return eng.forward(x.to(eng.device), t.to(eng.device), index=index, t_edit=t_edit, hs_coeff=hs_coeff,
                            ignore_timestep=ignore_timestep, delta_h=delta_h, use_mask=use_mask)
 

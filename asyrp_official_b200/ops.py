@@ -111,11 +111,13 @@ class ConvOp:
     table ([N][Ctot][2] fp32, GroupNorm finalise output) the operand becomes act(a*x + b), applied in shared memory
     inside the kernel (the activated tensor is never materialised).  The output is [N][H][W][Cout]; for MODE_3x3_S2
     the source is [N][2H][2W][C].  weight: packed fp16 [Cout][K] ([N][Cout][K] when weight_batched).
+    scales: device (acc_scale, res_scale) read at run time; with scales_stride > 0 it is sample 0's pair of a per-sample
+    table, sample n's pair scales_stride floats after sample n-1's.
     """
 
     def __init__(self, segs, weight, out=None, ebias=None, ebias_stride=0, residual=None, res_scale=1.0,
                  acc_scale=1.0, stats=None, out_planar=None, out_shape=None, weight_batched=False, a_heads=1,
-                 b_heads=1, out_heads=1, up2=False, scales=None, res_mode=0, sums_out=None):
+                 b_heads=1, out_heads=1, up2=False, scales=None, res_mode=0, sums_out=None, scales_stride=0):
         lib = _lib.load()
         segs = [tuple(sg) + (None, 0, 0) * (len(sg) == 2) for sg in segs]
         srcs = [sg[0] for sg in segs]
@@ -178,6 +180,11 @@ class ConvOp:
         if scales is not None:  # device-side (acc_scale, res_scale): overrides the two values above at run time
             assert scales.dtype == torch.float32 and scales.is_cuda and scales.numel() >= 2 and scales.is_contiguous()
             d.scales = scales.data_ptr()
+            # scales_stride > 0: `scales` is sample 0's pair of a table whose row n starts scales_stride floats further
+            if scales_stride > 0:
+                need = (scales.storage_offset() + (N - 1) * scales_stride + 2) * 4
+                assert need <= scales.untyped_storage().nbytes(), "scales table shorter than the batch"
+        d.scales_stride = int(scales_stride)
         d.out = out.data_ptr() if out is not None else None
         d.stats = stats.data_ptr() if stats is not None else None
         if sums_out is not None:

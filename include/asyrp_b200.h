@@ -129,6 +129,11 @@ typedef struct AsyrpConvDesc {
   /* optional [N][Cout/2][2] int64 accumulators of (sum, sum of squares) * 2^18 of the output, for a consumer's in-kernel
    * GroupNorm (AsyrpConvSeg.gn_*); requires `stats` */
   long long* sums_out;
+  /* layout of `scales`: 0 = one (acc_scale, res_scale) pair for every sample; > 0 = per-sample pairs, that of batch
+   * entry n at scales + n*scales_stride floats (requires `scales`; negative is rejected).  Lets one batch carry a
+   * different hs_coeff tuple per sample: an edit-strength sweep runs as one batch instead of one trajectory per tuple.
+   * Last field, so a zero-initialised descriptor keeps the shared-pair meaning. */
+  int scales_stride;
 } AsyrpConvDesc;
 
 /* number of tile slots of the stats buffer of a conv with this output geometry; has_3x3: the conv has an

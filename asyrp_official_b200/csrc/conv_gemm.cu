@@ -17,12 +17,13 @@
 // address, the descriptor's stride-byte-offset is the halo pitch); layers narrower than 8x16 pixels use three
 // dx-shifted copies whose dy taps are 1024B-aligned row offsets.  TMA's out-of-bounds zero fill is the padding.
 //
-// Warp roles (576 threads): warps 0..7 = two consumer warpgroups (wgmma into register accumulators, then the
-// epilogue: accumulators -> shared-memory staging tile -> bias/residual -> fp16 NHWC store + GroupNorm partial sums),
-// warps 8..15 = in-place operand transform (fused GroupNorm-apply + SiLU), warp 16 = activation TMA producer,
-// warp 17 = weight TMA producer (whole-warp uniform control flow, one elected lane issues).  Persistent: each CTA
-// loops over output tiles; the producers run ahead across tile boundaries, so the loads of tile i+1 overlap the
-// epilogue of tile i.
+// Warp roles (576 threads): warps 0..7 = two consumer warpgroups (wgmma into register accumulators, which go to a
+// shared-memory staging tile at the end of each tile), warps 8..15 = in-place operand transform (fused GroupNorm-apply
+// + SiLU) and the epilogue (staging tile -> bias/residual -> fp16 NHWC store + GroupNorm partial sums), warp 16 =
+// activation TMA producer, warp 17 = weight TMA producer (whole-warp uniform control flow, one elected lane issues).
+// Persistent: each CTA loops over output tiles; the producers run ahead across tile boundaries, and the staging tile
+// is handed over through a full / empty mbarrier pair, so the consumers start tile i+1's MMAs while warps 8..15 run
+// the epilogue of tile i.
 #include "common.h"
 #include "ptx.cuh"
 #include <cstring>
@@ -126,15 +127,17 @@ struct ConvParams {
 #endif
 };
 // Pipeline timeline of a diagnostic build (-DASYRP_TRACE, scripts/conv_trace.py): one elected lane per role stamps
-// clock64() at its hand-off points; compiled out of the product library.
+// clock64() at its hand-off points (role 10 holds a duration instead); compiled out of the product library.
 #ifdef ASYRP_TRACE
-static constexpr int kTraceRoles = 10, kTraceLen = 128;
-#define ASYRP_TRACE_STAMP(role, idx)                                                                    \
-  do {                                                                                                  \
-    if (p.trace != nullptr && lane == 0 && (idx) < kTraceLen)                                           \
-      p.trace[(static_cast<size_t>(blockIdx.x) * kTraceRoles + (role)) * kTraceLen + (idx)] = clock64(); \
+static constexpr int kTraceRoles = 11, kTraceLen = 128;
+#define ASYRP_TRACE_PUT(role, idx, val)                                                             \
+  do {                                                                                              \
+    if (p.trace != nullptr && lane == 0 && (idx) < kTraceLen)                                       \
+      p.trace[(static_cast<size_t>(blockIdx.x) * kTraceRoles + (role)) * kTraceLen + (idx)] = (val); \
   } while (0)
+#define ASYRP_TRACE_STAMP(role, idx) ASYRP_TRACE_PUT(role, idx, clock64())
 #else
+#define ASYRP_TRACE_PUT(role, idx, val) do { } while (0)
 #define ASYRP_TRACE_STAMP(role, idx) do { } while (0)
 #endif
 
@@ -310,6 +313,26 @@ __device__ __forceinline__ void gn_affine8(const ConvSegDev& sg, const float2* g
     cb[i] = b;
   }
 }
+// Recursive-halving reduce-scatter of 32 per-lane values over the warp: afterwards w[0] on lane L is the total of
+// slot L.  One template instance per step, so that every index is a constant and w[] stays in registers (written
+// as a loop over the step width, the steps were not unrolled and w[] went to local memory).
+template <int H>
+__device__ __forceinline__ void reduce_scatter_step(float (&w)[32], int lane) {
+  const bool up = (lane & H) != 0;
+#pragma unroll
+  for (int i = 0; i < H; ++i) {
+    const float send = up ? w[i] : w[i + H];
+    const float keep = up ? w[i + H] : w[i];
+    w[i] = keep + __shfl_xor_sync(0xffffffffu, send, H);
+  }
+}
+__device__ __forceinline__ void reduce_scatter32(float (&w)[32], int lane) {
+  reduce_scatter_step<16>(w, lane);
+  reduce_scatter_step<8>(w, lane);
+  reduce_scatter_step<4>(w, lane);
+  reduce_scatter_step<2>(w, lane);
+  reduce_scatter_step<1>(w, lane);
+}
 __device__ __forceinline__ void stat_atomic_add(long long* dst, float v) {
   atomicAdd(reinterpret_cast<unsigned long long*>(dst), static_cast<unsigned long long>(__float2ll_rn(v * kStatScale)));
 }
@@ -359,7 +382,9 @@ __global__ void __launch_bounds__(kNumThreads, 1) conv_gemm_kernel(const __grid_
   uint64_t* readyA = emptyA + n_aslots;
   uint64_t* fullB = readyA + n_aslots;
   uint64_t* emptyB = fullB + p.b_stages;
-  float* s_stats = reinterpret_cast<float*>(emptyB + p.b_stages);     // [2][4][BN/32][32]
+  uint64_t* stageFull = emptyB + p.b_stages;  // staging tile holds a tile's accumulators (consumers -> epilogue)
+  uint64_t* stageEmpty = stageFull + 1;       // the epilogue has read them out (epilogue -> consumers)
+  float* s_stats = reinterpret_cast<float*>(stageEmpty + 1);          // [2][4][BN/32][32]
   float2* s_gstat = reinterpret_cast<float2*>(s_stats + 2 * 4 * BN);  // [2][kMaxSeg][32] (mean, rstd), see gn_affine8
   const int THT = MT * p.TH;  // rows of the CTA tile
 
@@ -373,6 +398,8 @@ __global__ void __launch_bounds__(kNumThreads, 1) conv_gemm_kernel(const __grid_
       mbar_init(&fullB[i], 1);
       mbar_init(&emptyB[i], kNumConsumerWarps);
     }
+    mbar_init(stageFull, kNumConsumerWarps);
+    mbar_init(stageEmpty, kNumTransformWarps);
     fence_mbar_init();
   }
   if (warp == kWarpA && lane == 0) {
@@ -463,199 +490,410 @@ __global__ void __launch_bounds__(kNumThreads, 1) conv_gemm_kernel(const __grid_
       }
     }
   } else if (warp >= kWarpT) {
-    // ======================================================== operand transform warps, in place
-    if (p.any_transform) {
-      constexpr int kLanes = kNumTransformWarps * 4;  // pixels handled concurrently (8 threads per pixel)
-      const int tt = threadIdx.x - kWarpT * 32;
-      const int jl = tt & 7;                  // logical 16B chunk = channels [jl*8, jl*8+8) of the 64-channel slab
-      const int pl = tt >> 3;                 // pixel lane
-      const int toff = pl * 128 + ((jl ^ (pl & 7)) << 4);  // this thread's chunk of pixel `pl` inside a stage
-      // Pixel masks of this thread, bit m = pixel pl + 32*m.  Halo geometry ((TW+2) x (THT+2) pixels, tiles always
-      // whole): which pixels exist, and which sit in the left / right column or top / bottom row of the halo — those
-      // are outside the image exactly when the tile touches that image edge.  Plain geometry (1x1 stages): existence.
-      uint32_t h_vld = 0, h_l = 0, h_r = 0, h_t = 0, h_b = 0, d_vld = 0;
-      {
-        const int prow = p.TW + 2, rows = THT + 2;
+    // ======================================================== operand transform (in place) + epilogue warps
+    constexpr int kLanes = kNumTransformWarps * 4;  // pixels handled concurrently (8 threads per pixel)
+    const int tt = threadIdx.x - kWarpT * 32;
+    const int jl = tt & 7;                  // logical 16B chunk = channels [jl*8, jl*8+8) of the 64-channel slab
+    const int pl = tt >> 3;                 // pixel lane
+    const int toff = pl * 128 + ((jl ^ (pl & 7)) << 4);  // this thread's chunk of pixel `pl` inside a stage
+    // Pixel masks of this thread, bit m = pixel pl + 32*m.  Halo geometry ((TW+2) x (THT+2) pixels, tiles always
+    // whole): which pixels exist, and which sit in the left / right column or top / bottom row of the halo — those
+    // are outside the image exactly when the tile touches that image edge.  Plain geometry (1x1 stages): existence.
+    uint32_t h_vld = 0, h_l = 0, h_r = 0, h_t = 0, h_b = 0, d_vld = 0;
+    {
+      const int prow = p.TW + 2, rows = THT + 2;
 #pragma unroll 1
-        for (int m = 0, pk = pl; pk < rows * prow; ++m, pk += kLanes) {
-          const int hy = pk / prow, r = pk - hy * prow;
-          h_vld |= 1u << m;
-          if (r == 0) h_l |= 1u << m;
-          if (r == prow - 1) h_r |= 1u << m;
-          if (hy == 0) h_t |= 1u << m;
-          if (hy == rows - 1) h_b |= 1u << m;
-        }
-#pragma unroll 1
-        for (int m = 0, pk = pl; pk < THT * p.TW * p.NB; ++m, pk += kLanes) d_vld |= 1u << m;
+      for (int m = 0, pk = pl; pk < rows * prow; ++m, pk += kLanes) {
+        const int hy = pk / prow, r = pk - hy * prow;
+        h_vld |= 1u << m;
+        if (r == 0) h_l |= 1u << m;
+        if (r == prow - 1) h_r |= 1u << m;
+        if (hy == 0) h_t |= 1u << m;
+        if (hy == rows - 1) h_b |= 1u << m;
       }
-      int sa = 0, sl = 0;
-      uint32_t pa = 0, plt = 0;
-      [[maybe_unused]] int tr_n = 0;
-      // In-kernel GroupNorm: lane g of transform warp s computes (mean, rstd) of group g of segment s for the sample of a
-      // tile, ONE tile ahead (the buffer of tile i+1 is written while tile i is transformed; the named barrier at the
-      // top of tile i+1 publishes it).  fp64 like gn_finalize_kernel; 32 x nseg threads per tile, not every thread.
-      auto group_stats = [&](int tile_next, int buf) {
-        const int s = tt >> 5;
-        if (s < p.nseg && p.seg[s].gn_gamma != nullptr) {
-          const ConvSegDev& sg = p.seg[s];
-          const TileCoord tcn = tile_coord(p, tile_next);
-          const int n = tcn.tn < p.N ? tcn.tn : 0;  // NB == 1
-          const int cpg = (sg.gn_C[0] + sg.gn_C[1]) >> 5;
-          float m, r;
-          gn_group_stats(sg, n, tt & 31, cpg,
-                         static_cast<double>(sg.gn_inv_count) * (1.0 / static_cast<double>(kStatScale)), m, r);
-          s_gstat[(buf * kMaxSeg + s) * 32 + (tt & 31)] = make_float2(m, r);
-        }
-      };
-      if (p.any_gn && static_cast<int>(blockIdx.x) < total_tiles) group_stats(blockIdx.x, 0);
-      int git = 0;
-      for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x, ++git) {
-        const TileCoord tc = tile_coord(p, tile);
-        const int x0 = tc.tx * p.TW, y0 = tc.ty * THT, n0 = tc.tn * p.NB;
-        if (p.any_gn) {
-          named_bar_sync(2, kNumTransformWarps * 32);
-          if (tile + static_cast<int>(gridDim.x) < total_tiles) group_stats(tile + gridDim.x, (git + 1) & 1);
-        }
-        for (int e = 0; e < p.n_sched; ++e) {
-          const int s = p.sched[e] >> 6, ch = p.sched[e] & 63;
-          const ConvSegDev sg = p.seg[s];
-          const bool lt = p.l_stages != 0 && sg.mode == 0;
-          const int ncopies = (sg.mode == 0 || sg.mode == 3) ? 1 : (sg.mode == 1 ? 3 : 9);
-          const int pw = sg.mode == 3 ? p.TW + 2 : p.TW;      // pixels per (row, sample) in the stage
-          const int prow = pw * p.NB;                          // pixels per tile row
-          const int rows = (sg.mode == 1 || sg.mode == 3) ? THT + 2 : THT;
-          const int npix = rows * prow;
-          const int yoff = (sg.mode == 1 || sg.mode == 3) ? -1 : 0;
-          {
-            float ca[8], cb[8];
-            if (sg.affine != nullptr && p.NB == 1) {
-              const float4* ap = reinterpret_cast<const float4*>(
-                  sg.affine + static_cast<size_t>(n0 < p.N ? n0 : 0) * sg.aff_stride + (ch * 64 + jl * 8) * 2);
+#pragma unroll 1
+      for (int m = 0, pk = pl; pk < THT * p.TW * p.NB; ++m, pk += kLanes) d_vld |= 1u << m;
+    }
+    int sa = 0, sl = 0;
+    uint32_t pa = 0, plt = 0;
+    [[maybe_unused]] int tr_n = 0;
+    // In-kernel GroupNorm: lane g of transform warp s computes (mean, rstd) of group g of segment s for the sample of a
+    // tile, ONE tile ahead (the buffer of tile i+1 is written while tile i is transformed; the named barrier at the
+    // top of tile i+1 publishes it).  fp64 like gn_finalize_kernel; 32 x nseg threads per tile, not every thread.
+    auto group_stats = [&](int tile_next, int buf) {
+      const int s = tt >> 5;
+      if (s < p.nseg && p.seg[s].gn_gamma != nullptr) {
+        const ConvSegDev& sg = p.seg[s];
+        const TileCoord tcn = tile_coord(p, tile_next);
+        const int n = tcn.tn < p.N ? tcn.tn : 0;  // NB == 1
+        const int cpg = (sg.gn_C[0] + sg.gn_C[1]) >> 5;
+        float m, r;
+        gn_group_stats(sg, n, tt & 31, cpg,
+                       static_cast<double>(sg.gn_inv_count) * (1.0 / static_cast<double>(kStatScale)), m, r);
+        s_gstat[(buf * kMaxSeg + s) * 32 + (tt & 31)] = make_float2(m, r);
+      }
+    };
+    if (p.any_gn && static_cast<int>(blockIdx.x) < total_tiles) group_stats(blockIdx.x, 0);
+    // Epilogue, from the staging tile in shared memory (row = pixel of the sub-tile, column = sub * BN + channel):
+    // warp 8+w, (q, half) = (w & 3, w >> 2), owns pixel rows [32q, 32q+32) and drains the 32-channel column chunks
+    // half, half+2, ...  `it` counts the CTA's tiles: the phase of the staging barriers and the statistics buffer.
+    // Everything per thread is derived inside: the transform state stays live across the call.
+    constexpr int kEpThreads = kNumTransformWarps * 32;
+    auto drain = [&](int tile, int it) {
+      mbar_wait_suspend(stageFull, it & 1);
+      if (warp == kWarpT) ASYRP_TRACE_STAMP(7, it);
+      const int q = (warp - kWarpT) & 3;
+      const int half = (warp - kWarpT) >> 2;
+      const int ep_tid = tt;
+      const int row = q * 32 + lane;
+      const int xx = row % p.TW, nn = (row / p.TW) % p.NB, yy = row / (p.TW * p.NB);
+      const int tiles_per_sample = p.tiles_x * p.tiles_y * (p.up2 ? 4 : 1);  // statistics slots per sample
+      const uint32_t c_row = smem_u32(sC) + static_cast<uint32_t>(row * kCPitch) * 4u;
+
+      const TileCoord tc = tile_coord(p, tile);
+      const int tx = tc.tx, ty = tc.ty, tn = tc.tn;
+      // up2: the channel-tile index carries the sub-pixel phase (a, b); outputs land on the (2H, 2W) grid
+      int nt = tc.nt, ph = 0;
+      if (p.up2) {
+        const int cts = p.Cout / BN;
+        ph = nt / cts;
+        nt -= ph * cts;
+      }
+      const int ps = p.up2 ? 2 : 1, OH = p.H * ps, OW = p.W * ps, pa_ = ph >> 1, pb_ = ph & 1;
+      const int x = tx * p.TW + xx, n = tn * p.NB + nn;
+      const int tile_in_sample = (ty * p.tiles_x + tx) * (p.up2 ? 4 : 1) + ph;
+      float* st = s_stats + (it & 1) * (4 * BN);
+      if constexpr (BN == 16) {
+        // narrow-N tile of conv_out (3 / 6 real output channels, fp32 planar store): one 16-column load per sub-tile,
+        // warps of the second half have nothing to drain
+        if (half == 0) {
+#pragma unroll 1
+          for (int sub = 0; sub < MT; ++sub) {
+            const int y = ty * THT + sub * p.TH + yy;
+            const bool valid = (x < p.W) && (y < p.H) && (n < p.N);
+            uint32_t r[16];
+            ld_staged<16>(c_row + sub * BN * 4, r);
+            if (valid) {
+              const float* eb = p.ebias != nullptr ? p.ebias + static_cast<size_t>(n) * p.ebias_stride : nullptr;
+              const size_t hw = static_cast<size_t>(p.H) * p.W;
+              float* pp = p.out_planar + static_cast<size_t>(n) * p.planar_c * hw + static_cast<size_t>(y) * p.W + x;
+              const float acc_scale = conv_scale(p, n, 0);
 #pragma unroll
-              for (int k = 0; k < 4; ++k) {
-                const float4 t4 = ap[k];
-                ca[2 * k] = t4.x; cb[2 * k] = t4.y; ca[2 * k + 1] = t4.z; cb[2 * k + 1] = t4.w;
+              for (int i = 0; i < 8; ++i)
+                if (i < p.planar_c) pp[i * hw] = (__uint_as_float(r[i]) + (eb != nullptr ? eb[i] : 0.f)) * acc_scale;
+            }
+          }
+        }
+      } else {
+#pragma unroll 1
+        for (int cc = half; cc < BN / 32; cc += 2) {
+          const int c0 = nt * BN + cc * 32;
+          // statistics of this chunk: slot `lane` (see below) summed over the sub-tiles.  Reduced across the lanes once per
+          // sub-tile: per-lane partial sums kept alive across the sub-tile loop (32 more registers next to r[] and v[])
+          // would spill
+          float wtot = 0.f;
+#pragma unroll 1
+          for (int sub = 0; sub < MT; ++sub) {
+            float ws[32];
+#pragma unroll
+            for (int j = 0; j < 32; ++j) ws[j] = 0.f;
+            const int y = ty * THT + sub * p.TH + yy;
+            const bool valid = (x < p.W) && (y < p.H) && (n < p.N);
+            // output row of this pixel: batch entry n may be a (sample, head) pair writing a channel slice
+            const size_t pix = ((static_cast<size_t>(n / p.out_heads) * OH + y * ps + pa_) * OW + x * ps + pb_) * p.out_ld +
+                               static_cast<size_t>(n % p.out_heads) * p.Cout;
+            uint32_t r[32];
+            ld_staged<32>(c_row + (sub * BN + cc * 32) * 4, r);
+            float v[32];
+#pragma unroll
+            for (int i = 0; i < 32; ++i) v[i] = __uint_as_float(r[i]);
+            if (p.ebias != nullptr) {
+              const float* eb = p.ebias + static_cast<size_t>(valid ? n : 0) * p.ebias_stride + c0;
+#pragma unroll
+              for (int i = 0; i < 32; i += 4) {
+                const float4 b4 = *reinterpret_cast<const float4*>(eb + i);
+                v[i] += b4.x; v[i + 1] += b4.y; v[i + 2] += b4.z; v[i + 3] += b4.w;
               }
-            } else if (sg.gn_gamma != nullptr) {  // GroupNorm finalise in place of the table (NB == 1 by construction)
-              gn_affine8(sg, s_gstat + ((git & 1) * kMaxSeg + s) * 32, n0 < p.N ? n0 : 0, ch * 64 + jl * 8, ca, cb);
             }
-            if (sg.act == 2) {
+            const float acc_scale = conv_scale(p, n, 0);
+            if (acc_scale != 1.0f) {  // exact skip: multiplying by 1 changes nothing
 #pragma unroll
-              for (int k = 0; k < 8; ++k) { ca[k] *= 0.5f; cb[k] *= 0.5f; }
+              for (int i = 0; i < 32; ++i) v[i] *= acc_scale;
             }
-            for (int cp = 0; cp < ncopies; ++cp) {
-              const int slot = lt ? p.a_stages + sl : sa;
-              mbar_wait_suspend(&fullA[slot], lt ? plt : pa);
-              if (warp == kWarpT) ASYRP_TRACE_STAMP(1, tr_n);
-              if (sg.affine != nullptr || sg.gn_gamma != nullptr) {
-                uint8_t* stage = lt ? sL + sl * p.l_stage_bytes : sA + sa * p.a_stage_bytes;
-                const int xoff = sg.mode == 3 ? -1 : (sg.mode == 1 ? cp - 1 : 0);
-                // whole tile inside the image (always true for halo tiles; 1x1 stages of ragged layers fall back)
-                const bool whole = x0 + p.TW <= p.W && y0 + THT <= p.H && n0 < p.N;
-                if (p.NB == 1 && whole && (sg.mode == 3 || sg.mode == 0)) {
-                  // Up to 4 pixels in flight per thread (all shared-memory loads first, branch-free math, then the
-                  // stores); the last groups of a stage use the 2- and 1-wide variants instead of idle lanes (a
-                  // 180-pixel halo tile is 1.4 four-wide passes).  No per-pixel index arithmetic: see the masks above.
-                  uint32_t m_vld = d_vld, m_img = d_vld;
-                  bool m_plain = true;
-                  if (sg.mode == 3) {
-                    const bool el = x0 == 0, er = x0 + p.TW >= p.W, et = y0 == 0, eb = y0 + THT >= p.H;
-                    m_vld = h_vld;
-                    m_img = h_vld & ~((el ? h_l : 0u) | (er ? h_r : 0u) | (et ? h_t : 0u) | (eb ? h_b : 0u));
-                    m_plain = !(el || er || et || eb);
-                  }
-                  const uint32_t tb = smem_u32(stage) + toff;
-                  const int ng = (npix + kLanes - 1) / kLanes;  // 32-pixel groups of the stage (<= 11)
-                  int m = 0;
-                  if (m_plain)  // interior tile: only the last group (partial) needs the masks
-                    for (; m + 4 < ng; m += 4) transform_fast<4, false>(tb + m * 4096, 0u, 0u, ca, cb, sg.act);
-                  for (; m + 4 <= ng; m += 4)
-                    transform_fast<4, true>(tb + m * 4096, m_vld >> m, m_img >> m, ca, cb, sg.act);
-                  if (m + 2 <= ng) {
-                    transform_fast<2, true>(tb + m * 4096, m_vld >> m, m_img >> m, ca, cb, sg.act);
-                    m += 2;
-                  }
-                  if (m < ng) transform_fast<1, true>(tb + m * 4096, m_vld >> m, m_img >> m, ca, cb, sg.act);
-                } else if (p.NB == 1) {
-                  // three dx-shifted copies (mode 1): the in-image test depends on the copy
-                  // (hy, r) = (tile row, position inside the row) of pixel px, advanced incrementally (no divisions)
-                  int hy = pl / prow, r = pl - hy * prow;
-                  const int dhy = kLanes / prow, dr = kLanes - dhy * prow;
-                  const bool n_ok = n0 < p.N;
-                  int px = pl;
-                  for (; px - pl + 3 * kLanes < npix; px += 4 * kLanes)
-                    transform_pixels<4>(stage, px, jl, kLanes, npix, hy, r, dhy, dr, prow, x0 + xoff, y0 + yoff, p.W,
-                                        p.H, n_ok, ca, cb, sg.act);
-                  if (px - pl + kLanes < npix) {
-                    transform_pixels<2>(stage, px, jl, kLanes, npix, hy, r, dhy, dr, prow, x0 + xoff, y0 + yoff, p.W,
-                                        p.H, n_ok, ca, cb, sg.act);
-                    px += 2 * kLanes;
-                  }
-                  if (px - pl < npix)
-                    transform_pixels<1>(stage, px, jl, kLanes, npix, hy, r, dhy, dr, prow, x0 + xoff, y0 + yoff, p.W,
-                                        p.H, n_ok, ca, cb, sg.act);
-                } else {
-                  // tiles spanning several samples (layers below 16x16 when fused): per-pixel sample lookup
-                  for (int px = pl; px < npix; px += kLanes) {
-                    const int hy = px / prow, r = px - hy * prow;
-                    const int nn = r / pw, xx = r - nn * pw;
-                    const int x = x0 + xx + xoff, y = y0 + hy + yoff, n = n0 + nn;
-                    uint4* slot = reinterpret_cast<uint4*>(stage + px * 128 + ((jl ^ (px & 7)) << 4));
-                    uint4 u = make_uint4(0u, 0u, 0u, 0u);
-                    if (x >= 0 && x < p.W && y >= 0 && y < p.H && n < p.N) {
-                      const float4* ap = reinterpret_cast<const float4*>(
-                          sg.affine + static_cast<size_t>(n) * sg.aff_stride + (ch * 64 + jl * 8) * 2);
+            if (p.res != nullptr && valid) {
+              const float res_scale = conv_scale(p, n, 1);
+              if (p.res_mode == 2) {
+                // skip branch of a down ResBlock: 2x2 average of the double-resolution tensor, fp32
+                const size_t rW = static_cast<size_t>(p.W) * 2;
+                const __half* r0 = p.res + ((static_cast<size_t>(n) * p.H * 2 + y * 2) * rW + x * 2) * p.Cout + c0;
 #pragma unroll
-                      for (int k = 0; k < 4; ++k) {
-                        const float4 t4 = ap[k];
-                        ca[2 * k] = t4.x; cb[2 * k] = t4.y; ca[2 * k + 1] = t4.z; cb[2 * k + 1] = t4.w;
-                      }
-                      u = *slot;
-                      __half2* h2 = reinterpret_cast<__half2*>(&u);
+                for (int j = 0; j < 4; ++j) {
+                  float a8[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
 #pragma unroll
-                      for (int k = 0; k < 4; ++k) {
-                        float2 f = __half22float2(h2[k]);
-                        f.x = fmaf(ca[2 * k], f.x, cb[2 * k]);
-                        f.y = fmaf(ca[2 * k + 1], f.y, cb[2 * k + 1]);
-                        if (sg.act == 2) { f.x = silu_tanh_half(0.5f * f.x); f.y = silu_tanh_half(0.5f * f.y); }
-                        else if (sg.act) { f.x = silu_fast(f.x); f.y = silu_fast(f.y); }
-                        h2[k] = __floats2half2_rn(f.x, f.y);
-                      }
+                  for (int q4 = 0; q4 < 4; ++q4) {
+                    const uint4 u = *reinterpret_cast<const uint4*>(r0 + ((q4 >> 1) * rW + (q4 & 1)) * p.Cout + j * 8);
+                    const __half2* h2 = reinterpret_cast<const __half2*>(&u);
+#pragma unroll
+                    for (int k = 0; k < 4; ++k) {
+                      const float2 f = __half22float2(h2[k]);
+                      a8[2 * k] += f.x;
+                      a8[2 * k + 1] += f.y;
                     }
-                    *slot = u;
+                  }
+#pragma unroll
+                  for (int k = 0; k < 8; ++k) v[j * 8 + k] += res_scale * (0.25f * a8[k]);
+                }
+              } else {
+                // res_mode 1: nearest-x2 of the half-resolution tensor (skip branch of an up ResBlock)
+                const size_t rpix = p.res_mode == 1 ? ((static_cast<size_t>(n) * (p.H >> 1) + (y >> 1)) * (p.W >> 1) + (x >> 1)) *
+                                                          p.Cout
+                                                    : pix;
+                const uint4* rp = reinterpret_cast<const uint4*>(p.res + rpix + c0);
+#pragma unroll
+                for (int j = 0; j < 4; ++j) {
+                  const uint4 u = rp[j];
+                  const __half2* h2 = reinterpret_cast<const __half2*>(&u);
+#pragma unroll
+                  for (int k = 0; k < 4; ++k) {
+                    const float2 f = __half22float2(h2[k]);
+                    v[j * 8 + k * 2] += res_scale * f.x;
+                    v[j * 8 + k * 2 + 1] += res_scale * f.y;
                   }
                 }
-                fence_proxy_async_smem();  // generic-proxy writes -> visible to the tensor core's async-proxy reads
               }
-              __syncwarp();
-              if (warp == kWarpT) ASYRP_TRACE_STAMP(2, tr_n);
-              ++tr_n;
-              if (lane == 0) mbar_arrive(&readyA[slot]);
-              if (lt) {
-                if (++sl == p.l_stages) { sl = 0; plt ^= 1; }
+            }
+            if (p.out_planar != nullptr) {
+              if (valid && c0 == 0) {
+                const size_t hw = static_cast<size_t>(p.H) * p.W;
+                float* pp = p.out_planar + static_cast<size_t>(n) * p.planar_c * hw + static_cast<size_t>(y) * p.W + x;
+#pragma unroll
+                for (int i = 0; i < 8; ++i)
+                  if (i < p.planar_c) pp[i * hw] = v[i];
+              }
+            } else if (p.out_f32) {
+              if (valid) {
+                float4* op = reinterpret_cast<float4*>(reinterpret_cast<float*>(p.out) + pix + c0);
+#pragma unroll
+                for (int j = 0; j < 8; ++j) op[j] = make_float4(v[4 * j], v[4 * j + 1], v[4 * j + 2], v[4 * j + 3]);
+              }
+            } else if (valid) {
+              uint4* op = reinterpret_cast<uint4*>(p.out + pix + c0);
+#pragma unroll
+              for (int j = 0; j < 4; ++j) {
+                uint4 u;
+                __half2* h2 = reinterpret_cast<__half2*>(&u);
+#pragma unroll
+                for (int k = 0; k < 4; ++k) h2[k] = __floats2half2_rn(v[j * 8 + k * 2], v[j * 8 + k * 2 + 1]);
+                op[j] = u;
+              }
+            }
+            if (p.stats != nullptr) {
+              if (p.NB == 1) {
+                // slot j<16 : sum of channel pair j ; slot j>=16 : sum of squares of pair j-16 (this lane's pixel)
+                if (valid) {
+#pragma unroll
+                  for (int j = 0; j < 16; ++j) {
+                    ws[j] += v[2 * j] + v[2 * j + 1];
+                    ws[16 + j] += v[2 * j] * v[2 * j] + v[2 * j + 1] * v[2 * j + 1];
+                  }
+                }
               } else {
-                if (++sa == p.a_stages) { sa = 0; pa ^= 1; }
+                // tiles spanning several samples (tiny layers): one masked warp reduction per sample
+                for (int sn = 0; sn < p.NB; ++sn) {
+                  const bool mine = valid && (nn == sn);
+                  float w[32];
+#pragma unroll
+                  for (int j = 0; j < 16; ++j) {
+                    const float a = mine ? v[2 * j] : 0.f, b = mine ? v[2 * j + 1] : 0.f;
+                    w[j] = a + b;
+                    w[16 + j] = a * a + b * b;
+                  }
+                  reduce_scatter32(w, lane);
+                  const int ns = tn * p.NB + sn;
+                  if (ns < p.N) {  // one slot per (sample, tile, lane quarter): deterministic, no atomics
+                    float* g = p.stats + (((static_cast<size_t>(ns) * tiles_per_sample + tile_in_sample) * 4 + q) *
+                                              (p.Cout / 2) + (c0 / 2) + (lane & 15)) * 2 + (lane >> 4);
+                    *g = w[0];
+                  }
+                }
               }
+            }
+            if (p.stats != nullptr && p.NB == 1) {
+              reduce_scatter32(ws, lane);  // afterwards ws[0] on lane L is the total of slot L
+              wtot += ws[0];
+            }
+          }  // sub
+          if (p.stats != nullptr && p.NB == 1) st[(q * (BN / 32) + cc) * 32 + lane] = wtot;
+        }  // cc
+      }
+      // every read of the staging tile is done: the consumers may refill it
+      __syncwarp();
+      if (lane == 0) mbar_arrive(stageEmpty);
+      if (warp == kWarpT) ASYRP_TRACE_STAMP(8, it);
+
+      if (BN >= 32 && p.stats != nullptr && p.NB == 1) {
+        named_bar_sync(1, kEpThreads);
+        for (int e = ep_tid; e < BN; e += kEpThreads) {
+          const int cc = e >> 5, j = e & 31;
+          float tot = 0.f;
+#pragma unroll
+          for (int qq = 0; qq < 4; ++qq) tot += st[(qq * (BN / 32) + cc) * 32 + j];
+          float* g = p.stats + ((static_cast<size_t>(tn) * tiles_per_sample + tile_in_sample) * (p.Cout / 2) +
+                                (nt * BN + cc * 32) / 2 + (j & 15)) * 2 + (j >> 4);
+          *g = tot;
+          if (p.sums_out != nullptr)
+            stat_atomic_add(p.sums_out + (static_cast<size_t>(tn) * (p.Cout / 2) + (nt * BN + cc * 32) / 2 + (j & 15)) * 2 +
+                                (j >> 4), tot);
+        }
+      }
+    };
+    // The epilogue of tile i runs once the first K stage of tile i+1 is handed to the consumers, so that the tensor
+    // pipe works on tile i+1 meanwhile; without a transform, and after the CTA's last tile, it runs straight away.
+    int pend = -1;  // tile whose accumulators the consumers hand over next
+    for (int tile = blockIdx.x, git = 0;; tile += gridDim.x, ++git) {
+      const bool live = tile < total_tiles;
+      const int n_xf = live && p.any_transform ? p.n_sched : 0;  // K stages this warp transforms for the tile
+      const TileCoord tc = tile_coord(p, live ? tile : 0);
+      const int x0 = tc.tx * p.TW, y0 = tc.ty * THT, n0 = tc.tn * p.NB;
+      if (n_xf > 0 && p.any_gn) {
+        named_bar_sync(2, kNumTransformWarps * 32);
+        if (tile + static_cast<int>(gridDim.x) < total_tiles) group_stats(tile + gridDim.x, (git + 1) & 1);
+      }
+      for (int e = 0; e <= n_xf; ++e) {
+        if (e == min(n_xf, 1) && pend >= 0) drain(pend, git - 1);
+        if (e == n_xf) break;
+        const int s = p.sched[e] >> 6, ch = p.sched[e] & 63;
+        const ConvSegDev sg = p.seg[s];
+        const bool lt = p.l_stages != 0 && sg.mode == 0;
+        const int ncopies = (sg.mode == 0 || sg.mode == 3) ? 1 : (sg.mode == 1 ? 3 : 9);
+        const int pw = sg.mode == 3 ? p.TW + 2 : p.TW;      // pixels per (row, sample) in the stage
+        const int prow = pw * p.NB;                          // pixels per tile row
+        const int rows = (sg.mode == 1 || sg.mode == 3) ? THT + 2 : THT;
+        const int npix = rows * prow;
+        const int yoff = (sg.mode == 1 || sg.mode == 3) ? -1 : 0;
+        {
+          float ca[8], cb[8];
+          if (sg.affine != nullptr && p.NB == 1) {
+            const float4* ap = reinterpret_cast<const float4*>(
+                sg.affine + static_cast<size_t>(n0 < p.N ? n0 : 0) * sg.aff_stride + (ch * 64 + jl * 8) * 2);
+#pragma unroll
+            for (int k = 0; k < 4; ++k) {
+              const float4 t4 = ap[k];
+              ca[2 * k] = t4.x; cb[2 * k] = t4.y; ca[2 * k + 1] = t4.z; cb[2 * k + 1] = t4.w;
+            }
+          } else if (sg.gn_gamma != nullptr) {  // GroupNorm finalise in place of the table (NB == 1 by construction)
+            gn_affine8(sg, s_gstat + ((git & 1) * kMaxSeg + s) * 32, n0 < p.N ? n0 : 0, ch * 64 + jl * 8, ca, cb);
+          }
+          if (sg.act == 2) {
+#pragma unroll
+            for (int k = 0; k < 8; ++k) { ca[k] *= 0.5f; cb[k] *= 0.5f; }
+          }
+          for (int cp = 0; cp < ncopies; ++cp) {
+            const int slot = lt ? p.a_stages + sl : sa;
+            mbar_wait_suspend(&fullA[slot], lt ? plt : pa);
+            if (warp == kWarpT) ASYRP_TRACE_STAMP(1, tr_n);
+            if (sg.affine != nullptr || sg.gn_gamma != nullptr) {
+              uint8_t* stage = lt ? sL + sl * p.l_stage_bytes : sA + sa * p.a_stage_bytes;
+              const int xoff = sg.mode == 3 ? -1 : (sg.mode == 1 ? cp - 1 : 0);
+              // whole tile inside the image (always true for halo tiles; 1x1 stages of ragged layers fall back)
+              const bool whole = x0 + p.TW <= p.W && y0 + THT <= p.H && n0 < p.N;
+              if (p.NB == 1 && whole && (sg.mode == 3 || sg.mode == 0)) {
+                // Up to 4 pixels in flight per thread (all shared-memory loads first, branch-free math, then the
+                // stores); the last groups of a stage use the 2- and 1-wide variants instead of idle lanes (a
+                // 180-pixel halo tile is 1.4 four-wide passes).  No per-pixel index arithmetic: see the masks above.
+                uint32_t m_vld = d_vld, m_img = d_vld;
+                bool m_plain = true;
+                if (sg.mode == 3) {
+                  const bool el = x0 == 0, er = x0 + p.TW >= p.W, et = y0 == 0, eb = y0 + THT >= p.H;
+                  m_vld = h_vld;
+                  m_img = h_vld & ~((el ? h_l : 0u) | (er ? h_r : 0u) | (et ? h_t : 0u) | (eb ? h_b : 0u));
+                  m_plain = !(el || er || et || eb);
+                }
+                const uint32_t tb = smem_u32(stage) + toff;
+                const int ng = (npix + kLanes - 1) / kLanes;  // 32-pixel groups of the stage (<= 11)
+                int m = 0;
+                if (m_plain)  // interior tile: only the last group (partial) needs the masks
+                  for (; m + 4 < ng; m += 4) transform_fast<4, false>(tb + m * 4096, 0u, 0u, ca, cb, sg.act);
+                for (; m + 4 <= ng; m += 4)
+                  transform_fast<4, true>(tb + m * 4096, m_vld >> m, m_img >> m, ca, cb, sg.act);
+                if (m + 2 <= ng) {
+                  transform_fast<2, true>(tb + m * 4096, m_vld >> m, m_img >> m, ca, cb, sg.act);
+                  m += 2;
+                }
+                if (m < ng) transform_fast<1, true>(tb + m * 4096, m_vld >> m, m_img >> m, ca, cb, sg.act);
+              } else if (p.NB == 1) {
+                // three dx-shifted copies (mode 1): the in-image test depends on the copy
+                // (hy, r) = (tile row, position inside the row) of pixel px, advanced incrementally (no divisions)
+                int hy = pl / prow, r = pl - hy * prow;
+                const int dhy = kLanes / prow, dr = kLanes - dhy * prow;
+                const bool n_ok = n0 < p.N;
+                int px = pl;
+                for (; px - pl + 3 * kLanes < npix; px += 4 * kLanes)
+                  transform_pixels<4>(stage, px, jl, kLanes, npix, hy, r, dhy, dr, prow, x0 + xoff, y0 + yoff, p.W,
+                                      p.H, n_ok, ca, cb, sg.act);
+                if (px - pl + kLanes < npix) {
+                  transform_pixels<2>(stage, px, jl, kLanes, npix, hy, r, dhy, dr, prow, x0 + xoff, y0 + yoff, p.W,
+                                      p.H, n_ok, ca, cb, sg.act);
+                  px += 2 * kLanes;
+                }
+                if (px - pl < npix)
+                  transform_pixels<1>(stage, px, jl, kLanes, npix, hy, r, dhy, dr, prow, x0 + xoff, y0 + yoff, p.W,
+                                      p.H, n_ok, ca, cb, sg.act);
+              } else {
+                // tiles spanning several samples (layers below 16x16 when fused): per-pixel sample lookup
+                for (int px = pl; px < npix; px += kLanes) {
+                  const int hy = px / prow, r = px - hy * prow;
+                  const int nn = r / pw, xx = r - nn * pw;
+                  const int x = x0 + xx + xoff, y = y0 + hy + yoff, n = n0 + nn;
+                  uint4* slot = reinterpret_cast<uint4*>(stage + px * 128 + ((jl ^ (px & 7)) << 4));
+                  uint4 u = make_uint4(0u, 0u, 0u, 0u);
+                  if (x >= 0 && x < p.W && y >= 0 && y < p.H && n < p.N) {
+                    const float4* ap = reinterpret_cast<const float4*>(
+                        sg.affine + static_cast<size_t>(n) * sg.aff_stride + (ch * 64 + jl * 8) * 2);
+#pragma unroll
+                    for (int k = 0; k < 4; ++k) {
+                      const float4 t4 = ap[k];
+                      ca[2 * k] = t4.x; cb[2 * k] = t4.y; ca[2 * k + 1] = t4.z; cb[2 * k + 1] = t4.w;
+                    }
+                    u = *slot;
+                    __half2* h2 = reinterpret_cast<__half2*>(&u);
+#pragma unroll
+                    for (int k = 0; k < 4; ++k) {
+                      float2 f = __half22float2(h2[k]);
+                      f.x = fmaf(ca[2 * k], f.x, cb[2 * k]);
+                      f.y = fmaf(ca[2 * k + 1], f.y, cb[2 * k + 1]);
+                      if (sg.act == 2) { f.x = silu_tanh_half(0.5f * f.x); f.y = silu_tanh_half(0.5f * f.y); }
+                      else if (sg.act) { f.x = silu_fast(f.x); f.y = silu_fast(f.y); }
+                      h2[k] = __floats2half2_rn(f.x, f.y);
+                    }
+                  }
+                  *slot = u;
+                }
+              }
+              fence_proxy_async_smem();  // generic-proxy writes -> visible to the tensor core's async-proxy reads
+            }
+            __syncwarp();
+            if (warp == kWarpT) ASYRP_TRACE_STAMP(2, tr_n);
+            ++tr_n;
+            if (lane == 0) mbar_arrive(&readyA[slot]);
+            if (lt) {
+              if (++sl == p.l_stages) { sl = 0; plt ^= 1; }
+            } else {
+              if (++sa == p.a_stages) { sa = 0; pa ^= 1; }
             }
           }
         }
       }
+      if (!live) break;
+      pend = tile;
     }
   } else {
-    // ======================================================== consumers (warps 0..7): wgmma, then the epilogue
-    // Warpgroup wg accumulates rows [64 wg, 64 wg + 64) of every 128-pixel sub-tile in registers.  The epilogue works
-    // on the staging tile in shared memory (row = pixel of the sub-tile, column = sub * BN + channel): warp (q, half)
-    // owns pixel rows [32q, 32q+32) and drains the 32-channel column chunks half, half+2, ...
+    // ======================================================== consumers (warps 0..7): wgmma into registers
+    // Warpgroup wg accumulates rows [64 wg, 64 wg + 64) of every 128-pixel sub-tile in registers, hands them to the
+    // epilogue warps through the staging tile and starts the next tile's K loop.
     const int wg = warp >> 2;
-    const uint32_t b_lo0 = gmma_desc_lo(smem_u32(sB));
-    const uint32_t sC_addr = smem_u32(sC);
     const int q = warp & 3;
-    const int half = warp >> 2;
-    const int ep_tid = warp * 32 + lane;
-    const int row = q * 32 + lane;
-    const int xx = row % p.TW, nn = (row / p.TW) % p.NB, yy = row / (p.TW * p.NB);
-    const int tiles_per_sample = p.tiles_x * p.tiles_y * (p.up2 ? 4 : 1);  // statistics slots per sample
-    constexpr int kEpThreads = kNumConsumerWarps * 32;
+    const uint32_t b_lo0 = gmma_desc_lo(smem_u32(sB));
     // ring slots whose last reader is a wgmma group: handed back to the producers once that group has completed
     auto release = [&](int b, int a) {
       __syncwarp();
@@ -714,8 +952,15 @@ __global__ void __launch_bounds__(kNumThreads, 1) conv_gemm_kernel(const __grid_
           uint32_t a_lo =
               gmma_desc_lo(smem_u32(lt ? sL + sl * p.l_stage_bytes : sA + sa * p.a_stage_bytes)) + first16 + wg16;
           int kx = 0;
+          [[maybe_unused]] long long tr_bwait = 0;  // clocks this stage spent waiting for weight stages
           for (int tp = 0; tp < ntaps; ++tp) {
+#ifdef ASYRP_TRACE
+            const long long tr_b0 = clock64();
             mbar_wait(&fullB[sb], pb);
+            tr_bwait += clock64() - tr_b0;
+#else
+            mbar_wait(&fullB[sb], pb);
+#endif
             const uint32_t b_lo = b_lo0 + sb * (kBStage >> 4);
             wgmma_fence();
 #pragma unroll
@@ -736,6 +981,7 @@ __global__ void __launch_bounds__(kNumThreads, 1) conv_gemm_kernel(const __grid_
             if (++kx == kxn) { kx = 0; a_lo += wrap16; } else { a_lo += step16; }
           }
           ASYRP_TRACE_STAMP(9, tr_n - 1);
+          ASYRP_TRACE_PUT(10, tr_n - 1, tr_bwait);
           if (lt) {
             if (++sl == p.l_stages) { sl = 0; pl ^= 1; }
           } else {
@@ -748,9 +994,9 @@ __global__ void __launch_bounds__(kNumThreads, 1) conv_gemm_kernel(const __grid_
 #pragma unroll
       for (int sub = 0; sub < MT; ++sub) wgmma_fence_operands(acc[sub]);
 
-      // accumulators -> staging tile; the barrier before makes sure every consumer has drained the previous tile
-      named_bar_sync(3, kEpThreads);
-      if (warp == 0) ASYRP_TRACE_STAMP(7, it);
+      // accumulators -> staging tile, once the epilogue warps have drained the previous tile out of it
+      mbar_wait(stageEmpty, (it & 1) ^ 1);
+      ASYRP_TRACE_STAMP(6, it);
       {
         const int r0 = 64 * wg + 16 * q + (lane >> 2);
 #pragma unroll
@@ -762,221 +1008,8 @@ __global__ void __launch_bounds__(kNumThreads, 1) conv_gemm_kernel(const __grid_
               *reinterpret_cast<float2*>(sC + (r0 + 8 * h) * kCPitch + sub * BN + 8 * j + 2 * (lane & 3)) =
                   make_float2(acc[sub][4 * j + 2 * h], acc[sub][4 * j + 2 * h + 1]);
       }
-      named_bar_sync(3, kEpThreads);
-      const uint32_t c_row = sC_addr + static_cast<uint32_t>(row * kCPitch) * 4u;
-
-      const TileCoord tc = tile_coord(p, tile);
-      const int tx = tc.tx, ty = tc.ty, tn = tc.tn;
-      // up2: the channel-tile index carries the sub-pixel phase (a, b); outputs land on the (2H, 2W) grid
-      int nt = tc.nt, ph = 0;
-      if (p.up2) {
-        const int cts = p.Cout / BN;
-        ph = nt / cts;
-        nt -= ph * cts;
-      }
-      const int ps = p.up2 ? 2 : 1, OH = p.H * ps, OW = p.W * ps, pa_ = ph >> 1, pb_ = ph & 1;
-      const int x = tx * p.TW + xx, n = tn * p.NB + nn;
-      const int tile_in_sample = (ty * p.tiles_x + tx) * (p.up2 ? 4 : 1) + ph;
-      float* st = s_stats + (it & 1) * (4 * BN);
-      if constexpr (BN == 16) {
-        // narrow-N tile of conv_out (3 / 6 real output channels, fp32 planar store): one 16-column load per sub-tile,
-        // warps of the second half have nothing to drain
-        if (half == 0) {
-#pragma unroll 1
-          for (int sub = 0; sub < MT; ++sub) {
-            const int y = ty * THT + sub * p.TH + yy;
-            const bool valid = (x < p.W) && (y < p.H) && (n < p.N);
-            uint32_t r[16];
-            ld_staged<16>(c_row + sub * BN * 4, r);
-            if (valid) {
-              const float* eb = p.ebias != nullptr ? p.ebias + static_cast<size_t>(n) * p.ebias_stride : nullptr;
-              const size_t hw = static_cast<size_t>(p.H) * p.W;
-              float* pp = p.out_planar + static_cast<size_t>(n) * p.planar_c * hw + static_cast<size_t>(y) * p.W + x;
-              const float acc_scale = conv_scale(p, n, 0);
-#pragma unroll
-              for (int i = 0; i < 8; ++i)
-                if (i < p.planar_c) pp[i * hw] = (__uint_as_float(r[i]) + (eb != nullptr ? eb[i] : 0.f)) * acc_scale;
-            }
-          }
-        }
-      } else {
-#pragma unroll 1
-      for (int cc = half; cc < BN / 32; cc += 2) {
-        const int c0 = nt * BN + cc * 32;
-        // statistics of this chunk: slot `lane` (see below) summed over the sub-tiles.  Reduced across the lanes once per
-        // sub-tile: per-lane partial sums kept alive across the sub-tile loop (32 more registers next to r[] and v[])
-        // would spill
-        float wtot = 0.f;
-#pragma unroll 1
-        for (int sub = 0; sub < MT; ++sub) {
-          float ws[32];
-#pragma unroll
-          for (int j = 0; j < 32; ++j) ws[j] = 0.f;
-          const int y = ty * THT + sub * p.TH + yy;
-          const bool valid = (x < p.W) && (y < p.H) && (n < p.N);
-          // output row of this pixel: batch entry n may be a (sample, head) pair writing a channel slice
-          const size_t pix = ((static_cast<size_t>(n / p.out_heads) * OH + y * ps + pa_) * OW + x * ps + pb_) * p.out_ld +
-                             static_cast<size_t>(n % p.out_heads) * p.Cout;
-          uint32_t r[32];
-          ld_staged<32>(c_row + (sub * BN + cc * 32) * 4, r);
-          float v[32];
-#pragma unroll
-          for (int i = 0; i < 32; ++i) v[i] = __uint_as_float(r[i]);
-          if (p.ebias != nullptr) {
-            const float* eb = p.ebias + static_cast<size_t>(valid ? n : 0) * p.ebias_stride + c0;
-#pragma unroll
-            for (int i = 0; i < 32; i += 4) {
-              const float4 b4 = *reinterpret_cast<const float4*>(eb + i);
-              v[i] += b4.x; v[i + 1] += b4.y; v[i + 2] += b4.z; v[i + 3] += b4.w;
-            }
-          }
-          const float acc_scale = conv_scale(p, n, 0);
-          if (acc_scale != 1.0f) {  // exact skip: multiplying by 1 changes nothing
-#pragma unroll
-            for (int i = 0; i < 32; ++i) v[i] *= acc_scale;
-          }
-          if (p.res != nullptr && valid) {
-            const float res_scale = conv_scale(p, n, 1);
-            if (p.res_mode == 2) {
-              // skip branch of a down ResBlock: 2x2 average of the double-resolution tensor, fp32
-              const size_t rW = static_cast<size_t>(p.W) * 2;
-              const __half* r0 = p.res + ((static_cast<size_t>(n) * p.H * 2 + y * 2) * rW + x * 2) * p.Cout + c0;
-#pragma unroll
-              for (int j = 0; j < 4; ++j) {
-                float a8[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
-#pragma unroll
-                for (int q4 = 0; q4 < 4; ++q4) {
-                  const uint4 u = *reinterpret_cast<const uint4*>(r0 + ((q4 >> 1) * rW + (q4 & 1)) * p.Cout + j * 8);
-                  const __half2* h2 = reinterpret_cast<const __half2*>(&u);
-#pragma unroll
-                  for (int k = 0; k < 4; ++k) {
-                    const float2 f = __half22float2(h2[k]);
-                    a8[2 * k] += f.x;
-                    a8[2 * k + 1] += f.y;
-                  }
-                }
-#pragma unroll
-                for (int k = 0; k < 8; ++k) v[j * 8 + k] += res_scale * (0.25f * a8[k]);
-              }
-            } else {
-              // res_mode 1: nearest-x2 of the half-resolution tensor (skip branch of an up ResBlock)
-              const size_t rpix = p.res_mode == 1 ? ((static_cast<size_t>(n) * (p.H >> 1) + (y >> 1)) * (p.W >> 1) + (x >> 1)) *
-                                                        p.Cout
-                                                  : pix;
-              const uint4* rp = reinterpret_cast<const uint4*>(p.res + rpix + c0);
-#pragma unroll
-              for (int j = 0; j < 4; ++j) {
-                const uint4 u = rp[j];
-                const __half2* h2 = reinterpret_cast<const __half2*>(&u);
-#pragma unroll
-                for (int k = 0; k < 4; ++k) {
-                  const float2 f = __half22float2(h2[k]);
-                  v[j * 8 + k * 2] += res_scale * f.x;
-                  v[j * 8 + k * 2 + 1] += res_scale * f.y;
-                }
-              }
-            }
-          }
-          if (p.out_planar != nullptr) {
-            if (valid && c0 == 0) {
-              const size_t hw = static_cast<size_t>(p.H) * p.W;
-              float* pp = p.out_planar + static_cast<size_t>(n) * p.planar_c * hw + static_cast<size_t>(y) * p.W + x;
-#pragma unroll
-              for (int i = 0; i < 8; ++i)
-                if (i < p.planar_c) pp[i * hw] = v[i];
-            }
-          } else if (p.out_f32) {
-            if (valid) {
-              float4* op = reinterpret_cast<float4*>(reinterpret_cast<float*>(p.out) + pix + c0);
-#pragma unroll
-              for (int j = 0; j < 8; ++j) op[j] = make_float4(v[4 * j], v[4 * j + 1], v[4 * j + 2], v[4 * j + 3]);
-            }
-          } else if (valid) {
-            uint4* op = reinterpret_cast<uint4*>(p.out + pix + c0);
-#pragma unroll
-            for (int j = 0; j < 4; ++j) {
-              uint4 u;
-              __half2* h2 = reinterpret_cast<__half2*>(&u);
-#pragma unroll
-              for (int k = 0; k < 4; ++k) h2[k] = __floats2half2_rn(v[j * 8 + k * 2], v[j * 8 + k * 2 + 1]);
-              op[j] = u;
-            }
-          }
-          if (p.stats != nullptr) {
-            if (p.NB == 1) {
-              // slot j<16 : sum of channel pair j ; slot j>=16 : sum of squares of pair j-16 (this lane's pixel)
-              if (valid) {
-#pragma unroll
-                for (int j = 0; j < 16; ++j) {
-                  ws[j] += v[2 * j] + v[2 * j + 1];
-                  ws[16 + j] += v[2 * j] * v[2 * j] + v[2 * j + 1] * v[2 * j + 1];
-                }
-              }
-            } else {
-              // tiles spanning several samples (tiny layers): one masked warp reduction per sample
-              for (int sn = 0; sn < p.NB; ++sn) {
-                const bool mine = valid && (nn == sn);
-                float w[32];
-#pragma unroll
-                for (int j = 0; j < 16; ++j) {
-                  const float a = mine ? v[2 * j] : 0.f, b = mine ? v[2 * j + 1] : 0.f;
-                  w[j] = a + b;
-                  w[16 + j] = a * a + b * b;
-                }
-#pragma unroll
-                for (int h = 16; h >= 1; h >>= 1) {
-                  const bool up = (lane & h) != 0;
-#pragma unroll
-                  for (int i = 0; i < h; ++i) {
-                    const float send = up ? w[i] : w[i + h];
-                    const float keep = up ? w[i + h] : w[i];
-                    w[i] = keep + __shfl_xor_sync(0xffffffffu, send, h);
-                  }
-                }
-                const int ns = tn * p.NB + sn;
-                if (ns < p.N) {  // one slot per (sample, tile, lane quarter): deterministic, no atomics
-                  float* g = p.stats + (((static_cast<size_t>(ns) * tiles_per_sample + tile_in_sample) * 4 + q) *
-                                            (p.Cout / 2) + (c0 / 2) + (lane & 15)) * 2 + (lane >> 4);
-                  *g = w[0];
-                }
-              }
-            }
-          }
-          if (p.stats != nullptr && p.NB == 1) {
-            // recursive-halving reduce-scatter over the 32 lanes: afterwards ws[0] on lane L is the total of slot L
-#pragma unroll
-            for (int h = 16; h >= 1; h >>= 1) {
-              const bool up = (lane & h) != 0;
-#pragma unroll
-              for (int i = 0; i < h; ++i) {
-                const float send = up ? ws[i] : ws[i + h];
-                const float keep = up ? ws[i + h] : ws[i];
-                ws[i] = keep + __shfl_xor_sync(0xffffffffu, send, h);
-              }
-            }
-            wtot += ws[0];
-          }
-        }  // sub
-        if (p.stats != nullptr && p.NB == 1) st[(q * (BN / 32) + cc) * 32 + lane] = wtot;
-      }  // cc
-      }
-      if (warp == 0) ASYRP_TRACE_STAMP(8, it);
-
-      if (BN >= 32 && p.stats != nullptr && p.NB == 1) {
-        named_bar_sync(1, kEpThreads);
-        for (int e = ep_tid; e < BN; e += kEpThreads) {
-          const int cc = e >> 5, j = e & 31;
-          float tot = 0.f;
-#pragma unroll
-          for (int qq = 0; qq < 4; ++qq) tot += st[(qq * (BN / 32) + cc) * 32 + j];
-          float* g = p.stats + ((static_cast<size_t>(tn) * tiles_per_sample + tile_in_sample) * (p.Cout / 2) +
-                                (nt * BN + cc * 32) / 2 + (j & 15)) * 2 + (j >> 4);
-          *g = tot;
-          if (p.sums_out != nullptr)
-            stat_atomic_add(p.sums_out + (static_cast<size_t>(tn) * (p.Cout / 2) + (nt * BN + cc * 32) / 2 + (j & 15)) * 2 +
-                                (j >> 4), tot);
-        }
-      }
+      __syncwarp();
+      if (lane == 0) mbar_arrive(stageFull);
     }
   }
 }
@@ -1396,7 +1429,7 @@ ASYRP_API int asyrp_conv_create(const AsyrpConvDesc* d, void** out_op) {
                 "asyrp_conv_create: sums_out needs stats and tiles inside one sample");
   op->smem_bytes = 1024 + static_cast<size_t>(p.a_stages) * p.a_stage_bytes +
                    static_cast<size_t>(p.l_stages) * p.l_stage_bytes + static_cast<size_t>(p.b_stages) * b_stage +
-                   staging + (3 * (p.a_stages + p.l_stages) + 2 * p.b_stages) * 8 + 2 * 4 * op->BN * 4 +
+                   staging + (3 * (p.a_stages + p.l_stages) + 2 * p.b_stages + 2) * 8 + 2 * 4 * op->BN * 4 +
                    2 * kMaxSeg * 32 * sizeof(float2);
   ASYRP_REQUIRE(op->smem_bytes <= 227 * 1024, "asyrp_conv_create: smem %zu too large", op->smem_bytes);
   const int sms = sm_count();

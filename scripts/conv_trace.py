@@ -7,8 +7,17 @@
 Every role of conv_gemm_kernel stamps clock64() at its hand-off points (csrc/conv_gemm.cu ASYRP_TRACE_STAMP):
   0 A-producer: slot free, TMA issued      1 transform: stage landed      2 transform: stage done
   3 MMA: waits for the stage               4 MMA: stage ready             9 MMA: all MMAs of the stage issued
-  5 MMA: tile start                        6 MMA: accumulator free        7 epilogue: accumulator full   8 epilogue: drained
-The script saves the raw stamps and prints, per CTA, where the tensor pipe's idle time between stages comes from."""
+  5 MMA: tile start                        6 MMA: staging tile free (the previous tile's epilogue has read it)
+  7 epilogue: staging tile full            8 epilogue: staging tile drained
+  10 MMA: clocks the stage spent waiting for weight stages (a duration, not a time stamp)
+A library built before the staging handoff has 10 roles (--roles 10) and no stamp 6 or 10.
+
+Per CTA the script prints, as shares of the CTA's span (first tile start to last drain):
+  * tile boundaries: from the last MMA issue of tile i to the first stage of tile i+1 being ready (includes the last
+    wgmma group's execution), split into the wait for the staging tile and the rest (staging write, A-stage wait);
+  * A waits: the MMA warps waiting for a ready activation stage inside a tile;
+  * B waits: the MMA warps waiting for a weight stage;
+  * the epilogue's length per tile."""
 import argparse, ctypes as C, os, sys
 import numpy as np
 import torch
@@ -17,6 +26,7 @@ from asyrp_official_b200 import ops, _lib
 ap = argparse.ArgumentParser()
 ap.add_argument("spec")
 ap.add_argument("--out", default="gpurun_out/trace.npz")
+ap.add_argument("--roles", type=int, default=11, help="trace roles of the library (10 before the staging handoff)")
 a = ap.parse_args()
 dev = torch.device("cuda:0")
 N = 16
@@ -37,7 +47,7 @@ w = (torch.randn(Cout, K, device=dev) / K ** 0.5).half()
 out = torch.empty(N, H, H, Cout, device=dev, dtype=torch.float16)
 op = ops.ConvOp(segs, w, out=out, stats=ops.new_stats(N, H, H, Cout, dev, True))
 lib = _lib.load()
-ROLES, LEN = 10, 128
+ROLES, LEN = a.roles, 128
 buf = torch.zeros(132 * ROLES * LEN, dtype=torch.int64, device=dev)
 lib.asyrp_conv_set_trace.restype = C.c_int
 lib.asyrp_conv_set_trace.argtypes = [C.c_void_p, C.c_void_p]
@@ -50,19 +60,34 @@ e0.record(); op.launch(); e1.record(); torch.cuda.synchronize()
 us = e0.elapsed_time(e1) * 1e3
 t = buf.cpu().numpy().reshape(132, ROLES, LEN)[:grid]
 os.makedirs(os.path.dirname(a.out) or ".", exist_ok=True)
-np.savez_compressed(a.out, t=t, spec=a.spec, us=us, grid=grid)
+np.savez_compressed(a.out, t=t, spec=a.spec, us=us, grid=grid, roles=ROLES)
 print(f"{a.spec}: {us:.1f} us, grid {grid}, {2.0 * N * H * H * Cout * K / us / 1e6:.0f} TF/s")
-for cta in (0, 1, grid // 2, grid - 1):
+# K stages per tile: one per 64-channel chunk (halo tiles, 1x1 chunks), three dx-shifted copies per 3x3 chunk otherwise
+halo = H % 16 == 0
+spt = (Cin // 64) * (nseg * (1 if halo else 3) + n1)
+rows = []
+for cta in range(grid):
     r = t[cta]
-    ns = int((r[4] > 0).sum()); nt = int((r[5] > 0).sum())
-    t0 = r[5][0]
-    span = r[8][nt - 1] - t0
-    wait = (r[4][:ns] - r[3][:ns])
-    acc_wait = (r[6][:nt] - r[5][:nt])
-    issue = (r[9][:ns] - r[4][:ns])
-    xf = (r[2][:ns] - r[1][:ns])
-    land = (r[1][:ns] - r[0][:ns])
-    print(f"CTA {cta}: {nt} tiles, {ns} stages, span {span} clk = {span / max(nt, 1):.0f} per tile; MMA warp waits: stage-ready "
-          f"{wait.sum()} ({wait.sum() / span * 100:.1f}%), accumulator {acc_wait.sum()} ({acc_wait.sum() / span * 100:.1f}%); "
-          f"issue per stage {issue.mean():.0f}; transform per stage {xf.mean():.0f} (max {xf.max()}); TMA issue->landed "
-          f"{land.mean():.0f} (max {land.max()})")
+    nt = int((r[5] > 0).sum())
+    nts = min(nt, LEN // spt)  # tiles whose stages are all stamped
+    ns = nts * spt
+    span = r[8][nt - 1] - r[5][0]
+    first = np.arange(1, nts) * spt          # first stage of tiles 1..nts-1
+    gap = r[4][first] - r[9][first - 1]      # last MMA issue of tile i -> first stage of tile i+1 ready
+    st_wait = (r[6][:nts - 1] - r[9][first - 1]) if ROLES > 10 else np.zeros(0)
+    inner = np.setdiff1d(np.arange(ns), np.arange(0, ns, spt))
+    a_wait = r[4][inner] - r[3][inner]
+    b_wait = r[10][:ns] if ROLES > 10 else np.zeros(0)
+    epi = r[8][:nt] - r[7][:nt]
+    # shares of the stamped part of the span (stage stamps stop at LEN)
+    cov = (r[9][ns - 1] - r[5][0]) if nts < nt else span
+    rows.append((nt, span / nt, gap.sum() / cov, st_wait.sum() / cov, a_wait.sum() / cov, b_wait.sum() / cov,
+                 epi.mean(), (r[2][:ns] - r[1][:ns]).mean()))
+R = np.array(rows)
+print("CTA  tiles  clk/tile  boundary%  (staging wait%)  A-wait%  B-wait%  epilogue clk  transform clk/stage")
+for cta in sorted({0, 1, grid // 2, grid - 1}):
+    nt, pt, g, s, aw, bw, ep, xf = R[cta]
+    print(f"{cta:3d} {nt:6.0f} {pt:9.0f} {100 * g:9.1f}  ({100 * s:5.1f})       {100 * aw:6.1f}  {100 * bw:6.1f}  {ep:12.0f}  "
+          f"{xf:8.0f}")
+nt, pt, g, s, aw, bw, ep, xf = R.mean(0)
+print(f"all {nt:6.1f} {pt:9.0f} {100 * g:9.1f}  ({100 * s:5.1f})       {100 * aw:6.1f}  {100 * bw:6.1f}  {ep:12.0f}  {xf:8.0f}")

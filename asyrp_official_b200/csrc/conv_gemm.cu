@@ -313,25 +313,42 @@ __device__ __forceinline__ void gn_affine8(const ConvSegDev& sg, const float2* g
     cb[i] = b;
   }
 }
-// Recursive-halving reduce-scatter of 32 per-lane values over the warp: afterwards w[0] on lane L is the total of
-// slot L.  One template instance per step, so that every index is a constant and w[] stays in registers (written
-// as a loop over the step width, the steps were not unrolled and w[] went to local memory).
-template <int H>
-__device__ __forceinline__ void reduce_scatter_step(float (&w)[32], int lane) {
-  const bool up = (lane & H) != 0;
+// GroupNorm slot values of one output row's 8 channels (on == false: zeros): [k] = sum of channel pair k, [4 + k]
+// its sum of squares
+__device__ __forceinline__ void pair_sums(const float (&v)[8], bool on, float (&x)[8]) {
 #pragma unroll
-  for (int i = 0; i < H; ++i) {
-    const float send = up ? w[i] : w[i + H];
-    const float keep = up ? w[i + H] : w[i];
-    w[i] = keep + __shfl_xor_sync(0xffffffffu, send, H);
+  for (int k = 0; k < 4; ++k) {
+    const float a = on ? v[2 * k] : 0.f, b = on ? v[2 * k + 1] : 0.f;
+    x[k] = a + b;
+    x[4 + k] = a * a + b * b;
   }
 }
-__device__ __forceinline__ void reduce_scatter32(float (&w)[32], int lane) {
-  reduce_scatter_step<16>(w, lane);
-  reduce_scatter_step<8>(w, lane);
-  reduce_scatter_step<4>(w, lane);
-  reduce_scatter_step<2>(w, lane);
-  reduce_scatter_step<1>(w, lane);
+__host__ __device__ constexpr int bit_reverse(int t, int bits) {
+  int r = 0;
+  for (int b = 0; b < bits; ++b) r |= ((t >> b) & 1) << (bits - 1 - b);
+  return r;
+}
+__host__ __device__ constexpr int trailing_ones(int t) {
+  int n = 0;
+  while (t & 1) { t >>= 1; ++n; }
+  return n;
+}
+// Pairwise sum of the rows an epilogue lane visits, row t of the visit order at a time (t must be a constant after
+// unrolling): lv[l] holds the sum of the 2^l rows visited last while it waits for its sibling, lv[L-1] ends up
+// holding the total.  Rows visited in bit-reversed order of their row index i fold first over the top bit of i.
+template <int L>
+__device__ __forceinline__ void tree_add(float (&lv)[L][8], float (&x)[8], int t) {
+  const int m = trailing_ones(t);
+#pragma unroll
+  for (int l = 0; l < L - 1; ++l)
+    if (l < m)
+#pragma unroll
+      for (int k = 0; k < 8; ++k) x[k] = lv[l][k] + x[k];
+#pragma unroll
+  for (int l = 0; l < L; ++l)
+    if (l == m)
+#pragma unroll
+      for (int k = 0; k < 8; ++k) lv[l][k] = x[k];
 }
 __device__ __forceinline__ void stat_atomic_add(long long* dst, float v) {
   atomicAdd(reinterpret_cast<unsigned long long*>(dst), static_cast<unsigned long long>(__float2ll_rn(v * kStatScale)));
@@ -534,10 +551,10 @@ __global__ void __launch_bounds__(kNumThreads, 1) conv_gemm_kernel(const __grid_
       }
     };
     if (p.any_gn && static_cast<int>(blockIdx.x) < total_tiles) group_stats(blockIdx.x, 0);
-    // Epilogue, from the staging tile in shared memory (row = pixel of the sub-tile, column = sub * BN + channel):
-    // warp 8+w, (q, half) = (w & 3, w >> 2), owns pixel rows [32q, 32q+32) and drains the 32-channel column chunks
-    // half, half+2, ...  `it` counts the CTA's tiles: the phase of the staging barriers and the statistics buffer.
-    // Everything per thread is derived inside: the transform state stays live across the call.
+    // Epilogue, from the staging tile in shared memory (row = pixel of the sub-tile, column = sub * BN + channel).
+    // Warp 8+w, (q, half) = (w & 3, w >> 2), drains pixel rows [32q, 32q+32) of every sub-tile.  `it` counts the
+    // CTA's tiles: the phase of the staging barriers and the statistics buffer.  Everything per thread is derived
+    // inside: the transform state stays live across the call.
     constexpr int kEpThreads = kNumTransformWarps * 32;
     auto drain = [&](int tile, int it) {
       mbar_wait_suspend(stageFull, it & 1);
@@ -545,10 +562,7 @@ __global__ void __launch_bounds__(kNumThreads, 1) conv_gemm_kernel(const __grid_
       const int q = (warp - kWarpT) & 3;
       const int half = (warp - kWarpT) >> 2;
       const int ep_tid = tt;
-      const int row = q * 32 + lane;
-      const int xx = row % p.TW, nn = (row / p.TW) % p.NB, yy = row / (p.TW * p.NB);
       const int tiles_per_sample = p.tiles_x * p.tiles_y * (p.up2 ? 4 : 1);  // statistics slots per sample
-      const uint32_t c_row = smem_u32(sC) + static_cast<uint32_t>(row * kCPitch) * 4u;
 
       const TileCoord tc = tile_coord(p, tile);
       const int tx = tc.tx, ty = tc.ty, tn = tc.tn;
@@ -560,12 +574,15 @@ __global__ void __launch_bounds__(kNumThreads, 1) conv_gemm_kernel(const __grid_
         nt -= ph * cts;
       }
       const int ps = p.up2 ? 2 : 1, OH = p.H * ps, OW = p.W * ps, pa_ = ph >> 1, pb_ = ph & 1;
-      const int x = tx * p.TW + xx, n = tn * p.NB + nn;
       const int tile_in_sample = (ty * p.tiles_x + tx) * (p.up2 ? 4 : 1) + ph;
       float* st = s_stats + (it & 1) * (4 * BN);
       if constexpr (BN == 16) {
-        // narrow-N tile of conv_out (3 / 6 real output channels, fp32 planar store): one 16-column load per sub-tile,
-        // warps of the second half have nothing to drain
+        // narrow-N tile of conv_out (3 / 6 real output channels, fp32 planar store, contiguous along x): one lane per
+        // pixel row, one 16-column load per sub-tile; warps of the second half have nothing to drain
+        const int row = q * 32 + lane;
+        const int xx = row % p.TW, nn = (row / p.TW) % p.NB, yy = row / (p.TW * p.NB);
+        const int x = tx * p.TW + xx, n = tn * p.NB + nn;
+        const uint32_t c_row = smem_u32(sC) + static_cast<uint32_t>(row * kCPitch) * 4u;
         if (half == 0) {
 #pragma unroll 1
           for (int sub = 0; sub < MT; ++sub) {
@@ -585,146 +602,206 @@ __global__ void __launch_bounds__(kNumThreads, 1) conv_gemm_kernel(const __grid_
           }
         }
       } else {
+        // Warp (q, half) owns channels [half*BN/2, (half+1)*BN/2) of its 32 rows.  A lane owns 8 consecutive channels
+        // (one 16-byte fp16 store) of kNI rows; the kLPP lanes of a pixel row cover its BN/2 channels, so every global
+        // access of the epilogue covers whole 128-byte lines (BN 128) or whole halves of them (BN 64), and a lane
+        // needs the bias of its 8 channels only (one row per tile unless the tile's samples have rows of their own).
+        constexpr int kLPP = BN / 16;  // lanes per pixel row: 8 or 4
+        constexpr int kPG = 32 / kLPP;  // pixel rows per warp access: 4 or 8
+        constexpr int kNI = 32 / kPG;   // rows per lane: 8 or 4
+        constexpr int kLog = kNI == 8 ? 3 : 2;
+        // lane bits 0-1: low bits of the channel group, bit 2: bit 0 of the row group.  The 8 lanes of a quarter-warp
+        // thus read 32-byte column groups 0, 2, 4, 6 (x 16 B) of two adjacent staging rows, whose pitch is 16 B mod
+        // 128 B: their 16-byte reads fall in 8 distinct bank quads (8 groups of one row would collide pairwise).
+        const int cg = (lane & 3) | (kLPP == 8 ? ((lane >> 3) & 1) << 2 : 0);
+        const int g = kLPP == 8 ? (((lane >> 2) & 1) | ((lane >> 4) << 1)) : (lane >> 2);
+        const int cw = half * (BN / 2) + 8 * cg;  // first of the lane's channels in the tile
+        const int ch = nt * BN + cw;              // ... in the output
+        const int lw = __ffs(p.TW) - 1, ln = __ffs(p.NB) - 1;  // TW * TH * NB == 128: all three are powers of two
+        struct Px { int x, y, n; bool valid; };
+        auto row_px = [&](int sub, int i) {
+          const int r = 32 * q + kPG * i + g;
+          Px w;
+          w.x = tx * p.TW + (r & (p.TW - 1));
+          w.n = tn * p.NB + ((r >> lw) & (p.NB - 1));
+          w.y = ty * THT + sub * p.TH + (r >> (lw + ln));
+          w.valid = w.x < p.W && w.y < p.H && w.n < p.N;
+          return w;
+        };
+        auto row_addr = [&](int sub, int i) {
+          return smem_u32(sC) + static_cast<uint32_t>((32 * q + kPG * i + g) * kCPitch + sub * BN + cw) * 4u;
+        };
+        // output element of the lane's first channel: batch entry n may be a (sample, head) pair writing a slice
+        auto out_off = [&](const Px& w) {
+          const int nh = p.out_heads == 1 ? w.n : w.n / p.out_heads;
+          return ((static_cast<size_t>(nh) * OH + w.y * ps + pa_) * OW + w.x * ps + pb_) * p.out_ld +
+                 static_cast<size_t>(w.n - nh * p.out_heads) * p.Cout + ch;
+        };
+        // residual of a row, res_mode 0 (output geometry) or 1 (nearest-x2 of the half-resolution tensor, skip branch of
+        // an up ResBlock); res_mode 2 (2x2 average of the double-resolution tensor, down ResBlock) loads in the row
+        auto load_res = [&](const Px& w) {
+          uint4 u = make_uint4(0u, 0u, 0u, 0u);
+          if (p.res != nullptr && p.res_mode != 2 && w.valid) {
+            const size_t off = p.res_mode == 1 ? ((static_cast<size_t>(w.n) * (p.H >> 1) + (w.y >> 1)) * (p.W >> 1) +
+                                                  (w.x >> 1)) * p.Cout + ch
+                                               : out_off(w);
+            u = *reinterpret_cast<const uint4*>(p.res + off);
+          }
+          return u;
+        };
+        float eb[8];
+        auto load_bias = [&](int n) {
+          const float4* b4 = reinterpret_cast<const float4*>(p.ebias + static_cast<size_t>(n) * p.ebias_stride + ch);
+          const float4 lo = b4[0], hi = b4[1];
+          eb[0] = lo.x; eb[1] = lo.y; eb[2] = lo.z; eb[3] = lo.w; eb[4] = hi.x; eb[5] = hi.y; eb[6] = hi.z; eb[7] = hi.w;
+        };
+        // one bias row for the tile, unless its rows belong to several samples with rows of their own
+        const bool eb_rows = p.ebias != nullptr && p.ebias_stride > 0 && p.NB > 1;
+        if (p.ebias != nullptr && !eb_rows) load_bias(tn);
+        // statistics of tiles spanning several samples (MT == 1: stacked sub-tiles are whole tiles of one sample): the
+        // epilogue values go back into the staging tile, and one masked pass per sample sums them
+        const bool nb_stats = MT == 1 && p.stats != nullptr && p.NB > 1;
+        // NB == 1: the lane's slots in the statistics scratch; slot j < 16 of a 32-channel column chunk is the sum of
+        // its channel pair j, slot 16 + j the sum of squares
+        float* st_lane = st + (q * (BN / 32) + (cw >> 5)) * 32 + ((cw & 31) >> 1);
+        // Statistics summation order: a quarter's 32 rows are summed as a fixed tree over the row bits, bit 4 first
+        // and bit 0 last.  Row 32q + kPG*i + g: the bits of i are the row's top bits (tree_add over the rows in
+        // bit-reversed order of i), the bits of g the low ones (shuffles across the row groups, highest bit first).
+        auto rowgroup_sum = [&](float (&x)[8]) {
+#pragma unroll
+          for (int k = 0; k < 8; ++k) {
+            x[k] += __shfl_xor_sync(0xffffffffu, x[k], 16);
+            if (kLPP == 4) x[k] += __shfl_xor_sync(0xffffffffu, x[k], 8);
+            x[k] += __shfl_xor_sync(0xffffffffu, x[k], 4);
+          }
+        };
 #pragma unroll 1
-        for (int cc = half; cc < BN / 32; cc += 2) {
-          const int c0 = nt * BN + cc * 32;
-          // statistics of this chunk: slot `lane` (see below) summed over the sub-tiles.  Reduced across the lanes once per
-          // sub-tile: per-lane partial sums kept alive across the sub-tile loop (32 more registers next to r[] and v[])
-          // would spill
-          float wtot = 0.f;
-#pragma unroll 1
-          for (int sub = 0; sub < MT; ++sub) {
-            float ws[32];
+        for (int sub = 0; sub < MT; ++sub) {
+          float lv[kLog + 1][8];
+          Px wn = row_px(sub, 0);
+          uint4 un = load_res(wn);  // residual of the next row: in flight while the current row is computed
 #pragma unroll
-            for (int j = 0; j < 32; ++j) ws[j] = 0.f;
-            const int y = ty * THT + sub * p.TH + yy;
-            const bool valid = (x < p.W) && (y < p.H) && (n < p.N);
-            // output row of this pixel: batch entry n may be a (sample, head) pair writing a channel slice
-            const size_t pix = ((static_cast<size_t>(n / p.out_heads) * OH + y * ps + pa_) * OW + x * ps + pb_) * p.out_ld +
-                               static_cast<size_t>(n % p.out_heads) * p.Cout;
-            uint32_t r[32];
-            ld_staged<32>(c_row + (sub * BN + cc * 32) * 4, r);
-            float v[32];
-#pragma unroll
-            for (int i = 0; i < 32; ++i) v[i] = __uint_as_float(r[i]);
-            if (p.ebias != nullptr) {
-              const float* eb = p.ebias + static_cast<size_t>(valid ? n : 0) * p.ebias_stride + c0;
-#pragma unroll
-              for (int i = 0; i < 32; i += 4) {
-                const float4 b4 = *reinterpret_cast<const float4*>(eb + i);
-                v[i] += b4.x; v[i + 1] += b4.y; v[i + 2] += b4.z; v[i + 3] += b4.w;
-              }
+          for (int t = 0; t < kNI; ++t) {
+            const int i = bit_reverse(t, kLog);
+            const Px w = wn;
+            const uint4 u = un;
+            if (t + 1 < kNI) {
+              wn = row_px(sub, bit_reverse(t + 1, kLog));
+              un = load_res(wn);
             }
-            const float acc_scale = conv_scale(p, n, 0);
+            uint32_t r[8];
+            ld_staged<8>(row_addr(sub, i), r);
+            float v[8];
+#pragma unroll
+            for (int k = 0; k < 8; ++k) v[k] = __uint_as_float(r[k]);
+            if (p.ebias != nullptr) {
+              if (eb_rows) load_bias(w.valid ? w.n : 0);
+#pragma unroll
+              for (int k = 0; k < 8; ++k) v[k] += eb[k];
+            }
+            const float acc_scale = conv_scale(p, w.n, 0);
             if (acc_scale != 1.0f) {  // exact skip: multiplying by 1 changes nothing
 #pragma unroll
-              for (int i = 0; i < 32; ++i) v[i] *= acc_scale;
+              for (int k = 0; k < 8; ++k) v[k] *= acc_scale;
             }
-            if (p.res != nullptr && valid) {
-              const float res_scale = conv_scale(p, n, 1);
+            if (p.res != nullptr && w.valid) {
+              const float res_scale = conv_scale(p, w.n, 1);
               if (p.res_mode == 2) {
-                // skip branch of a down ResBlock: 2x2 average of the double-resolution tensor, fp32
                 const size_t rW = static_cast<size_t>(p.W) * 2;
-                const __half* r0 = p.res + ((static_cast<size_t>(n) * p.H * 2 + y * 2) * rW + x * 2) * p.Cout + c0;
+                const __half* r0 = p.res + ((static_cast<size_t>(w.n) * p.H * 2 + w.y * 2) * rW + w.x * 2) * p.Cout + ch;
+                float a8[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
 #pragma unroll
-                for (int j = 0; j < 4; ++j) {
-                  float a8[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
-#pragma unroll
-                  for (int q4 = 0; q4 < 4; ++q4) {
-                    const uint4 u = *reinterpret_cast<const uint4*>(r0 + ((q4 >> 1) * rW + (q4 & 1)) * p.Cout + j * 8);
-                    const __half2* h2 = reinterpret_cast<const __half2*>(&u);
-#pragma unroll
-                    for (int k = 0; k < 4; ++k) {
-                      const float2 f = __half22float2(h2[k]);
-                      a8[2 * k] += f.x;
-                      a8[2 * k + 1] += f.y;
-                    }
-                  }
-#pragma unroll
-                  for (int k = 0; k < 8; ++k) v[j * 8 + k] += res_scale * (0.25f * a8[k]);
-                }
-              } else {
-                // res_mode 1: nearest-x2 of the half-resolution tensor (skip branch of an up ResBlock)
-                const size_t rpix = p.res_mode == 1 ? ((static_cast<size_t>(n) * (p.H >> 1) + (y >> 1)) * (p.W >> 1) + (x >> 1)) *
-                                                          p.Cout
-                                                    : pix;
-                const uint4* rp = reinterpret_cast<const uint4*>(p.res + rpix + c0);
-#pragma unroll
-                for (int j = 0; j < 4; ++j) {
-                  const uint4 u = rp[j];
-                  const __half2* h2 = reinterpret_cast<const __half2*>(&u);
+                for (int q4 = 0; q4 < 4; ++q4) {
+                  const uint4 u4 = *reinterpret_cast<const uint4*>(r0 + ((q4 >> 1) * rW + (q4 & 1)) * p.Cout);
+                  const __half2* h2 = reinterpret_cast<const __half2*>(&u4);
 #pragma unroll
                   for (int k = 0; k < 4; ++k) {
                     const float2 f = __half22float2(h2[k]);
-                    v[j * 8 + k * 2] += res_scale * f.x;
-                    v[j * 8 + k * 2 + 1] += res_scale * f.y;
+                    a8[2 * k] += f.x;
+                    a8[2 * k + 1] += f.y;
                   }
                 }
-              }
-            }
-            if (p.out_planar != nullptr) {
-              if (valid && c0 == 0) {
-                const size_t hw = static_cast<size_t>(p.H) * p.W;
-                float* pp = p.out_planar + static_cast<size_t>(n) * p.planar_c * hw + static_cast<size_t>(y) * p.W + x;
 #pragma unroll
-                for (int i = 0; i < 8; ++i)
-                  if (i < p.planar_c) pp[i * hw] = v[i];
-              }
-            } else if (p.out_f32) {
-              if (valid) {
-                float4* op = reinterpret_cast<float4*>(reinterpret_cast<float*>(p.out) + pix + c0);
-#pragma unroll
-                for (int j = 0; j < 8; ++j) op[j] = make_float4(v[4 * j], v[4 * j + 1], v[4 * j + 2], v[4 * j + 3]);
-              }
-            } else if (valid) {
-              uint4* op = reinterpret_cast<uint4*>(p.out + pix + c0);
-#pragma unroll
-              for (int j = 0; j < 4; ++j) {
-                uint4 u;
-                __half2* h2 = reinterpret_cast<__half2*>(&u);
-#pragma unroll
-                for (int k = 0; k < 4; ++k) h2[k] = __floats2half2_rn(v[j * 8 + k * 2], v[j * 8 + k * 2 + 1]);
-                op[j] = u;
-              }
-            }
-            if (p.stats != nullptr) {
-              if (p.NB == 1) {
-                // slot j<16 : sum of channel pair j ; slot j>=16 : sum of squares of pair j-16 (this lane's pixel)
-                if (valid) {
-#pragma unroll
-                  for (int j = 0; j < 16; ++j) {
-                    ws[j] += v[2 * j] + v[2 * j + 1];
-                    ws[16 + j] += v[2 * j] * v[2 * j] + v[2 * j + 1] * v[2 * j + 1];
-                  }
-                }
+                for (int k = 0; k < 8; ++k) v[k] += res_scale * (0.25f * a8[k]);
               } else {
-                // tiles spanning several samples (tiny layers): one masked warp reduction per sample
-                for (int sn = 0; sn < p.NB; ++sn) {
-                  const bool mine = valid && (nn == sn);
-                  float w[32];
+                const __half2* h2 = reinterpret_cast<const __half2*>(&u);
 #pragma unroll
-                  for (int j = 0; j < 16; ++j) {
-                    const float a = mine ? v[2 * j] : 0.f, b = mine ? v[2 * j + 1] : 0.f;
-                    w[j] = a + b;
-                    w[16 + j] = a * a + b * b;
-                  }
-                  reduce_scatter32(w, lane);
-                  const int ns = tn * p.NB + sn;
-                  if (ns < p.N) {  // one slot per (sample, tile, lane quarter): deterministic, no atomics
-                    float* g = p.stats + (((static_cast<size_t>(ns) * tiles_per_sample + tile_in_sample) * 4 + q) *
-                                              (p.Cout / 2) + (c0 / 2) + (lane & 15)) * 2 + (lane >> 4);
-                    *g = w[0];
-                  }
+                for (int k = 0; k < 4; ++k) {
+                  const float2 f = __half22float2(h2[k]);
+                  v[2 * k] += res_scale * f.x;
+                  v[2 * k + 1] += res_scale * f.y;
                 }
               }
             }
-            if (p.stats != nullptr && p.NB == 1) {
-              reduce_scatter32(ws, lane);  // afterwards ws[0] on lane L is the total of slot L
-              wtot += ws[0];
+            if (w.valid) {
+              if (p.out_planar != nullptr) {
+                if (ch == 0) {
+                  const size_t hw = static_cast<size_t>(p.H) * p.W;
+                  float* pp = p.out_planar + static_cast<size_t>(w.n) * p.planar_c * hw + static_cast<size_t>(w.y) * p.W + w.x;
+#pragma unroll
+                  for (int k = 0; k < 8; ++k)
+                    if (k < p.planar_c) pp[k * hw] = v[k];
+                }
+              } else if (p.out_f32) {
+                float4* op = reinterpret_cast<float4*>(reinterpret_cast<float*>(p.out) + out_off(w));
+                op[0] = make_float4(v[0], v[1], v[2], v[3]);
+                op[1] = make_float4(v[4], v[5], v[6], v[7]);
+              } else {
+                uint4 o;
+                __half2* h2 = reinterpret_cast<__half2*>(&o);
+#pragma unroll
+                for (int k = 0; k < 4; ++k) h2[k] = __floats2half2_rn(v[2 * k], v[2 * k + 1]);
+                *reinterpret_cast<uint4*>(p.out + out_off(w)) = o;
+              }
             }
-          }  // sub
-          if (p.stats != nullptr && p.NB == 1) st[(q * (BN / 32) + cc) * 32 + lane] = wtot;
-        }  // cc
+            if (nb_stats) {
+              const uint32_t a = row_addr(sub, i);
+              sts128(a, make_uint4(__float_as_uint(v[0]), __float_as_uint(v[1]), __float_as_uint(v[2]), __float_as_uint(v[3])));
+              sts128(a + 16, make_uint4(__float_as_uint(v[4]), __float_as_uint(v[5]), __float_as_uint(v[6]), __float_as_uint(v[7])));
+            } else if (p.stats != nullptr) {
+              float x[8];
+              pair_sums(v, w.valid, x);
+              tree_add(lv, x, t);
+            }
+          }
+          if (p.stats != nullptr && p.NB == 1) {
+            rowgroup_sum(lv[kLog]);
+            if (g == 0) {  // summed over the sub-tiles in order, from 0
+#pragma unroll
+              for (int k = 0; k < 4; ++k) {
+                st_lane[k] = (sub == 0 ? 0.f : st_lane[k]) + lv[kLog][k];
+                st_lane[16 + k] = (sub == 0 ? 0.f : st_lane[16 + k]) + lv[kLog][4 + k];
+              }
+            }
+          }
+          if (nb_stats) {
+#pragma unroll 1
+            for (int sn = 0; sn < p.NB; ++sn) {
+              const int ns = tn * p.NB + sn;
+#pragma unroll
+              for (int t = 0; t < kNI; ++t) {
+                const int i = bit_reverse(t, kLog);
+                const Px w = row_px(sub, i);
+                uint32_t r[8];
+                ld_staged<8>(row_addr(sub, i), r);
+                float v[8], x[8];
+#pragma unroll
+                for (int k = 0; k < 8; ++k) v[k] = __uint_as_float(r[k]);
+                pair_sums(v, w.valid && w.n == ns, x);
+                tree_add(lv, x, t);
+              }
+              rowgroup_sum(lv[kLog]);
+              if (ns < p.N && g == 0) {  // one slot per (sample, tile, quarter): deterministic, no atomics
+                const float* s = lv[kLog];
+                float4* d = reinterpret_cast<float4*>(
+                    p.stats + (((static_cast<size_t>(ns) * tiles_per_sample + tile_in_sample) * 4 + q) * (p.Cout / 2) +
+                               ch / 2) * 2);
+                d[0] = make_float4(s[0], s[4], s[1], s[5]);
+                d[1] = make_float4(s[2], s[6], s[3], s[7]);
+              }
+            }
+          }
+        }  // sub
       }
       // every read of the staging tile is done: the consumers may refill it
       __syncwarp();

@@ -1304,7 +1304,8 @@ ASYRP_API int asyrp_conv_create(const AsyrpConvDesc* d, void** out_op) {
   if (d->up2)
     ASYRP_REQUIRE(halo && d->nseg == 1 && !d->weight_batched && !d->out_f32 &&
                       d->out_planar == nullptr && d->out_heads <= 1 && d->a_heads <= 1 && d->residual == nullptr,
-                  "asyrp_conv_create: up2 needs one plain 3x3 segment on a source of H %% 16 == 0, W %% 8 == 0");
+                  "asyrp_conv_create: up2 needs one 3x3 segment (raw, fused affine or in-kernel GroupNorm) on a source "
+                  "of H %% 16 == 0, W %% 8 == 0, an fp16 NHWC output and no residual, heads or batched weights");
   p.up2 = d->up2 ? 1 : 0;
   conv_config(d->H, d->W, d->Cout, halo, &op->BN, &op->MT, p.up2 ? 4 : 1);
   p.MT = op->MT;

@@ -25,13 +25,18 @@ from .ops import MODE_1x1, MODE_3x3, MODE_3x3_S2, RESAMPLE_AVGPOOL2, RESAMPLE_NO
 # ASYRP_DUAL_STREAM=0: run the two decoder passes of an edit step one after the other (A/B measurements)
 DUAL_STREAM = os.environ.get("ASYRP_DUAL_STREAM", "1") != "0"
 # layers narrower than this keep a pointwise GroupNorm-apply launch instead of the in-kernel operand transform
-# (ASYRP_FUSE_MIN_H=8 fuses the 8x8 layers too: 28 launches fewer per edit evaluation)
+# (ASYRP_FUSE_MIN_H=8 fuses the 8x8 layers too: 28 apply launches fewer per edit evaluation of the DDPM UNet, 38 of
+# ADM ImageNet)
 FUSE_MIN_H = int(os.environ.get("ASYRP_FUSE_MIN_H", "16"))
 # ASYRP_GN_FOLD=1: GroupNorm finalised inside the consuming conv kernel from integer-atomic per-sample sums the
-# producers' epilogues accumulate (no gn_finalize launch, no affine table) for every layer of at least 16x16: 226 instead
-# of 315 launches per edit evaluation — at the price of per-tile group statistics on the transform warps' critical
-# path and 64-bit atomics in every epilogue.  Off by default; the path is complete and covered by tests
-# (test_groupnorm_finalised_inside_the_consumer_conv).
+# producers' epilogues accumulate (no gn_finalize launch, no affine table) for every layer of at least 16x16 except the
+# ADM downsampling ResBlocks' first norm (pointwise apply + average pool): 226 instead of 315 launches per edit
+# evaluation of the DDPM UNet, 345 instead of 464 for ADM ImageNet, 189 instead of 267 for ADM AFHQ (the 4 timestep-MLP launches,
+# which sample() runs outside the graph, not counted) — at the price of per-tile group statistics on the transform
+# warps' critical path and 64-bit atomics in every epilogue.  Off by default.  Covered by tests/test_engine_options_gpu.py
+# (every launch of the plans against fp64, whole trajectories, in-kernel GroupNorm past one wave in <128,1>, <64,1> and
+# up2) and by the kernel tests test_groupnorm_finalised_inside_the_consumer_conv and test_conv_coverage_gpu.py's
+# halo64x2_gn_* cases.
 GN_FOLD = os.environ.get("ASYRP_GN_FOLD", "0") in ("1", "2")
 GN_FOLD_PRODUCERS_ONLY = os.environ.get("ASYRP_GN_FOLD", "0") == "2"  # diagnostic: atomics on, consumers use tables
 # ResBlock identity skips x + h ride conv2's K loop as an identity weight block (C extra MACs per output, exact: fp16 x

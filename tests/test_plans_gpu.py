@@ -39,6 +39,7 @@ G = os.path.join(os.path.dirname(__file__), "golden")
 TOL_RAW, TOL_FUSED, TOL_FUSED_UP2, TOL_F32, TOL_STATS = 1.5e-3, 2.5e-3, 3e-3, 2e-5, 2e-3
 TOL_GN, TOL_APPLY, TOL_ATTN, TOL_SOFTMAX_ABS, TOL_LINEAR, TOL_TEMB_ABS, TOL_SLERP = \
     1e-4, 1e-3, 1.5e-3, 6e-4, 1e-5, 2e-4, 1e-3
+TOL_GN_FOLD = 3e-3  # test_conv_coverage_gpu.py: GroupNorm finalised inside the consuming conv
 TOL_TRAJ = 1e-3  # test_model_gpu.py: N-step x_0 vs the reference's own output
 # fp64 work (multiply-adds) per launch above which only samples 0, B//2 and B-1 are compared
 FULL_BATCH_MACS = 1 << 36
@@ -173,6 +174,16 @@ class Recorder:
             self.tags.add(tag)
 
     # ---------------------------------------------------------------------------------------------- conv
+    def seg_inputs(self, i, aff):
+        """the tensors segment i's operand transform reads (snapshotted, checked unchanged)"""
+        assert not isinstance(aff, ops.GNSpec), "in-kernel GroupNorm operands are not part of the default plans"
+        return {f"aff{i}": aff}
+
+    def seg_affine(self, snap, i, aff, off, C, idx):
+        """(a, b), each [samples idx][C], of segment i's operand transform y = a*x + b, from the snapshot"""
+        ab = snap[f"aff{i}"][idx].double()[:, off:off + C]
+        return ab[..., 0], ab[..., 1]
+
     def conv(self, op):
         segs, weight, kw = op._rec
         if kw.get("weight_batched"):
@@ -190,15 +201,17 @@ class Recorder:
             st = kw.get("ebias_stride", 0)
             ins["ebias"] = torch.as_strided(eb, (N, Cout), (st, 1), eb.storage_offset())
         for i, (src, mode, aff, off, act) in enumerate(segs):
-            assert not isinstance(aff, ops.GNSpec), "in-kernel GroupNorm operands are not part of the default plans"
             ins[f"src{i}"] = src
-            ins[f"aff{i}"] = aff
+            if aff is not None:
+                ins.update(self.seg_inputs(i, aff))
         outs = {"out": out, "stats": kw.get("stats"), "out_planar": planar}
         ktot = weight.shape[-1]
         ns = self.samples(Ho * Wo * Cout * ktot)
         fused = any(sg[2] is not None for sg in segs)
         tol = (TOL_FUSED_UP2 if fused else TOL_FUSED) if up2 else \
             (TOL_FUSED if fused else (TOL_F32 if planar is not None or out.dtype == torch.float32 else TOL_RAW))
+        if any(isinstance(sg[2], ops.GNSpec) for sg in segs):
+            tol = TOL_GN_FOLD
 
         def reference(snap, got):
             idx = torch.tensor(ns, device=weight.device)
@@ -208,8 +221,8 @@ class Recorder:
                 y = _nchw(snap[f"src{i}"][idx])
                 C = y.shape[1]
                 if aff is not None:
-                    ab = snap[f"aff{i}"][idx].double()[:, off:off + C]
-                    y = y * ab[..., 0, None, None] + ab[..., 1, None, None]
+                    a, b = self.seg_affine(snap, i, aff, off, C, idx)
+                    y = y * a[..., None, None] + b[..., None, None]
                     if act:
                         y = _silu(y)
                     y = _h32(y)

@@ -60,6 +60,7 @@ SIGNATURES = {
     "asyrp_conv_launch": (c_int, [c_void_p, c_void_p]),
     "asyrp_conv_set_scales": (c_int, [c_void_p, c_float, c_float]),
     "asyrp_conv_destroy": (None, [c_void_p]),
+    "asyrp_conv_drain_at": (c_int, [c_void_p]),
     "asyrp_gn_finalize": (c_int, [c_void_p, c_int, c_int, c_void_p, c_int, c_int, c_void_p, c_void_p, c_float,
                                   c_int, c_int, c_void_p, c_int, c_void_p, c_void_p]),
     "asyrp_apply": (c_int, [c_void_p, c_int, c_void_p, c_int, c_void_p, c_int, c_void_p, c_int, c_int, c_int, c_int,

@@ -122,6 +122,9 @@ struct ConvParams {
   // K-loop order: entries (segment << 6 | 64-channel chunk), see asyrp_conv_create().
   int n_sched;
   uint8_t sched[64];
+  // K-schedule entries of tile i+1 the transform warps ready before they run the epilogue of tile i (>= 1): as many as
+  // the activation rings hold while tile i's MMAs still read its last stage, see asyrp_conv_create()
+  int drain_at;
 #ifdef ASYRP_TRACE
   long long* trace;  // diagnostic build only: [CTA][kTraceRoles][kTraceLen] clock64() stamps, see scripts/conv_trace.py
 #endif
@@ -129,7 +132,7 @@ struct ConvParams {
 // Pipeline timeline of a diagnostic build (-DASYRP_TRACE, scripts/conv_trace.py): one elected lane per role stamps
 // clock64() at its hand-off points (role 10 holds a duration instead); compiled out of the product library.
 #ifdef ASYRP_TRACE
-static constexpr int kTraceRoles = 11, kTraceLen = 128;
+static constexpr int kTraceRoles = 12, kTraceLen = 128;
 #define ASYRP_TRACE_PUT(role, idx, val)                                                             \
   do {                                                                                              \
     if (p.trace != nullptr && lane == 0 && (idx) < kTraceLen)                                       \
@@ -374,8 +377,12 @@ __device__ __forceinline__ void ld_staged(uint32_t addr, uint32_t (&r)[NV]) {
 
 // BN output channels x MT sub-tiles of 128 pixels per CTA tile; each consumer warpgroup accumulates MT x BN/2 fp32
 // registers per thread.  MT * BN <= 128 bounds them to 64: ptxas allocates 96 registers per thread to every
-// instantiation at 576 threads, and the 64- and 128-channel ones still spill ~100 bytes outside the wgmma chain.
-template <int BN, int MT>
+// instantiation at 576 threads, and the 64- and 128-channel ones still spill outside the wgmma chain.
+// PLAIN: tiles inside one sample (NB == 1) and one fp16 NHWC output (out_heads == 1, no fp32 or planar output), as
+// every 128x128-and-larger layer has.  The epilogue and transform code of the other modes then drops out, and with it
+// the values they keep live across the epilogue's row loop: about half the spill traffic, and none of it reloaded
+// between the row loop's global stores.
+template <int BN, int MT, bool PLAIN>
 __global__ void __launch_bounds__(kNumThreads, 1) conv_gemm_kernel(const __grid_constant__ ConvParams p) {
   pdl_trigger();  // the next kernel of the stream may be scheduled as soon as every CTA of this grid is running
   extern __shared__ uint8_t smem_raw[];
@@ -509,6 +516,7 @@ __global__ void __launch_bounds__(kNumThreads, 1) conv_gemm_kernel(const __grid_
   } else if (warp >= kWarpT) {
     // ======================================================== operand transform (in place) + epilogue warps
     constexpr int kLanes = kNumTransformWarps * 4;  // pixels handled concurrently (8 threads per pixel)
+    const int NB = PLAIN ? 1 : p.NB;                // samples per tile
     const int tt = threadIdx.x - kWarpT * 32;
     const int jl = tt & 7;                  // logical 16B chunk = channels [jl*8, jl*8+8) of the 64-channel slab
     const int pl = tt >> 3;                 // pixel lane
@@ -529,7 +537,7 @@ __global__ void __launch_bounds__(kNumThreads, 1) conv_gemm_kernel(const __grid_
         if (hy == rows - 1) h_b |= 1u << m;
       }
 #pragma unroll 1
-      for (int m = 0, pk = pl; pk < THT * p.TW * p.NB; ++m, pk += kLanes) d_vld |= 1u << m;
+      for (int m = 0, pk = pl; pk < THT * p.TW * NB; ++m, pk += kLanes) d_vld |= 1u << m;
     }
     int sa = 0, sl = 0;
     uint32_t pa = 0, plt = 0;
@@ -617,13 +625,13 @@ __global__ void __launch_bounds__(kNumThreads, 1) conv_gemm_kernel(const __grid_
         const int g = kLPP == 8 ? (((lane >> 2) & 1) | ((lane >> 4) << 1)) : (lane >> 2);
         const int cw = half * (BN / 2) + 8 * cg;  // first of the lane's channels in the tile
         const int ch = nt * BN + cw;              // ... in the output
-        const int lw = __ffs(p.TW) - 1, ln = __ffs(p.NB) - 1;  // TW * TH * NB == 128: all three are powers of two
+        const int lw = __ffs(p.TW) - 1, ln = __ffs(NB) - 1;  // TW * TH * NB == 128: all three are powers of two
         struct Px { int x, y, n; bool valid; };
         auto row_px = [&](int sub, int i) {
           const int r = 32 * q + kPG * i + g;
           Px w;
           w.x = tx * p.TW + (r & (p.TW - 1));
-          w.n = tn * p.NB + ((r >> lw) & (p.NB - 1));
+          w.n = tn * NB + ((r >> lw) & (NB - 1));
           w.y = ty * THT + sub * p.TH + (r >> (lw + ln));
           w.valid = w.x < p.W && w.y < p.H && w.n < p.N;
           return w;
@@ -633,9 +641,10 @@ __global__ void __launch_bounds__(kNumThreads, 1) conv_gemm_kernel(const __grid_
         };
         // output element of the lane's first channel: batch entry n may be a (sample, head) pair writing a slice
         auto out_off = [&](const Px& w) {
-          const int nh = p.out_heads == 1 ? w.n : w.n / p.out_heads;
+          const int heads = PLAIN ? 1 : p.out_heads;
+          const int nh = heads == 1 ? w.n : w.n / heads;
           return ((static_cast<size_t>(nh) * OH + w.y * ps + pa_) * OW + w.x * ps + pb_) * p.out_ld +
-                 static_cast<size_t>(w.n - nh * p.out_heads) * p.Cout + ch;
+                 static_cast<size_t>(w.n - nh * heads) * p.Cout + ch;
         };
         // residual of a row, res_mode 0 (output geometry) or 1 (nearest-x2 of the half-resolution tensor, skip branch of
         // an up ResBlock); res_mode 2 (2x2 average of the double-resolution tensor, down ResBlock) loads in the row
@@ -656,11 +665,11 @@ __global__ void __launch_bounds__(kNumThreads, 1) conv_gemm_kernel(const __grid_
           eb[0] = lo.x; eb[1] = lo.y; eb[2] = lo.z; eb[3] = lo.w; eb[4] = hi.x; eb[5] = hi.y; eb[6] = hi.z; eb[7] = hi.w;
         };
         // one bias row for the tile, unless its rows belong to several samples with rows of their own
-        const bool eb_rows = p.ebias != nullptr && p.ebias_stride > 0 && p.NB > 1;
+        const bool eb_rows = p.ebias != nullptr && p.ebias_stride > 0 && NB > 1;
         if (p.ebias != nullptr && !eb_rows) load_bias(tn);
         // statistics of tiles spanning several samples (MT == 1: stacked sub-tiles are whole tiles of one sample): the
         // epilogue values go back into the staging tile, and one masked pass per sample sums them
-        const bool nb_stats = MT == 1 && p.stats != nullptr && p.NB > 1;
+        const bool nb_stats = MT == 1 && p.stats != nullptr && NB > 1;
         // NB == 1: the lane's slots in the statistics scratch; slot j < 16 of a 32-channel column chunk is the sum of
         // its channel pair j, slot 16 + j the sum of squares
         float* st_lane = st + (q * (BN / 32) + (cw >> 5)) * 32 + ((cw & 31) >> 1);
@@ -734,7 +743,7 @@ __global__ void __launch_bounds__(kNumThreads, 1) conv_gemm_kernel(const __grid_
               }
             }
             if (w.valid) {
-              if (p.out_planar != nullptr) {
+              if (!PLAIN && p.out_planar != nullptr) {
                 if (ch == 0) {
                   const size_t hw = static_cast<size_t>(p.H) * p.W;
                   float* pp = p.out_planar + static_cast<size_t>(w.n) * p.planar_c * hw + static_cast<size_t>(w.y) * p.W + w.x;
@@ -742,7 +751,7 @@ __global__ void __launch_bounds__(kNumThreads, 1) conv_gemm_kernel(const __grid_
                   for (int k = 0; k < 8; ++k)
                     if (k < p.planar_c) pp[k * hw] = v[k];
                 }
-              } else if (p.out_f32) {
+              } else if (!PLAIN && p.out_f32) {
                 float4* op = reinterpret_cast<float4*>(reinterpret_cast<float*>(p.out) + out_off(w));
                 op[0] = make_float4(v[0], v[1], v[2], v[3]);
                 op[1] = make_float4(v[4], v[5], v[6], v[7]);
@@ -764,7 +773,7 @@ __global__ void __launch_bounds__(kNumThreads, 1) conv_gemm_kernel(const __grid_
               tree_add(lv, x, t);
             }
           }
-          if (p.stats != nullptr && p.NB == 1) {
+          if (p.stats != nullptr && NB == 1) {
             rowgroup_sum(lv[kLog]);
             if (g == 0) {  // summed over the sub-tiles in order, from 0
 #pragma unroll
@@ -776,8 +785,8 @@ __global__ void __launch_bounds__(kNumThreads, 1) conv_gemm_kernel(const __grid_
           }
           if (nb_stats) {
 #pragma unroll 1
-            for (int sn = 0; sn < p.NB; ++sn) {
-              const int ns = tn * p.NB + sn;
+            for (int sn = 0; sn < NB; ++sn) {
+              const int ns = tn * NB + sn;
 #pragma unroll
               for (int t = 0; t < kNI; ++t) {
                 const int i = bit_reverse(t, kLog);
@@ -808,7 +817,7 @@ __global__ void __launch_bounds__(kNumThreads, 1) conv_gemm_kernel(const __grid_
       if (lane == 0) mbar_arrive(stageEmpty);
       if (warp == kWarpT) ASYRP_TRACE_STAMP(8, it);
 
-      if (BN >= 32 && p.stats != nullptr && p.NB == 1) {
+      if (BN >= 32 && p.stats != nullptr && NB == 1) {
         named_bar_sync(1, kEpThreads);
         for (int e = ep_tid; e < BN; e += kEpThreads) {
           const int cc = e >> 5, j = e & 31;
@@ -824,33 +833,37 @@ __global__ void __launch_bounds__(kNumThreads, 1) conv_gemm_kernel(const __grid_
         }
       }
     };
-    // The epilogue of tile i runs once the first K stage of tile i+1 is handed to the consumers, so that the tensor
-    // pipe works on tile i+1 meanwhile; without a transform, and after the CTA's last tile, it runs straight away.
+    // The epilogue of tile i runs once the first drain_at K-schedule entries of tile i+1 are handed to the consumers,
+    // so that the tensor pipe works on tile i+1 meanwhile; without a transform, and after the CTA's last tile, it runs
+    // straight away.  No drain_at in [1, n_xf] can deadlock: the consumers finish tile i's K loop and fill the staging
+    // tile without drain(i) — they need only the stages of tile i, readied in the previous iteration, and stageEmpty
+    // from drain(i-1), which also ran there.  So every ring slot that an entry of tile i+1 waits for before drain(i) is
+    // released by tile i's MMAs or by tile i+1's earlier entries, which this loop has already readied.
     int pend = -1;  // tile whose accumulators the consumers hand over next
     for (int tile = blockIdx.x, git = 0;; tile += gridDim.x, ++git) {
       const bool live = tile < total_tiles;
       const int n_xf = live && p.any_transform ? p.n_sched : 0;  // K stages this warp transforms for the tile
       const TileCoord tc = tile_coord(p, live ? tile : 0);
-      const int x0 = tc.tx * p.TW, y0 = tc.ty * THT, n0 = tc.tn * p.NB;
+      const int x0 = tc.tx * p.TW, y0 = tc.ty * THT, n0 = tc.tn * NB;
       if (n_xf > 0 && p.any_gn) {
         named_bar_sync(2, kNumTransformWarps * 32);
         if (tile + static_cast<int>(gridDim.x) < total_tiles) group_stats(tile + gridDim.x, (git + 1) & 1);
       }
       for (int e = 0; e <= n_xf; ++e) {
-        if (e == min(n_xf, 1) && pend >= 0) drain(pend, git - 1);
+        if (e == min(n_xf, p.drain_at) && pend >= 0) drain(pend, git - 1);
         if (e == n_xf) break;
         const int s = p.sched[e] >> 6, ch = p.sched[e] & 63;
         const ConvSegDev sg = p.seg[s];
         const bool lt = p.l_stages != 0 && sg.mode == 0;
         const int ncopies = (sg.mode == 0 || sg.mode == 3) ? 1 : (sg.mode == 1 ? 3 : 9);
         const int pw = sg.mode == 3 ? p.TW + 2 : p.TW;      // pixels per (row, sample) in the stage
-        const int prow = pw * p.NB;                          // pixels per tile row
+        const int prow = pw * NB;                            // pixels per tile row
         const int rows = (sg.mode == 1 || sg.mode == 3) ? THT + 2 : THT;
         const int npix = rows * prow;
         const int yoff = (sg.mode == 1 || sg.mode == 3) ? -1 : 0;
         {
           float ca[8], cb[8];
-          if (sg.affine != nullptr && p.NB == 1) {
+          if (sg.affine != nullptr && NB == 1) {
             const float4* ap = reinterpret_cast<const float4*>(
                 sg.affine + static_cast<size_t>(n0 < p.N ? n0 : 0) * sg.aff_stride + (ch * 64 + jl * 8) * 2);
 #pragma unroll
@@ -874,7 +887,7 @@ __global__ void __launch_bounds__(kNumThreads, 1) conv_gemm_kernel(const __grid_
               const int xoff = sg.mode == 3 ? -1 : (sg.mode == 1 ? cp - 1 : 0);
               // whole tile inside the image (always true for halo tiles; 1x1 stages of ragged layers fall back)
               const bool whole = x0 + p.TW <= p.W && y0 + THT <= p.H && n0 < p.N;
-              if (p.NB == 1 && whole && (sg.mode == 3 || sg.mode == 0)) {
+              if (NB == 1 && whole && (sg.mode == 3 || sg.mode == 0)) {
                 // Up to 4 pixels in flight per thread (all shared-memory loads first, branch-free math, then the
                 // stores); the last groups of a stage use the 2- and 1-wide variants instead of idle lanes (a
                 // 180-pixel halo tile is 1.4 four-wide passes).  No per-pixel index arithmetic: see the masks above.
@@ -898,7 +911,7 @@ __global__ void __launch_bounds__(kNumThreads, 1) conv_gemm_kernel(const __grid_
                   m += 2;
                 }
                 if (m < ng) transform_fast<1, true>(tb + m * 4096, m_vld >> m, m_img >> m, ca, cb, sg.act);
-              } else if (p.NB == 1) {
+              } else if (NB == 1) {
                 // three dx-shifted copies (mode 1): the in-image test depends on the copy
                 // (hy, r) = (tile row, position inside the row) of pixel px, advanced incrementally (no divisions)
                 int hy = pl / prow, r = pl - hy * prow;
@@ -947,6 +960,7 @@ __global__ void __launch_bounds__(kNumThreads, 1) conv_gemm_kernel(const __grid_
                   *slot = u;
                 }
               }
+              if (warp == kWarpT) ASYRP_TRACE_STAMP(11, tr_n);
               fence_proxy_async_smem();  // generic-proxy writes -> visible to the tensor core's async-proxy reads
             }
             __syncwarp();
@@ -1098,6 +1112,7 @@ struct ConvOp {
   ConvParams p;
   int BN;
   int MT;
+  bool plain;  // conv_gemm_kernel<BN, MT, true> serves it
   int grid;
   size_t smem_bytes;
 };
@@ -1106,12 +1121,15 @@ struct ConvOp {
 
 using namespace asyrp;
 
-static const void* conv_kernel_ptr(int BN, int MT) {
-  if (BN == 16) return MT == 2 ? reinterpret_cast<const void*>(&conv_gemm_kernel<16, 2>)
-                               : reinterpret_cast<const void*>(&conv_gemm_kernel<16, 1>);
-  if (BN == 128) return reinterpret_cast<const void*>(&conv_gemm_kernel<128, 1>);
-  return MT == 2 ? reinterpret_cast<const void*>(&conv_gemm_kernel<64, 2>)
-                 : reinterpret_cast<const void*>(&conv_gemm_kernel<64, 1>);
+static const void* conv_kernel_ptr(int BN, int MT, bool plain) {
+  if (BN == 16) return MT == 2 ? reinterpret_cast<const void*>(&conv_gemm_kernel<16, 2, false>)
+                               : reinterpret_cast<const void*>(&conv_gemm_kernel<16, 1, false>);
+  if (BN == 128) return plain ? reinterpret_cast<const void*>(&conv_gemm_kernel<128, 1, true>)
+                              : reinterpret_cast<const void*>(&conv_gemm_kernel<128, 1, false>);
+  if (MT == 2) return plain ? reinterpret_cast<const void*>(&conv_gemm_kernel<64, 2, true>)
+                            : reinterpret_cast<const void*>(&conv_gemm_kernel<64, 2, false>);
+  return plain ? reinterpret_cast<const void*>(&conv_gemm_kernel<64, 1, true>)
+               : reinterpret_cast<const void*>(&conv_gemm_kernel<64, 1, false>);
 }
 
 extern "C" {
@@ -1481,6 +1499,32 @@ ASYRP_API int asyrp_conv_create(const AsyrpConvDesc* d, void** out_op) {
     if (cap >= 2 && p.b_stages > cap) p.b_stages = cap;
   }
 #endif
+  {
+    // Epilogue placement (see the transform warps' tile loop): the transform warps ready the leading K-schedule entries
+    // of tile i+1 that the activation rings hold while tile i's MMAs still read its last stage — every slot of a ring
+    // but, in the ring of tile i's last entry, that stage's — and then drain tile i, whose epilogue so overlaps the
+    // MMAs of those entries.  An entry of mode 1 / 2 takes one slot per shifted copy.  At least one entry.
+    int cap_h = p.a_stages, cap_l = p.l_stages;
+    const int last = p.sched[p.n_sched - 1] >> 6;
+    const bool last_lt = p.l_stages != 0 && p.seg[last].mode == 0;
+    --(last_lt ? cap_l : cap_h);
+    int e = 0;
+    for (; e < p.n_sched; ++e) {
+      const ConvSegDev& sg = p.seg[p.sched[e] >> 6];
+      const bool lt = p.l_stages != 0 && sg.mode == 0;
+      int& cap = lt ? cap_l : cap_h;
+      const int ncopies = (sg.mode == 0 || sg.mode == 3) ? 1 : (sg.mode == 1 ? 3 : 9);
+      if (ncopies > cap) break;
+      cap -= ncopies;
+    }
+    p.drain_at = e > 1 ? e : 1;
+#ifdef ASYRP_TRACE
+    if (const char* s = getenv("ASYRP_DRAIN_AT")) {  // diagnostic build: epilogue placement from the environment
+      const int v = atoi(s);
+      if (v >= 1) p.drain_at = v;
+    }
+#endif
+  }
   p.ebias = d->ebias;
   p.ebias_stride = d->ebias_stride;
   p.out_planar = d->out_planar;
@@ -1514,7 +1558,8 @@ ASYRP_API int asyrp_conv_create(const AsyrpConvDesc* d, void** out_op) {
   if (sms <= 0) return ASYRP_ERR_NO_DEVICE;
   const int total = p.m_tiles * p.n_tiles;
   op->grid = total < sms ? total : sms;
-  cudaError_t e = cudaFuncSetAttribute(conv_kernel_ptr(op->BN, op->MT),
+  op->plain = op->BN >= 64 && p.NB == 1 && p.out_heads == 1 && !p.out_f32 && p.out_planar == nullptr;
+  cudaError_t e = cudaFuncSetAttribute(conv_kernel_ptr(op->BN, op->MT, op->plain),
                                        cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
   if (e != cudaSuccess) {
     set_error("asyrp_conv_create: cudaFuncSetAttribute: %s", cudaGetErrorString(e));
@@ -1541,7 +1586,7 @@ ASYRP_API int asyrp_conv_launch(void* handle, void* stream) {
     attr[cfg.numAttrs].val.programmaticStreamSerializationAllowed = 1;
     ++cfg.numAttrs;
   }
-  ASYRP_CHECK_CUDA(cudaLaunchKernelExC(&cfg, conv_kernel_ptr(op->BN, op->MT), args));
+  ASYRP_CHECK_CUDA(cudaLaunchKernelExC(&cfg, conv_kernel_ptr(op->BN, op->MT, op->plain), args));
   return ASYRP_OK;
 }
 
@@ -1556,6 +1601,11 @@ ASYRP_API int asyrp_conv_set_scales(void* handle, float acc_scale, float res_sca
 }
 
 ASYRP_API void asyrp_conv_destroy(void* handle) { delete static_cast<ConvOp*>(handle); }
+
+ASYRP_API int asyrp_conv_drain_at(void* handle) {
+  ASYRP_REQUIRE(handle, "asyrp_conv_drain_at: null op");
+  return static_cast<ConvOp*>(handle)->p.drain_at;
+}
 
 #ifdef ASYRP_TRACE
 // diagnostic build only: device buffer [grid][kTraceRoles][kTraceLen] int64 receiving the pipeline timeline

@@ -208,6 +208,11 @@ class ConvOp:
     def set_scales(self, acc_scale, res_scale):
         check(self._lib.asyrp_conv_set_scales(self._h, acc_scale, res_scale), "asyrp_conv_set_scales")
 
+    @property
+    def drain_at(self):
+        """K-schedule entries of tile i+1 the kernel readies before it runs the epilogue of tile i"""
+        return self._lib.asyrp_conv_drain_at(self._h)
+
     def __del__(self):
         if getattr(self, "_h", None):
             self._lib.asyrp_conv_destroy(self._h)

@@ -153,6 +153,8 @@ int asyrp_conv_create(const AsyrpConvDesc* desc, void** op); /* encodes TMA desc
 int asyrp_conv_launch(void* op, void* stream);
 int asyrp_conv_set_scales(void* op, float acc_scale, float res_scale); /* hs_coeff of forward(), diffusion.py:512-516 */
 void asyrp_conv_destroy(void* op);
+/* K-schedule entries of a tile the op's operand-transform warps ready before they run the previous tile's epilogue */
+int asyrp_conv_drain_at(void* op);
 
 /* ---- GroupNorm(32) statistics -> per-(sample, channel) affine ------------------------------------------
  * Replaces torch.nn.GroupNorm in Normalize (ddpm/diffusion.py:68-69, eps 1e-6) and GroupNorm32

@@ -10,14 +10,17 @@ Every role of conv_gemm_kernel stamps clock64() at its hand-off points (csrc/con
   5 MMA: tile start                        6 MMA: staging tile free (the previous tile's epilogue has read it)
   7 epilogue: staging tile full            8 epilogue: staging tile drained
   10 MMA: clocks the stage spent waiting for weight stages (a duration, not a time stamp)
-A library built before the staging handoff has 10 roles (--roles 10) and no stamp 6 or 10.
+  11 transform: stage transformed, before the proxy fence (stages without a transform have no stamp)
+A library built before the staging handoff has 10 roles (--roles 10) and no stamp 6 or 10; one built before the fence
+stamp has 11 (--roles 11).
 
 Per CTA the script prints, as shares of the CTA's span (first tile start to last drain):
   * tile boundaries: from the last MMA issue of tile i to the first stage of tile i+1 being ready (includes the last
     wgmma group's execution), split into the wait for the staging tile and the rest (staging write, A-stage wait);
   * A waits: the MMA warps waiting for a ready activation stage inside a tile;
   * B waits: the MMA warps waiting for a weight stage;
-  * the epilogue's length per tile."""
+  * the epilogue's length per tile, the transform warps' clocks per stage, and how many of them the proxy fence after
+    the transform takes."""
 import argparse, ctypes as C, os, sys
 import numpy as np
 import torch
@@ -26,7 +29,8 @@ from asyrp_official_b200 import ops, _lib
 ap = argparse.ArgumentParser()
 ap.add_argument("spec")
 ap.add_argument("--out", default="gpurun_out/trace.npz")
-ap.add_argument("--roles", type=int, default=11, help="trace roles of the library (10 before the staging handoff)")
+ap.add_argument("--roles", type=int, default=12,
+                help="trace roles of the library (10 before the staging handoff, 11 before the fence stamp)")
 a = ap.parse_args()
 dev = torch.device("cuda:0")
 N = 16
@@ -81,13 +85,16 @@ for cta in range(grid):
     epi = r[8][:nt] - r[7][:nt]
     # shares of the stamped part of the span (stage stamps stop at LEN)
     cov = (r[9][ns - 1] - r[5][0]) if nts < nt else span
+    fenced = (r[11][:ns] > 0) if ROLES > 11 else np.zeros(ns, bool)
+    fence = (r[2][:ns] - r[11][:ns])[fenced].mean() if fenced.any() else 0.0
     rows.append((nt, span / nt, gap.sum() / cov, st_wait.sum() / cov, a_wait.sum() / cov, b_wait.sum() / cov,
-                 epi.mean(), (r[2][:ns] - r[1][:ns]).mean()))
+                 epi.mean(), (r[2][:ns] - r[1][:ns]).mean(), fence))
 R = np.array(rows)
-print("CTA  tiles  clk/tile  boundary%  (staging wait%)  A-wait%  B-wait%  epilogue clk  transform clk/stage")
+print("CTA  tiles  clk/tile  boundary%  (staging wait%)  A-wait%  B-wait%  epilogue clk  transform clk/stage  fence clk")
 for cta in sorted({0, 1, grid // 2, grid - 1}):
-    nt, pt, g, s, aw, bw, ep, xf = R[cta]
+    nt, pt, g, s, aw, bw, ep, xf, fc = R[cta]
     print(f"{cta:3d} {nt:6.0f} {pt:9.0f} {100 * g:9.1f}  ({100 * s:5.1f})       {100 * aw:6.1f}  {100 * bw:6.1f}  {ep:12.0f}  "
-          f"{xf:8.0f}")
-nt, pt, g, s, aw, bw, ep, xf = R.mean(0)
-print(f"all {nt:6.1f} {pt:9.0f} {100 * g:9.1f}  ({100 * s:5.1f})       {100 * aw:6.1f}  {100 * bw:6.1f}  {ep:12.0f}  {xf:8.0f}")
+          f"{xf:8.0f}  {fc:8.0f}")
+nt, pt, g, s, aw, bw, ep, xf, fc = R.mean(0)
+print(f"all {nt:6.1f} {pt:9.0f} {100 * g:9.1f}  ({100 * s:5.1f})       {100 * aw:6.1f}  {100 * bw:6.1f}  {ep:12.0f}  {xf:8.0f}  "
+      f"{fc:8.0f}")

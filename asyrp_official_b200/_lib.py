@@ -88,6 +88,13 @@ SIGNATURES = {
     "asyrp_lpips_distance_chunks": (c_int, [c_int]),
     "asyrp_lpips_distance": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p,
                                      c_void_p, c_int, c_void_p]),
+    "asyrp_clip_embed": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p]),
+    "asyrp_clip_layernorm": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_void_p]),
+    "asyrp_clip_linear": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int,
+                                  c_void_p]),
+    "asyrp_clip_attention": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p]),
+    "asyrp_clip_pool": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p]),
+    "asyrp_clip_cosine": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_float, c_void_p]),
 }
 
 _lib = None

@@ -8,15 +8,19 @@ Mirrors, with the same attribute / flag names:
   Asyrp.save_image             :445-544                     the reverse loops + PNG grid
   Asyrp.random_noise_pairs     :1087-1188                   x_T = N(0,1) per image
   Asyrp.set_t_edit_t_addnoise  :1308-1416                   user-defined values or LPIPS-table lookup given a cosine
+                                                            (--clip_cosine, or CLIP's text cosine on the GPU)
   Asyrp.compute_lpips_distance :1191-1303                   --lpips: the LPIPS(x_t, x0) / LPIPS(x0_t, x0) tables of an
                                                             inversion, which set_t_edit_t_addnoise reads
 
 Differences (documented in INTEGRATION.md): the reverse loop is UNetEngine.sample() — one CUDA graph per
 (batch, schedule) instead of 40 Python iterations; pretrained weights come from --model_path (no URL download);
-CLIP is not available, so t_edit / t_addnoise come from --user_defined_t_edit/_t_addnoise or from the shipped
-LPIPS tables with an explicit --clip_cosine.  With torch.distributed initialised (one process per GPU) the image
-batches are sharded round-robin across ranks; the only collective is the initial weight broadcast.
+the CLIP text cosine that picks t_edit runs on this library's kernels (clip_text.CLIPText) from --clip_weights and
+--clip_vocab, or is given as --clip_cosine; SRC_TRG_TXT_DIC is read from --text_dic (default utils/text_dic.py).
+With torch.distributed initialised (one process per GPU) the image batches are sharded round-robin across ranks;
+the only collective is the initial weight broadcast, and each rank computes the CLIP cosine itself (the kernels are
+deterministic, so every rank picks the same t_edit).
 """
+import ast
 import os
 import time
 
@@ -86,7 +90,8 @@ class Asyrp(object):
         """t_edit = first t with LPIPS(x0_t, x0) >= LPIPS_th * cosine; t_addnoise = first t with LPIPS >= LPIPS_addnoise_th
         on the x_t table (--add_noise_from_xt) or the same x0_t table (diffusion_latent.py:1331-1410).  Each of
         --user_defined_t_edit / --user_defined_t_addnoise overrides its value.  The cosine is CLIP's text-direction
-        similarity in the reference (:1319-1329); CLIP is unavailable offline, so it is the explicit --clip_cosine.
+        similarity in the reference (:1319-1329): the `cosine` argument, else --clip_cosine, else, when t_edit is
+        needed, CLIPText on --clip_weights / --clip_vocab with the texts of --edit_attr (or --src_txts / --trg_txts).
         Tables: <lpips_table_dir>/<config stem>_LPIPS_distance_{x0_t,x}.tsv (the reference ships them under utils/)."""
         a = self.args
         ut, ua = getattr(a, "user_defined_t_edit", None), getattr(a, "user_defined_t_addnoise", None)
@@ -100,9 +105,12 @@ class Asyrp(object):
         if name == "custom":
             name = getattr(a, "custom_dataset_name", "celeba")
         p0 = os.path.join(tdir, f"{name}_LPIPS_distance_x0_t.tsv")
-        if not os.path.exists(p0) or (ut is None and cosine is None):
+        if not os.path.exists(p0) or (ut is None and cosine is None and not self.clip_configured()):
             raise ValueError(f"t_edit / t_addnoise undefined: pass --user_defined_t_edit and --user_defined_t_addnoise, "
-                             f"or --clip_cosine with --lpips_table_dir (looked for {p0}; CLIP is not available offline)")
+                             f"or --clip_cosine, or --clip_weights and --clip_vocab, with --lpips_table_dir (looked "
+                             f"for {p0})")
+        if ut is None and cosine is None:
+            cosine = self.clip_cosines([self.edit_texts()])[0]
         table = _read_tsv(p0)
         self.t_edit = ut if ut is not None else next(t for t, v in table if v >= LPIPS_th * cosine)
         if ua is not None:
@@ -112,6 +120,67 @@ class Asyrp(object):
                 table = _read_tsv(os.path.join(tdir, f"{name}_LPIPS_distance_x.tsv"))
             self.t_addnoise = next(t for t, v in table if v >= LPIPS_addnoise_th)
         return cosine
+
+    def clip_configured(self):
+        return bool(getattr(self.args, "clip_weights", None)) and bool(getattr(self.args, "clip_vocab", None))
+
+    def needs_clip(self):
+        """t_edit must come from CLIP's text cosine: no --user_defined_t_edit, no --clip_cosine"""
+        a = self.args
+        return getattr(a, "user_defined_t_edit", None) is None and getattr(a, "clip_cosine", None) is None
+
+    def text_dic(self):
+        return read_text_dic(getattr(self.args, "text_dic", None) or os.path.join("utils", "text_dic.py"))
+
+    def edit_texts(self, attr=None):
+        """(src_txts, trg_txts) of an attribute as the reference's __init__ picks them (:66-73): --src_txts /
+        --trg_txts for --edit_attr None, SRC_TRG_TXT_DIC[attr] otherwise; the dictionary is read only here"""
+        a = self.args
+        attr = attr if attr is not None else getattr(a, "edit_attr", None)
+        if attr is None:
+            src, trg = getattr(a, "src_txts", None), getattr(a, "trg_txts", None)
+            if not src or not trg:
+                raise ValueError("--edit_attr None needs --src_txts and --trg_txts")
+            return list(src), list(trg)
+        if attr == "attribute":
+            raise ValueError("--edit_attr attribute has no texts: CLIP's cosine needs --multiple_attr, an attribute "
+                             "of SRC_TRG_TXT_DIC or --src_txts / --trg_txts")
+        dic = self.text_dic()
+        if attr not in dic:
+            raise ValueError(f"attribute {attr!r} is not in SRC_TRG_TXT_DIC")
+        return list(dic[attr][0]), list(dic[attr][1])
+
+    @torch.no_grad()
+    def clip_cosines(self, pairs):
+        """CLIP's text-direction cosine of each (src_txts, trg_txts) pair (:1319-1329), printed as the reference
+        prints it.  Each pair must hold one text per side (the reference takes .item()).  The encoder is built here
+        and dropped before returning, so its buffers are gone before the UNet is loaded."""
+        from .clip_text import CLIPText
+        a = self.args
+        clip = CLIPText(a.clip_weights, a.clip_vocab, device=self.device)
+        try:
+            out = []
+            for src, trg in pairs:
+                print("Texts:", src, trg)
+                cos = clip.text_cosine(src, trg)
+                if cos.numel() != 1:
+                    raise ValueError(f"CLIP's cosine takes one source and one target text, got {src} and {trg}")
+                print("text_cos_distance", cos.item())
+                out.append(cos.item())
+        finally:
+            del clip
+            torch.cuda.empty_cache()
+        return out
+
+    def choose_attribute(self, attrs):
+        """--multiple_attr (:640-652): the attribute of the largest CLIP cosine (the first on a tie); sets
+        src_txts / trg_txts to its texts and returns its cosine"""
+        texts = [self.edit_texts(attr) for attr in attrs]
+        cosines = self.clip_cosines(texts)
+        best = max(range(len(attrs)), key=lambda i: (cosines[i], -i))
+        print(f"Max cosine: {cosines[best]}, Max attribute: {attrs[best]}")
+        self.src_txts, self.trg_txts = texts[best]
+        return cosines[best]
 
     # ------------------------------------------------------------------------------------------
     @torch.no_grad()
@@ -424,7 +493,11 @@ class Asyrp(object):
         if getattr(a, "warigari", 0.0):
             print("--warigari is accepted and has no effect (the reference's branch returns the same values, "
                   "utils/diffusion_utils.py:103-109)")
-        self.set_t_edit_t_addnoise(LPIPS_th=a.lpips_edit_th, LPIPS_addnoise_th=a.lpips_addnoise_th)
+        if a.multiple_attr and self.needs_clip() and self.clip_configured():
+            cosine = self.choose_attribute(a.multiple_attr.split(' '))  # :640-652
+            self.set_t_edit_t_addnoise(LPIPS_th=a.lpips_edit_th, LPIPS_addnoise_th=a.lpips_addnoise_th, cosine=cosine)
+        else:
+            self.set_t_edit_t_addnoise(LPIPS_th=a.lpips_edit_th, LPIPS_addnoise_th=a.lpips_addnoise_th)
         # ----------- sequences (:560-574)
         if a.n_train_step != 0:
             seq_train = np.linspace(0, 1, a.n_train_step) * a.t_0
@@ -594,6 +667,21 @@ def plan_sweep(n_tuples, bs, max_rows):
     rows, the last one padded (pad_rows), so that one plan and one captured graph serve them all."""
     tpc = min(n_tuples, max(1, max_rows // bs))
     return tpc, [list(range(k, min(k + tpc, n_tuples))) for k in range(0, n_tuples, tpc)]
+
+
+def read_text_dic(path):
+    """SRC_TRG_TXT_DIC of the reference's utils/text_dic.py: the literal assigned to that name, read with ast (the
+    file is parsed, never imported or executed)"""
+    if not os.path.exists(path):
+        raise FileNotFoundError(f"{path} not found: pass --text_dic <file defining SRC_TRG_TXT_DIC> (the reference's "
+                                "utils/text_dic.py)")
+    with open(path, encoding="utf-8") as f:
+        tree = ast.parse(f.read(), filename=path)
+    for node in tree.body:
+        if isinstance(node, ast.Assign) and any(isinstance(t, ast.Name) and t.id == "SRC_TRG_TXT_DIC"
+                                                for t in node.targets):
+            return ast.literal_eval(node.value)
+    raise ValueError(f"{path} assigns no SRC_TRG_TXT_DIC literal")
 
 
 def lpips_tables(seq_inv, seq_inv_next, per_image):

@@ -64,6 +64,8 @@ def build_parser():
     p.add_argument('--verbose', type=str, default='info')
     p.add_argument('--ni', type=int, default=1)
     p.add_argument('--edit_attr', type=str, default=None)
+    p.add_argument('--src_txts', type=str, action='append')
+    p.add_argument('--trg_txts', type=str, action='append')
     p.add_argument('--t_0', type=int, default=999)
     p.add_argument('--n_inv_step', type=int, default=40)
     p.add_argument('--n_train_step', type=int, default=6)
@@ -84,7 +86,14 @@ def build_parser():
     p.add_argument('--n_iter', type=int, default=1)
     # additions of this build (documented in INTEGRATION.md)
     p.add_argument('--synthetic_weights', **sa, help='seeded random UNet weights instead of --model_path')
-    p.add_argument('--clip_cosine', type=float, help='text-direction cosine CLIP would give (no CLIP offline)')
+    p.add_argument('--clip_cosine', type=float, help='text-direction cosine to use instead of computing it with CLIP')
+    p.add_argument('--clip_weights', type=str, default=None,
+                   help="CLIP's model file (e.g. ~/.cache/clip/ViT-B-16.pt, or a torch.save of its state dict): the "
+                        "text tower computes the cosine that picks t_edit")
+    p.add_argument('--clip_vocab', type=str, default=None,
+                   help="CLIP's bpe_simple_vocab_16e6.txt.gz (inside the installed clip package)")
+    p.add_argument('--text_dic', type=str, default=None,
+                   help='file defining SRC_TRG_TXT_DIC, read with ast (default utils/text_dic.py)')
     p.add_argument('--lpips_table_dir', type=str,
                    help='directory with <config stem>_LPIPS_distance_{x,x0_t}.tsv (read by --run_test, written by '
                         '--lpips; default utils)')

@@ -374,6 +374,74 @@ def lpips_distance(probe, ref, lin_w, partial, counters, d, accumulate):
                                    _ptr(counters), _ptr(d), int(accumulate), _stream()), "asyrp_lpips_distance")
 
 
+CLIP_EPI_BIAS, CLIP_EPI_QUICK_GELU, CLIP_EPI_RESIDUAL = 1, 2, 3
+
+
+def clip_embed(ids, token_embedding, positional_embedding, out):
+    """out [P][T][w] = token_embedding[ids] + positional_embedding; ids int32 [P][T]"""
+    lib = _lib.load()
+    P, T = ids.shape
+    w = token_embedding.shape[1]
+    _need_cuda(ids, token_embedding, positional_embedding, out)
+    assert ids.dtype == torch.int32 and ids.is_contiguous() and tuple(positional_embedding.shape) == (T, w)
+    assert tuple(out.shape) == (P, T, w) and out.dtype == torch.float32
+    check(lib.asyrp_clip_embed(_ptr(ids), _ptr(token_embedding), _ptr(positional_embedding), _ptr(out), P, T, w,
+                               _stream()), "asyrp_clip_embed")
+
+
+def clip_layernorm(x, gamma, beta, out):
+    """LayerNorm(eps 1e-5) over the last dim of fp32 x; out may be x"""
+    lib = _lib.load()
+    w = x.shape[-1]
+    _need_cuda(x, gamma, beta, out)
+    assert x.is_contiguous() and out.shape == x.shape and gamma.numel() == w and beta.numel() == w
+    check(lib.asyrp_clip_layernorm(_ptr(x), _ptr(gamma), _ptr(beta), _ptr(out), x.numel() // w, w, _stream()),
+          "asyrp_clip_layernorm")
+
+
+def clip_linear(x, weight, bias, out, epilogue=CLIP_EPI_BIAS, residual=None):
+    """out = epilogue(x @ weight.T + bias) over the last dim, TF32 tensor cores (the LPIPS conv's GEMM); weight fp32
+    [N][K] (nn.Linear layout), bias [N] or None; CLIP_EPI_RESIDUAL adds residual (which may be out)"""
+    lib = _lib.load()
+    K = x.shape[-1]
+    N = weight.shape[0]
+    M = x.numel() // K
+    _need_cuda(x, weight, bias, out, residual)
+    assert x.is_contiguous() and weight.is_contiguous() and tuple(weight.shape) == (N, K)
+    assert out.is_contiguous() and out.numel() == M * N and out.shape[-1] == N
+    assert residual is None or (residual.is_contiguous() and residual.shape == out.shape)
+    check(lib.asyrp_clip_linear(_ptr(x), _ptr(weight), _ptr(bias), _ptr(residual), _ptr(out), M, K, N, int(epilogue),
+                                _stream()), "asyrp_clip_linear")
+
+
+def clip_attention(qkv, out, heads):
+    """causal multi-head attention (head size 64): qkv [P][T][3w] (q | k | v), out [P][T][w]"""
+    lib = _lib.load()
+    P, T, w3 = qkv.shape
+    _need_cuda(qkv, out)
+    assert qkv.is_contiguous() and w3 == 3 * 64 * heads and tuple(out.shape) == (P, T, 64 * heads)
+    check(lib.asyrp_clip_attention(_ptr(qkv), _ptr(out), P, T, heads, _stream()), "asyrp_clip_attention")
+
+
+def clip_pool(x, ids, gamma, beta, out):
+    """out [P][w] = LayerNorm(x[p][first argmax of ids[p]]); x [P][T][w], ids int32 [P][T]"""
+    lib = _lib.load()
+    P, T, w = x.shape
+    _need_cuda(x, ids, gamma, beta, out)
+    assert ids.dtype == torch.int32 and tuple(ids.shape) == (P, T) and tuple(out.shape) == (P, w)
+    check(lib.asyrp_clip_pool(_ptr(x), _ptr(ids), _ptr(gamma), _ptr(beta), _ptr(out), P, T, w, _stream()),
+          "asyrp_clip_pool")
+
+
+def clip_cosine(a, b, out, eps=1e-6):
+    """out[n] = torch.nn.CosineSimilarity(dim=1, eps)(a, b)[n]; a, b fp32 [n][dim]"""
+    lib = _lib.load()
+    n, dim = a.shape
+    _need_cuda(a, b, out)
+    assert a.is_contiguous() and b.is_contiguous() and b.shape == a.shape and out.numel() == n
+    check(lib.asyrp_clip_cosine(_ptr(a), _ptr(b), _ptr(out), n, dim, float(eps), _stream()), "asyrp_clip_cosine")
+
+
 def ddpm_update(x, et, z, x_next, at, bt, logvar, learned_sigma, mask):
     lib = _lib.load()
     N, Cx, H, W = x.shape

@@ -24,6 +24,59 @@ def lpips_state_dict(seed=1234):
     return {k: (v.abs() if k.startswith("lin") else v) for k, v in sd.items()}
 
 
+def clip_text_state_dict(seed=1234, width=512, layers=12, context=77, vocab=49408, embed_dim=512):
+    """seeded CLIP text-tower weights in CLIP's state-dict layout (asyrp_official_b200.clip_text), at the scales of
+    CLIP's initialize_parameters: token embedding N(0, .02^2), positional N(0, .01^2), in_proj / text_projection
+    std width^-1/2, out_proj / c_proj std width^-1/2 (2 layers)^-1/2, c_fc std (2 width)^-1/2.  No term is zero:
+    the biases are N(0, .02^2) and the LayerNorm affines 1 + N(0, .1^2) / N(0, .02^2), so a dropped term shows."""
+    from .clip_text import text_key_shapes
+    std = {"token_embedding.weight": 0.02, "positional_embedding": 0.01, "text_projection": width ** -0.5,
+           "attn.in_proj_weight": width ** -0.5, "attn.out_proj.weight": width ** -0.5 * (2 * layers) ** -0.5,
+           "mlp.c_fc.weight": (2 * width) ** -0.5, "mlp.c_proj.weight": width ** -0.5 * (2 * layers) ** -0.5}
+    sd = {}
+    for name, shp in text_key_shapes(width, layers, context, vocab, embed_dim).items():
+        g = torch.Generator()
+        g.manual_seed((zlib.crc32(name.encode()) ^ (seed * 0x9E3779B1)) & 0x7FFFFFFF)
+        key = name.split(".", 3)[-1] if name.startswith("transformer.") else name
+        z = torch.randn(shp, generator=g)
+        if key in std:
+            sd[name] = z * std[key]
+        elif key.startswith("ln") and key.endswith(".weight"):
+            sd[name] = 1.0 + 0.1 * z
+        else:  # biases
+            sd[name] = 0.02 * z
+    return sd
+
+
+def clip_bpe_merges(texts):
+    """BPE merges that build every word of texts (after CLIP's cleaning and pre-tokenisation) left to right from its
+    byte symbols: a small vocabulary for tests and smoke runs in place of bpe_simple_vocab_16e6.txt.gz"""
+    import regex
+
+    from .clip_text import _PAT, byte_symbols, clean_text
+    enc, merges, seen = byte_symbols(), [], set()
+    for text in texts:
+        for token in regex.findall(_PAT, clean_text(text), regex.IGNORECASE):
+            sym = [enc[b] for b in token.encode("utf-8")]
+            sym[-1] += "</w>"
+            cur = sym[0]
+            for s in sym[1:]:
+                if (cur, s) not in seen:
+                    seen.add((cur, s))
+                    merges.append((cur, s))
+                cur += s
+    return merges
+
+
+def write_clip_vocab(path, merges):
+    """write merges as a bpe_simple_vocab_16e6.txt.gz-style file (a header line, then one 'a b' merge per line);
+    returns the vocabulary size: 512 byte symbols + the merges + 2"""
+    import gzip
+    with gzip.open(path, "wt", encoding="utf-8") as f:
+        f.write("\n".join(["#version: 0.2"] + [f"{a} {b}" for a, b in merges]))
+    return 512 + len(merges) + 2
+
+
 def _draw(shapes, seed, style):
     fan = {k[:-7]: math.prod(v[1:]) for k, v in shapes.items() if k.endswith(".weight") and len(v) >= 2}
     new = {}

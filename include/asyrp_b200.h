@@ -245,6 +245,31 @@ int asyrp_lpips_distance_chunks(int HW); /* host only */
 int asyrp_lpips_distance(const float* probe, const float* ref, int N, int B, int HW, int C, const float* lin_w,
                          float* partial, int* counters, float* d, int accumulate, void* stream);
 
+/* ---- CLIP text tower: OpenAI CLIP's encode_text and the text-direction cosine --------------------------------------
+ * Replaces the clip_loss_func.encode_text / CosineSimilarity calls of Asyrp.set_t_edit_t_addnoise
+ * (diffusion_latent.py:1319-1329).  Activations are fp32 [P][T][width], P prompts of T tokens, rows = P*T.
+ * asyrp_clip_embed: out = token_embedding[ids] + positional_embedding; ids int32 [P][T] (each < the vocabulary),
+ *   token_embedding [vocab][width], positional_embedding [T][width].
+ * asyrp_clip_layernorm: LayerNorm over width, eps 1e-5, per row of [rows][width]; out may be in.
+ * asyrp_clip_linear: out[M][N] = epilogue(in[M][K] @ weight[N][K]^T + bias) (nn.Linear's weight layout), TF32
+ *   operands rounded to nearest, fp32 accumulation, the LPIPS conv's GEMM.  K % 32 == 0, N % 64 == 0.  epilogue 1:
+ *   identity (bias may be null), 2: QuickGELU z*sigmoid(1.702z), 3: residual + z (residual [M][N], may be out).
+ * asyrp_clip_attention: causal multi-head attention, head size 64, scale 1/8; qkv [P*T][3*64*heads] as
+ *   nn.MultiheadAttention's in_proj packs q | k | v, out [P*T][64*heads] (T <= 128).
+ * asyrp_clip_pool: out [P][width] = LayerNorm(x[p][eot]) with eot the first argmax of ids[p].
+ * asyrp_clip_cosine: cos[n] = torch.nn.CosineSimilarity(dim=1, eps) of rows a[n], b[n] of [n][dim].
+ * Fixed-order reductions, no float atomics, no kernel mixes prompts: a prompt's features do not depend on P. */
+int asyrp_clip_embed(const int* ids, const float* token_embedding, const float* positional_embedding, float* out,
+                     int P, int T, int width, void* stream);
+int asyrp_clip_layernorm(const float* in, const float* gamma, const float* beta, float* out, int rows, int width,
+                         void* stream);
+int asyrp_clip_linear(const float* in, const float* weight, const float* bias, const float* residual, float* out, int M,
+                      int K, int N, int epilogue, void* stream);
+int asyrp_clip_attention(const float* qkv, float* out, int P, int T, int heads, void* stream);
+int asyrp_clip_pool(const float* x, const int* ids, const float* gamma, const float* beta, float* out, int P, int T,
+                    int width, void* stream);
+int asyrp_clip_cosine(const float* a, const float* b, float* cos, int n, int dim, float eps, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -95,6 +95,12 @@ SIGNATURES = {
     "asyrp_clip_attention": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p]),
     "asyrp_clip_pool": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p]),
     "asyrp_clip_cosine": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_float, c_void_p]),
+    "asyrp_clip_layernorm_rows": (c_int, [c_void_p, C.c_longlong, c_void_p, c_void_p, c_void_p, c_int, c_int,
+                                          c_void_p]),
+    "asyrp_clip_attention_full": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p]),
+    "asyrp_clip_image_patches": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p]),
+    "asyrp_clip_image_tokens": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p]),
+    "asyrp_clip_direction": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_float, c_void_p]),
 }
 
 _lib = None

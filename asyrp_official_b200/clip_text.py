@@ -120,17 +120,20 @@ class Tokenizer:
 
 # ---------------------------------------------------------------------------------------------------------------------
 # weights
-def text_key_shapes(width, layers, context, vocab, embed_dim):
-    """name -> shape of every text-tower tensor of a CLIP state dict"""
-    shapes = {"token_embedding.weight": (vocab, width), "positional_embedding": (context, width),
-              "ln_final.weight": (width,), "ln_final.bias": (width,), "text_projection": (width, embed_dim)}
+def block_key_shapes(width, layers):
+    """name -> shape of every tensor of CLIP's Transformer (transformer.resblocks.*), the same in both towers"""
     per = {"ln_1.weight": (width,), "ln_1.bias": (width,), "attn.in_proj_weight": (3 * width, width),
            "attn.in_proj_bias": (3 * width,), "attn.out_proj.weight": (width, width), "attn.out_proj.bias": (width,),
            "ln_2.weight": (width,), "ln_2.bias": (width,), "mlp.c_fc.weight": (4 * width, width),
            "mlp.c_fc.bias": (4 * width,), "mlp.c_proj.weight": (width, 4 * width), "mlp.c_proj.bias": (width,)}
-    for i in range(layers):
-        for k, s in per.items():
-            shapes[f"transformer.resblocks.{i}.{k}"] = s
+    return {f"transformer.resblocks.{i}.{k}": s for i in range(layers) for k, s in per.items()}
+
+
+def text_key_shapes(width, layers, context, vocab, embed_dim):
+    """name -> shape of every text-tower tensor of a CLIP state dict"""
+    shapes = {"token_embedding.weight": (vocab, width), "positional_embedding": (context, width),
+              "ln_final.weight": (width,), "ln_final.bias": (width,), "text_projection": (width, embed_dim)}
+    shapes.update(block_key_shapes(width, layers))
     return shapes
 
 
@@ -184,6 +187,25 @@ def load_state_dict(sd_or_path, vocab_size=None):
 
 
 # ---------------------------------------------------------------------------------------------------------------------
+def residual_blocks(sd, layers, heads, x, causal):
+    """CLIP's Transformer on x [P][T][w] (device, fp32), in place: per block x += out_proj(mha(ln_1(x))),
+    x += c_proj(quick_gelu(c_fc(ln_2(x)))), with the weights sd[f"transformer.resblocks.{i}.{key}"].  The attention is
+    causal in the text tower and full in the image tower."""
+    P, T, w = x.shape
+    h = torch.empty_like(x)
+    qkv = x.new_empty(P, T, 3 * w)
+    mlp = x.new_empty(P, T, 4 * w)
+    for i in range(layers):
+        b = {k: sd[f"transformer.resblocks.{i}.{k}"] for k in BLOCK_KEYS}
+        ops.clip_layernorm(x, b["ln_1.weight"], b["ln_1.bias"], h)
+        ops.clip_linear(h, b["attn.in_proj_weight"], b["attn.in_proj_bias"], qkv)
+        ops.clip_attention(qkv, h, heads, causal=causal)
+        ops.clip_linear(h, b["attn.out_proj.weight"], b["attn.out_proj.bias"], x, ops.CLIP_EPI_RESIDUAL, residual=x)
+        ops.clip_layernorm(x, b["ln_2.weight"], b["ln_2.bias"], h)
+        ops.clip_linear(h, b["mlp.c_fc.weight"], b["mlp.c_fc.bias"], mlp, ops.CLIP_EPI_QUICK_GELU)
+        ops.clip_linear(mlp, b["mlp.c_proj.weight"], b["mlp.c_proj.bias"], x, ops.CLIP_EPI_RESIDUAL, residual=x)
+
+
 class CLIPText:
     """CLIPText(weights, vocab_path).text_cosine(src_txts, trg_txts) -> fp32 [n] on the host, the cosine of each
     source / target pair's encode_text features.  Every operation is a kernel of libasyrp_b200.so; a prompt's
@@ -217,21 +239,8 @@ class CLIPText:
         with torch.cuda.device(self.device):
             ids = ids.to(torch.int32).contiguous().to(self.device)
             x = torch.empty(P, T, w, **f32)
-            h = torch.empty(P, T, w, **f32)
-            qkv = torch.empty(P, T, 3 * w, **f32)
-            mlp = torch.empty(P, T, 4 * w, **f32)
             ops.clip_embed(ids, sd["token_embedding.weight"], sd["positional_embedding"], x)
-            for i in range(d["layers"]):
-                b = {k: sd[f"transformer.resblocks.{i}.{k}"] for k in BLOCK_KEYS}
-                ops.clip_layernorm(x, b["ln_1.weight"], b["ln_1.bias"], h)
-                ops.clip_linear(h, b["attn.in_proj_weight"], b["attn.in_proj_bias"], qkv)
-                ops.clip_attention(qkv, h, d["heads"])
-                ops.clip_linear(h, b["attn.out_proj.weight"], b["attn.out_proj.bias"], x, ops.CLIP_EPI_RESIDUAL,
-                                residual=x)
-                ops.clip_layernorm(x, b["ln_2.weight"], b["ln_2.bias"], h)
-                ops.clip_linear(h, b["mlp.c_fc.weight"], b["mlp.c_fc.bias"], mlp, ops.CLIP_EPI_QUICK_GELU)
-                ops.clip_linear(mlp, b["mlp.c_proj.weight"], b["mlp.c_proj.bias"], x, ops.CLIP_EPI_RESIDUAL,
-                                residual=x)
+            residual_blocks(sd, d["layers"], d["heads"], x, causal=True)
             pooled = torch.empty(P, w, **f32)
             ops.clip_pool(x, ids, sd["ln_final.weight"], sd["ln_final.bias"], pooled)
             feats = torch.empty(P, d["embed_dim"], **f32)

@@ -1,5 +1,6 @@
 // CLIP's text tower (OpenAI CLIP `encode_text`) and the text-direction cosine Asyrp.set_t_edit_t_addnoise takes from
-// it (diffusion_latent.py:1319-1329).  Activations are fp32 [P][T][width] (P prompts, T = 77 tokens).
+// it (diffusion_latent.py:1319-1329).  The LayerNorm, the residual blocks' linear layers and the attention (full
+// rather than causal) also serve the image tower (clip_image.cu).  Activations are fp32 [P][T][width] (P prompts, T = 77 tokens).
 //
 //   x = token_embedding[id] + positional_embedding
 //   layers x:  x = x + out_proj(causal_mha(ln_1(x)));  x = x + c_proj(quick_gelu(c_fc(ln_2(x))))
@@ -20,8 +21,11 @@ namespace asyrp {
 namespace {
 
 constexpr int kHeadDim = 64;
-constexpr int kMaxTokens = 128;     // keys per query row: four per lane
+constexpr int kMaxTokens = 128;     // text tower: keys per query row, four per lane
 constexpr int kAttnWarps = 4;
+constexpr int kMaxImageTokens = 257;  // image tower: 1 + G^2 tokens, G <= 16 (ViT-L/14 at 224)
+constexpr int kImageAttnSlots = 288;  // kMaxImageTokens rounded up to whole lanes: nine keys per lane
+constexpr int kImageAttnWarps = 8;
 constexpr int kRowThreads = 256;    // LayerNorm / cosine: one warp per row
 
 __device__ __forceinline__ float warp_sum(float v) {
@@ -65,30 +69,34 @@ __global__ void clip_embed_kernel(const int* __restrict__ ids, const float* __re
   }
 }
 
+// row r of in starts at in + r * ld (ld = w for a dense matrix; the image tower's ln_post reads the class-token rows
+// with ld = T * w); out is dense [rows][w]
 __global__ void __launch_bounds__(kRowThreads) clip_layernorm_kernel(const float* in, const float* __restrict__ gamma,
                                                                      const float* __restrict__ beta, float* out,
-                                                                     int rows, int w) {
+                                                                     int rows, int w, size_t ld) {
   pdl_trigger();
   pdl_wait();
   const int row = blockIdx.x * (kRowThreads / 32) + (threadIdx.x >> 5);
   if (row >= rows) return;
-  layernorm_row(in + static_cast<size_t>(row) * w, gamma, beta, out + static_cast<size_t>(row) * w, w,
+  layernorm_row(in + static_cast<size_t>(row) * ld, gamma, beta, out + static_cast<size_t>(row) * w, w,
                 threadIdx.x & 31);
 }
 
-// Causal multi-head attention of one (head, prompt) per CTA.  qkv [P*T][3w] packs q | k | v as
-// nn.MultiheadAttention's in_proj does, head h in columns h*64 .. h*64+63 of each; out [P*T][w], the heads
-// concatenated.  A warp per query row i: lane j scores keys j, j+32, ... <= i (64-term dot in d order, times scale),
-// softmax with the row max subtracted, then out[d] = sum_{j <= i} p_j v_j[d] in j order.
-__global__ void __launch_bounds__(kAttnWarps * 32) clip_attention_kernel(const float* __restrict__ qkv,
-                                                                         float* __restrict__ out, int T, int w,
-                                                                         float scale) {
+// Multi-head attention of one (head, sample) per CTA, causal (text tower) or full (image tower).  qkv [P*T][3w]
+// packs q | k | v as nn.MultiheadAttention's in_proj does, head h in columns h*64 .. h*64+63 of each; out [P*T][w],
+// the heads concatenated.  A warp per query row i: lane j scores keys j, j+32, ... <= last (last = i when causal,
+// T-1 otherwise; 64-term dot in d order, times scale), softmax with the row max subtracted, then
+// out[d] = sum_{j <= last} p_j v_j[d] in j order.
+template <bool kCausal, int kSlots, int kWarps>
+__global__ void __launch_bounds__(kWarps * 32) clip_attention_kernel(const float* __restrict__ qkv,
+                                                                     float* __restrict__ out, int T, int w,
+                                                                     float scale) {
   pdl_trigger();
   extern __shared__ __align__(16) float sm[];
   float* Ks = sm;                                   // [T][65]
   float* Vs = Ks + T * (kHeadDim + 1);              // [T][64]
   float* Qs = Vs + T * kHeadDim;                    // [warps][64]
-  float* Ps = Qs + kAttnWarps * kHeadDim;           // [warps][kMaxTokens]
+  float* Ps = Qs + kWarps * kHeadDim;               // [warps][kSlots]
   const int h = blockIdx.x, p = blockIdx.y;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const size_t ld = static_cast<size_t>(3) * w;
@@ -101,18 +109,19 @@ __global__ void __launch_bounds__(kAttnWarps * 32) clip_attention_kernel(const f
   }
   __syncthreads();
   float* q = Qs + warp * kHeadDim;
-  float* pr = Ps + warp * kMaxTokens;
-  for (int i = warp; i < T; i += kAttnWarps) {
+  float* pr = Ps + warp * kSlots;
+  for (int i = warp; i < T; i += kWarps) {
+    const int last = kCausal ? i : T - 1;
     q[lane] = base[i * ld + lane];
     q[lane + 32] = base[i * ld + lane + 32];
     __syncwarp();
-    float s[kMaxTokens / 32];
+    float s[kSlots / 32];
     float mx = -FLT_MAX;
 #pragma unroll
-    for (int kk = 0; kk < kMaxTokens / 32; ++kk) {
+    for (int kk = 0; kk < kSlots / 32; ++kk) {
       const int j = lane + 32 * kk;
       s[kk] = -FLT_MAX;
-      if (j <= i) {
+      if (j <= last) {
         const float* kr = Ks + j * (kHeadDim + 1);
         float dot = 0.f;
 #pragma unroll 16
@@ -122,19 +131,19 @@ __global__ void __launch_bounds__(kAttnWarps * 32) clip_attention_kernel(const f
       }
     }
     mx = warp_max(mx);
-    float e[kMaxTokens / 32], sum = 0.f;
+    float e[kSlots / 32], sum = 0.f;
 #pragma unroll
-    for (int kk = 0; kk < kMaxTokens / 32; ++kk) {
-      e[kk] = lane + 32 * kk <= i ? expf(s[kk] - mx) : 0.f;
+    for (int kk = 0; kk < kSlots / 32; ++kk) {
+      e[kk] = lane + 32 * kk <= last ? expf(s[kk] - mx) : 0.f;
       sum += e[kk];
     }
     sum = warp_sum(sum);
 #pragma unroll
-    for (int kk = 0; kk < kMaxTokens / 32; ++kk)
-      if (lane + 32 * kk <= i) pr[lane + 32 * kk] = e[kk] / sum;
+    for (int kk = 0; kk < kSlots / 32; ++kk)
+      if (lane + 32 * kk <= last) pr[lane + 32 * kk] = e[kk] / sum;
     __syncwarp();
     float o0 = 0.f, o1 = 0.f;
-    for (int j = 0; j <= i; ++j) {
+    for (int j = 0; j <= last; ++j) {
       o0 += pr[j] * Vs[j * kHeadDim + lane];
       o1 += pr[j] * Vs[j * kHeadDim + lane + 32];
     }
@@ -196,8 +205,19 @@ inline int grid_cap(size_t total, int block) {
   return static_cast<int>(g < cap ? (g > 0 ? g : 1) : cap);
 }
 
-inline size_t attention_smem(int T) {
-  return (static_cast<size_t>(T) * (2 * kHeadDim + 1) + kAttnWarps * (kHeadDim + kMaxTokens)) * sizeof(float);
+inline size_t attention_smem(int T, int warps, int slots) {
+  return (static_cast<size_t>(T) * (2 * kHeadDim + 1) + warps * (kHeadDim + slots)) * sizeof(float);
+}
+
+template <bool kCausal, int kSlots, int kWarps>
+int launch_attention(const float* qkv, float* out, int P, int T, int heads, cudaStream_t stream) {
+  const size_t smem = attention_smem(T, kWarps, kSlots);
+  auto kernel = clip_attention_kernel<kCausal, kSlots, kWarps>;
+  ASYRP_CHECK_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)));
+  ASYRP_LAUNCH(kernel, dim3(heads, P), dim3(kWarps * 32), smem, stream, qkv, out, T, heads * kHeadDim,
+               1.f / sqrtf(static_cast<float>(kHeadDim)));
+  ASYRP_CHECK_CUDA(cudaGetLastError());
+  return ASYRP_OK;
 }
 
 }  // namespace
@@ -222,7 +242,20 @@ ASYRP_API int asyrp_clip_layernorm(const float* in, const float* gamma, const fl
   ASYRP_REQUIRE(rows > 0 && width > 0, "asyrp_clip_layernorm: bad shape rows=%d width=%d", rows, width);
   const int per = kRowThreads / 32;
   ASYRP_LAUNCH(clip_layernorm_kernel, dim3((rows + per - 1) / per), dim3(kRowThreads), 0,
-               static_cast<cudaStream_t>(stream), in, gamma, beta, out, rows, width);
+               static_cast<cudaStream_t>(stream), in, gamma, beta, out, rows, width, static_cast<size_t>(width));
+  ASYRP_CHECK_CUDA(cudaGetLastError());
+  return ASYRP_OK;
+}
+
+ASYRP_API int asyrp_clip_layernorm_rows(const float* in, long long ld, const float* gamma, const float* beta,
+                                        float* out, int rows, int width, void* stream) {
+  ASYRP_REQUIRE(rows > 0 && width > 0 && ld >= width, "asyrp_clip_layernorm_rows: bad shape rows=%d width=%d ld=%lld",
+                rows, width, ld);
+  ASYRP_REQUIRE(out + static_cast<size_t>(rows) * width <= in || in + static_cast<size_t>(rows - 1) * ld + width <= out,
+                "asyrp_clip_layernorm_rows: out must not overlap in");
+  const int per = kRowThreads / 32;
+  ASYRP_LAUNCH(clip_layernorm_kernel, dim3((rows + per - 1) / per), dim3(kRowThreads), 0,
+               static_cast<cudaStream_t>(stream), in, gamma, beta, out, rows, width, static_cast<size_t>(ld));
   ASYRP_CHECK_CUDA(cudaGetLastError());
   return ASYRP_OK;
 }
@@ -254,13 +287,14 @@ ASYRP_API int asyrp_clip_linear(const float* in, const float* weight, const floa
 ASYRP_API int asyrp_clip_attention(const float* qkv, float* out, int P, int T, int heads, void* stream) {
   ASYRP_REQUIRE(P > 0 && heads > 0 && T > 0 && T <= kMaxTokens,
                 "asyrp_clip_attention: bad shape P=%d T=%d heads=%d (T <= %d)", P, T, heads, kMaxTokens);
-  const size_t smem = attention_smem(T);
-  ASYRP_CHECK_CUDA(cudaFuncSetAttribute(clip_attention_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                        static_cast<int>(smem)));
-  ASYRP_LAUNCH(clip_attention_kernel, dim3(heads, P), dim3(kAttnWarps * 32), smem, static_cast<cudaStream_t>(stream),
-               qkv, out, T, heads * kHeadDim, 1.f / sqrtf(static_cast<float>(kHeadDim)));
-  ASYRP_CHECK_CUDA(cudaGetLastError());
-  return ASYRP_OK;
+  return launch_attention<true, kMaxTokens, kAttnWarps>(qkv, out, P, T, heads, static_cast<cudaStream_t>(stream));
+}
+
+ASYRP_API int asyrp_clip_attention_full(const float* qkv, float* out, int P, int T, int heads, void* stream) {
+  ASYRP_REQUIRE(P > 0 && heads > 0 && T > 0 && T <= kMaxImageTokens,
+                "asyrp_clip_attention_full: bad shape P=%d T=%d heads=%d (T <= %d)", P, T, heads, kMaxImageTokens);
+  return launch_attention<false, kImageAttnSlots, kImageAttnWarps>(qkv, out, P, T, heads,
+                                                                   static_cast<cudaStream_t>(stream));
 }
 
 ASYRP_API int asyrp_clip_pool(const float* x, const int* ids, const float* gamma, const float* beta, float* out, int P,

@@ -11,6 +11,8 @@ Mirrors, with the same attribute / flag names:
                                                             (--clip_cosine, or CLIP's text cosine on the GPU)
   Asyrp.compute_lpips_distance :1191-1303                   --lpips: the LPIPS(x_t, x0) / LPIPS(x0_t, x0) tables of an
                                                             inversion, which set_t_edit_t_addnoise reads
+  --DirectionalClipSmilarity   main.py:101, losses/clip_loss.py  run_test scores every edit with CLIPLoss's directional
+                                                            similarity (clip_image.CLIPLoss), written next to the PNG
 
 Differences (documented in INTEGRATION.md): the reverse loop is UNetEngine.sample() — one CUDA graph per
 (batch, schedule) instead of 40 Python iterations; pretrained weights come from --model_path (no URL download);
@@ -58,6 +60,7 @@ class Asyrp(object):
         self.t_addnoise = getattr(args, "user_defined_t_addnoise", None)
         self.rank = int(os.environ.get("RANK", "0"))
         self.world = int(os.environ.get("WORLD_SIZE", "1"))
+        self.directional_clip = {}  # --DirectionalClipSmilarity: save_image's file name -> S_dir [tuples][images]
 
     # ------------------------------------------------------------------------------------------
     def load_pretrained_model(self):
@@ -149,6 +152,44 @@ class Asyrp(object):
         if attr not in dic:
             raise ValueError(f"attribute {attr!r} is not in SRC_TRG_TXT_DIC")
         return list(dic[attr][0]), list(dic[attr][1])
+
+    def directional_clip_setup(self):
+        """--DirectionalClipSmilarity's requirements, checked before any model is loaded; raises ValueError with the
+        reason.  Returns (src_txt, trg_txt, templates): src_txts[0] / trg_txts[0] of edit_texts(), the pair
+        run_training scores (diffusion_latent.py:343), and imagenet_templates from --text_templates."""
+        from .clip_image import read_templates
+        a = self.args
+        if getattr(a, "multiple_attr", ""):
+            raise ValueError("--DirectionalClipSmilarity scores one source / target text pair: a --multiple_attr edit "
+                             "has none")
+        if getattr(a, "pass_editing", False):
+            raise ValueError("--DirectionalClipSmilarity scores the edited images: with --pass_editing nothing is "
+                             "edited")
+        if not self.clip_configured():
+            raise ValueError("--DirectionalClipSmilarity needs --clip_weights and --clip_vocab")
+        for flag, path in (("--clip_weights", a.clip_weights), ("--clip_vocab", a.clip_vocab)):
+            if not os.path.isfile(path):
+                raise ValueError(f"--DirectionalClipSmilarity: {flag} {path!r} is not a file")
+        try:
+            templates = read_templates(getattr(a, "text_templates", None)
+                                       or os.path.join("utils", "text_templates.py"))
+        except FileNotFoundError as e:
+            raise ValueError(f"--DirectionalClipSmilarity: {e}") from None
+        src, trg = self.edit_texts()
+        return src[0], trg[0], templates
+
+    def write_directional_clip(self, path, coeffs, s_dir):
+        """the TSV of one batch: one row per (hs_coeff tuple, image) in grid order, S_dir = 1 -
+        clip_directional_loss of that row; prints each tuple's mean"""
+        with open(path, "w") as f:
+            f.write("image\ttuple\ths_coeff\tS_dir\n")
+            for k, row in enumerate(s_dir.tolist()):
+                tup = ",".join(f"{float(c):.6g}" for c in coeffs[k])
+                for i, v in enumerate(row):
+                    f.write(f"{i}\t{k}\t{tup}\t{v!r}\n")
+        for k, row in enumerate(s_dir):
+            print(f"directional CLIP similarity, hs_coeff {tuple(float(c) for c in coeffs[k])}: mean "
+                  f"{row.double().mean().item():.6f} over {row.numel()} images")
 
     @torch.no_grad()
     def clip_cosines(self, pairs):
@@ -323,26 +364,35 @@ class Asyrp(object):
     @torch.no_grad()
     def save_image(self, model, x_lat_tensor, seq_inv, seq_inv_next, save_x0=False, save_x_origin=False,
                    save_process_delta_h=False, save_process_origin=False, x0_tensor=None, delta_h_dict=None,
-                   get_delta_hs=False, folder_dir="", file_name="", hs_coeff=(1.0, 1.0)):
+                   get_delta_hs=False, folder_dir="", file_name="", hs_coeff=(1.0, 1.0), directional_clip=None):
         """rows of the grid: [x0] [origin DDIM] one row per hs_coeff tuple  (diffusion_latent.py:445-544).
 
         delta_h_dict: {t: None | Δh tensor}.  Entries that are tensors select the explicit-Δh branch for that step
         (raw-Δh checkpoints, mean Δh); get_delta_hs: run the DeltaBlocks and ADD their per-step output into
-        delta_h_dict (mean-Δh extraction, :528-532)."""
+        delta_h_dict (mean-Δh extraction, :528-532).
+        directional_clip: (CLIPLoss, src_txt, trg_txt) for --DirectionalClipSmilarity: every tuple's edited rows are
+        scored against the origin pass of the same x_T (run for this even without save_x_origin, then left out of the
+        grid), written to <file_name>_ngen<n_train_step>_directional_clip.tsv and kept in
+        self.directional_clip[file_name]."""
         import torchvision.utils as tvu
         a = self.args
         time_s = time.time()
         eng = model.engine
         bs = x_lat_tensor.shape[0]
-        x_list = []
+        x_list, edited = [], []
         if save_x0 and x0_tensor is not None:
             x_list.append(x0_tensor.cpu())
-        if save_x_origin:
+        if save_x_origin or directional_clip is not None:
             sch = self.make_schedule(seq_inv, seq_inv_next, (1.0,), edit=False,
                                      addnoise=bool(getattr(a, "origin_process_addnoise", False)))
-            x_list.append(self.edit_batch(model, x_lat_tensor, sch, record_process=save_process_origin))
-            if save_process_origin:
-                self._write_process(eng, sch, os.path.join(folder_dir, file_name), "origin", bs)
+            if save_x_origin:
+                origin = self.edit_batch(model, x_lat_tensor, sch, record_process=save_process_origin)
+                x_list.append(origin)
+                if save_process_origin:
+                    self._write_process(eng, sch, os.path.join(folder_dir, file_name), "origin", bs)
+            else:  # the pass only the score needs leaves the random stream as it was: the edits draw the same noise
+                with torch.random.fork_rng(devices=[eng.device]):
+                    origin = self.edit_batch(model, x_lat_tensor, sch)
         if not getattr(a, "pass_editing", False):
             coeffs = hs_coeff if isinstance(hs_coeff, list) else [hs_coeff]
             # the reference replays the trajectory once per tuple (:495-532); the tuples share x_T and the schedule, so
@@ -390,6 +440,7 @@ class Asyrp(object):
                 x0 = self.edit_batch(model, rows_x, sch, noise=noise, record_process=save_process_delta_h, **kw)
                 for j in range(len(chunk)):
                     x_list.append(x0[j * bs:(j + 1) * bs].clone())
+                    edited.append(x_list[-1])
                 if save_process_delta_h and chunk is chunks[-1]:  # each tuple rewrote these files: the last one stays
                     j = len(chunk) - 1
                     self._write_process(eng, sch, os.path.join(folder_dir, file_name), "delta_h", bs,
@@ -405,6 +456,12 @@ class Asyrp(object):
         os.makedirs(folder_dir, exist_ok=True)
         path = os.path.join(folder_dir, f'{file_name}_ngen{a.n_train_step}.png')
         tvu.save_image(grid, path)
+        if directional_clip is not None and edited:
+            clip_loss, src_txt, trg_txt = directional_clip
+            s_dir = clip_loss.directional_similarity(origin, src_txt, torch.cat(edited), trg_txt).view(len(edited), bs)
+            self.directional_clip[file_name] = s_dir
+            self.write_directional_clip(
+                os.path.join(folder_dir, f'{file_name}_ngen{a.n_train_step}_directional_clip.tsv'), coeffs, s_dir)
         print(f'{time.time() - time_s} seconds, {file_name}_ngen{a.n_train_step}.png is saved')
         return x_list
 
@@ -493,6 +550,7 @@ class Asyrp(object):
         if getattr(a, "warigari", 0.0):
             print("--warigari is accepted and has no effect (the reference's branch returns the same values, "
                   "utils/diffusion_utils.py:103-109)")
+        sdir = self.directional_clip_setup() if getattr(a, "DirectionalClipSmilarity", False) else None
         if a.multiple_attr and self.needs_clip() and self.clip_configured():
             cosine = self.choose_attribute(a.multiple_attr.split(' '))  # :640-652
             self.set_t_edit_t_addnoise(LPIPS_th=a.lpips_edit_th, LPIPS_addnoise_th=a.lpips_addnoise_th, cosine=cosine)
@@ -610,7 +668,10 @@ class Asyrp(object):
         if getattr(a, "target_image_id", None):
             target_ids = [int(i) for i in str(a.target_image_id).split(" ")]
             assert a.bs_train == 1, "target_image_id is only supported for batch_size == 1"
-        results = {}
+        results, directional_clip = {}, None
+        if sdir is not None:  # the image tower lives for this run_test only
+            from .clip_image import CLIPLoss
+            directional_clip = (CLIPLoss(a.clip_weights, a.clip_vocab, sdir[2], device=self.device), sdir[0], sdir[1])
         try:
             for mode, do, n_img in (("train", a.do_train, a.n_train_img), ("test", a.do_test, a.n_test_img)):
                 if not do:
@@ -633,7 +694,8 @@ class Asyrp(object):
                             get_delta_hs=bool(num_mean),
                             save_process_origin=bool(getattr(a, "save_process_origin", False)),
                             save_process_delta_h=bool(getattr(a, "save_process_delta_h", False)),
-                            folder_dir=a.test_image_folder, file_name=f'{mode}_{step}_{a.n_iter - 1}', hs_coeff=hs_coeff)
+                            folder_dir=a.test_image_folder, file_name=f'{mode}_{step}_{a.n_iter - 1}', hs_coeff=hs_coeff,
+                            directional_clip=directional_clip)
                     batch_idx += 1
                     if step == n_img - 1:
                         break
@@ -657,6 +719,9 @@ class Asyrp(object):
                     x_lat_tensor, x0_tensor = None, None
         finally:
             a.train_delta_h = a_train_delta_h_prev
+            if directional_clip is not None:
+                del directional_clip
+                torch.cuda.empty_cache()
         self.last_delta_h_dict = delta_h_dict
         return results
 

@@ -57,6 +57,7 @@ def build_parser():
     p.add_argument('--choose_checkpoint_num', type=str, default='')
     p.add_argument('--load_from_checkpoint', type=str)
     p.add_argument('--pass_editing', **sa)
+    p.add_argument('--DirectionalClipSmilarity', **sa)
     p.add_argument('--warigari', type=float, default=0.0)
     p.add_argument('--config', type=str, required=True)
     p.add_argument('--seed', type=int, default=1234)
@@ -94,6 +95,9 @@ def build_parser():
                    help="CLIP's bpe_simple_vocab_16e6.txt.gz (inside the installed clip package)")
     p.add_argument('--text_dic', type=str, default=None,
                    help='file defining SRC_TRG_TXT_DIC, read with ast (default utils/text_dic.py)')
+    p.add_argument('--text_templates', type=str, default=None,
+                   help='file defining imagenet_templates, read with ast, for --DirectionalClipSmilarity (default '
+                        'utils/text_templates.py)')
     p.add_argument('--lpips_table_dir', type=str,
                    help='directory with <config stem>_LPIPS_distance_{x,x0_t}.tsv (read by --run_test, written by '
                         '--lpips; default utils)')

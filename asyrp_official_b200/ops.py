@@ -414,13 +414,70 @@ def clip_linear(x, weight, bias, out, epilogue=CLIP_EPI_BIAS, residual=None):
                                 _stream()), "asyrp_clip_linear")
 
 
-def clip_attention(qkv, out, heads):
-    """causal multi-head attention (head size 64): qkv [P][T][3w] (q | k | v), out [P][T][w]"""
+def clip_attention(qkv, out, heads, causal=True):
+    """multi-head attention (head size 64): qkv [P][T][3w] (q | k | v), out [P][T][w]; causal (the text tower,
+    T <= 128) or full (the image tower, T <= 257)"""
     lib = _lib.load()
     P, T, w3 = qkv.shape
     _need_cuda(qkv, out)
     assert qkv.is_contiguous() and w3 == 3 * 64 * heads and tuple(out.shape) == (P, T, 64 * heads)
-    check(lib.asyrp_clip_attention(_ptr(qkv), _ptr(out), P, T, heads, _stream()), "asyrp_clip_attention")
+    if causal:
+        check(lib.asyrp_clip_attention(_ptr(qkv), _ptr(out), P, T, heads, _stream()), "asyrp_clip_attention")
+    else:
+        check(lib.asyrp_clip_attention_full(_ptr(qkv), _ptr(out), P, T, heads, _stream()),
+              "asyrp_clip_attention_full")
+
+
+def clip_layernorm_rows(x, gamma, beta, out):
+    """out [B][w] = LayerNorm(eps 1e-5)(x[:, 0]) of x [B][T][w]: ln_post of the class token, read in place"""
+    lib = _lib.load()
+    B, T, w = x.shape
+    _need_cuda(x, gamma, beta, out)
+    assert x.is_contiguous() and tuple(out.shape) == (B, w) and out.is_contiguous()
+    assert gamma.numel() == w and beta.numel() == w
+    check(lib.asyrp_clip_layernorm_rows(_ptr(x), T * w, _ptr(gamma), _ptr(beta), _ptr(out), B, w, _stream()),
+          "asyrp_clip_layernorm_rows")
+
+
+def clip_image_kpad(patch):
+    """columns of the patch matrix: 3 * patch^2 rounded up to the GEMM's K multiple (32)"""
+    return -(-3 * patch * patch // 32) * 32
+
+
+def clip_image_patches(x, out, grid, patch):
+    """CLIPLoss.preprocess + patchify: x fp32 [B][3][S][S] in [-1, 1] -> out [B*grid^2][clip_image_kpad(patch)]
+    (asyrp_b200.h gives the resize, normalisation and layout)"""
+    lib = _lib.load()
+    B, C, S, S2 = x.shape
+    _need_cuda(x, out)
+    kpad = clip_image_kpad(patch)
+    assert C == 3 and S == S2 and x.dtype == torch.float32 and x.is_contiguous()
+    assert tuple(out.shape) == (B * grid * grid, kpad) and out.is_contiguous()
+    check(lib.asyrp_clip_image_patches(_ptr(x), _ptr(out), B, S, grid, patch, kpad, _stream()),
+          "asyrp_clip_image_patches")
+
+
+def clip_image_tokens(patch_emb, class_embedding, positional_embedding, out):
+    """out [B][T][w]: row 0 = class_embedding + pos[0], row 1+p = patch_emb[b*(T-1) + p] + pos[1+p]"""
+    lib = _lib.load()
+    B, T, w = out.shape
+    _need_cuda(patch_emb, class_embedding, positional_embedding, out)
+    assert patch_emb.is_contiguous() and patch_emb.numel() == B * (T - 1) * w and class_embedding.numel() == w
+    assert tuple(positional_embedding.shape) == (T, w) and out.is_contiguous()
+    check(lib.asyrp_clip_image_tokens(_ptr(patch_emb), _ptr(class_embedding), _ptr(positional_embedding), _ptr(out), B,
+                                      T, w, _stream()), "asyrp_clip_image_tokens")
+
+
+def clip_direction(src, trg, out, group_rows, add_eps):
+    """out[g] = d / (|d| + add_eps), d = mean over the group's rows i of trg_i/|trg_i| - src_i/|src_i|; src, trg fp32
+    [groups * group_rows][dim], out [groups][dim]"""
+    lib = _lib.load()
+    n, dim = src.shape
+    _need_cuda(src, trg, out)
+    assert src.is_contiguous() and trg.is_contiguous() and trg.shape == src.shape and n % group_rows == 0
+    assert tuple(out.shape) == (n // group_rows, dim) and out.is_contiguous()
+    check(lib.asyrp_clip_direction(_ptr(src), _ptr(trg), _ptr(out), n // group_rows, group_rows, dim, float(add_eps),
+                                   _stream()), "asyrp_clip_direction")
 
 
 def clip_pool(x, ids, gamma, beta, out):

@@ -30,21 +30,41 @@ def clip_text_state_dict(seed=1234, width=512, layers=12, context=77, vocab=4940
     std width^-1/2, out_proj / c_proj std width^-1/2 (2 layers)^-1/2, c_fc std (2 width)^-1/2.  No term is zero:
     the biases are N(0, .02^2) and the LayerNorm affines 1 + N(0, .1^2) / N(0, .02^2), so a dropped term shows."""
     from .clip_text import text_key_shapes
-    std = {"token_embedding.weight": 0.02, "positional_embedding": 0.01, "text_projection": width ** -0.5,
-           "attn.in_proj_weight": width ** -0.5, "attn.out_proj.weight": width ** -0.5 * (2 * layers) ** -0.5,
+    std = {"token_embedding.weight": 0.02, "positional_embedding": 0.01, "text_projection": width ** -0.5}
+    return _draw_clip(text_key_shapes(width, layers, context, vocab, embed_dim), "", std, width, layers, seed)
+
+
+def clip_image_state_dict(seed=1234, width=768, layers=12, patch=16, grid=14, embed_dim=512):
+    """seeded CLIP image-tower (VisionTransformer) weights under visual.* in CLIP's state-dict layout
+    (asyrp_official_b200.clip_image), at CLIP's init scales: class_embedding, positional_embedding and proj std
+    width^-1/2, conv1 torch's Conv2d default U(-b, b), b = (3 patch^2)^-1/2, the blocks as in clip_text_state_dict.
+    No term is zero: biases N(0, .02^2), LayerNorm affines 1 + N(0, .1^2) / N(0, .02^2).  Defaults: ViT-B/16."""
+    from .clip_image import image_key_shapes
+    std = {"class_embedding": width ** -0.5, "positional_embedding": width ** -0.5, "proj": width ** -0.5}
+    sd = _draw_clip(image_key_shapes(width, layers, patch, grid, embed_dim), "visual.", std, width, layers, seed)
+    sd["visual.conv1.weight"] = (2 * sd["visual.conv1.weight"] - 1) * (3 * patch * patch) ** -0.5
+    return sd
+
+
+def _draw_clip(shapes, prefix, std, width, layers, seed):
+    """CLIP weights of `shapes` (names without `prefix`), each from its own generator seeded by crc32(prefix + name)"""
+    std = {**std, "attn.in_proj_weight": width ** -0.5, "attn.out_proj.weight": width ** -0.5 * (2 * layers) ** -0.5,
            "mlp.c_fc.weight": (2 * width) ** -0.5, "mlp.c_proj.weight": width ** -0.5 * (2 * layers) ** -0.5}
     sd = {}
-    for name, shp in text_key_shapes(width, layers, context, vocab, embed_dim).items():
+    for name, shp in shapes.items():
         g = torch.Generator()
-        g.manual_seed((zlib.crc32(name.encode()) ^ (seed * 0x9E3779B1)) & 0x7FFFFFFF)
+        g.manual_seed((zlib.crc32((prefix + name).encode()) ^ (seed * 0x9E3779B1)) & 0x7FFFFFFF)
         key = name.split(".", 3)[-1] if name.startswith("transformer.") else name
+        if key == "conv1.weight":  # U(0, 1), scaled by the caller
+            sd[prefix + name] = torch.rand(shp, generator=g)
+            continue
         z = torch.randn(shp, generator=g)
         if key in std:
-            sd[name] = z * std[key]
+            sd[prefix + name] = z * std[key]
         elif key.startswith("ln") and key.endswith(".weight"):
-            sd[name] = 1.0 + 0.1 * z
+            sd[prefix + name] = 1.0 + 0.1 * z
         else:  # biases
-            sd[name] = 0.02 * z
+            sd[prefix + name] = 0.02 * z
     return sd
 
 

@@ -270,6 +270,31 @@ int asyrp_clip_pool(const float* x, const int* ids, const float* gamma, const fl
                     int width, void* stream);
 int asyrp_clip_cosine(const float* a, const float* b, float* cos, int n, int dim, float eps, void* stream);
 
+/* ---- CLIP image tower and the directional similarity: OpenAI CLIP's VisionTransformer.forward and CLIPLoss's
+ * clip_directional_loss (losses/clip_loss.py:102-117,170-180).  Activations are fp32 [B][T][width], T = 1 + grid^2.
+ * asyrp_clip_image_patches: CLIPLoss.preprocess and the patch layout of conv1.  x fp32 [B][3][S][S] in [-1, 1]
+ *   (square) -> (x+1)/2 -> F.interpolate(R x R, bicubic, align_corners=False, no antialiasing, A = -0.75, taps clamped
+ *   at the edges), R = grid*patch -> (v - mean_c) / std_c with CLIP's mean and std -> out [B*grid^2][kpad]: row
+ *   gy*grid + gx of image b, column c*patch^2 + ky*patch + kx (conv1.weight.reshape(width, -1)'s order), columns
+ *   3*patch^2 .. kpad-1 zero; kpad = 3*patch^2 rounded up to a multiple of 32.
+ * asyrp_clip_image_tokens: out[b][0] = class_embedding + pos[0], out[b][1+p] = patch_emb[b*(T-1) + p] + pos[1+p];
+ *   patch_emb [B*(T-1)][width], positional_embedding [T][width].
+ * asyrp_clip_layernorm_rows: LayerNorm (eps 1e-5) of rows in + r*ld, r < rows, into dense out [rows][width] (ln_post
+ *   of the class token: ld = T*width).  out must not overlap in.
+ * asyrp_clip_attention_full: asyrp_clip_attention without the causal mask, T <= 257.
+ * asyrp_clip_direction: for each group g of n rows of src and trg [groups*n][dim]:
+ *   d = mean_i(trg_i/|trg_i| - src_i/|src_i|), out[g] = d / (|d| + add_eps).  Images: n = 1, add_eps = 1e-7; text
+ *   templates: one group, add_eps = 0.  2n + dim <= 12288.
+ * Fixed-order reductions, no float atomics, no kernel mixes images or groups. */
+int asyrp_clip_image_patches(const float* x, float* out, int B, int S, int grid, int patch, int kpad, void* stream);
+int asyrp_clip_image_tokens(const float* patch_emb, const float* class_embedding, const float* positional_embedding,
+                            float* out, int B, int T, int width, void* stream);
+int asyrp_clip_layernorm_rows(const float* in, long long ld, const float* gamma, const float* beta, float* out,
+                              int rows, int width, void* stream);
+int asyrp_clip_attention_full(const float* qkv, float* out, int P, int T, int heads, void* stream);
+int asyrp_clip_direction(const float* src, const float* trg, float* out, int groups, int n, int dim, float add_eps,
+                         void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -17,10 +17,11 @@
 // address, the descriptor's stride-byte-offset is the halo pitch); layers narrower than 8x16 pixels use three
 // dx-shifted copies whose dy taps are 1024B-aligned row offsets.  TMA's out-of-bounds zero fill is the padding.
 //
-// Warp roles (576 threads): warps 0..7 = two consumer warpgroups (wgmma into register accumulators, which go to a
-// shared-memory staging tile at the end of each tile), warps 8..15 = in-place operand transform (fused GroupNorm-apply
-// + SiLU) and the epilogue (staging tile -> bias/residual -> fp16 NHWC store + GroupNorm partial sums), warp 16 =
-// activation TMA producer, warp 17 = weight TMA producer (whole-warp uniform control flow, one elected lane issues).
+// Warp roles (640 threads, five warpgroups): warps 0..7 = two consumer warpgroups (wgmma into register accumulators,
+// which go to a shared-memory staging tile at the end of each tile), warps 8..15 = in-place operand transform (fused
+// GroupNorm-apply + SiLU) and the epilogue (staging tile -> bias/residual -> fp16 NHWC store + GroupNorm partial sums),
+// warp 16 = activation TMA producer, warp 17 = weight TMA producer (whole-warp uniform control flow, one elected lane
+// issues), warps 18..19 only complete the producers' warpgroup: setmaxnreg moves registers from it to warps 8..15.
 // Persistent: each CTA loops over output tiles; the producers run ahead across tile boundaries, and the staging tile
 // is handed over through a full / empty mbarrier pair, so the consumers start tile i+1's MMAs while warps 8..15 run
 // the epilogue of tile i.
@@ -37,7 +38,15 @@ static constexpr int kNumTransformWarps = 8;
 static constexpr int kWarpT = kNumConsumerWarps;                // first transform warp
 static constexpr int kWarpA = kWarpT + kNumTransformWarps;      // activation (A operand) producer warp
 static constexpr int kWarpB = kWarpA + 1;                       // weight (B operand) producer warp
-static constexpr int kNumThreads = 32 * (kWarpB + 1);
+static constexpr int kNumThreads = 32 * (kWarpA + 4);          // the producers' warpgroup is filled up with idle warps
+// Registers per thread.  The launch allocates kRegsLaunch for every thread (what ptxas grants 640 threads of a 64K
+// register file); after the prologue the producers' warpgroup gives back all but kRegsProducer and the transform /
+// epilogue warpgroups grow to kRegsTransform.  setmaxnreg.inc can only take what setmaxnreg.dec has freed.
+static constexpr int kRegsLaunch = 96, kRegsProducer = 40, kRegsTransform = 120;
+static_assert(kNumThreads * kRegsLaunch <= 65536, "registers of an SM");
+static_assert(32 * (kNumConsumerWarps * kRegsLaunch + kNumTransformWarps * kRegsTransform + 4 * kRegsProducer) <=
+                  kNumThreads * kRegsLaunch,
+              "the transform warps' increase must fit into what the producers' warpgroup released");
 
 struct ConvSegDev {
   int nchunks;  // C / 64
@@ -376,12 +385,12 @@ __device__ __forceinline__ void ld_staged(uint32_t addr, uint32_t (&r)[NV]) {
 }
 
 // BN output channels x MT sub-tiles of 128 pixels per CTA tile; each consumer warpgroup accumulates MT x BN/2 fp32
-// registers per thread.  MT * BN <= 128 bounds them to 64: ptxas allocates 96 registers per thread to every
-// instantiation at 576 threads, and the 64- and 128-channel ones still spill outside the wgmma chain.
+// registers per thread.  MT * BN <= 128 bounds them to 64, which fits the 96 registers a thread has at launch (a
+// consumer warpgroup cannot give any up: at 88 ptxas refuses the limit for the 64-accumulator tiles).
 // PLAIN: tiles inside one sample (NB == 1) and one fp16 NHWC output (out_heads == 1, no fp32 or planar output), as
 // every 128x128-and-larger layer has.  The epilogue and transform code of the other modes then drops out, and with it
-// the values they keep live across the epilogue's row loop: about half the spill traffic, and none of it reloaded
-// between the row loop's global stores.
+// the values they keep live across the epilogue's row loop: at kRegsTransform registers its row loop has no spill
+// traffic (the generic instantiations keep a few spilled values, see DESIGN.md section 5).
 template <int BN, int MT, bool PLAIN>
 __global__ void __launch_bounds__(kNumThreads, 1) conv_gemm_kernel(const __grid_constant__ ConvParams p) {
   pdl_trigger();  // the next kernel of the stream may be scheduled as soon as every CTA of this grid is running
@@ -437,83 +446,88 @@ __global__ void __launch_bounds__(kNumThreads, 1) conv_gemm_kernel(const __grid_
 
   const int total_tiles = p.m_tiles * p.n_tiles;
 
-  if (warp == kWarpA) {
-    // ======================================================== TMA producer, A operand (activations)
-    // A and B have independent rings and independent producer threads, so the activation prefetch (which the
-    // transform warps must also touch) runs a full A-ring ahead regardless of the weight ring's depth.
-    // Whole warp, uniform control flow; one elected lane issues (see elect_one()).
-    int sa = 0, sl = 0;      // heavy / light ring cursors
-    uint32_t pa = 0, pl = 0;
-    [[maybe_unused]] int tr_n = 0;
-    for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
-      const TileCoord tc = tile_coord(p, tile);
-      const int x0 = tc.tx * p.TW, y0 = tc.ty * THT, n0 = tc.tn * p.NB;
-      for (int e = 0; e < p.n_sched; ++e) {
-        const int s = p.sched[e] >> 6, ch = p.sched[e] & 63;
-        const ConvSegDev sg = p.seg[s];
-        const bool lt = p.l_stages != 0 && sg.mode == 0;
-        const int ncopies = (sg.mode == 0 || sg.mode == 3) ? 1 : (sg.mode == 1 ? 3 : 9);
-        const uint32_t a_bytes = sg.mode == 3 ? (THT + 2) * (p.TW + 2) * 128u
-                                              : (sg.mode == 1 ? (THT + 2) : THT) * p.row_bytes;
-        for (int cp = 0; cp < ncopies; ++cp) {
-          const int slot = lt ? p.a_stages + sl : sa;
-          mbar_wait_suspend(&emptyA[slot], (lt ? pl : pa) ^ 1);
-          ASYRP_TRACE_STAMP(0, tr_n);
-          ++tr_n;
-          uint8_t* dst = lt ? sL + sl * p.l_stage_bytes : sA + sa * p.a_stage_bytes;
-          int c0 = ch * 64, c1, c2 = n0, c3 = 0, c4;
-          if (sg.mode == 3) {
-            c1 = x0 - 1; c4 = y0 - 1;
-          } else if (sg.mode == 0) {
-            c1 = x0; c2 = n0 / p.a_heads; c3 = n0 % p.a_heads; c4 = y0;
-          } else if (sg.mode == 1) {
-            c1 = x0 + cp - 1; c4 = y0 - 1;
-          } else {
-            const int ky = cp / 3, kx = cp % 3;
-            c0 += (kx & 1) * sg.C; c1 = x0 + (kx >> 1); c3 = ky & 1; c4 = y0 + (ky >> 1);
-          }
-          if (elect_one()) {
-            mbar_arrive_expect_tx(&fullA[slot], a_bytes);
-            tma_load_5d(dst, &p.tmA[s], &fullA[slot], c0, c1, c2, c3, c4);
-          }
-          if (lt) {
-            if (++sl == p.l_stages) { sl = 0; pl ^= 1; }
-          } else {
-            if (++sa == p.a_stages) { sa = 0; pa ^= 1; }
+  if (warp >= kWarpA) {
+    // the producers' warpgroup keeps what two TMA loops need; warps 18..19 have nothing else to do
+    setmaxnreg_dec<kRegsProducer>();
+    if (warp == kWarpA) {
+      // ======================================================== TMA producer, A operand (activations)
+      // A and B have independent rings and independent producer threads, so the activation prefetch (which the
+      // transform warps must also touch) runs a full A-ring ahead regardless of the weight ring's depth.
+      // Whole warp, uniform control flow; one elected lane issues (see elect_one()).
+      int sa = 0, sl = 0;      // heavy / light ring cursors
+      uint32_t pa = 0, pl = 0;
+      [[maybe_unused]] int tr_n = 0;
+      for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
+        const TileCoord tc = tile_coord(p, tile);
+        const int x0 = tc.tx * p.TW, y0 = tc.ty * THT, n0 = tc.tn * p.NB;
+        for (int e = 0; e < p.n_sched; ++e) {
+          const int s = p.sched[e] >> 6, ch = p.sched[e] & 63;
+          const ConvSegDev sg = p.seg[s];
+          const bool lt = p.l_stages != 0 && sg.mode == 0;
+          const int ncopies = (sg.mode == 0 || sg.mode == 3) ? 1 : (sg.mode == 1 ? 3 : 9);
+          const uint32_t a_bytes = sg.mode == 3 ? (THT + 2) * (p.TW + 2) * 128u
+                                                : (sg.mode == 1 ? (THT + 2) : THT) * p.row_bytes;
+          for (int cp = 0; cp < ncopies; ++cp) {
+            const int slot = lt ? p.a_stages + sl : sa;
+            mbar_wait_suspend(&emptyA[slot], (lt ? pl : pa) ^ 1);
+            ASYRP_TRACE_STAMP(0, tr_n);
+            ++tr_n;
+            uint8_t* dst = lt ? sL + sl * p.l_stage_bytes : sA + sa * p.a_stage_bytes;
+            int c0 = ch * 64, c1, c2 = n0, c3 = 0, c4;
+            if (sg.mode == 3) {
+              c1 = x0 - 1; c4 = y0 - 1;
+            } else if (sg.mode == 0) {
+              c1 = x0; c2 = n0 / p.a_heads; c3 = n0 % p.a_heads; c4 = y0;
+            } else if (sg.mode == 1) {
+              c1 = x0 + cp - 1; c4 = y0 - 1;
+            } else {
+              const int ky = cp / 3, kx = cp % 3;
+              c0 += (kx & 1) * sg.C; c1 = x0 + (kx >> 1); c3 = ky & 1; c4 = y0 + (ky >> 1);
+            }
+            if (elect_one()) {
+              mbar_arrive_expect_tx(&fullA[slot], a_bytes);
+              tma_load_5d(dst, &p.tmA[s], &fullA[slot], c0, c1, c2, c3, c4);
+            }
+            if (lt) {
+              if (++sl == p.l_stages) { sl = 0; pl ^= 1; }
+            } else {
+              if (++sa == p.a_stages) { sa = 0; pa ^= 1; }
+            }
           }
         }
       }
-    }
-  } else if (warp == kWarpB) {
-    // ======================================================== TMA producer, B operand (weights)
-    int sb = 0;
-    uint32_t pb = 0;
-    for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
-      const TileCoord tc = tile_coord(p, tile);
-      const int nt = tc.nt, tn = tc.tn;
-      const int bz = p.b_batched ? tn * p.NB : 0;
-      const int b_n = bz / p.b_heads, b_h = bz % p.b_heads;
-      for (int e = 0; e < p.n_sched; ++e) {
-        const int s = p.sched[e] >> 6, ch = p.sched[e] & 63;
-        const ConvSegDev sg = p.seg[s];
-        const int ncopies = (sg.mode == 0 || sg.mode == 3) ? 1 : (sg.mode == 1 ? 3 : 9);
-        const int ntaps = sg.mode == 1 ? 3 : (sg.mode == 3 ? (p.up2 ? 4 : 9) : 1);
-        for (int cp = 0; cp < ncopies; ++cp) {
-          for (int tp = 0; tp < ntaps; ++tp) {
-            // tap index in the weight matrix: ky*3+kx (up2: dy*2+dx of the phase's 2x2 kernel; the weight rows
-            // nt*BN already select the phase)
-            const int tap = sg.mode == 0 ? 0 : (sg.mode == 1 ? tp * 3 + cp : (sg.mode == 3 ? tp : cp));
-            mbar_wait_suspend(&emptyB[sb], pb ^ 1);
-            if (elect_one()) {
-              mbar_arrive_expect_tx(&fullB[sb], kBStage);
-              tma_load_4d(sB + sb * kBStage, &p.tmB, &fullB[sb], sg.kbase + tap * sg.C + ch * 64, nt * BN, b_h, b_n);
+    } else if (warp == kWarpB) {
+      // ======================================================== TMA producer, B operand (weights)
+      int sb = 0;
+      uint32_t pb = 0;
+      for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
+        const TileCoord tc = tile_coord(p, tile);
+        const int nt = tc.nt, tn = tc.tn;
+        const int bz = p.b_batched ? tn * p.NB : 0;
+        const int b_n = bz / p.b_heads, b_h = bz % p.b_heads;
+        for (int e = 0; e < p.n_sched; ++e) {
+          const int s = p.sched[e] >> 6, ch = p.sched[e] & 63;
+          const ConvSegDev sg = p.seg[s];
+          const int ncopies = (sg.mode == 0 || sg.mode == 3) ? 1 : (sg.mode == 1 ? 3 : 9);
+          const int ntaps = sg.mode == 1 ? 3 : (sg.mode == 3 ? (p.up2 ? 4 : 9) : 1);
+          for (int cp = 0; cp < ncopies; ++cp) {
+            for (int tp = 0; tp < ntaps; ++tp) {
+              // tap index in the weight matrix: ky*3+kx (up2: dy*2+dx of the phase's 2x2 kernel; the weight rows
+              // nt*BN already select the phase)
+              const int tap = sg.mode == 0 ? 0 : (sg.mode == 1 ? tp * 3 + cp : (sg.mode == 3 ? tp : cp));
+              mbar_wait_suspend(&emptyB[sb], pb ^ 1);
+              if (elect_one()) {
+                mbar_arrive_expect_tx(&fullB[sb], kBStage);
+                tma_load_4d(sB + sb * kBStage, &p.tmB, &fullB[sb], sg.kbase + tap * sg.C + ch * 64, nt * BN, b_h, b_n);
+              }
+              if (++sb == p.b_stages) { sb = 0; pb ^= 1; }
             }
-            if (++sb == p.b_stages) { sb = 0; pb ^= 1; }
           }
         }
       }
     }
   } else if (warp >= kWarpT) {
+    setmaxnreg_inc<kRegsTransform>();
     // ======================================================== operand transform (in place) + epilogue warps
     constexpr int kLanes = kNumTransformWarps * 4;  // pixels handled concurrently (8 threads per pixel)
     const int NB = PLAIN ? 1 : p.NB;                // samples per tile
@@ -687,22 +701,25 @@ __global__ void __launch_bounds__(kNumThreads, 1) conv_gemm_kernel(const __grid_
 #pragma unroll 1
         for (int sub = 0; sub < MT; ++sub) {
           float lv[kLog + 1][8];
+          // Two rows in flight: the staged accumulators and the residual of the next row are loaded before the current
+          // row's arithmetic and store, so a row's shared- and global-memory latencies overlap the row before it.
           Px wn = row_px(sub, 0);
-          uint4 un = load_res(wn);  // residual of the next row: in flight while the current row is computed
+          uint4 un = load_res(wn);
+          uint32_t rn[8];
+          ld_staged<8>(row_addr(sub, 0), rn);
 #pragma unroll
           for (int t = 0; t < kNI; ++t) {
             const int i = bit_reverse(t, kLog);
             const Px w = wn;
             const uint4 u = un;
+            float v[8];
+#pragma unroll
+            for (int k = 0; k < 8; ++k) v[k] = __uint_as_float(rn[k]);
             if (t + 1 < kNI) {
               wn = row_px(sub, bit_reverse(t + 1, kLog));
               un = load_res(wn);
+              ld_staged<8>(row_addr(sub, bit_reverse(t + 1, kLog)), rn);
             }
-            uint32_t r[8];
-            ld_staged<8>(row_addr(sub, i), r);
-            float v[8];
-#pragma unroll
-            for (int k = 0; k < 8; ++k) v[k] = __uint_as_float(r[k]);
             if (p.ebias != nullptr) {
               if (eb_rows) load_bias(w.valid ? w.n : 0);
 #pragma unroll

@@ -200,6 +200,19 @@ __device__ __forceinline__ uint64_t gmma_desc(uint32_t lo, uint32_t hi) {
 __device__ __forceinline__ void pdl_trigger() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
 
+// ---------------------------------------------------------------- per-warpgroup register budget
+// setmaxnreg: every warp of a warpgroup executes the same instruction.  dec returns registers above N to the CTA's
+// pool; inc blocks until the pool (what the launch allocated, minus what other warpgroups hold) can raise this
+// warpgroup to N.  N is a multiple of 8 in [24, 256]; ptxas allocates the code that follows under the new limit.
+template <int N>
+__device__ __forceinline__ void setmaxnreg_dec() {
+  asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N));
+}
+template <int N>
+__device__ __forceinline__ void setmaxnreg_inc() {
+  asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N));
+}
+
 // ---------------------------------------------------------------- misc
 __device__ __forceinline__ void named_bar_sync(uint32_t id, uint32_t nthreads) {
   asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");

@@ -101,6 +101,15 @@ SIGNATURES = {
     "asyrp_clip_image_patches": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p]),
     "asyrp_clip_image_tokens": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p]),
     "asyrp_clip_direction": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_float, c_void_p]),
+    "asyrp_arcface_preprocess": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p]),
+    "asyrp_arcface_conv": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int,
+                                   c_int, c_int, c_int, c_void_p]),
+    "asyrp_arcface_affine": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, C.c_longlong, c_int, c_void_p]),
+    "asyrp_arcface_se_scale": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p]),
+    "asyrp_arcface_se_apply": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int,
+                                       c_int, c_int, c_int, c_int, c_int, c_int, c_void_p]),
+    "asyrp_arcface_l2norm": (c_int, [c_void_p, c_void_p, c_int, c_int, c_void_p]),
+    "asyrp_arcface_dot": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p]),
 }
 
 _lib = None

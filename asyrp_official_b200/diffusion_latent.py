@@ -13,6 +13,9 @@ Mirrors, with the same attribute / flag names:
                                                             inversion, which set_t_edit_t_addnoise reads
   --DirectionalClipSmilarity   main.py:101, losses/clip_loss.py  run_test scores every edit with CLIPLoss's directional
                                                             similarity (clip_image.CLIPLoss), written next to the PNG
+  --id_similarity              losses/id_loss.py            run_test scores every edit with 1 - IDLoss (ArcFace IR-SE50,
+                                                            arcface.ArcFace), written next to the PNG; the reference
+                                                            uses IDLoss only in training
 
 Differences (documented in INTEGRATION.md): the reverse loop is UNetEngine.sample() — one CUDA graph per
 (batch, schedule) instead of 40 Python iterations; pretrained weights come from --model_path (no URL download);
@@ -61,6 +64,7 @@ class Asyrp(object):
         self.rank = int(os.environ.get("RANK", "0"))
         self.world = int(os.environ.get("WORLD_SIZE", "1"))
         self.directional_clip = {}  # --DirectionalClipSmilarity: save_image's file name -> S_dir [tuples][images]
+        self.id_similarity = {}  # --id_similarity: save_image's file name -> 1 - IDLoss [tuples][images]
 
     # ------------------------------------------------------------------------------------------
     def load_pretrained_model(self):
@@ -181,15 +185,33 @@ class Asyrp(object):
     def write_directional_clip(self, path, coeffs, s_dir):
         """the TSV of one batch: one row per (hs_coeff tuple, image) in grid order, S_dir = 1 -
         clip_directional_loss of that row; prints each tuple's mean"""
-        with open(path, "w") as f:
-            f.write("image\ttuple\ths_coeff\tS_dir\n")
-            for k, row in enumerate(s_dir.tolist()):
-                tup = ",".join(f"{float(c):.6g}" for c in coeffs[k])
-                for i, v in enumerate(row):
-                    f.write(f"{i}\t{k}\t{tup}\t{v!r}\n")
-        for k, row in enumerate(s_dir):
-            print(f"directional CLIP similarity, hs_coeff {tuple(float(c) for c in coeffs[k])}: mean "
-                  f"{row.double().mean().item():.6f} over {row.numel()} images")
+        write_scores(path, coeffs, s_dir, "S_dir", "directional CLIP similarity")
+
+    def id_similarity_setup(self):
+        """--id_similarity's requirements, checked before any model is loaded; raises ValueError with the reason.
+        Returns the validated --id_weights state dict (arcface.load_state_dict)."""
+        from .arcface import check_image_size, load_state_dict
+        a = self.args
+        if getattr(a, "pass_editing", False):
+            raise ValueError("--id_similarity scores the edited images: with --pass_editing nothing is edited")
+        size = self.config.data.image_size
+        try:
+            check_image_size(size, size)
+        except ValueError as e:
+            raise ValueError(f"--id_similarity: {e}") from None
+        path = getattr(a, "id_weights", None)
+        if not path or not os.path.isfile(path):
+            raise ValueError(f"--id_similarity: --id_weights {path!r} is not a file (the reference's "
+                             "pretrained/model_ir_se50.pth)")
+        try:
+            return load_state_dict(path)
+        except ValueError as e:
+            raise ValueError(f"--id_similarity: {e}") from None
+
+    def write_id_similarity(self, path, coeffs, ids):
+        """the TSV of one batch: one row per (hs_coeff tuple, image) in grid order, ID = 1 - IDLoss(origin, edit) of
+        that row; prints each tuple's mean"""
+        write_scores(path, coeffs, ids, "ID", "identity similarity")
 
     @torch.no_grad()
     def clip_cosines(self, pairs):
@@ -364,7 +386,8 @@ class Asyrp(object):
     @torch.no_grad()
     def save_image(self, model, x_lat_tensor, seq_inv, seq_inv_next, save_x0=False, save_x_origin=False,
                    save_process_delta_h=False, save_process_origin=False, x0_tensor=None, delta_h_dict=None,
-                   get_delta_hs=False, folder_dir="", file_name="", hs_coeff=(1.0, 1.0), directional_clip=None):
+                   get_delta_hs=False, folder_dir="", file_name="", hs_coeff=(1.0, 1.0), directional_clip=None,
+                   id_scorer=None):
         """rows of the grid: [x0] [origin DDIM] one row per hs_coeff tuple  (diffusion_latent.py:445-544).
 
         delta_h_dict: {t: None | Δh tensor}.  Entries that are tensors select the explicit-Δh branch for that step
@@ -373,7 +396,10 @@ class Asyrp(object):
         directional_clip: (CLIPLoss, src_txt, trg_txt) for --DirectionalClipSmilarity: every tuple's edited rows are
         scored against the origin pass of the same x_T (run for this even without save_x_origin, then left out of the
         grid), written to <file_name>_ngen<n_train_step>_directional_clip.tsv and kept in
-        self.directional_clip[file_name]."""
+        self.directional_clip[file_name].
+        id_scorer: an arcface.ArcFace for --id_similarity: the same for 1 - IDLoss against the same origin pass (which
+        runs once for both scores), written to <file_name>_ngen<n_train_step>_id_similarity.tsv and kept in
+        self.id_similarity[file_name]."""
         import torchvision.utils as tvu
         a = self.args
         time_s = time.time()
@@ -382,7 +408,7 @@ class Asyrp(object):
         x_list, edited = [], []
         if save_x0 and x0_tensor is not None:
             x_list.append(x0_tensor.cpu())
-        if save_x_origin or directional_clip is not None:
+        if save_x_origin or directional_clip is not None or id_scorer is not None:
             sch = self.make_schedule(seq_inv, seq_inv_next, (1.0,), edit=False,
                                      addnoise=bool(getattr(a, "origin_process_addnoise", False)))
             if save_x_origin:
@@ -462,6 +488,11 @@ class Asyrp(object):
             self.directional_clip[file_name] = s_dir
             self.write_directional_clip(
                 os.path.join(folder_dir, f'{file_name}_ngen{a.n_train_step}_directional_clip.tsv'), coeffs, s_dir)
+        if id_scorer is not None and edited:
+            ids = id_scorer.id_similarity(origin, torch.cat(edited)).view(len(edited), bs)
+            self.id_similarity[file_name] = ids
+            self.write_id_similarity(
+                os.path.join(folder_dir, f'{file_name}_ngen{a.n_train_step}_id_similarity.tsv'), coeffs, ids)
         print(f'{time.time() - time_s} seconds, {file_name}_ngen{a.n_train_step}.png is saved')
         return x_list
 
@@ -551,6 +582,7 @@ class Asyrp(object):
             print("--warigari is accepted and has no effect (the reference's branch returns the same values, "
                   "utils/diffusion_utils.py:103-109)")
         sdir = self.directional_clip_setup() if getattr(a, "DirectionalClipSmilarity", False) else None
+        id_sd = self.id_similarity_setup() if getattr(a, "id_similarity", False) else None
         if a.multiple_attr and self.needs_clip() and self.clip_configured():
             cosine = self.choose_attribute(a.multiple_attr.split(' '))  # :640-652
             self.set_t_edit_t_addnoise(LPIPS_th=a.lpips_edit_th, LPIPS_addnoise_th=a.lpips_addnoise_th, cosine=cosine)
@@ -668,11 +700,15 @@ class Asyrp(object):
         if getattr(a, "target_image_id", None):
             target_ids = [int(i) for i in str(a.target_image_id).split(" ")]
             assert a.bs_train == 1, "target_image_id is only supported for batch_size == 1"
-        results, directional_clip = {}, None
+        results, directional_clip, id_scorer = {}, None, None
         if sdir is not None:  # the image tower lives for this run_test only
             from .clip_image import CLIPLoss
             directional_clip = (CLIPLoss(a.clip_weights, a.clip_vocab, sdir[2], device=self.device), sdir[0], sdir[1])
         try:
+            if id_sd is not None:  # so does ArcFace
+                from .arcface import ArcFace
+                id_scorer = ArcFace(id_sd, device=self.device)
+                id_sd = None
             for mode, do, n_img in (("train", a.do_train, a.n_train_img), ("test", a.do_test, a.n_test_img)):
                 if not do:
                     continue
@@ -695,7 +731,7 @@ class Asyrp(object):
                             save_process_origin=bool(getattr(a, "save_process_origin", False)),
                             save_process_delta_h=bool(getattr(a, "save_process_delta_h", False)),
                             folder_dir=a.test_image_folder, file_name=f'{mode}_{step}_{a.n_iter - 1}', hs_coeff=hs_coeff,
-                            directional_clip=directional_clip)
+                            directional_clip=directional_clip, id_scorer=id_scorer)
                     batch_idx += 1
                     if step == n_img - 1:
                         break
@@ -719,11 +755,25 @@ class Asyrp(object):
                     x_lat_tensor, x0_tensor = None, None
         finally:
             a.train_delta_h = a_train_delta_h_prev
-            if directional_clip is not None:
-                del directional_clip
+            if directional_clip is not None or id_scorer is not None:
+                del directional_clip, id_scorer
                 torch.cuda.empty_cache()
         self.last_delta_h_dict = delta_h_dict
         return results
+
+
+def write_scores(path, coeffs, scores, column, label):
+    """a per-edit score table: one row per (hs_coeff tuple, image) in grid order, columns image, tuple, hs_coeff and
+    `column`; prints each tuple's mean as `label`"""
+    with open(path, "w") as f:
+        f.write(f"image\ttuple\ths_coeff\t{column}\n")
+        for k, row in enumerate(scores.tolist()):
+            tup = ",".join(f"{float(c):.6g}" for c in coeffs[k])
+            for i, v in enumerate(row):
+                f.write(f"{i}\t{k}\t{tup}\t{v!r}\n")
+    for k, row in enumerate(scores):
+        print(f"{label}, hs_coeff {tuple(float(c) for c in coeffs[k])}: mean {row.double().mean().item():.6f} over "
+              f"{row.numel()} images")
 
 
 def plan_sweep(n_tuples, bs, max_rows):

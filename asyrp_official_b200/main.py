@@ -98,6 +98,11 @@ def build_parser():
     p.add_argument('--text_templates', type=str, default=None,
                    help='file defining imagenet_templates, read with ast, for --DirectionalClipSmilarity (default '
                         'utils/text_templates.py)')
+    p.add_argument('--id_similarity', **sa,
+                   help='--run_test: score every edit for identity preservation, 1 - IDLoss (ArcFace IR-SE50) against '
+                        'the unedited DDIM pass of the same x_T, written next to the PNG')
+    p.add_argument('--id_weights', type=str, default='pretrained/model_ir_se50.pth',
+                   help="the reference's ArcFace weights (MODEL_PATHS['ir_se50']) for --id_similarity")
     p.add_argument('--lpips_table_dir', type=str,
                    help='directory with <config stem>_LPIPS_distance_{x,x0_t}.tsv (read by --run_test, written by '
                         '--lpips; default utils)')

@@ -499,6 +499,87 @@ def clip_cosine(a, b, out, eps=1e-6):
     check(lib.asyrp_clip_cosine(_ptr(a), _ptr(b), _ptr(out), n, dim, float(eps), _stream()), "asyrp_clip_cosine")
 
 
+def arcface_preprocess(x, out):
+    """IDLoss's crop x[:, :, 35:223, 32:220] and AdaptiveAvgPool2d(112): x fp32 [B][3][H][W] -> out fp32 NHWC
+    [B][112][112][4], channel 3 zero"""
+    lib = _lib.load()
+    B, C, H, W = x.shape
+    _need_cuda(x, out)
+    assert C == 3 and x.dtype == torch.float32 and x.is_contiguous() and tuple(out.shape) == (B, 112, 112, 4)
+    check(lib.asyrp_arcface_preprocess(_ptr(x), _ptr(out), B, H, W, _stream()), "asyrp_arcface_preprocess")
+
+
+def arcface_conv(inp, weight, bias, out, k, stride, pad, prelu=None):
+    """out = conv(inp) + bias (bias may be None), then PReLU with per-channel slopes when prelu is given; fp32 NHWC,
+    TF32 tensor cores; weight from pack_lpips_conv_weight"""
+    lib = _lib.load()
+    N, H, W, cin = inp.shape
+    cout = out.shape[-1]
+    _need_cuda(inp, weight, bias, out, prelu)
+    assert inp.is_contiguous() and out.is_contiguous()
+    assert tuple(weight.shape) == (cout, lpips_conv_kpad(cin, k, k)) and weight.dtype == torch.float32
+    assert tuple(out.shape) == (N, (H + 2 * pad - k) // stride + 1, (W + 2 * pad - k) // stride + 1, cout)
+    check(lib.asyrp_arcface_conv(_ptr(inp), _ptr(weight), _ptr(bias), _ptr(prelu), _ptr(out), N, H, W, cin, cout, k,
+                                 stride, pad, _stream()), "asyrp_arcface_conv")
+
+
+def arcface_affine(inp, scale, shift, out):
+    """out = inp * scale[c] + shift[c] over the last dim of fp32 inp"""
+    lib = _lib.load()
+    C = inp.shape[-1]
+    _need_cuda(inp, scale, shift, out)
+    assert inp.is_contiguous() and out.is_contiguous() and out.shape == inp.shape
+    assert scale.numel() == C and shift.numel() == C
+    check(lib.asyrp_arcface_affine(_ptr(inp), _ptr(scale), _ptr(shift), _ptr(out), inp.numel() // C, C, _stream()),
+          "asyrp_arcface_affine")
+
+
+def arcface_se_scale(res, fc1, fc2, scale):
+    """SEModule's gate: scale [N][C] = sigmoid(fc2 relu(fc1 mean_hw(res))) of res [N][H][W][C]; fc1 [C/16][C],
+    fc2 [C][C/16]"""
+    lib = _lib.load()
+    N, H, W, C = res.shape
+    _need_cuda(res, fc1, fc2, scale)
+    assert res.is_contiguous() and tuple(fc1.shape) == (C // 16, C) and tuple(fc2.shape) == (C, C // 16)
+    assert fc1.is_contiguous() and fc2.is_contiguous() and tuple(scale.shape) == (N, C)
+    check(lib.asyrp_arcface_se_scale(_ptr(res), _ptr(fc1), _ptr(fc2), _ptr(scale), N, H * W, C, _stream()),
+          "asyrp_arcface_se_scale")
+
+
+def arcface_se_apply(res, scale, shortcut, out, stride=1, bn=None, out2=None):
+    """out = res * scale[n][c] + shortcut[:, ::stride, ::stride]; with bn = (scale, shift) also out2 = out * bn_scale +
+    bn_shift (the next block's pre-conv BatchNorm)"""
+    lib = _lib.load()
+    N, Ho, Wo, C = res.shape
+    _, Hs, Ws, Cs = shortcut.shape
+    bs, bt = bn if bn is not None else (None, None)
+    _need_cuda(res, scale, shortcut, out, bs, bt, out2)
+    assert Cs == C and shortcut.shape[0] == N and res.is_contiguous() and shortcut.is_contiguous()
+    assert out.shape == res.shape and out.is_contiguous() and tuple(scale.shape) == (N, C)
+    assert (bn is None) == (out2 is None) and (out2 is None or (out2.shape == res.shape and out2.is_contiguous()))
+    check(lib.asyrp_arcface_se_apply(_ptr(res), _ptr(scale), _ptr(shortcut), _ptr(out), _ptr(bs), _ptr(bt), _ptr(out2),
+                                     N, Ho, Wo, C, Hs, Ws, stride, _stream()), "asyrp_arcface_se_apply")
+
+
+def arcface_l2norm(x, out):
+    """out = x / |x| per row of fp32 [rows][dim] (no epsilon); out must not be x"""
+    lib = _lib.load()
+    rows, dim = x.shape
+    _need_cuda(x, out)
+    assert x.is_contiguous() and out.is_contiguous() and out.shape == x.shape and out.data_ptr() != x.data_ptr()
+    check(lib.asyrp_arcface_l2norm(_ptr(x), _ptr(out), rows, dim, _stream()), "asyrp_arcface_l2norm")
+
+
+def arcface_dot(src, edited, out):
+    """out[j] = edited[j] . src[j % B]; src [B][dim], edited [n][dim] fp32"""
+    lib = _lib.load()
+    B, dim = src.shape
+    n = edited.shape[0]
+    _need_cuda(src, edited, out)
+    assert src.is_contiguous() and edited.is_contiguous() and edited.shape[1] == dim and out.numel() >= n
+    check(lib.asyrp_arcface_dot(_ptr(src), _ptr(edited), _ptr(out), n, B, dim, _stream()), "asyrp_arcface_dot")
+
+
 def ddpm_update(x, et, z, x_next, at, bt, logvar, learned_sigma, mask):
     lib = _lib.load()
     N, Cx, H, W = x.shape

@@ -46,6 +46,37 @@ def clip_image_state_dict(seed=1234, width=768, layers=12, patch=16, grid=14, em
     return sd
 
 
+def arcface_state_dict(seed=1234):
+    """seeded ArcFace Backbone(112, 50, 'ir_se') weights in its state-dict layout (asyrp_official_b200.arcface), every
+    term non-degenerate: convs U(-b, b) with b = 1.5 fan_in^-1/2 (at torch's default b = fan_in^-1/2 the BatchNorm
+    shifts drown an image in [-1, 1] and unrelated images score ID ~.997; at Kaiming's (6 / fan_in)^1/2 the 24 blocks
+    amplify TF32 rounding into a different feature), the linear layer and its bias U(-b, b), b = fan_in^-1/2; BatchNorms
+    weight 1 + N(0, .1^2), bias, running_mean N(0, .1^2), running_var exp(N(0, .2^2)) > 0; PReLU slopes
+    .25 + N(0, .05^2); num_batches_tracked 0 (ignored by eval-mode BatchNorm)"""
+    from .arcface import _bn_prefixes, state_dict_shapes
+    sd = {}
+    for name, shp in state_dict_shapes().items():
+        g = torch.Generator()
+        g.manual_seed((zlib.crc32(name.encode()) ^ (seed * 0x9E3779B1)) & 0x7FFFFFFF)
+        if name == "output_layer.3.bias":
+            sd[name] = (torch.rand(shp, generator=g) * 2 - 1) * (512 * 49) ** -0.5
+        elif name == "output_layer.3.weight":
+            sd[name] = (torch.rand(shp, generator=g) * 2 - 1) * shp[1] ** -0.5
+        elif len(shp) >= 2:
+            sd[name] = (torch.rand(shp, generator=g) * 2 - 1) * 1.5 * math.prod(shp[1:]) ** -0.5
+        elif name.endswith("running_var"):
+            sd[name] = torch.exp(0.2 * torch.randn(shp, generator=g))
+        elif name.endswith(".weight") and ".res_layer.2." in name or name == "input_layer.2.weight":
+            sd[name] = 0.25 + 0.05 * torch.randn(shp, generator=g)
+        elif name.endswith(".weight"):
+            sd[name] = 1.0 + 0.1 * torch.randn(shp, generator=g)
+        else:
+            sd[name] = 0.1 * torch.randn(shp, generator=g)
+    for prefix in _bn_prefixes():
+        sd[prefix + ".num_batches_tracked"] = torch.tensor(0, dtype=torch.long)
+    return sd
+
+
 def _draw_clip(shapes, prefix, std, width, layers, seed):
     """CLIP weights of `shapes` (names without `prefix`), each from its own generator seeded by crc32(prefix + name)"""
     std = {**std, "attn.in_proj_weight": width ** -0.5, "attn.out_proj.weight": width ** -0.5 * (2 * layers) ** -0.5,

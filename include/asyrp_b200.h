@@ -295,6 +295,37 @@ int asyrp_clip_attention_full(const float* qkv, float* out, int P, int T, int he
 int asyrp_clip_direction(const float* src, const float* trg, float* out, int groups, int n, int dim, float add_eps,
                          void* stream);
 
+/* ---- ArcFace IR-SE50 and the identity similarity: the reference's Backbone(112, 50, 'ir_se') and IDLoss
+ * (models/insight_face/model_irse.py, losses/id_loss.py).  Activations are fp32 NHWC.
+ * asyrp_arcface_preprocess: IDLoss.extract_feats's crop x[:, :, 35:223, 32:220] and AdaptiveAvgPool2d((112, 112)):
+ *   x fp32 NCHW [B][3][H][W] (H >= 223, W >= 220) -> out fp32 NHWC [B][112][112][4], channel 3 zero.  Bin i covers
+ *   crop rows [floor(188 i / 112), ceil(188 (i+1) / 112)), likewise columns; summed row by row, left to right.
+ * asyrp_arcface_conv: out = epilogue(conv(in) + bias), k x k, zero padding `pad`, any stride, the LPIPS conv's TF32
+ *   implicit GEMM; prelu null: bias alone (bias may be null), else PReLU with per-channel slopes prelu [Cout] (bias
+ *   may be null).  in [N][H][W][Cin] (Cin % 4 == 0), out [N][Ho][Wo][Cout] (Cout % 64 == 0), weight fp32
+ *   [Cout][asyrp_lpips_conv_kpad(Cin, k, k)].
+ * asyrp_arcface_affine: out = in * scale[c] + shift[c] over [rows][C] (C % 4 == 0): a folded eval-mode BatchNorm.
+ * asyrp_arcface_se_scale: SEModule's gate, one CTA per sample: scale[n][c] = sigmoid(fc2 relu(fc1 mean_hw(res[n])))
+ *   with res [N][HW][C], fc1 [C/16][C], fc2 [C][C/16]; C a multiple of 16 that divides 512.
+ * asyrp_arcface_se_apply: out = res * scale[n][c] + shortcut[n][y*ss][x*ss][c], res and out [N][Ho][Wo][C], shortcut
+ *   [N][Hs][Ws][C], ss 1 (identity, conv shortcut) or 2 (MaxPool2d(1, 2)); out2 (optional, with bn_scale / bn_shift
+ *   [C]) = out * bn_scale + bn_shift, the next block's pre-conv BatchNorm.
+ * asyrp_arcface_l2norm: out[r] = in[r] / |in[r]| (no epsilon) over [rows][dim]; out must not alias in.
+ * asyrp_arcface_dot: id[j] = edited[j] . src[j % B] over rows of dim floats (IDLoss = 1 - id).
+ * Fixed-order reductions, no float atomics, no kernel mixes samples. */
+int asyrp_arcface_preprocess(const float* x, float* out, int B, int H, int W, void* stream);
+int asyrp_arcface_conv(const float* in, const float* weight, const float* bias, const float* prelu, float* out, int N,
+                       int H, int W, int Cin, int Cout, int k, int stride, int pad, void* stream);
+int asyrp_arcface_affine(const float* in, const float* scale, const float* shift, float* out, long long rows, int C,
+                         void* stream);
+int asyrp_arcface_se_scale(const float* res, const float* fc1, const float* fc2, float* scale, int N, int HW, int C,
+                           void* stream);
+int asyrp_arcface_se_apply(const float* res, const float* scale, const float* shortcut, float* out,
+                           const float* bn_scale, const float* bn_shift, float* out2, int N, int Ho, int Wo, int C,
+                           int Hs, int Ws, int ss, void* stream);
+int asyrp_arcface_l2norm(const float* in, float* out, int rows, int dim, void* stream);
+int asyrp_arcface_dot(const float* src, const float* edited, float* id, int n, int B, int dim, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -16,7 +16,9 @@ namespace asyrp {
 namespace {
 
 constexpr int kDirThreads = 256;
-constexpr int kDirSmemFloats = 12288;  // 48 KB: 2 * rows per group + dim, no opt-in needed
+// 48 KB of dynamic shared memory (2 * rows per group + dim floats); with the kernel's static red[] that is past the
+// default 48 KB per block, so the launch opts in
+constexpr int kDirSmemFloats = 12288;
 // CLIP's Normalize
 __constant__ float kClipMean[3] = {0.48145466f, 0.4578275f, 0.40821073f};
 __constant__ float kClipStd[3] = {0.26862954f, 0.26130258f, 0.27577711f};
@@ -192,6 +194,8 @@ ASYRP_API int asyrp_clip_direction(const float* src, const float* trg, float* ou
                 kDirSmemFloats);
   ASYRP_REQUIRE(add_eps >= 0.f, "asyrp_clip_direction: add_eps=%g must be >= 0", add_eps);
   const size_t smem = static_cast<size_t>(2 * n + dim) * sizeof(float);
+  ASYRP_CHECK_CUDA(cudaFuncSetAttribute(clip_direction_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                        kDirSmemFloats * static_cast<int>(sizeof(float))));
   ASYRP_LAUNCH(clip_direction_kernel, dim3(groups), dim3(kDirThreads), smem, static_cast<cudaStream_t>(stream), src,
                trg, out, n, dim, add_eps);
   ASYRP_CHECK_CUDA(cudaGetLastError());

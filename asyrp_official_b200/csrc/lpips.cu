@@ -163,6 +163,8 @@ ASYRP_API int asyrp_lpips_conv(const float* in, const float* weight, const float
   ASYRP_REQUIRE(Cin > 0 && Cin % 4 == 0, "asyrp_lpips_conv: Cin=%d must be a positive multiple of 4", Cin);
   ASYRP_REQUIRE(Cout > 0 && Cout % kBN == 0, "asyrp_lpips_conv: Cout=%d must be a positive multiple of %d", Cout, kBN);
   ASYRP_REQUIRE(kh > 0 && kw > 0 && stride > 0 && pad >= 0, "asyrp_lpips_conv: bad kernel geometry");
+  ASYRP_REQUIRE(bias != nullptr, "asyrp_lpips_conv: the ReLU epilogue needs a bias");
+  ASYRP_REQUIRE(in != out, "asyrp_lpips_conv: out must not alias in");
   tf32gemm::Tf32ConvParams p;
   p.in = in; p.w = weight; p.bias = bias; p.residual = nullptr; p.out = out;
   p.N = N; p.H = H; p.W = W; p.Cin = Cin; p.Cout = Cout; p.kw = kw; p.stride = stride; p.pad = pad;

@@ -342,6 +342,7 @@ def lpips_conv(inp, weight, bias, out, kh, kw, stride, pad):
     N, H, W, cin = inp.shape
     cout = out.shape[-1]
     _need_cuda(inp, weight, bias, out)
+    assert inp.is_contiguous() and out.is_contiguous() and weight.is_contiguous()
     assert tuple(weight.shape) == (cout, lpips_conv_kpad(cin, kh, kw)) and weight.dtype == torch.float32
     assert tuple(out.shape) == (N, (H + 2 * pad - kh) // stride + 1, (W + 2 * pad - kw) // stride + 1, cout)
     check(lib.asyrp_lpips_conv(_ptr(inp), _ptr(weight), _ptr(bias), _ptr(out), N, H, W, cin, cout, kh, kw, stride, pad,
@@ -516,7 +517,7 @@ def arcface_conv(inp, weight, bias, out, k, stride, pad, prelu=None):
     N, H, W, cin = inp.shape
     cout = out.shape[-1]
     _need_cuda(inp, weight, bias, out, prelu)
-    assert inp.is_contiguous() and out.is_contiguous()
+    assert inp.is_contiguous() and out.is_contiguous() and weight.is_contiguous()
     assert tuple(weight.shape) == (cout, lpips_conv_kpad(cin, k, k)) and weight.dtype == torch.float32
     assert tuple(out.shape) == (N, (H + 2 * pad - k) // stride + 1, (W + 2 * pad - k) // stride + 1, cout)
     check(lib.asyrp_arcface_conv(_ptr(inp), _ptr(weight), _ptr(bias), _ptr(prelu), _ptr(out), N, H, W, cin, cout, k,

@@ -229,7 +229,7 @@ int asyrp_softmax_rows(const void* S, void* P, long long rows, int T, float scal
  * asyrp_lpips_conv: out = relu(conv(in) + bias), zero padding `pad`, any kh x kw and stride; implicit GEMM on the tensor
  *   cores with TF32 operands (round to nearest) and fp32 accumulation.  in [N][H][W][Cin] (Cin % 4 == 0), out
  *   [N][Ho][Wo][Cout] (Cout % 64 == 0), weight fp32 [Cout][asyrp_lpips_conv_kpad(Cin, kh, kw)]: K = kh*kw*Cin
- *   tap-major / channel-minor, zero columns past K.
+ *   tap-major / channel-minor, zero columns past K.  bias [Cout] is required; out must not alias in.
  * asyrp_lpips_maxpool: MaxPool2d(3, 2), no padding, floor mode, [N][H][W][C] -> [N][(H-3)/2+1][(W-3)/2+1][C].
  * asyrp_lpips_distance: one layer term of the distance: per pixel, f/(sqrt(sum_c f^2) + 1e-10) of probe row n and of
  *   ref row n % B, squared difference, lin_w [C] (the 1x1 conv C -> 1), mean over the HW pixels; d[n] = term

@@ -51,7 +51,7 @@ def test_preprocess_and_patches(cuda_device, S, P, G):
     assert torch.equal(out[:, 3 * P * P:], torch.zeros(3 * G * G, kpad - 3 * P * P))
 
 
-@pytest.mark.parametrize("T", [50, 197, 257])
+@pytest.mark.parametrize("T", [50, 197, 257, 1, 33])
 def test_full_attention(cuda_device, T):
     heads, P = 12, 3
     w = 64 * heads

@@ -99,10 +99,12 @@ def test_linear_epilogues(cuda_device, epi):
         assert ((o2.cpu().double() - ref2).abs() <= bound + 1e-6 * (1 + ref2.abs())).all()
 
 
-@pytest.mark.parametrize("heads", [8, 12])
-def test_causal_attention(cuda_device, heads):
-    g = _g(heads)
-    P, T, w = 3, 77, 64 * heads
+@pytest.mark.parametrize("heads,T", [pytest.param(8, 77, id="8"), pytest.param(12, 77, id="12"),
+                                     pytest.param(8, 1, id="8-T1"), pytest.param(8, 33, id="8-T33"),
+                                     pytest.param(12, 128, id="12-T128")])  # T <= 128: the most the kernel admits
+def test_causal_attention(cuda_device, heads, T):
+    g = _g(heads + T)
+    P, w = 3, 64 * heads
     qkv = torch.randn(P, T, 3 * w, generator=g) * 2
     out = torch.empty(P, T, w, device=cuda_device)
     ops.clip_attention(qkv.to(cuda_device), out, heads)

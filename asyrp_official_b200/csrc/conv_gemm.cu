@@ -1204,8 +1204,8 @@ struct AsyrpConvDesc {
 
 static void conv_tile_shape(int H, int W, int halo, int* TW, int* TH, int* NB);
 
-// The fused operand transform evaluates SiLU with ONE special-function op (tanh.approx.f32, 11 bits: absolute error
-// <= 2^-12 |x|, the size of the fp16 rounding the operand receives anyway) instead of ex2 + rcp: 4 instead of 7.5
+// The fused operand transform evaluates SiLU with ONE special-function op (tanh.approx.f32, 11 bits: error <= 2^-12 |x|,
+// absolute in |x|, not relative to the result: see silu_tanh_half) instead of ex2 + rcp: 4 instead of 7.5
 // instructions per element on the transform warps, whose work per 3x3 stage is comparable to that stage's MMAs.
 // ASYRP_SILU_TANH=0 / asyrp_set_silu_tanh(0): the 2-MUFU form.
 static int g_silu_tanh = -1;

@@ -228,8 +228,9 @@ __device__ __forceinline__ float silu_fast(float x) {
 }
 
 // SiLU from ONE special-function op: with h = x/2, x*sigmoid(x) = h + h*tanh(h).  tanh.approx.f32 carries 11 bits
-// (max relative error 2^-11): the absolute error is <= 2^-12 |x|, the size of the fp16 rounding the operand gets
-// anyway.  Takes h, not x: callers fold the 1/2 into the affine that precedes the activation.
+// (max relative error 2^-11): the error is <= 2^-12 |x|, absolute in |x| and not relative to the result, so in the
+// negative tail it is far above the result's fp16 rounding (x = -6: up to 1.5e-3 on silu = -0.0148).  Takes h, not x:
+// callers fold the 1/2 into the affine that precedes the activation.
 __device__ __forceinline__ float silu_tanh_half(float h) {
   float t;
   asm("tanh.approx.f32 %0, %1;" : "=f"(t) : "f"(h));

@@ -292,6 +292,7 @@ def slerp_h(h, dh, h2, stats, t, use_mask=False):
     """h2 = slerp(t, h, |h|*dh/|dh|): h, h2 NHWC fp16; dh fp32 [C][H][W] (shared) or [N][C][H][W]; stats [N][T][C/2][2]"""
     lib = _lib.load()
     N, H, W, Cc = h.shape
+    assert dh.is_contiguous() or (dh.dim() == 4 and dh[0].is_contiguous()), "dh must be dense [C][H][W] per sample"
     stride = dh.stride(0) if dh.dim() == 4 else 0
     check(lib.asyrp_slerp_h(_ptr(h), _ptr(dh), stride, _ptr(h2), _ptr(stats), stats.shape[1], N, Cc, H, W, float(t),
                             int(use_mask), _stream()), "asyrp_slerp_h")

@@ -194,6 +194,8 @@ using namespace asyrp;
 
 extern "C" ASYRP_API int asyrp_transpose_tc(const void* in, void* out, int N, int T, int C, int ld, void* stream) {
   ASYRP_REQUIRE(C % 32 == 0, "asyrp_transpose_tc: C=%d must be a multiple of 32", C);
+  ASYRP_REQUIRE(N >= 1 && N <= kMaxGridYZ, "asyrp_transpose_tc: N=%d out of range (1..%d: the grid's z dimension)", N,
+                kMaxGridYZ);
   dim3 grid((T + 31) / 32, C / 32, N);
   ASYRP_LAUNCH(transpose_tc_kernel, dim3(grid), dim3(256), 0, static_cast<cudaStream_t>(stream), static_cast<const __half*>(in),
                                                                            static_cast<__half*>(out), T, C, ld);
@@ -211,6 +213,9 @@ extern "C" ASYRP_API int asyrp_softmax_rows(const void* S, void* P, long long ro
 
 extern "C" ASYRP_API int asyrp_attention(const void* qkv, void* out, int N, int T, int heads, int head_dim,
                                          float scale, void* stream) {
+  ASYRP_REQUIRE(N >= 1 && N <= kMaxGridYZ && heads >= 1 && heads <= kMaxGridYZ,
+                "asyrp_attention: N=%d, heads=%d out of range (1..%d: the grid's z and y dimensions)", N, heads,
+                kMaxGridYZ);
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   switch (head_dim) {
     case 64: return launch_attention<64>(qkv, out, N, T, heads, scale, st);

@@ -58,6 +58,9 @@ int encode_tensor_map(CUtensorMap* out, CUtensorMapDataType dt, uint32_t rank, c
 
 int sm_count();
 
+// largest grid y / z dimension of a launch; kernels that put the batch there refuse a larger one up front
+constexpr int kMaxGridYZ = 65535;
+
 // Programmatic dependent launch (PDL).  Every kernel of the library starts with `griddepcontrol.launch_dependents`
 // and executes `griddepcontrol.wait` before its first global-memory access; launched with the
 // programmaticStreamSerialization attribute, kernel i+1 is scheduled (and runs its prologue: barrier init,

@@ -27,7 +27,9 @@
 // the epilogue of tile i.
 #include "common.h"
 #include "ptx.cuh"
+#include <algorithm>
 #include <cstring>
+#include <initializer_list>
 #include <memory>
 
 namespace asyrp {
@@ -1324,6 +1326,8 @@ ASYRP_API int asyrp_conv_create(const AsyrpConvDesc* d, void** out_op) {
   ASYRP_REQUIRE(d->Cout % 64 == 0 || (d->Cout == 16 && d->out_planar != nullptr && d->stats == nullptr &&
                                       d->residual == nullptr && !d->up2 && !d->weight_batched),
                 "asyrp_conv_create: Cout=%d must be a multiple of 64 (or 16 with a planar fp32 output)", d->Cout);
+  ASYRP_REQUIRE(d->N >= 1 && d->H >= 1 && d->W >= 1, "asyrp_conv_create: empty geometry N=%d H=%d W=%d", d->N, d->H,
+                d->W);
   // owned here until it is handed out, so that every rejection below frees it
   std::unique_ptr<ConvOp> op(new ConvOp());
   ConvParams& p = op->p;
@@ -1345,14 +1349,21 @@ ASYRP_API int asyrp_conv_create(const AsyrpConvDesc* d, void** out_op) {
   conv_config(d->H, d->W, d->Cout, halo, &op->BN, &op->MT, p.up2 ? 4 : 1);
   p.MT = op->MT;
   const int THT = p.TH * p.MT;
-  p.tiles_x = (d->W + p.TW - 1) / p.TW;
-  p.tiles_y = (d->H + THT - 1) / THT;
-  p.tiles_n = (d->N + p.NB - 1) / p.NB;
-  p.m_tiles = p.tiles_x * p.tiles_y * p.tiles_n;
+  // ceil(a / b) without forming a + b - 1, which overflows int for a near INT_MAX
+  p.tiles_x = (d->W - 1) / p.TW + 1;
+  p.tiles_y = (d->H - 1) / THT + 1;
+  p.tiles_n = (d->N - 1) / p.NB + 1;
   p.n_tiles = (d->Cout / op->BN) * (p.up2 ? 4 : 1);
   {
+    // the tile count, saturated at 2^31 (every factor is below 2^31, so no product overflows 64 bits): the kernel
+    // indexes tiles with int
+    unsigned long long xmax = 1;
+    for (const int f : {p.tiles_x, p.tiles_y, p.tiles_n, p.n_tiles})
+      xmax = std::min(xmax * static_cast<unsigned long long>(f), 1ull << 31);
+    ASYRP_REQUIRE(xmax < (1ull << 31), "asyrp_conv_create: %d x %d x %d x %d tiles exceed the tile-index range",
+                  p.tiles_x, p.tiles_y, p.tiles_n, p.n_tiles);
+    p.m_tiles = p.tiles_x * p.tiles_y * p.tiles_n;
     // x / dv == umulhi(x, 2^32/dv + 1) for all x with x*dv < 2^32; the largest dividend is the tile count
-    const unsigned long long xmax = static_cast<unsigned long long>(p.m_tiles) * p.n_tiles;
     auto magic = [xmax](uint32_t dv) -> uint32_t {
       if (dv <= 1) return 0u;
       if (xmax * dv >= (1ull << 32)) return 1u;
@@ -1361,7 +1372,6 @@ ASYRP_API int asyrp_conv_create(const AsyrpConvDesc* d, void** out_op) {
     p.mul_m = magic(p.m_tiles);
     p.mul_x = magic(p.tiles_x);
     p.mul_xy = magic(p.tiles_x * p.tiles_y);
-    ASYRP_REQUIRE(xmax < (1ull << 31), "asyrp_conv_create: %llu tiles exceed the tile-index range", xmax);
   }
   p.row_bytes = p.NB * p.TW * 128;
   p.nseg = d->nseg;

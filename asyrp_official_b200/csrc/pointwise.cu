@@ -482,6 +482,8 @@ ASYRP_API int asyrp_gn_finalize(const float* st_a, int Ca, int Ta, const float* 
                                 const float* scale_shift, int ss_stride, float* affine, void* stream) {
   const int C = Ca + Cb;
   ASYRP_REQUIRE(C % 64 == 0, "asyrp_gn_finalize: C=%d must be a multiple of 64", C);
+  ASYRP_REQUIRE(N >= 1 && N <= kMaxGridYZ, "asyrp_gn_finalize: N=%d out of range (1..%d: the grid's y dimension)", N,
+                kMaxGridYZ);
   const float count = static_cast<float>(HW) * (C / 32);
   ASYRP_LAUNCH(gn_finalize_kernel, dim3(dim3(32, N)), dim3(256), 0, static_cast<cudaStream_t>(stream), 
       st_a, Ca, Ta, st_b, Cb, Tb, gamma, beta, eps, count, scale_shift, ss_stride, affine);
@@ -492,6 +494,11 @@ ASYRP_API int asyrp_gn_finalize(const float* st_a, int Ca, int Ta, const float* 
 ASYRP_API int asyrp_apply(const void* src_a, int Ca, const void* src_b, int Cb, const float* affine,
                           int affine_stride, void* out, int N, int Hi, int Wi, int act, int resample, void* stream) {
   ASYRP_REQUIRE(Ca % 8 == 0 && Cb % 8 == 0, "asyrp_apply: channels must be multiples of 8");
+  ASYRP_REQUIRE(resample >= 0 && resample <= 2, "asyrp_apply: resample=%d (0 none, 1 avg-pool 2x2, 2 nearest x2)",
+                resample);
+  ASYRP_REQUIRE(act == 0 || act == 1, "asyrp_apply: act=%d (0 none, 1 SiLU)", act);
+  ASYRP_REQUIRE(N >= 1 && N <= kMaxGridYZ, "asyrp_apply: N=%d out of range (1..%d: the grid's y dimension)", N,
+                kMaxGridYZ);
   ApplyParams p;
   p.src_a = static_cast<const __half*>(src_a); p.Ca = Ca;
   p.src_b = static_cast<const __half*>(src_b); p.Cb = Cb;

@@ -346,6 +346,32 @@ __global__ void ddim_update_kernel(const float* __restrict__ x, const float* __r
   }
 }
 
+// Per-row DDIM update: the kernel above with (c1, c2) read per sample from c12 [N][2], so that the rows of one batch can
+// follow different eta schedules (an attribute sweep: every row its own t_addnoise).  Per row the operations, their
+// order and their rounding are those of ddim_update_kernel with that row's scalars; z is read only by rows whose c1 is
+// non-zero (the scalar kernel is launched without z for eta = 0 steps).
+__global__ void ddim_update_rows_kernel(const float* __restrict__ x, const float* __restrict__ et,
+                                        const float* __restrict__ em, const float* __restrict__ z,
+                                        float* __restrict__ x_next, float* __restrict__ x0_out, int N, int Cx, int Ce,
+                                        int HW, float at, float an, const float* __restrict__ c12) {
+  pdl_trigger();
+  pdl_wait();
+  const float sq1 = sqrtf(1.0f - at), sqa = sqrtf(at), sqn = sqrtf(an);
+  const size_t total = static_cast<size_t>(N) * Cx * HW;
+  for (size_t idx = static_cast<size_t>(blockIdx.x) * blockDim.x + threadIdx.x; idx < total;
+       idx += static_cast<size_t>(gridDim.x) * blockDim.x) {
+    const size_t n = idx / (static_cast<size_t>(Cx) * HW), r = idx % (static_cast<size_t>(Cx) * HW);
+    const size_t eidx = n * Ce * HW + r;
+    const float c1 = c12[2 * n], c2 = c12[2 * n + 1];
+    const float e = et[eidx], m = em[eidx];
+    const float x0 = __fdiv_rn(__fsub_rn(x[idx], __fmul_rn(m, sq1)), sqa);
+    float nx = __fadd_rn(__fmul_rn(sqn, x0), __fmul_rn(c2, e));
+    if (z != nullptr && c1 != 0.0f) nx = __fadd_rn(nx, __fmul_rn(c1, z[idx]));
+    x_next[idx] = nx;
+    if (x0_out) x0_out[idx] = x0;
+  }
+}
+
 // ---------------------------------------------------------------------------------------------
 // DDPM ancestral update (utils/diffusion_utils.py:74-82, sampling_type='ddpm'):
 //   mean = 1/sqrt(1-bt) * (x - bt/sqrt(1-at) * et);  x_next = mean + mask * exp(0.5*logvar) * z
@@ -577,6 +603,17 @@ ASYRP_API int asyrp_ddim_update(const float* x, const float* et, const float* em
   const size_t total = static_cast<size_t>(N) * Cx * HW;
   ASYRP_LAUNCH(ddim_update_kernel, dim3(grid_for(total, 256, 8)), dim3(256), 0, static_cast<cudaStream_t>(stream), 
       x, et, em, z, x_next, x0_out, N, Cx, Ce, HW, at, an, c1, c2, z != nullptr);
+  ASYRP_CHECK_CUDA(cudaGetLastError());
+  return ASYRP_OK;
+}
+
+ASYRP_API int asyrp_ddim_update_rows(const float* x, const float* et, const float* em, const float* z, float* x_next,
+                                     float* x0_out, int N, int Cx, int Ce, int HW, float at, float an, const float* c12,
+                                     void* stream) {
+  ASYRP_REQUIRE(c12 != nullptr, "asyrp_ddim_update_rows: c12 is NULL");
+  const size_t total = static_cast<size_t>(N) * Cx * HW;
+  ASYRP_LAUNCH(ddim_update_rows_kernel, dim3(grid_for(total, 256, 8)), dim3(256), 0, static_cast<cudaStream_t>(stream),
+      x, et, em, z, x_next, x0_out, N, Cx, Ce, HW, at, an, c12);
   ASYRP_CHECK_CUDA(cudaGetLastError());
   return ASYRP_OK;
 }

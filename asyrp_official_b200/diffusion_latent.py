@@ -33,7 +33,7 @@ import numpy as np
 import torch
 
 from .modules import DDPM, guided_Diffusion, i_DDPM
-from .schedule import Schedule
+from .schedule import RowSchedule, Schedule
 from .utils.diffusion_utils import get_beta_schedule
 
 
@@ -157,10 +157,11 @@ class Asyrp(object):
             raise ValueError(f"attribute {attr!r} is not in SRC_TRG_TXT_DIC")
         return list(dic[attr][0]), list(dic[attr][1])
 
-    def directional_clip_setup(self):
+    def directional_clip_setup(self, attrs=None):
         """--DirectionalClipSmilarity's requirements, checked before any model is loaded; raises ValueError with the
         reason.  Returns (src_txt, trg_txt, templates): src_txts[0] / trg_txts[0] of edit_texts(), the pair
-        run_training scores (diffusion_latent.py:343), and imagenet_templates from --text_templates."""
+        run_training scores (diffusion_latent.py:343), and imagenet_templates from --text_templates.  With attrs (an
+        attribute sweep): ([(src_txt, trg_txt)] of every attribute, templates)."""
         from .clip_image import read_templates
         a = self.args
         if getattr(a, "multiple_attr", ""):
@@ -179,6 +180,8 @@ class Asyrp(object):
                                        or os.path.join("utils", "text_templates.py"))
         except FileNotFoundError as e:
             raise ValueError(f"--DirectionalClipSmilarity: {e}") from None
+        if attrs is not None:
+            return [tuple(t[0] for t in self.edit_texts(attr)) for attr in attrs], templates
         src, trg = self.edit_texts()
         return src[0], trg[0], templates
 
@@ -574,9 +577,27 @@ class Asyrp(object):
         return tables
 
     # ------------------------------------------------------------------------------------------
+    def checkpoint_name(self):
+        """the Δh checkpoint run_test loads (:594-614); --multiple_attr and --attr_sweep replace 'attribute' in it"""
+        a = self.args
+        exp_id = os.path.split(a.exp)[-1]
+        ckdir = getattr(a, "checkpoint_dir", "checkpoint")
+        if a.load_from_checkpoint:
+            save_name = (f'{ckdir}/{a.load_from_checkpoint}_LC_{self.config.data.category}_t{a.t_0}_ninv'
+                         f'{a.n_inv_step}_ngen{a.n_train_step}_{a.n_iter - 1}.pth')
+        else:
+            save_name = f'{ckdir}/{exp_id}_{a.n_iter - 1}.pth'
+        if a.manual_checkpoint_name:
+            save_name = os.path.join(ckdir, a.manual_checkpoint_name)
+        elif a.choose_checkpoint_num:
+            save_name = save_name[:-4] + f'_{a.choose_checkpoint_num}.pth'
+        return save_name
+
     @torch.no_grad()
     def run_test(self):
         a = self.args
+        if getattr(a, "attr_sweep", ""):
+            return self.run_attr_sweep()
         print("Running Test")
         if getattr(a, "warigari", 0.0):
             print("--warigari is accepted and has no effect (the reference's branch returns the same values, "
@@ -605,16 +626,7 @@ class Asyrp(object):
             model.setattr_layers(a.get_h_num)
         # ----------- Δh checkpoint name resolution (:594-614)
         exp_id = os.path.split(a.exp)[-1]
-        ckdir = getattr(a, "checkpoint_dir", "checkpoint")
-        if a.load_from_checkpoint:
-            save_name = (f'{ckdir}/{a.load_from_checkpoint}_LC_{self.config.data.category}_t{a.t_0}_ninv'
-                         f'{a.n_inv_step}_ngen{a.n_train_step}_{a.n_iter - 1}.pth')
-        else:
-            save_name = f'{ckdir}/{exp_id}_{a.n_iter - 1}.pth'
-        if a.manual_checkpoint_name:
-            save_name = os.path.join(ckdir, a.manual_checkpoint_name)
-        elif a.choose_checkpoint_num:
-            save_name = save_name[:-4] + f'_{a.choose_checkpoint_num}.pth'
+        save_name = self.checkpoint_name()
         # ----------- global / mean Δh (:616-627): load the cached dict if it exists, else compute it below
         num_mean, load_dict = a.num_mean_of_delta_hs, False
         train_delta_h, train_delta_block = bool(getattr(a, "train_delta_h", False)), bool(a.train_delta_block)
@@ -762,18 +774,216 @@ class Asyrp(object):
         return results
 
 
-def write_scores(path, coeffs, scores, column, label):
+    # ------------------------------------------------------------------------------------------
+    def attr_sweep_setup(self):
+        """--attr_sweep's requirements, checked before any model is loaded; raises ValueError with the reason.
+        Returns (attributes, their DeltaBlock checkpoints): the checkpoint name with 'attribute' replaced by each
+        attribute, as --multiple_attr resolves them."""
+        a = self.args
+        attrs = [t for t in str(a.attr_sweep).split(" ") if t]
+        if not attrs:
+            raise ValueError("--attr_sweep names no attribute")
+        if len(set(attrs)) != len(attrs):
+            raise ValueError(f"--attr_sweep names an attribute twice: {attrs}")
+        for flag, on in (("--multiple_attr", bool(a.multiple_attr)), ("--delta_interpolation", a.delta_interpolation),
+                         ("--num_mean_of_delta_hs", bool(a.num_mean_of_delta_hs)),
+                         ("--train_delta_h", bool(getattr(a, "train_delta_h", False)))):
+            if on:
+                raise ValueError(f"--attr_sweep edits with one DeltaBlock per attribute: it does not combine with {flag}")
+        if getattr(a, "sample_type", "ddim") != "ddim":
+            raise ValueError(f"--attr_sweep needs --sample_type ddim (every row its own eta schedule), got "
+                             f"{a.sample_type!r}")
+        if a.get_h_num != 1:
+            raise ValueError(f"--attr_sweep loads one DeltaBlock per attribute: --get_h_num must be 1, got {a.get_h_num}")
+        if getattr(a, "pass_editing", False):
+            raise ValueError("--attr_sweep edits every image: it does not combine with --pass_editing")
+        name = self.checkpoint_name()
+        if "attribute" not in os.path.basename(name):
+            raise ValueError(f"--attr_sweep: the checkpoint name {name!r} has no 'attribute' to replace by each "
+                             "attribute (e.g. --manual_checkpoint_name attribute_LC_CelebA_HQ_t999_ninv40_ngen40_0.pth)")
+        dirname, base = os.path.split(name)
+        paths = [os.path.join(dirname, base.replace("attribute", attr)) for attr in attrs]
+        missing = [p for p in paths if not os.path.isfile(p)]
+        if missing:
+            raise ValueError(f"--attr_sweep: checkpoint(s) {missing} do not exist")
+        return attrs, paths
+
+    def attr_sweep_schedules(self, attrs):
+        """(t_edit, t_addnoise) of every attribute: --user_defined_t_edit / --user_defined_t_addnoise for all of them,
+        else set_t_edit_t_addnoise with the attribute's CLIP text cosine, the K cosines from one clip_cosines call
+        (or --clip_cosine for all)"""
+        a = self.args
+        cosines = [None] * len(attrs)
+        both = getattr(a, "user_defined_t_edit", None) is not None and \
+            getattr(a, "user_defined_t_addnoise", None) is not None
+        if not both and self.needs_clip() and self.clip_configured():
+            cosines = self.clip_cosines([self.edit_texts(attr) for attr in attrs])
+        out = []
+        for attr, cos in zip(attrs, cosines):
+            self.set_t_edit_t_addnoise(LPIPS_th=a.lpips_edit_th, LPIPS_addnoise_th=a.lpips_addnoise_th, cosine=cos)
+            out.append((int(self.t_edit), int(self.t_addnoise)))
+            print(f"attribute {attr}: t_edit {out[-1][0]}, t_addnoise {out[-1][1]}")
+        return out
+
+    @torch.no_grad()
+    def run_attr_sweep(self):
+        """--run_test --attr_sweep "a b ..": every image edited with every attribute in one batched trajectory per
+        chunk of rows (attributes x images).  Row (attribute k, image i) is what --run_test --edit_attr <k> gives
+        image i: the attribute's own DeltaBlock, t_edit and t_addnoise (schedule.RowSchedule)."""
+        a = self.args
+        print("Running Test (attribute sweep)")
+        attrs, paths = self.attr_sweep_setup()
+        sdir = None
+        if getattr(a, "DirectionalClipSmilarity", False):
+            sdir = self.directional_clip_setup(attrs)
+        id_sd = self.id_similarity_setup() if getattr(a, "id_similarity", False) else None
+        times = self.attr_sweep_schedules(attrs)
+        self.sweep_times = dict(zip(attrs, times))
+        seq_test = [int(s + 1e-6) for s in list(np.linspace(0, 1, a.n_test_step) * a.t_0)]
+        seq_test_next = [-1] + list(seq_test[:-1])
+        model = self.load_pretrained_model()
+        # the latents below come from the global random stream, after the model is built: advance it as run_test does
+        # (one DeltaBlock's default init), then create the K blocks, whose initial values the checkpoints replace,
+        # without touching it, so that every image gets the x_T of its --edit_attr run
+        model.setattr_layers(a.get_h_num)
+        with torch.random.fork_rng(devices=[]):
+            model.setattr_layers(len(attrs))
+        for i, path in enumerate(paths):  # packed as layer_0 .. layer_{K-1}
+            print(f"{path} exists. load checkpoint")
+            ck = torch.load(path, map_location="cpu", weights_only=True)
+            getattr(model, f"layer_{i}").load_state_dict(ck["0"])
+        scaling_factor = a.n_train_step / a.n_test_step * a.hs_coeff_delta_h  # :626
+        coeffs = [tuple([1.0 * a.hs_coeff_origin_h] + [1.0 * scaling_factor if j == k else 0.0
+                                                        for j in range(len(attrs))]) for k in range(len(attrs))]
+        model = model.to(self.device)
+        if self.world > 1 and torch.distributed.is_initialized():
+            broadcast_weights(model)
+        if a.load_random_noise:
+            pairs = self.random_noise_pairs(model, saved_noise=bool(getattr(a, "saved_random_noise", False)))
+        else:
+            pairs = self.precompute_pairs(model)
+        target_ids = [int(i) for i in str(a.target_image_id).split(" ")] if getattr(a, "target_image_id", None) \
+            else None
+        results, directional_clip, id_scorer = {}, None, None
+        if sdir is not None:
+            from .clip_image import CLIPLoss
+            directional_clip = (CLIPLoss(a.clip_weights, a.clip_vocab, sdir[1], device=self.device), sdir[0])
+        try:
+            if id_sd is not None:
+                from .arcface import ArcFace
+                id_scorer = ArcFace(id_sd, device=self.device)
+                id_sd = None
+            for mode, do, n_img in (("train", a.do_train, a.n_train_img), ("test", a.do_test, a.n_test_img)):
+                if not do:
+                    continue
+                x_lat_tensor, x0_tensor, batch_idx = None, None, 0
+                for step, (x0, _, x_lat) in enumerate(pairs[mode]):
+                    if (target_ids is not None and step not in target_ids) or a.start_image_id > step:
+                        continue
+                    x_lat_tensor = x_lat if x_lat_tensor is None else torch.cat((x_lat_tensor, x_lat), dim=0)
+                    if a.use_x0_tensor:
+                        x0_tensor = x0 if x0_tensor is None else torch.cat((x0_tensor, x0), dim=0)
+                    if (step + 1) % a.bs_train != 0:
+                        continue
+                    if batch_idx % self.world == self.rank:  # batch-sharded across ranks, as run_test
+                        results[(mode, step)] = self.save_image_sweep(
+                            model, x_lat_tensor, seq_test, seq_test_next, attrs, times, coeffs, save_x0=a.save_x0,
+                            save_x_origin=a.save_x_origin, x0_tensor=x0_tensor,
+                            folder_dir=a.test_image_folder, file_name=f'{mode}_{step}_{a.n_iter - 1}',
+                            directional_clip=directional_clip, id_scorer=id_scorer)
+                    batch_idx += 1
+                    if step == n_img - 1:
+                        break
+                    x_lat_tensor, x0_tensor = None, None
+        finally:
+            if directional_clip is not None or id_scorer is not None:
+                del directional_clip, id_scorer
+                torch.cuda.empty_cache()
+        return results
+
+    def sweep_schedule(self, seq, seq_next, times, coeffs):
+        """the RowSchedule of sweep rows: row r has t_edit / t_addnoise times[r] and coefficients coeffs[r], with the
+        flags save_image's edit pass gives a single-attribute schedule (make_schedule)"""
+        a = self.args
+        return RowSchedule(self.betas, seq, seq_next, t_edit=[t[0] for t in times], t_addnoise=[t[1] for t in times],
+                           hs_coeffs=coeffs, sample_type=getattr(a, "sample_type", "ddim"),
+                           dt_lambda=getattr(a, "dt_lambda", 1.0), dt_end=999,
+                           ignore_timestep=bool(getattr(a, "ignore_timesteps", False)), logvars=self.logvar)
+
+    @torch.no_grad()
+    def save_image_sweep(self, model, x_lat_tensor, seq_inv, seq_inv_next, attrs, times, coeffs, save_x0=False,
+                         save_x_origin=False, x0_tensor=None, folder_dir="", file_name="", directional_clip=None,
+                         id_scorer=None):
+        """save_image for an attribute sweep: grid rows [x0] [origin DDIM] then one row per attribute in the order
+        given.  Rows of the trajectory are (attribute, image), attribute-major, run in chunks of whole attributes of
+        at most --max_rows_per_replay rows (sweep_chunks).  directional_clip = (CLIPLoss, [(src_txt, trg_txt)] per
+        attribute): each attribute's rows are scored with its own texts.  The score TSVs name the attribute of each
+        row in an appended `attr` column; `tuple` is the attribute's index."""
+        import torchvision.utils as tvu
+        a = self.args
+        time_s = time.time()
+        eng = model.engine
+        bs = x_lat_tensor.shape[0]
+        x_list, edited, origin = [], [], None
+        if save_x0 and x0_tensor is not None:
+            x_list.append(x0_tensor.cpu())
+        if save_x_origin or directional_clip is not None or id_scorer is not None:
+            sch = self.make_schedule(seq_inv, seq_inv_next, (1.0,), edit=False,
+                                     addnoise=bool(getattr(a, "origin_process_addnoise", False)))
+            if save_x_origin:
+                origin = self.edit_batch(model, x_lat_tensor, sch)
+                x_list.append(origin)
+            else:
+                with torch.random.fork_rng(devices=[eng.device]):
+                    origin = self.edit_batch(model, x_lat_tensor, sch)
+        tpc, chunks = plan_sweep(len(attrs), bs, getattr(a, "max_rows_per_replay", 16))
+        for chunk in chunks:
+            rows = sweep_rows(chunk, tpc, bs)
+            sch = self.sweep_schedule(seq_inv, seq_inv_next, [times[k] for k in rows], [coeffs[k] for k in rows])
+            rows_x = pad_rows(x_lat_tensor.repeat(len(chunk), 1, 1, 1), tpc * bs)
+            x0 = self.edit_batch(model, rows_x, sch)
+            for j in range(len(chunk)):
+                x_list.append(x0[j * bs:(j + 1) * bs].clone())
+                edited.append(x_list[-1])
+        x = (torch.cat(x_list, dim=0) + 1) * 0.5
+        grid = tvu.make_grid(x, nrow=a.bs_train, padding=1)
+        os.makedirs(folder_dir, exist_ok=True)
+        tvu.save_image(grid, os.path.join(folder_dir, f'{file_name}_ngen{a.n_train_step}.png'))
+        if directional_clip is not None:
+            clip_loss, texts = directional_clip
+            s_dir = torch.stack([clip_loss.directional_similarity(origin, texts[k][0], edited[k], texts[k][1]).view(bs)
+                                 for k in range(len(attrs))])
+            self.directional_clip[file_name] = s_dir
+            write_scores(os.path.join(folder_dir, f'{file_name}_ngen{a.n_train_step}_directional_clip.tsv'), coeffs,
+                         s_dir, "S_dir", "directional CLIP similarity", attrs=attrs)
+        if id_scorer is not None:
+            ids = id_scorer.id_similarity(origin, torch.cat(edited)).view(len(edited), bs)
+            self.id_similarity[file_name] = ids
+            write_scores(os.path.join(folder_dir, f'{file_name}_ngen{a.n_train_step}_id_similarity.tsv'), coeffs,
+                         ids, "ID", "identity similarity", attrs=attrs)
+        print(f'{time.time() - time_s} seconds, {file_name}_ngen{a.n_train_step}.png is saved')
+        return x_list
+
+
+def sweep_rows(chunk, tpc, bs):
+    """the attribute of every trajectory row of one sweep chunk: attribute-major (attribute, image) rows, padded to
+    tpc * bs rows with the last attribute (padding rows are discarded)"""
+    rows = [k for k in chunk for _ in range(bs)]
+    return rows + [rows[-1]] * (tpc * bs - len(rows))
+
+def write_scores(path, coeffs, scores, column, label, attrs=None):
     """a per-edit score table: one row per (hs_coeff tuple, image) in grid order, columns image, tuple, hs_coeff and
-    `column`; prints each tuple's mean as `label`"""
+    `column`; prints each tuple's mean as `label`.  attrs (an attribute sweep): tuple k is attribute k, named in an
+    appended `attr` column"""
     with open(path, "w") as f:
-        f.write(f"image\ttuple\ths_coeff\t{column}\n")
+        f.write(f"image\ttuple\ths_coeff\t{column}" + ("\tattr" if attrs is not None else "") + "\n")
         for k, row in enumerate(scores.tolist()):
             tup = ",".join(f"{float(c):.6g}" for c in coeffs[k])
             for i, v in enumerate(row):
-                f.write(f"{i}\t{k}\t{tup}\t{v!r}\n")
+                f.write(f"{i}\t{k}\t{tup}\t{v!r}" + (f"\t{attrs[k]}" if attrs is not None else "") + "\n")
     for k, row in enumerate(scores):
-        print(f"{label}, hs_coeff {tuple(float(c) for c in coeffs[k])}: mean {row.double().mean().item():.6f} over "
-              f"{row.numel()} images")
+        name = f"attribute {attrs[k]}" if attrs is not None else f"hs_coeff {tuple(float(c) for c in coeffs[k])}"
+        print(f"{label}, {name}: mean {row.double().mean().item():.6f} over {row.numel()} images")
 
 
 def plan_sweep(n_tuples, bs, max_rows):

@@ -20,6 +20,7 @@ import torch
 from . import ops
 from .arch import Arch, Attn, Res, Resample
 from .ops import MODE_1x1, MODE_3x3, MODE_3x3_S2, RESAMPLE_AVGPOOL2, RESAMPLE_NONE, RESAMPLE_UP2
+from .schedule import RowSchedule
 
 
 # ASYRP_DUAL_STREAM=0: run the two decoder passes of an edit step one after the other (A/B measurements)
@@ -277,6 +278,39 @@ def coeff_table(hs_coeffs, N, n_delta):
         raise ops._lib.AsyrpError(f"hs_coeffs must be a float [{N}][{1 + n_delta}] table (batch x (1 + DeltaBlocks)), "
                                   f"got {t.dtype} {tuple(t.shape)}")
     return t.to(torch.float32)
+
+
+def sweep_pairs(coeffs):
+    """per-row coefficients [..][N][1 + K] -> the pairs of the independent DeltaBlocks of a per-row schedule,
+    [..][N][K][2]: block i of row n computes c_{i+1}*(conv + bias) + c0*h, i.e. (acc_scale, res_scale) = (c_{i+1}, c0)"""
+    t = torch.as_tensor(coeffs, dtype=torch.float32)
+    out = torch.empty(*t.shape[:-1], t.shape[-1] - 1, 2, dtype=torch.float32)
+    out[..., 0] = t[..., 1:]
+    out[..., 1] = t[..., :1]
+    return out
+
+
+def own_blocks(hs_coeffs):
+    """the DeltaBlock each row of a per-row schedule edits with: the one non-zero c_{i+1} of its coefficients (block
+    0 when all are zero).  Rows combining several blocks have no single-block run to equal and are refused."""
+    own = []
+    for n, row in enumerate(hs_coeffs):
+        nz = [i for i, c in enumerate(row[1:]) if float(c) != 0.0]
+        if len(nz) > 1:
+            raise ops._lib.AsyrpError(f"per-row schedule: row {n} has non-zero coefficients on DeltaBlocks {nz}; each "
+                                      "row edits with one block")
+        own.append(nz[0] if nz else 0)
+    return tuple(own)
+
+
+def row_runs(rows):
+    """maximal runs [a, b) of consecutive rows with equal values: [(a, b, value)]"""
+    runs, a = [], 0
+    for n in range(1, len(rows) + 1):
+        if n == len(rows) or rows[n] != rows[a]:
+            runs.append((a, n, rows[a]))
+            a = n
+    return runs
 
 
 def shared_c0(table):
@@ -660,6 +694,19 @@ class Plan:
             self._free(h2_prev)
         return h2
 
+    def build_sweep(self):
+        """The DeltaBlocks of a per-row schedule (an attribute sweep), built on first use: block i computes
+        D_i = c_{i+1}*layer_i(h) + c0*h from middle_h, with its own output and GroupNorm sums, so that a row's D_i is
+        the h2 that a plan with only block i packed computes for it.  The trajectory copies each editing row's D_i
+        into h2 (and its sums), where the second decoder reads it.  Buffers come from a pool of their own."""
+        if getattr(self, "sweep_ops", None) is not None:
+            return
+        main_pool, self.pool = self.pool, Pool(self.eng.device)
+        main_cur, self.sweep_ops = self._cur, []
+        self._cur = self.sweep_ops
+        self.sweep_h2 = [self._delta_block(i, self.middle_h, self.middle_h, last=False) for i in range(self.eng.n_delta)]
+        self.sweep_pool, self.pool, self._cur = self.pool, main_pool, main_cur
+
     def _decoder(self, h_in, out_planar):
         a, W = self.eng.arch, self.eng.W
         h = h_in
@@ -756,6 +803,27 @@ class Plan:
     def run_decoder(self):
         for f in self.dec_ops:
             f()
+
+    def run_sweep_and_decoder(self, select):
+        """edit step of a per-row schedule: every DeltaBlock from middle_h, `select()` (the row copies into h2), the
+        decoder on h2 — and, concurrently on the side stream, the decoder on h"""
+        def edit():
+            for f in self.sweep_ops:
+                f()
+            select()
+            for f in self.dec_mod_ops:
+                f()
+
+        if not DUAL_STREAM:
+            edit()
+            self.run_decoder()
+            return
+        cur = torch.cuda.current_stream()
+        self.side_stream.wait_stream(cur)
+        with torch.cuda.stream(self.side_stream):
+            self.run_decoder()
+        edit()
+        cur.wait_stream(self.side_stream)
 
     def run_edit_and_decoder(self, explicit=False):
         """edit step: Δh injection + decoder(h2) on the current stream, decoder(h) concurrently on the side stream
@@ -957,6 +1025,122 @@ class UNetEngine:
             g["graph"] = cg
         return g
 
+    def _build_row_trajectory(self, P, schedule, use_graph, own, record_process):
+        """the trajectory of a per-row schedule (schedule.RowSchedule): per step the step's rows of the DeltaBlock pair
+        table and of the (c1, c2) table are copied into the buffers the kernels read, as the timestep-embedding row is;
+        on edit steps every DeltaBlock runs from middle_h, each editing row's output is copied into h2, and the rows
+        that do not edit take et as et_mod; the update is ddim_update_rows"""
+        steps = schedule.steps
+        N, dev = P.x.shape[0], self.device
+        n_sto = schedule.n_stochastic
+        P.build_sweep()
+        zbuf = torch.zeros((max(n_sto, 1), *P.x.shape), dtype=torch.float32, device=dev)
+        emb_table = torch.empty((len(steps), *P.emb_all.shape), dtype=torch.float32, device=dev)
+        for k, s in enumerate(steps):
+            P.t.fill_(float(s.t))
+            P.run_temb()
+            emb_table[k].copy_(P.emb_all)
+        pair_table = torch.zeros((len(steps), *P.coef.shape), dtype=torch.float32, device=dev)
+        c_table = torch.zeros((len(steps), N, 2), dtype=torch.float32, device=dev)
+        c12 = torch.zeros((N, 2), dtype=torch.float32, device=dev)
+        rec = {}
+        if record_process:
+            rec["x"] = torch.zeros((len(steps), *P.x.shape), dtype=torch.float32, device=dev)
+            rec["x0_t"] = torch.zeros((len(steps), *P.x.shape), dtype=torch.float32, device=dev)
+        h2 = P.h2
+
+        def selector(s):
+            def select():
+                for a, b, (edit, i) in row_runs([(e, o) for e, o in zip(s.edit_rows, own)]):
+                    if edit:
+                        src = P.sweep_h2[i]
+                        h2.t[a:b].copy_(src.t[a:b])
+                        h2.stats[a:b].copy_(src.stats[a:b])
+            return select
+
+        def body():
+            zi = 0
+            for k, s in enumerate(steps):
+                P.emb_all.copy_(emb_table[k])
+                P.coef.copy_(pair_table[k])
+                c12.copy_(c_table[k])
+                P.run_encoder()
+                if s.edit:
+                    P.run_sweep_and_decoder(selector(s))
+                    for a, b, edit in row_runs(list(s.edit_rows)):
+                        if not edit:  # h2 = h: the second decoder pass equals the first (ddpm/diffusion.py:510)
+                            P.et_mod[a:b].copy_(P.et[a:b])
+                else:
+                    P.run_decoder()
+                z = None
+                if s.stochastic:
+                    z = zbuf[zi]
+                    zi += 1
+                ops.ddim_update_rows(P.x, P.et, P.et_mod if s.edit else P.et, z, P.x,
+                                     rec["x0_t"][k] if record_process else None, s.at, s.an, c12)
+                if record_process:
+                    rec["x"][k].copy_(P.x)
+
+        n_edit = sum(1 for s in steps if s.edit)
+        n_launch = sum(len(P.launches(False, temb=False)) + 1 for s in steps) + \
+            n_edit * (len(P.sweep_ops) + len(P.dec_mod_ops))
+        g = {"zbuf": zbuf, "emb_table": emb_table, "pairs": pair_table, "c": c_table, "body": body, "graph": None,
+             "launches": n_launch, "rec": rec, "n_edit": n_edit}
+        if use_graph:
+            s_ = torch.cuda.Stream(device=dev)
+            s_.wait_stream(torch.cuda.current_stream())
+            with torch.cuda.stream(s_):  # warm-up outside capture
+                P.emb_all.copy_(emb_table[0])
+                P.run_encoder()
+                P.run_sweep_and_decoder(lambda: None)
+            torch.cuda.current_stream().wait_stream(s_)
+            torch.cuda.synchronize(dev)
+            cg = torch.cuda.CUDAGraph()
+            with torch.cuda.graph(cg):
+                body()
+            g["graph"] = cg
+        return g
+
+    def _sample_rows(self, x_T, schedule, noise, use_graph, out, record_process):
+        N = x_T.shape[0]
+        if schedule.N != N:
+            raise ops._lib.AsyrpError(f"per-row schedule has {schedule.N} rows, x_T {N}")
+        if schedule.n_delta != self.n_delta or self.n_delta == 0:
+            raise ops._lib.AsyrpError(f"per-row schedule carries coefficients for {schedule.n_delta} DeltaBlocks; the "
+                                      f"engine packed {self.n_delta}")
+        if GN_FOLD:
+            raise ops._lib.AsyrpError("per-row schedules are not built with ASYRP_GN_FOLD (in-kernel GroupNorm sums)")
+        own = own_blocks(schedule.hs_coeffs)
+        P = self.plan(N)
+        key = (N, bool(use_graph), schedule.key(), own, bool(record_process))
+        with torch.cuda.device(self.device):
+            n_sto = schedule.n_stochastic
+            if n_sto and (noise is None or noise.shape[0] != n_sto or noise.shape[1] != N):
+                raise ops._lib.AsyrpError(f"pre-drawn noise [{n_sto}][{N}][..] required for the stochastic steps")
+            self.state["ignore_timestep"] = schedule.ignore_timestep
+            self.state["slerp_t"], self.state["use_mask"] = 0.0, False
+            g = self.graphs.pop(key, None)
+            if g is None:
+                g = self._build_row_trajectory(P, schedule, use_graph, own, record_process)
+                while len(self.graphs) >= self.MAX_GRAPHS:
+                    self.graphs.pop(next(iter(self.graphs)))
+            self.graphs[key] = g
+            self.last_launches = g["launches"]
+            self.last_records = g["rec"]
+            g["pairs"].copy_(sweep_pairs(schedule.coeffs))
+            g["c"].copy_(schedule.c)
+            P.x.copy_(x_T, non_blocking=True)
+            if n_sto:
+                g["zbuf"].copy_(noise, non_blocking=True)
+            if g["graph"] is not None:
+                g["graph"].replay()
+            else:
+                g["body"]()
+            if out is None:
+                return P.x.clone()
+            out.copy_(P.x)
+            return out
+
     def sample(self, x_T, schedule, noise=None, use_graph=True, out=None, delta_hs=None, use_mask=False,
                record_dh=False, record_process=False, hs_coeffs=None, lpips=None):
         """Run the reverse trajectory of `schedule` (sampler.Schedule) from x_T; returns x_0 (fp32 NCHW).
@@ -980,7 +1164,17 @@ class UNetEngine:
         lpips: an asyrp_official_b200.lpips.LPIPS.  The graph then computes the LPIPS features of its starting image
         once, at its head, and after every step's DDIM update the distances of x_t and of x0_t to it
         (compute_lpips_distance, diffusion_latent.py:1255-1268): `last_records["lpips_x"]` and
-        `last_records["lpips_x0_t"]`, [steps][N] fp32.  DDIM steps only."""
+        `last_records["lpips_x0_t"]`, [steps][N] fp32.  DDIM steps only.
+
+        schedule may also be a schedule.RowSchedule: every row its own t_edit, t_addnoise and coefficients, each row
+        editing with one DeltaBlock.  Row n then equals, bit for bit, a run of its own Schedule on an engine with only
+        its block packed, fed the noise entries of the steps at which it is stochastic (RowSchedule.noise_rows).
+        noise: [n_stochastic][N][C][H][W] over the steps at which any row is stochastic.  delta_hs, record_dh, hs_coeffs
+        and lpips do not apply."""
+        if isinstance(schedule, RowSchedule):
+            if delta_hs is not None or record_dh or hs_coeffs is not None or lpips is not None:
+                raise ops._lib.AsyrpError("a per-row schedule takes no delta_hs, record_dh, hs_coeffs or lpips")
+            return self._sample_rows(x_T, schedule, noise, use_graph, out, record_process)
         N = x_T.shape[0]
         P = self.plan(N)
         explicit = delta_hs is not None

@@ -112,6 +112,10 @@ def build_parser():
     p.add_argument('--max_rows_per_replay', type=int, default=16,
                    help='rows (hs_coeff tuples x images) of one batched trajectory in save_image; bounds the memory of '
                         'the per-batch plan (DDPM 256x256: about 4.3 GB at 16 rows); 1 = one replay per tuple')
+    p.add_argument('--attr_sweep', type=str, default='',
+                   help='--run_test: edit every image with each of these attributes ("smiling angry young"), one grid '
+                        'row per attribute, each row what --edit_attr <attribute> gives with its own t_edit / '
+                        't_addnoise; the checkpoint name\'s "attribute" is replaced by each attribute')
     return p
 
 

@@ -270,6 +270,19 @@ def ddim_update(x, et, em, z, x_next, x0_out, at, an, c1, c2):
                                 at, an, c1, c2, _stream()), "asyrp_ddim_update")
 
 
+def ddim_update_rows(x, et, em, z, x_next, x0_out, at, an, c12):
+    """ddim_update with one (c1, c2) pair per sample: c12 fp32 [N][2] on the device (row n gives the bits of
+    ddim_update with scalars c12[n]; z is read only by rows with c1 != 0)"""
+    lib = _lib.load()
+    N, Cx, H, W = x.shape
+    Ce = et.shape[1]
+    if not (c12.is_cuda and c12.dtype == torch.float32 and tuple(c12.shape) == (N, 2) and c12.is_contiguous()):
+        raise _lib.AsyrpError(f"ddim_update_rows: c12 must be a contiguous fp32 [{N}][2] device tensor, got "
+                              f"{c12.dtype} {tuple(c12.shape)} on {c12.device}")
+    check(lib.asyrp_ddim_update_rows(_ptr(x), _ptr(et), _ptr(em), _ptr(z), _ptr(x_next), _ptr(x0_out), N, Cx, Ce,
+                                     H * W, at, an, _ptr(c12), _stream()), "asyrp_ddim_update_rows")
+
+
 def attention(qkv, out, heads, head_dim, scale):
     lib = _lib.load()
     N, T, _ = qkv.shape

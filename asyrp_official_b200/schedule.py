@@ -96,3 +96,92 @@ class Schedule:
     @property
     def n_edit(self):
         return sum(1 for s in self.steps if s.edit)
+
+
+@dataclass(frozen=True)
+class RowStep:
+    """one step of a RowSchedule: what the whole batch shares, and which rows edit"""
+    t: int
+    t_next: int
+    at: float
+    an: float
+    edit_rows: Tuple[bool, ...]   # row n edits at this step: t >= t_edit[n] and its coefficients are not (1, 0, ..)
+    stochastic: bool              # any row has eta = 1 at this step (c1 != 0)
+    kind: str = "ddim"
+
+    @property
+    def edit(self):
+        return any(self.edit_rows)
+
+
+class RowSchedule:
+    """A trajectory whose rows follow their own schedules: row n is the single-row
+    Schedule(betas, seq, seq_next, t_edit[n], t_addnoise[n], hs_coeffs[n], ...).  The step list (t, t_next, alpha-bars)
+    is the same for every row; what differs per row lives in tables:
+
+      c         fp32 [steps][N][2]        (c1, c2) of each row, the values of its own Schedule
+      coeffs    fp32 [steps][N][1 + K]    DeltaBlock coefficients: hs_coeffs[n] while the row edits, (1, 0, .., 0)
+                                          below its t_edit (h2 = h, the reference's t[0] < t_edit branch)
+
+    A step edits when any row edits and is stochastic when any row has eta = 1.  'ddpm' sampling is refused: its
+    ancestral step has no per-row form here."""
+
+    def __init__(self, betas, seq, seq_next, t_edit, t_addnoise, hs_coeffs, sample_type="ddim", dt_lambda=1.0,
+                 dt_end=999, ignore_timestep=False, logvars=None):
+        if sample_type != "ddim":
+            raise ValueError(f"a per-row schedule needs sample_type 'ddim', got {sample_type!r}")
+        t_edit, t_addnoise = [int(v) for v in t_edit], [int(v) for v in t_addnoise]
+        coeffs = [tuple(float(c) for c in row) for row in hs_coeffs]
+        N = len(t_edit)
+        if not N or len(t_addnoise) != N or len(coeffs) != N:
+            raise ValueError(f"t_edit, t_addnoise and hs_coeffs need one entry per row, got {len(t_edit)}, "
+                             f"{len(t_addnoise)} and {len(coeffs)}")
+        if len({len(r) for r in coeffs}) != 1 or len(coeffs[0]) < 1:
+            raise ValueError("every row of hs_coeffs needs the same length 1 + K")
+        self.rows = [Schedule(betas, seq, seq_next, t_edit=t_edit[n], t_addnoise=t_addnoise[n], hs_coeff=coeffs[n],
+                              sample_type="ddim", dt_lambda=dt_lambda, dt_end=dt_end, ignore_timestep=ignore_timestep,
+                              logvars=logvars) for n in range(N)]
+        K1 = len(coeffs[0])
+        gate = (1.0,) + (0.0,) * (K1 - 1)
+        steps: List[RowStep] = []
+        c = torch.zeros(len(self.rows[0].steps), N, 2, dtype=torch.float32)
+        co = torch.zeros(len(self.rows[0].steps), N, K1, dtype=torch.float32)
+        for k, row_steps in enumerate(zip(*(r.steps for r in self.rows))):
+            s0 = row_steps[0]
+            edit_rows = []
+            for n, s in enumerate(row_steps):
+                c[k, n, 0], c[k, n, 1] = s.c1, s.c2
+                co[k, n] = torch.tensor(coeffs[n] if s.edit else gate, dtype=torch.float32)
+                edit_rows.append(bool(s.edit) and tuple(co[k, n].tolist()) != gate)
+            steps.append(RowStep(s0.t, s0.t_next, s0.at, s0.an, tuple(edit_rows), any(s.stochastic for s in row_steps)))
+        self.steps = steps
+        self.c, self.coeffs = c, co
+        self.t_edit, self.t_addnoise, self.hs_coeffs = t_edit, t_addnoise, coeffs
+        self.ignore_timestep = bool(ignore_timestep)
+
+    @property
+    def N(self):
+        return len(self.rows)
+
+    @property
+    def n_delta(self):
+        return self.coeffs.shape[2] - 1
+
+    def key(self):
+        """identifies the captured graph: the step list and which rows edit where; (c1, c2) and the DeltaBlock
+        coefficients are device-side tables, filled before every replay"""
+        return ("rows", tuple(self.steps), self.ignore_timestep, self.n_delta)
+
+    @property
+    def n_stochastic(self):
+        return sum(1 for s in self.steps if s.stochastic)
+
+    @property
+    def n_edit(self):
+        return sum(1 for s in self.steps if s.edit)
+
+    def noise_rows(self, n, noise):
+        """the noise a row's own Schedule consumes, [its n_stochastic][1][...], taken from a RowSchedule noise tensor
+        [n_stochastic][N][...]: the entries of the steps at which row n is stochastic"""
+        ks = [k for k, s in enumerate(self.steps) if s.stochastic]
+        return noise[[zi for zi, k in enumerate(ks) if self.rows[n].steps[k].stochastic], n:n + 1]

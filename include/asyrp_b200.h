@@ -192,6 +192,12 @@ int asyrp_ddim_update(const float* x, const float* et, const float* em, const fl
                       float* x0_out, int N, int Cx, int Ce, int HW, float at, float an, float c1, float c2,
                       void* stream);
 
+/* asyrp_ddim_update with a (c1, c2) pair per sample: c12 is a DEVICE array [N][2].  Row n gives exactly the bits of
+ * asyrp_ddim_update with scalars c12[n]; z (may be NULL) is read only where c1 != 0. */
+int asyrp_ddim_update_rows(const float* x, const float* et, const float* em, const float* z, float* x_next,
+                           float* x0_out, int N, int Cx, int Ce, int HW, float at, float an, const float* c12,
+                           void* stream);
+
 /* DDPM ancestral update (utils/diffusion_utils.py:74-82, sampling_type 'ddpm'):
  *   x_next = (x - bt/sqrt(1-at)*et)/sqrt(1-bt) + mask*exp(0.5*logvar)*z;  learned_sigma: logvar = et channels [Cx, 2Cx) */
 int asyrp_ddpm_update(const float* x, const float* et, const float* z, float* x_next, int N, int Cx, int Ce, int HW,

@@ -79,6 +79,8 @@ SIGNATURES = {
     "asyrp_unpack_nchw": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p]),
     "asyrp_slerp_h": (c_int, [c_void_p, c_void_p, C.c_longlong, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int,
                               c_float, c_int, c_void_p]),
+    "asyrp_slerp_h_rows": (c_int, [c_void_p, c_void_p, C.c_longlong, c_void_p, c_void_p, c_int, c_int, c_int, c_int,
+                                   c_int, c_void_p, c_int, c_void_p]),
     "asyrp_transpose_tc": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p]),
     "asyrp_softmax_rows": (c_int, [c_void_p, c_void_p, C.c_longlong, c_int, c_float, c_void_p]),
     "asyrp_attention": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_float, c_void_p]),

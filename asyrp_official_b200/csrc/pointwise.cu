@@ -443,13 +443,11 @@ __device__ __forceinline__ float block_sum(float v, float* sh) {
   return t;
 }
 
-__global__ void __launch_bounds__(256) slerp_h_kernel(const __half* __restrict__ h, const float* __restrict__ dh,
-                                                      long long dh_stride, __half* __restrict__ h2,
-                                                      float* __restrict__ stats, int T, int C, int H, int W, float t,
-                                                      int use_mask) {
-  pdl_trigger();
-  pdl_wait();
-  __shared__ float sh[8];
+// The body of both slerp kernels: sample n = blockIdx.x with slerp weight t.  The per-row kernel only reads t from
+// device memory, so row n performs exactly the scalar kernel's operations.
+__device__ __forceinline__ void slerp_h_sample(const __half* __restrict__ h, const float* __restrict__ dh,
+                                               long long dh_stride, __half* __restrict__ h2, float* __restrict__ stats,
+                                               int T, int C, int H, int W, float t, int use_mask, float* sh) {
   const int n = blockIdx.x, HW = H * W;
   const __half* hn = h + static_cast<size_t>(n) * HW * C;
   const float* dn = dh + static_cast<size_t>(n) * dh_stride;
@@ -487,6 +485,27 @@ __global__ void __launch_bounds__(256) slerp_h_kernel(const __half* __restrict__
     st[pr * 2] = s; st[pr * 2 + 1] = ss;
     for (int tt = 1; tt < T; ++tt) { st[(tt * (C / 2) + pr) * 2] = 0.f; st[(tt * (C / 2) + pr) * 2 + 1] = 0.f; }
   }
+}
+
+__global__ void __launch_bounds__(256) slerp_h_kernel(const __half* __restrict__ h, const float* __restrict__ dh,
+                                                      long long dh_stride, __half* __restrict__ h2,
+                                                      float* __restrict__ stats, int T, int C, int H, int W, float t,
+                                                      int use_mask) {
+  pdl_trigger();
+  pdl_wait();
+  __shared__ float sh[8];
+  slerp_h_sample(h, dh, dh_stride, h2, stats, T, C, H, W, t, use_mask, sh);
+}
+
+// per-sample slerp weight t_rows[n] (a graph input: one captured graph serves every weight table)
+__global__ void __launch_bounds__(256) slerp_h_rows_kernel(const __half* __restrict__ h, const float* __restrict__ dh,
+                                                           long long dh_stride, __half* __restrict__ h2,
+                                                           float* __restrict__ stats, int T, int C, int H, int W,
+                                                           const float* __restrict__ t_rows, int use_mask) {
+  pdl_trigger();
+  pdl_wait();
+  __shared__ float sh[8];
+  slerp_h_sample(h, dh, dh_stride, h2, stats, T, C, H, W, t_rows[blockIdx.x], use_mask, sh);
 }
 
 }  // namespace asyrp
@@ -642,6 +661,18 @@ ASYRP_API int asyrp_slerp_h(const void* h, const float* dh, long long dh_sample_
   ASYRP_LAUNCH(slerp_h_kernel, dim3(N), dim3(256), 0, static_cast<cudaStream_t>(stream), static_cast<const __half*>(h), dh, dh_sample_stride,
                                                                     static_cast<__half*>(h2), stats, stats_tiles, C, H,
                                                                     W, t, use_mask);
+  ASYRP_CHECK_CUDA(cudaGetLastError());
+  return ASYRP_OK;
+}
+
+ASYRP_API int asyrp_slerp_h_rows(const void* h, const float* dh, long long dh_sample_stride, void* h2, float* stats,
+                                 int stats_tiles, int N, int C, int H, int W, const float* t_rows, int use_mask,
+                                 void* stream) {
+  ASYRP_REQUIRE(C % 2 == 0 && stats_tiles >= 1, "asyrp_slerp_h_rows: bad arguments");
+  ASYRP_REQUIRE(t_rows != nullptr, "asyrp_slerp_h_rows: t_rows is NULL");
+  ASYRP_LAUNCH(slerp_h_rows_kernel, dim3(N), dim3(256), 0, static_cast<cudaStream_t>(stream),
+               static_cast<const __half*>(h), dh, dh_sample_stride, static_cast<__half*>(h2), stats, stats_tiles, C, H,
+               W, t_rows, use_mask);
   ASYRP_CHECK_CUDA(cudaGetLastError());
   return ASYRP_OK;
 }

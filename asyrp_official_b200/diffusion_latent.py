@@ -16,6 +16,11 @@ Mirrors, with the same attribute / flag names:
   --id_similarity              losses/id_loss.py            run_test scores every edit with 1 - IDLoss (ArcFace IR-SE50,
                                                             arcface.ArcFace), written next to the PNG; the reference
                                                             uses IDLoss only in training
+  Asyrp.precompute_pairs_with_h :877-947                    DDIM inversion of one image keeping the bottleneck h of
+                                                            every step (batched here, same cache file)
+  Asyrp.run_diff_style         main.py:192-202              --diff_style (DiffStyle content injection): this build's
+                                                            composition of the functions above with denoising_step's
+                                                            delta_h branch; the reference declares the flags only
 
 Differences (documented in INTEGRATION.md): the reverse loop is UNetEngine.sample() — one CUDA graph per
 (batch, schedule) instead of 40 Python iterations; pretrained weights come from --model_path (no URL download);
@@ -33,7 +38,7 @@ import numpy as np
 import torch
 
 from .modules import DDPM, guided_Diffusion, i_DDPM
-from .schedule import RowSchedule, Schedule
+from .schedule import RowSchedule, Schedule, make_sequences
 from .utils.diffusion_utils import get_beta_schedule
 
 
@@ -963,6 +968,204 @@ class Asyrp(object):
                          ids, "ID", "identity similarity", attrs=attrs)
         print(f'{time.time() - time_s} seconds, {file_name}_ngen{a.n_train_step}.png is saved')
         return x_list
+
+    # ------------------------------------------------------------------------------------------
+    def diff_style_setup(self):
+        """--diff_style's requirements, checked before any model is loaded; raises ValueError with the reason.
+        Returns (content image paths, style image paths, the hs_coeff values γ, one result per pair each)."""
+        a = self.args
+        if getattr(a, "run_test", False) or getattr(a, "lpips", False):
+            raise ValueError("--diff_style is a mode of its own: it does not combine with --run_test or --lpips")
+        if getattr(a, "user_defined_t_edit", None) is None:
+            raise ValueError("--diff_style needs --user_defined_t_edit: DiffStyle edits with no text, so neither CLIP's "
+                             "cosine nor the LPIPS tables can choose t_edit")
+        if getattr(a, "sample_type", "ddim") != "ddim":
+            raise ValueError(f"--diff_style needs --sample_type ddim, got {a.sample_type!r}: the reference's 'ddpm' step "
+                             "never reads et_modified, so nothing would be injected")
+        gammas = diff_style_gammas(getattr(a, "hs_coeff", 0.9), getattr(a, "hs_coeff_list", ""))
+        paths = []
+        for flag in ("content_dir", "style_dir"):
+            d = getattr(a, flag, None)
+            if not d or not os.path.isdir(d):
+                raise ValueError(f"--diff_style: --{flag} {d!r} is not a directory")
+            found = image_paths(d)
+            if not found:
+                raise ValueError(f"--diff_style: --{flag} {d!r} holds no png / jpg image")
+            paths.append(found)
+        names = {}
+        for p in dict.fromkeys(paths[0] + paths[1]):
+            c = diff_style_cache_path(self.config.data.category, a.n_inv_step, p)
+            if names.setdefault(c, p) != p:
+                raise ValueError(f"--diff_style: {names[c]!r} and {p!r} share the inversion cache {c!r} (the "
+                                 "reference's name keeps the parent directory and the stem only)")
+        return paths[0], paths[1], gammas
+
+    @torch.no_grad()
+    def precompute_pairs_with_h(self, model, img_paths):
+        """[x0, 0, x_T, h_dic] of every image (diffusion_latent.py:877-947): DDIM inversion over
+        zip(seq_inv_next[1:], seq_inv[1:]) with the plain UNet, h_dic[t] = the bottleneck h ([1,C,h,w] fp32) of the
+        step that evaluated the UNet at t.  Cached on the CPU as precomputed/<category>_inv<n_inv_step>_<dir>_<stem>.pt
+        in the reference's format; an existing cache (the reference's own included) is read unless --re_precompute.
+        The images to invert run --bs_train per replay, h recorded inside the graph (UNetEngine.sample(record_h=True)).
+        Under torchrun rank 0 inverts and writes the caches (temp file + rename), the other ranks load them after a
+        barrier.  Returns {path: [x0, 0, x_T, h_dic]}; self.n_inverted counts the images inverted here."""
+        a = self.args
+        seq_inv, seq_inv_next = make_sequences(a.t_0, a.n_inv_step)
+        os.makedirs('precomputed', exist_ok=True)
+        out, todo = {}, []
+        for p in dict.fromkeys(img_paths):
+            cache = diff_style_cache_path(self.config.data.category, a.n_inv_step, p)
+            if os.path.exists(cache) and not getattr(a, "re_precompute", False):
+                out[p] = torch.load(cache, map_location="cpu", weights_only=True)
+            else:
+                todo.append((p, cache))
+        self.n_inverted = 0
+        if todo and self.rank == 0:
+            eng = model.engine
+            sch = Schedule.inversion(self.betas, seq_inv, seq_inv_next)
+            bs = min(max(1, a.bs_train), len(todo))
+            for k in range(0, len(todo), bs):  # every replay bs rows (the last one padded): one captured graph
+                chunk = todo[k:k + bs]
+                x0 = torch.cat([diff_style_image(p, self.config.data.image_size) for p, _ in chunk])
+                x_lat = eng.sample(pad_rows(x0, bs).to(eng.device), sch, record_h=True).cpu()
+                hs = eng.last_records["h"].cpu()
+                for i, (p, cache) in enumerate(chunk):
+                    h_dic = {int(st.t): hs[j][i:i + 1].clone() for j, st in enumerate(sch.steps)}
+                    out[p] = [x0[i:i + 1].clone(), 0, x_lat[i:i + 1].clone(), h_dic]
+                    _atomic_save(out[p], cache)
+            self.n_inverted = len(todo)
+        if todo and self.world > 1 and torch.distributed.is_available() and torch.distributed.is_initialized():
+            torch.distributed.barrier()
+            for p, cache in todo:
+                out.setdefault(p, torch.load(cache, map_location="cpu", weights_only=True))
+        print(f"DiffStyle: {len(out)} images, {self.n_inverted} inverted, {len(out) - self.n_inverted} from cache")
+        return out
+
+    def diff_style_schedule(self, gamma):
+        """the generation steps zip(reversed(seq_inv), reversed(seq_inv_next)) as the mode calls denoising_step:
+        DDIM, t_edit = --user_defined_t_edit, eta = 1 below --t_noise, --dt_lambda from --dt_end on (save_image passes
+        999 as dt_end; this mode passes --dt_end), hs_coeff = (γ,)"""
+        a = self.args
+        seq_inv, seq_inv_next = make_sequences(a.t_0, a.n_inv_step)
+        return Schedule(self.betas, seq_inv, seq_inv_next, t_edit=a.user_defined_t_edit, t_addnoise=a.t_noise,
+                        hs_coeff=(float(gamma),), sample_type="ddim", dt_lambda=a.dt_lambda, dt_end=a.dt_end)
+
+    @torch.no_grad()
+    def run_diff_style(self):
+        """--diff_style: inject every content image's h into every style image's trajectory.  Row (content c, style s,
+        γ) starts from the style's x_T and runs diff_style_schedule(γ) with delta_h = the content's h at each edit
+        step: h2 = slerp(1 - γ, h, |h| h_c/|h_c|) (γ is forward's hs_coeff[0], so the weight on the content is 1 - γ).
+        The content h at t_0, which the inversion never evaluates, is the bottleneck h of the content's x_T at t_0.
+        Rows are (pair, γ), whole pairs per replay of at most --max_rows_per_replay rows; each row draws its own
+        noise for the eta = 1 steps.  Writes <save_dir>/<content stem>__<style stem>.png: content x0, style x0, one
+        result per γ.  Returns {(content path, style path): results [len(γ)][3][S][S]}."""
+        import torchvision.utils as tvu
+        a = self.args
+        contents, styles, gammas = self.diff_style_setup()
+        print(f"DiffStyle: hs_coeff {gammas} (slerp weight on the content h: 1 - hs_coeff)")
+        model = self.load_pretrained_model().to(self.device)
+        if self.world > 1 and torch.distributed.is_initialized():
+            broadcast_weights(model)
+        eng = model.engine
+        cached = self.precompute_pairs_with_h(model, contents + styles)
+        sch = self.diff_style_schedule(gammas[0])
+        t0 = sch.steps[0].t
+        # content h at t_0: one plain UNet evaluation of each content's x_T
+        h_c = {}
+        bs = min(max(1, a.bs_train), len(contents))
+        for k in range(0, len(contents), bs):
+            chunk = contents[k:k + bs]
+            x_T = pad_rows(torch.cat([cached[p][2] for p in chunk]), bs).to(eng.device)
+            mid = eng.forward(x_T, torch.full((bs,), float(t0), device=eng.device))[3].cpu()
+            for i, p in enumerate(chunk):
+                h_c[p] = dict(cached[p][3])
+                h_c[p][t0] = mid[i:i + 1].clone()
+        pairs = [(c, s_) for c in contents for s_ in styles]
+        ppc, chunks = plan_sweep(len(pairs), len(gammas), getattr(a, "max_rows_per_replay", 16))
+        R = ppc * len(gammas)
+        edit_ts = [st.t for st in sch.steps if st.edit]
+        print(f"DiffStyle: {len(pairs)} pairs, {len(pairs) * len(gammas)} rows, {len(chunks)} replays of {R} rows")
+        os.makedirs(a.save_dir, exist_ok=True)
+        results = {}
+        for ci, chunk in enumerate(chunks):
+            if ci % self.world != self.rank:  # chunks sharded round-robin across ranks
+                continue
+            rows = [(pairs[q], g) for q in chunk for g in gammas]
+            rows += [rows[-1]] * (R - len(rows))
+            x_T = torch.cat([cached[s_][2] for (_, s_), _ in rows])
+            kw = {"hs_coeffs": torch.tensor([[g] for _, g in rows], dtype=torch.float32), "use_mask": bool(a.use_mask)}
+            if edit_ts:
+                kw["delta_hs"] = diff_style_delta_hs([h_c[c] for (c, _), _ in rows], edit_ts)
+            noise = None
+            if sch.n_stochastic:  # one draw per row, made on the device up front
+                noise = torch.cat([torch.randn((sch.n_stochastic, 1, *x_T.shape[1:]), device=eng.device)
+                                   for _ in range(len(chunk) * len(gammas))], dim=1)
+                noise = pad_rows(noise.transpose(0, 1), R).transpose(0, 1).contiguous()
+            x0 = self.edit_batch(model, x_T, sch, noise=noise, **kw)
+            for j, q in enumerate(chunk):
+                c, s_ = pairs[q]
+                res = x0[j * len(gammas):(j + 1) * len(gammas)].clone()
+                results[(c, s_)] = res
+                grid = (torch.cat([cached[c][0].cpu(), cached[s_][0].cpu(), res]) + 1) * 0.5
+                tvu.save_image(tvu.make_grid(grid, nrow=grid.shape[0], padding=1),
+                               os.path.join(a.save_dir, f"{_stem(c)}__{_stem(s_)}.png"))
+        return results
+
+
+def diff_style_gammas(hs_coeff, hs_coeff_list):
+    """the hs_coeff values of a --diff_style run: --hs_coeff_list ("0.9 0.7 0.5"), else [--hs_coeff]"""
+    if not hs_coeff_list:
+        return [float(hs_coeff)]
+    if float(hs_coeff) != 0.9:
+        raise ValueError(f"--diff_style: give either --hs_coeff ({hs_coeff}) or --hs_coeff_list, not both")
+    try:
+        gammas = [float(v) for v in str(hs_coeff_list).split()]
+    except ValueError:
+        raise ValueError(f"--hs_coeff_list {hs_coeff_list!r} is not a list of numbers") from None
+    if not gammas:
+        raise ValueError("--hs_coeff_list names no value")
+    return gammas
+
+
+def image_paths(folder):
+    """every png / jpg of a directory, sorted"""
+    return sorted(os.path.join(folder, f) for f in os.listdir(folder) if f.lower().endswith((".png", ".jpg", ".jpeg")))
+
+
+def diff_style_cache_path(category, n_inv_step, img_path):
+    """precompute_pairs_with_h's cache file (diffusion_latent.py:883-885), the reference's expression kept as is: the
+    last two '/'-parts of the text before the path's last dot ("c/x.png" -> c_x; a dot in a directory name cuts the
+    directories before it, "a.b/c/x.png" -> c_x, and a dotted stem keeps its last part only, "c/x.v1.png" -> v1)"""
+    name = "_".join(img_path.split(".")[-2].split('/')[-2:])
+    return os.path.join('precomputed', category + '_inv' + str(n_inv_step) + '_' + name + '.pt')
+
+
+def diff_style_image(path, size):
+    """precompute_pairs_with_h's transform (:896-906): centre crop to the shorter side, Resize((size, size)),
+    ToTensor, Normalize(0.5, 0.5) -> [1,3,size,size] in [-1, 1]"""
+    from PIL import Image
+    from torchvision import transforms
+    image = Image.open(path).convert('RGB')
+    image = transforms.CenterCrop(min(image.size))(image)
+    tf = transforms.Compose([transforms.Resize((size, size)), transforms.ToTensor(),
+                             transforms.Normalize((0.5, 0.5, 0.5), (0.5, 0.5, 0.5))])
+    return tf(image)[None]
+
+
+def diff_style_delta_hs(h_dics, edit_ts):
+    """delta_hs of UNetEngine.sample for rows with their own content h: [edit steps][rows][C][h][w], row r's h_dics[r][t]
+    at every edit step t"""
+    out = []
+    for t in edit_ts:
+        missing = [r for r, d in enumerate(h_dics) if int(t) not in d]
+        if missing:
+            raise KeyError(f"DiffStyle: no content h at edit step t={t} (rows {missing})")
+        out.append(torch.cat([d[int(t)].float() for d in h_dics]))
+    return torch.stack(out)
+
+
+def _stem(path):
+    return os.path.splitext(os.path.basename(path))[0]
 
 
 def sweep_rows(chunk, tpc, bs):

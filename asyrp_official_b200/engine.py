@@ -322,6 +322,15 @@ def shared_c0(table):
     return float(c0[0])
 
 
+def slerp_rows(table):
+    """the per-sample slerp weights of explicit Δh rows, fp32 [N]: float(1 - c0_n), rounded as the scalar weight
+    1 - c0 is when it is passed to the kernel; None when c0 is one value (the scalar kernel serves the batch)"""
+    c0 = table[:, 0].cpu()
+    if bool((c0 == c0[0]).all()):
+        return None
+    return torch.tensor([1.0 - float(c) for c in c0], dtype=torch.float32)
+
+
 class Plan:
     """Static launch sequence for one batch size"""
 
@@ -639,11 +648,19 @@ class Plan:
         # explicit delta_h (DiffStyle / raw delta_h checkpoints): h2 = slerp(1-c0, h, |h| dh/|dh|), written into the same
         # h2 buffer (+ its GroupNorm partial sums) the DeltaBlock path produces, so the decoder plan is shared
         self.dh_user = torch.zeros(N, a.mid_ch, h.H, h.W, dtype=torch.float32, device=dev)
+        # per-sample slerp weights (state "slerp_rows"): a graph input, so every weight table replays one graph
+        self.slerp_w = torch.zeros(N, dtype=torch.float32, device=dev)
         self.slerp_ops = []
         self._cur = self.slerp_ops
         st = eng.state
-        self._emit(lambda: ops.slerp_h(self.middle_h.t, self.dh_user, self.h2.t, self.h2.stats, st["slerp_t"],
-                                       st["use_mask"]), "slerp")
+
+        def slerp():
+            if st["slerp_rows"]:
+                ops.slerp_h_rows(self.middle_h.t, self.dh_user, self.h2.t, self.h2.stats, self.slerp_w, st["use_mask"])
+            else:
+                ops.slerp_h(self.middle_h.t, self.dh_user, self.h2.t, self.h2.stats, st["slerp_t"], st["use_mask"])
+
+        self._emit(slerp, "slerp")
         # ---- decoders: (h2 -> et_mod) and (h -> et); same weights, same skip tensors.  The second pass allocates from
         # its own pool: in an edit step the two passes are independent and run CONCURRENTLY on two streams
         # (run_edit_and_decoder) — a persistent conv kernel leaves SMs idle in its last wave (512 tiles on 132 SMs =
@@ -848,7 +865,7 @@ class UNetEngine:
             raise ops._lib.AsyrpError("UNetEngine needs a CUDA device (sm_90a); there is no CPU path")
         ops._lib.load()
         self.arch, self.device, self.n_delta = arch, torch.device(device), n_delta
-        self.state = {"ignore_timestep": False, "slerp_t": 0.0, "use_mask": False}
+        self.state = {"ignore_timestep": False, "slerp_t": 0.0, "use_mask": False, "slerp_rows": False}
         with torch.cuda.device(self.device):
             self.W, self.emb_off, self.emb_total = pack_weights(arch, state_dict, self.device, n_delta)
         self.plans = {}
@@ -888,6 +905,7 @@ class UNetEngine:
                 P.dh_user.copy_(dh if dh.dim() == 4 else dh[None].expand_as(P.dh_user))
                 c0 = shared_c0(table) if table is not None else float(hs_coeff[0])
                 self.state["slerp_t"], self.state["use_mask"] = 1.0 - c0, bool(use_mask)
+                self.state["slerp_rows"] = False
                 P.run_edit(explicit=True)
                 delta = delta_h  # the reference returns the tensor it was given
             elif edit:
@@ -916,7 +934,8 @@ class UNetEngine:
     # ---- whole trajectory --------------------------------------------------------------------------
     MAX_GRAPHS = 4  # captured trajectory graphs kept per engine (least recently used is dropped)
 
-    def _build_trajectory(self, P, schedule, use_graph, explicit, record_dh, record_process, lpips=None):
+    def _build_trajectory(self, P, schedule, use_graph, explicit, record_dh, record_process, lpips=None,
+                          record_h=False):
         """per-(batch, schedule) state: the timestep-embedding table, the noise buffer, the step loop and its graph"""
         steps = schedule.steps
         n_sto = schedule.n_stochastic
@@ -942,6 +961,8 @@ class UNetEngine:
         if record_process:  # x_t and x0_t after every step (save_process_*, :485-491,523-527)
             rec["x"] = torch.zeros((len(steps), *P.x.shape), dtype=torch.float32, device=self.device)
             rec["x0_t"] = torch.zeros((len(steps), *P.x.shape), dtype=torch.float32, device=self.device)
+        if record_h:  # the bottleneck h of every step (precompute_pairs_with_h's h_dic, diffusion_latent.py:931-939)
+            rec["h"] = torch.zeros((len(steps), *P.mid_f32.shape), dtype=torch.float32, device=self.device)
         N = P.x.shape[0]
         if lpips is not None:
             # LPIPS(x_t, x_start) and LPIPS(x0_t, x_start) after every step (compute_lpips_distance,
@@ -971,6 +992,8 @@ class UNetEngine:
             for k, s in enumerate(steps):
                 P.emb_all.copy_(emb_table[k])
                 P.run_encoder()
+                if record_h:
+                    ops.unpack_nchw(P.middle_h.t, rec["h"][k])
                 edit = is_edit(s)
                 if edit:
                     if explicit:
@@ -995,7 +1018,7 @@ class UNetEngine:
                 if lpips is not None:
                     lpips_step(k)
 
-        n_launch = sum(len(P.launches(False, temb=False)) + 1 for s in steps)
+        n_launch = sum(len(P.launches(False, temb=False)) + 1 + int(record_h) for s in steps)
         n_launch += n_edit * ((len(P.slerp_ops) if explicit else len(P.delta_ops)) + len(P.dec_mod_ops) + int(record_dh))
         if lpips is not None:
             from .lpips import LAUNCHES_DISTANCE, LAUNCHES_FEATURES
@@ -1118,7 +1141,7 @@ class UNetEngine:
             if n_sto and (noise is None or noise.shape[0] != n_sto or noise.shape[1] != N):
                 raise ops._lib.AsyrpError(f"pre-drawn noise [{n_sto}][{N}][..] required for the stochastic steps")
             self.state["ignore_timestep"] = schedule.ignore_timestep
-            self.state["slerp_t"], self.state["use_mask"] = 0.0, False
+            self.state["slerp_t"], self.state["use_mask"], self.state["slerp_rows"] = 0.0, False, False
             g = self.graphs.pop(key, None)
             if g is None:
                 g = self._build_row_trajectory(P, schedule, use_graph, own, record_process)
@@ -1142,7 +1165,7 @@ class UNetEngine:
             return out
 
     def sample(self, x_T, schedule, noise=None, use_graph=True, out=None, delta_hs=None, use_mask=False,
-               record_dh=False, record_process=False, hs_coeffs=None, lpips=None):
+               record_dh=False, record_process=False, hs_coeffs=None, lpips=None, record_h=False):
         """Run the reverse trajectory of `schedule` (sampler.Schedule) from x_T; returns x_0 (fp32 NCHW).
 
         The step list, the edit/plain/stochastic phase of every step and all sampler coefficients are host-side
@@ -1158,8 +1181,14 @@ class UNetEngine:
 
         hs_coeffs: per-sample coefficients, fp32 [N][1 + n_delta] (host or device), overriding schedule.hs_coeff row by
         row.  Like the tuple they are graph inputs: every table replays the same captured graph, and sample n's result
-        is bit-identical to a batch-1 run with row n as schedule.hs_coeff.  With delta_hs the c0 column must be constant
-        (one slerp weight for the batch).
+        is bit-identical to a batch-1 run with row n as schedule.hs_coeff.  With delta_hs shared by the batch
+        ([n_edit][C][h][w]) the c0 column must be constant (one slerp weight for the batch).  With per-sample delta_hs
+        rows ([n_edit][N][C][h][w], DiffStyle's content h per row) it may differ: sample n's slerp weight
+        float(1 - c0_n) is then read from a device array (ops.slerp_h_rows), a graph input like the table itself, and
+        sample n equals a batch-1 run with c0_n bit for bit.
+
+        record_h: keep the bottleneck h (the middle_h forward() returns) of every step in `last_records["h"]`,
+        [steps][N][C][h][w] fp32 (precompute_pairs_with_h's h_dic).  Recording does not change the trajectory.
 
         lpips: an asyrp_official_b200.lpips.LPIPS.  The graph then computes the LPIPS features of its starting image
         once, at its head, and after every step's DDIM update the distances of x_t and of x0_t to it
@@ -1169,34 +1198,45 @@ class UNetEngine:
         schedule may also be a schedule.RowSchedule: every row its own t_edit, t_addnoise and coefficients, each row
         editing with one DeltaBlock.  Row n then equals, bit for bit, a run of its own Schedule on an engine with only
         its block packed, fed the noise entries of the steps at which it is stochastic (RowSchedule.noise_rows).
-        noise: [n_stochastic][N][C][H][W] over the steps at which any row is stochastic.  delta_hs, record_dh, hs_coeffs
-        and lpips do not apply."""
+        noise: [n_stochastic][N][C][H][W] over the steps at which any row is stochastic.  delta_hs, record_dh, hs_coeffs,
+        lpips and record_h do not apply."""
         if isinstance(schedule, RowSchedule):
-            if delta_hs is not None or record_dh or hs_coeffs is not None or lpips is not None:
-                raise ops._lib.AsyrpError("a per-row schedule takes no delta_hs, record_dh, hs_coeffs or lpips")
+            if delta_hs is not None or record_dh or hs_coeffs is not None or lpips is not None or record_h:
+                raise ops._lib.AsyrpError("a per-row schedule takes no delta_hs, record_dh, hs_coeffs, lpips or "
+                                          "record_h")
             return self._sample_rows(x_T, schedule, noise, use_graph, out, record_process)
         N = x_T.shape[0]
         P = self.plan(N)
         explicit = delta_hs is not None
         table = coeff_table(hs_coeffs, N, self.n_delta) if hs_coeffs is not None else None
-        if explicit:
+        rows_w = None
+        if explicit and table is not None and delta_hs.dim() == 5:
+            rows_w = slerp_rows(table)
+        if rows_w is not None:
+            slerp_t = "rows"
+        elif explicit:
             slerp_t = 1.0 - (shared_c0(table) if table is not None else float(schedule.hs_coeff[0]))
         else:
             slerp_t = 0.0
         key = (N, bool(use_graph), schedule.key(), explicit, slerp_t, bool(use_mask) if explicit else False,
-               bool(record_dh), bool(record_process)) + ((lpips,) if lpips is not None else ())
+               bool(record_dh), bool(record_process)) + ((lpips,) if lpips is not None else ()) + \
+            (("record_h",) if record_h else ())
         with torch.cuda.device(self.device):
             n_sto = schedule.n_stochastic
             if n_sto:
                 assert noise is not None and noise.shape[0] == n_sto, "pre-drawn noise required for stochastic steps"
             # kernel variants / parameters baked at capture time (all part of `key`)
             self.state["ignore_timestep"] = schedule.ignore_timestep
-            self.state["slerp_t"], self.state["use_mask"] = slerp_t, bool(use_mask)
+            self.state["slerp_t"] = 0.0 if rows_w is not None else slerp_t
+            self.state["use_mask"], self.state["slerp_rows"] = bool(use_mask), rows_w is not None
             if record_dh and (explicit or self.n_delta == 0):
                 raise ops._lib.AsyrpError("record_dh needs the DeltaBlock path")
+            if rows_w is not None:
+                P.slerp_w.copy_(rows_w)
             g = self.graphs.pop(key, None)
             if g is None:
-                g = self._build_trajectory(P, schedule, use_graph, explicit, record_dh, record_process, lpips)
+                g = self._build_trajectory(P, schedule, use_graph, explicit, record_dh, record_process, lpips,
+                                           record_h)
                 while len(self.graphs) >= self.MAX_GRAPHS:
                     self.graphs.pop(next(iter(self.graphs)))
             self.graphs[key] = g  # most recently used last

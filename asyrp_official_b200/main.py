@@ -6,6 +6,12 @@
         --manual_checkpoint_name smiling_LC_CelebA_HQ_t999_ninv40_ngen40_0.pth --model_path celeba_hq.ckpt \
         --n_test_img 32 --bs_train 16 --n_test_step 40 --n_train_step 40
 
+DiffStyle content injection (main.py:192-202; the loop is this build's composition of the reference's functions):
+
+    python -m asyrp_official_b200.main --diff_style --config celeba.yml --model_path celeba_hq.ckpt \
+        --content_dir content --style_dir style --save_dir results --user_defined_t_edit 400 \
+        --hs_coeff_list "0.9 0.7 0.5" --t_noise 200 --dt_lambda 0.9985 --dt_end 950 --bs_train 8
+
 Multi-GPU: launch with torchrun (one process per GPU); image batches are sharded across ranks.
 """
 import argparse
@@ -84,6 +90,14 @@ def build_parser():
     p.add_argument('--custom_test_dataset_dir', type=str, default="./custom/test")
     p.add_argument('--dt_lambda', type=float, default=1.0)
     p.add_argument('--dt_end', type=int, default=950)
+    # DiffStyle (main.py:192-202)
+    p.add_argument('--diff_style', **sa)
+    p.add_argument('--content_dir', type=str, default="./source_images/content")
+    p.add_argument('--style_dir', type=str, default="./source_images/style")
+    p.add_argument('--save_dir', type=str, default="./results")
+    p.add_argument('--hs_coeff', type=float, default=0.9)
+    p.add_argument('--use_mask', **sa)
+    p.add_argument('--t_noise', type=int, default=0)
     p.add_argument('--n_iter', type=int, default=1)
     # additions of this build (documented in INTEGRATION.md)
     p.add_argument('--synthetic_weights', **sa, help='seeded random UNet weights instead of --model_path')
@@ -112,6 +126,9 @@ def build_parser():
     p.add_argument('--max_rows_per_replay', type=int, default=16,
                    help='rows (hs_coeff tuples x images) of one batched trajectory in save_image; bounds the memory of '
                         'the per-batch plan (DDPM 256x256: about 4.3 GB at 16 rows); 1 = one replay per tuple')
+    p.add_argument('--hs_coeff_list', type=str, default='',
+                   help='--diff_style: several hs_coeff values ("0.9 0.7 0.5"), one result per value for every '
+                        'content / style pair, run as rows of one batch')
     p.add_argument('--attr_sweep', type=str, default='',
                    help='--run_test: edit every image with each of these attributes ("smiling angry young"), one grid '
                         'row per attribute, each row what --edit_attr <attribute> gives with its own t_edit / '
@@ -152,12 +169,14 @@ def main(argv=None):
         dist.init_process_group("nccl")
     runner = Asyrp(args, config)
     try:
-        if args.run_test:
+        if args.diff_style:
+            runner.run_diff_style()
+        elif args.run_test:
             runner.run_test()
         elif args.lpips:
             runner.compute_lpips_distance()
         else:
-            print('Choose one mode! (this build implements --run_test and --lpips)')
+            print('Choose one mode! (this build implements --run_test, --lpips and --diff_style)')
             raise ValueError
     except Exception:
         logging.error(traceback.format_exc())

@@ -311,6 +311,20 @@ def slerp_h(h, dh, h2, stats, t, use_mask=False):
                             int(use_mask), _stream()), "asyrp_slerp_h")
 
 
+def slerp_h_rows(h, dh, h2, stats, t_rows, use_mask=False):
+    """slerp_h with sample n's weight read from t_rows[n]: t_rows fp32 [N] on the device (row n gives the bits of
+    slerp_h with t = t_rows[n])"""
+    lib = _lib.load()
+    N, H, W, Cc = h.shape
+    assert dh.is_contiguous() or (dh.dim() == 4 and dh[0].is_contiguous()), "dh must be dense [C][H][W] per sample"
+    if not (t_rows.is_cuda and t_rows.dtype == torch.float32 and tuple(t_rows.shape) == (N,) and t_rows.is_contiguous()):
+        raise _lib.AsyrpError(f"slerp_h_rows: t_rows must be a contiguous fp32 [{N}] device tensor, got "
+                              f"{t_rows.dtype} {tuple(t_rows.shape)} on {t_rows.device}")
+    stride = dh.stride(0) if dh.dim() == 4 else 0
+    check(lib.asyrp_slerp_h_rows(_ptr(h), _ptr(dh), stride, _ptr(h2), _ptr(stats), stats.shape[1], N, Cc, H, W,
+                                 _ptr(t_rows), int(use_mask), _stream()), "asyrp_slerp_h_rows")
+
+
 def transpose_tc(inp, out):
     """inp [N][T][C] (may be a channel slice: last-dim stride 1, row stride ld) -> out [N][C][T] fp16"""
     lib = _lib.load()

@@ -213,6 +213,11 @@ int asyrp_axpby(const void* a, const void* b, void* out, float alpha, float beta
 int asyrp_slerp_h(const void* h, const float* dh, long long dh_sample_stride, void* h2, float* stats, int stats_tiles,
                   int N, int C, int H, int W, float t, int use_mask, void* stream);
 
+/* asyrp_slerp_h with the slerp weight of sample n read from t_rows[n] (fp32 [N], device memory); sample n gives the
+ * bits of asyrp_slerp_h with t = t_rows[n] (DiffStyle rows with their own hs_coeff in one batch). */
+int asyrp_slerp_h_rows(const void* h, const float* dh, long long dh_sample_stride, void* h2, float* stats,
+                       int stats_tiles, int N, int C, int H, int W, const float* t_rows, int use_mask, void* stream);
+
 /* NHWC fp16 [N][HW][C] -> NCHW fp32 (API-visible delta_h / middle_h) */
 int asyrp_unpack_nchw(const void* in, float* out, int N, int C, int HW, void* stream);
 

@@ -114,6 +114,17 @@ SIGNATURES = {
                                        c_int, c_int, c_int, c_int, c_int, c_int, c_void_p]),
     "asyrp_arcface_l2norm": (c_int, [c_void_p, c_void_p, c_int, c_int, c_void_p]),
     "asyrp_arcface_dot": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p]),
+    "asyrp_faceparse_pack": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p]),
+    "asyrp_faceparse_conv": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int,
+                                     c_int, c_int, c_int, c_int, c_int, c_void_p]),
+    "asyrp_faceparse_maxpool": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p]),
+    "asyrp_faceparse_gate": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p, c_int, c_int,
+                                     c_void_p, c_int, c_int, c_int, c_void_p]),
+    "asyrp_faceparse_apply": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_int, c_int, c_int, c_int, c_int,
+                                      c_void_p]),
+    "asyrp_faceparse_labels": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p]),
+    "asyrp_faceparse_agreement": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_int,
+                                          c_int, c_int, c_void_p]),
 }
 
 _lib = None

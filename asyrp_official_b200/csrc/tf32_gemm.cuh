@@ -1,6 +1,6 @@
 // The fp32-in / fp32-out implicit GEMM on the tensor cores shared by the LPIPS convs (lpips.cu), the CLIP towers'
-// linear layers (clip_text.cu, a linear layer being a 1x1 conv over a 1 x M image) and the ArcFace IR-SE50 convs
-// (arcface.cu): mma.sync m16n8k8, TF32
+// linear layers (clip_text.cu, a linear layer being a 1x1 conv over a 1 x M image), the ArcFace IR-SE50 convs
+// (arcface.cu) and the face-parsing BiSeNet convs (face_parsing.cu): mma.sync m16n8k8, TF32
 // operands rounded to nearest, fp32 accumulation, M = N*Ho*Wo output pixels, N = Cout, K = kh*kw*Cin tap-major /
 // channel-minor.  The epilogue is a template parameter; the main loop is the same code for every epilogue, so an
 // output element is the same fixed-order accumulation whichever layer or batch it belongs to.
@@ -27,6 +27,7 @@ enum Epilogue : int {
   kEpiQuickGelu = 2,  // v * sigmoid(1.702 v)       (CLIP's QuickGELU)
   kEpiResidual = 3,   // residual + v               (residual may be out: read and written by the same thread)
   kEpiPrelu = 4,      // v > 0 ? v : prelu[c] * v   (ArcFace's per-channel PReLU; bias may be null)
+  kEpiResidualRelu = 5,  // max(residual + v, 0)    (BiSeNet's BasicBlock end; bias may be null)
 };
 
 __device__ __forceinline__ void cp_async16(uint32_t dst, const void* src, int bytes) {
@@ -54,7 +55,7 @@ struct Tf32ConvParams {
   const float* in;        // [N][H][W][Cin]
   const float* w;         // [Cout][Kpad], K = kh*kw*Cin tap-major / channel-minor, zero columns past K
   const float* bias;      // [Cout]
-  const float* residual;  // [M][Cout] (kEpiResidual only)
+  const float* residual;  // [M][Cout] (kEpiResidual, kEpiResidualRelu)
   const float* prelu;     // [Cout] PReLU slopes (kEpiPrelu only)
   float* out;             // [N][Ho][Wo][Cout]
   int N, H, W, Cin, Ho, Wo, Cout, kw, stride, pad, K, Kpad, M;
@@ -194,6 +195,9 @@ __global__ void __launch_bounds__(kThreads) tf32_conv_kernel(const Tf32ConvParam
           } else if (kEpi == kEpiResidual) {
             const float2 r = *reinterpret_cast<const float2*>(p.residual + o);
             v = make_float2(r.x + v.x, r.y + v.y);
+          } else if (kEpi == kEpiResidualRelu) {
+            const float2 r = *reinterpret_cast<const float2*>(p.residual + o);
+            v = make_float2(fmaxf(r.x + v.x, 0.f), fmaxf(r.y + v.y, 0.f));
           } else if (kEpi == kEpiPrelu) {
             v = make_float2(v.x > 0.f ? v.x : p.prelu[c] * v.x, v.y > 0.f ? v.y : p.prelu[c + 1] * v.y);
           }

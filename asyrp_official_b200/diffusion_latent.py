@@ -16,6 +16,9 @@ Mirrors, with the same attribute / flag names:
   --id_similarity              losses/id_loss.py            run_test scores every edit with 1 - IDLoss (ArcFace IR-SE50,
                                                             arcface.ArcFace), written next to the PNG; the reference
                                                             uses IDLoss only in training
+  --seg_consistency            (none)                       run_test scores every edit with the segmentation consistency
+                                                            of a face-parsing BiSeNet (face_parsing.FaceParser), written
+                                                            next to the PNG; this build's definition
   Asyrp.precompute_pairs_with_h :877-947                    DDIM inversion of one image keeping the bottleneck h of
                                                             every step (batched here, same cache file)
   Asyrp.run_diff_style         main.py:192-202              --diff_style (DiffStyle content injection): this build's
@@ -70,6 +73,7 @@ class Asyrp(object):
         self.world = int(os.environ.get("WORLD_SIZE", "1"))
         self.directional_clip = {}  # --DirectionalClipSmilarity: save_image's file name -> S_dir [tuples][images]
         self.id_similarity = {}  # --id_similarity: save_image's file name -> 1 - IDLoss [tuples][images]
+        self.seg_consistency = {}  # --seg_consistency: save_image's file name -> SC [tuples][images]
 
     # ------------------------------------------------------------------------------------------
     def load_pretrained_model(self):
@@ -215,6 +219,22 @@ class Asyrp(object):
             return load_state_dict(path)
         except ValueError as e:
             raise ValueError(f"--id_similarity: {e}") from None
+
+    def seg_consistency_setup(self):
+        """--seg_consistency's requirements, checked before any model is loaded; raises ValueError with the reason.
+        Returns the validated --seg_weights state dict (face_parsing.load_state_dict)."""
+        from .face_parsing import load_state_dict
+        a = self.args
+        if getattr(a, "pass_editing", False):
+            raise ValueError("--seg_consistency scores the edited images: with --pass_editing nothing is edited")
+        path = getattr(a, "seg_weights", None)
+        if not path or not os.path.isfile(path):
+            raise ValueError(f"--seg_consistency: --seg_weights {path!r} is not a file (a torch.save of the face-parsing "
+                             "BiSeNet(n_classes=19) state dict, e.g. 79999_iter.pth)")
+        try:
+            return load_state_dict(path)
+        except ValueError as e:
+            raise ValueError(f"--seg_consistency: {e}") from None
 
     def write_id_similarity(self, path, coeffs, ids):
         """the TSV of one batch: one row per (hs_coeff tuple, image) in grid order, ID = 1 - IDLoss(origin, edit) of
@@ -395,7 +415,7 @@ class Asyrp(object):
     def save_image(self, model, x_lat_tensor, seq_inv, seq_inv_next, save_x0=False, save_x_origin=False,
                    save_process_delta_h=False, save_process_origin=False, x0_tensor=None, delta_h_dict=None,
                    get_delta_hs=False, folder_dir="", file_name="", hs_coeff=(1.0, 1.0), directional_clip=None,
-                   id_scorer=None):
+                   id_scorer=None, seg_scorer=None):
         """rows of the grid: [x0] [origin DDIM] one row per hs_coeff tuple  (diffusion_latent.py:445-544).
 
         delta_h_dict: {t: None | Δh tensor}.  Entries that are tensors select the explicit-Δh branch for that step
@@ -407,7 +427,10 @@ class Asyrp(object):
         self.directional_clip[file_name].
         id_scorer: an arcface.ArcFace for --id_similarity: the same for 1 - IDLoss against the same origin pass (which
         runs once for both scores), written to <file_name>_ngen<n_train_step>_id_similarity.tsv and kept in
-        self.id_similarity[file_name]."""
+        self.id_similarity[file_name].
+        seg_scorer: a face_parsing.FaceParser for --seg_consistency: the same for the segmentation consistency against
+        the same origin pass, written to <file_name>_ngen<n_train_step>_seg_consistency.tsv and kept in
+        self.seg_consistency[file_name]."""
         import torchvision.utils as tvu
         a = self.args
         time_s = time.time()
@@ -416,7 +439,7 @@ class Asyrp(object):
         x_list, edited = [], []
         if save_x0 and x0_tensor is not None:
             x_list.append(x0_tensor.cpu())
-        if save_x_origin or directional_clip is not None or id_scorer is not None:
+        if save_x_origin or directional_clip is not None or id_scorer is not None or seg_scorer is not None:
             sch = self.make_schedule(seq_inv, seq_inv_next, (1.0,), edit=False,
                                      addnoise=bool(getattr(a, "origin_process_addnoise", False)))
             if save_x_origin:
@@ -501,6 +524,11 @@ class Asyrp(object):
             self.id_similarity[file_name] = ids
             self.write_id_similarity(
                 os.path.join(folder_dir, f'{file_name}_ngen{a.n_train_step}_id_similarity.tsv'), coeffs, ids)
+        if seg_scorer is not None and edited:
+            sc = seg_scorer.seg_consistency(origin, torch.cat(edited)).view(len(edited), bs)
+            self.seg_consistency[file_name] = sc
+            write_scores(os.path.join(folder_dir, f'{file_name}_ngen{a.n_train_step}_seg_consistency.tsv'), coeffs, sc,
+                         "SC", "segmentation consistency")
         print(f'{time.time() - time_s} seconds, {file_name}_ngen{a.n_train_step}.png is saved')
         return x_list
 
@@ -609,6 +637,7 @@ class Asyrp(object):
                   "utils/diffusion_utils.py:103-109)")
         sdir = self.directional_clip_setup() if getattr(a, "DirectionalClipSmilarity", False) else None
         id_sd = self.id_similarity_setup() if getattr(a, "id_similarity", False) else None
+        seg_sd = self.seg_consistency_setup() if getattr(a, "seg_consistency", False) else None
         if a.multiple_attr and self.needs_clip() and self.clip_configured():
             cosine = self.choose_attribute(a.multiple_attr.split(' '))  # :640-652
             self.set_t_edit_t_addnoise(LPIPS_th=a.lpips_edit_th, LPIPS_addnoise_th=a.lpips_addnoise_th, cosine=cosine)
@@ -717,7 +746,7 @@ class Asyrp(object):
         if getattr(a, "target_image_id", None):
             target_ids = [int(i) for i in str(a.target_image_id).split(" ")]
             assert a.bs_train == 1, "target_image_id is only supported for batch_size == 1"
-        results, directional_clip, id_scorer = {}, None, None
+        results, directional_clip, id_scorer, seg_scorer = {}, None, None, None
         if sdir is not None:  # the image tower lives for this run_test only
             from .clip_image import CLIPLoss
             directional_clip = (CLIPLoss(a.clip_weights, a.clip_vocab, sdir[2], device=self.device), sdir[0], sdir[1])
@@ -726,6 +755,10 @@ class Asyrp(object):
                 from .arcface import ArcFace
                 id_scorer = ArcFace(id_sd, device=self.device)
                 id_sd = None
+            if seg_sd is not None:  # and the face parser
+                from .face_parsing import FaceParser
+                seg_scorer = FaceParser(seg_sd, device=self.device)
+                seg_sd = None
             for mode, do, n_img in (("train", a.do_train, a.n_train_img), ("test", a.do_test, a.n_test_img)):
                 if not do:
                     continue
@@ -748,7 +781,7 @@ class Asyrp(object):
                             save_process_origin=bool(getattr(a, "save_process_origin", False)),
                             save_process_delta_h=bool(getattr(a, "save_process_delta_h", False)),
                             folder_dir=a.test_image_folder, file_name=f'{mode}_{step}_{a.n_iter - 1}', hs_coeff=hs_coeff,
-                            directional_clip=directional_clip, id_scorer=id_scorer)
+                            directional_clip=directional_clip, id_scorer=id_scorer, seg_scorer=seg_scorer)
                     batch_idx += 1
                     if step == n_img - 1:
                         break
@@ -772,8 +805,8 @@ class Asyrp(object):
                     x_lat_tensor, x0_tensor = None, None
         finally:
             a.train_delta_h = a_train_delta_h_prev
-            if directional_clip is not None or id_scorer is not None:
-                del directional_clip, id_scorer
+            if directional_clip is not None or id_scorer is not None or seg_scorer is not None:
+                del directional_clip, id_scorer, seg_scorer
                 torch.cuda.empty_cache()
         self.last_delta_h_dict = delta_h_dict
         return results
@@ -842,6 +875,7 @@ class Asyrp(object):
         if getattr(a, "DirectionalClipSmilarity", False):
             sdir = self.directional_clip_setup(attrs)
         id_sd = self.id_similarity_setup() if getattr(a, "id_similarity", False) else None
+        seg_sd = self.seg_consistency_setup() if getattr(a, "seg_consistency", False) else None
         times = self.attr_sweep_schedules(attrs)
         self.sweep_times = dict(zip(attrs, times))
         seq_test = [int(s + 1e-6) for s in list(np.linspace(0, 1, a.n_test_step) * a.t_0)]
@@ -869,7 +903,7 @@ class Asyrp(object):
             pairs = self.precompute_pairs(model)
         target_ids = [int(i) for i in str(a.target_image_id).split(" ")] if getattr(a, "target_image_id", None) \
             else None
-        results, directional_clip, id_scorer = {}, None, None
+        results, directional_clip, id_scorer, seg_scorer = {}, None, None, None
         if sdir is not None:
             from .clip_image import CLIPLoss
             directional_clip = (CLIPLoss(a.clip_weights, a.clip_vocab, sdir[1], device=self.device), sdir[0])
@@ -878,6 +912,10 @@ class Asyrp(object):
                 from .arcface import ArcFace
                 id_scorer = ArcFace(id_sd, device=self.device)
                 id_sd = None
+            if seg_sd is not None:
+                from .face_parsing import FaceParser
+                seg_scorer = FaceParser(seg_sd, device=self.device)
+                seg_sd = None
             for mode, do, n_img in (("train", a.do_train, a.n_train_img), ("test", a.do_test, a.n_test_img)):
                 if not do:
                     continue
@@ -895,14 +933,14 @@ class Asyrp(object):
                             model, x_lat_tensor, seq_test, seq_test_next, attrs, times, coeffs, save_x0=a.save_x0,
                             save_x_origin=a.save_x_origin, x0_tensor=x0_tensor,
                             folder_dir=a.test_image_folder, file_name=f'{mode}_{step}_{a.n_iter - 1}',
-                            directional_clip=directional_clip, id_scorer=id_scorer)
+                            directional_clip=directional_clip, id_scorer=id_scorer, seg_scorer=seg_scorer)
                     batch_idx += 1
                     if step == n_img - 1:
                         break
                     x_lat_tensor, x0_tensor = None, None
         finally:
-            if directional_clip is not None or id_scorer is not None:
-                del directional_clip, id_scorer
+            if directional_clip is not None or id_scorer is not None or seg_scorer is not None:
+                del directional_clip, id_scorer, seg_scorer
                 torch.cuda.empty_cache()
         return results
 
@@ -918,7 +956,7 @@ class Asyrp(object):
     @torch.no_grad()
     def save_image_sweep(self, model, x_lat_tensor, seq_inv, seq_inv_next, attrs, times, coeffs, save_x0=False,
                          save_x_origin=False, x0_tensor=None, folder_dir="", file_name="", directional_clip=None,
-                         id_scorer=None):
+                         id_scorer=None, seg_scorer=None):
         """save_image for an attribute sweep: grid rows [x0] [origin DDIM] then one row per attribute in the order
         given.  Rows of the trajectory are (attribute, image), attribute-major, run in chunks of whole attributes of
         at most --max_rows_per_replay rows (sweep_chunks).  directional_clip = (CLIPLoss, [(src_txt, trg_txt)] per
@@ -932,7 +970,7 @@ class Asyrp(object):
         x_list, edited, origin = [], [], None
         if save_x0 and x0_tensor is not None:
             x_list.append(x0_tensor.cpu())
-        if save_x_origin or directional_clip is not None or id_scorer is not None:
+        if save_x_origin or directional_clip is not None or id_scorer is not None or seg_scorer is not None:
             sch = self.make_schedule(seq_inv, seq_inv_next, (1.0,), edit=False,
                                      addnoise=bool(getattr(a, "origin_process_addnoise", False)))
             if save_x_origin:
@@ -966,6 +1004,11 @@ class Asyrp(object):
             self.id_similarity[file_name] = ids
             write_scores(os.path.join(folder_dir, f'{file_name}_ngen{a.n_train_step}_id_similarity.tsv'), coeffs,
                          ids, "ID", "identity similarity", attrs=attrs)
+        if seg_scorer is not None:
+            sc = seg_scorer.seg_consistency(origin, torch.cat(edited)).view(len(edited), bs)
+            self.seg_consistency[file_name] = sc
+            write_scores(os.path.join(folder_dir, f'{file_name}_ngen{a.n_train_step}_seg_consistency.tsv'), coeffs,
+                         sc, "SC", "segmentation consistency", attrs=attrs)
         print(f'{time.time() - time_s} seconds, {file_name}_ngen{a.n_train_step}.png is saved')
         return x_list
 

@@ -117,6 +117,12 @@ def build_parser():
                         'the unedited DDIM pass of the same x_T, written next to the PNG')
     p.add_argument('--id_weights', type=str, default='pretrained/model_ir_se50.pth',
                    help="the reference's ArcFace weights (MODEL_PATHS['ir_se50']) for --id_similarity")
+    p.add_argument('--seg_consistency', **sa,
+                   help='--run_test: score every edit for segmentation consistency, the fraction of 512 x 512 pixels '
+                        'whose face-parsing BiSeNet label equals that of the unedited DDIM pass of the same x_T, '
+                        'written next to the PNG')
+    p.add_argument('--seg_weights', type=str, default='pretrained/79999_iter.pth',
+                   help='torch.save of the face-parsing BiSeNet(n_classes=19) state dict for --seg_consistency')
     p.add_argument('--lpips_table_dir', type=str,
                    help='directory with <config stem>_LPIPS_distance_{x,x0_t}.tsv (read by --run_test, written by '
                         '--lpips; default utils)')

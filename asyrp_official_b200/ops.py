@@ -609,6 +609,101 @@ def arcface_dot(src, edited, out):
     check(lib.asyrp_arcface_dot(_ptr(src), _ptr(edited), _ptr(out), n, B, dim, _stream()), "asyrp_arcface_dot")
 
 
+FP_ACT_NONE, FP_ACT_RELU, FP_ACT_SIGMOID = 0, 1, 2
+
+
+def faceparse_pack(x, out):
+    """x fp32 [B][3][H][W] in [-1, 1] -> out fp32 NHWC [B][S][S][4]: clamp, map to [0, 1], bilinear resize to S x S
+    (align_corners=False), ImageNet normalisation; channel 3 zero"""
+    lib = _lib.load()
+    B, C, H, W = x.shape
+    S = out.shape[1]
+    _need_cuda(x, out)
+    assert C == 3 and x.dtype == torch.float32 and x.is_contiguous() and tuple(out.shape) == (B, S, S, 4)
+    assert out.dtype == torch.float32 and out.is_contiguous()
+    check(lib.asyrp_faceparse_pack(_ptr(x), _ptr(out), B, H, W, S, _stream()), "asyrp_faceparse_pack")
+
+
+def faceparse_conv(inp, weight, bias, out, k, stride, pad, relu=False, residual=None):
+    """out = conv(inp) + bias (bias may be None), then max(., 0) with relu, or max(residual + ., 0) with residual (the
+    BasicBlock end); fp32 NHWC, TF32 tensor cores; weight from pack_lpips_conv_weight"""
+    lib = _lib.load()
+    N, H, W, cin = inp.shape
+    cout = out.shape[-1]
+    _need_cuda(inp, weight, bias, out, residual)
+    assert inp.is_contiguous() and out.is_contiguous() and weight.is_contiguous()
+    assert tuple(weight.shape) == (cout, lpips_conv_kpad(cin, k, k)) and weight.dtype == torch.float32
+    assert tuple(out.shape) == (N, (H + 2 * pad - k) // stride + 1, (W + 2 * pad - k) // stride + 1, cout)
+    assert residual is None or (residual.shape == out.shape and residual.is_contiguous())
+    check(lib.asyrp_faceparse_conv(_ptr(inp), _ptr(weight), _ptr(bias), _ptr(residual), _ptr(out), N, H, W, cin, cout,
+                                   k, stride, pad, int(relu or residual is not None), _stream()),
+          "asyrp_faceparse_conv")
+
+
+def faceparse_maxpool(inp, out):
+    """MaxPool2d(3, 2, padding 1) over fp32 NHWC"""
+    lib = _lib.load()
+    N, H, W, Cc = inp.shape
+    _need_cuda(inp, out)
+    assert inp.is_contiguous() and out.is_contiguous() and tuple(out.shape) == (N, (H - 1) // 2 + 1, (W - 1) // 2 + 1,
+                                                                               Cc)
+    check(lib.asyrp_faceparse_maxpool(_ptr(inp), _ptr(out), N, H, W, Cc, _stream()), "asyrp_faceparse_maxpool")
+
+
+def faceparse_gate(inp, w1, b1, act1, out, w2=None, b2=None, act2=FP_ACT_NONE):
+    """per sample n of inp [N][H][W][C]: h = act1(w1 mean_hw(inp[n]) + b1), out[n] = act2(w2 h + b2), or h without w2;
+    w1 [C1][C], w2 [C2][C1], biases may be None"""
+    lib = _lib.load()
+    N, H, W, Cc = inp.shape
+    C1 = w1.shape[0]
+    C2 = w2.shape[0] if w2 is not None else 0
+    _need_cuda(inp, w1, b1, w2, b2, out)
+    assert inp.is_contiguous() and w1.is_contiguous() and tuple(w1.shape) == (C1, Cc)
+    assert w2 is None or (w2.is_contiguous() and tuple(w2.shape) == (C2, C1))
+    assert (b1 is None or b1.numel() == C1) and (b2 is None or b2.numel() == C2)
+    assert out.is_contiguous() and tuple(out.shape) == (N, C2 if w2 is not None else C1)
+    check(lib.asyrp_faceparse_gate(_ptr(inp), _ptr(w1), _ptr(b1), C1, int(act1), _ptr(w2), _ptr(b2), C2, int(act2),
+                                   _ptr(out), N, H * W, Cc, _stream()), "asyrp_faceparse_gate")
+
+
+def faceparse_apply(f, gate, add, out, up=1):
+    """out[n][y][x][c] = f[n][y/up][x/up][c] * gate[n][c] + add, add [N][C] (broadcast) or the size of f"""
+    lib = _lib.load()
+    N, H, W, Cc = f.shape
+    _need_cuda(f, gate, add, out)
+    add_map = add.dim() == 4
+    assert f.is_contiguous() and gate.is_contiguous() and add.is_contiguous() and out.is_contiguous()
+    assert tuple(gate.shape) == (N, Cc) and (add.shape == f.shape if add_map else tuple(add.shape) == (N, Cc))
+    assert tuple(out.shape) == (N, H * up, W * up, Cc)
+    check(lib.asyrp_faceparse_apply(_ptr(f), _ptr(gate), _ptr(add), int(add_map), _ptr(out), N, H, W, Cc, up,
+                                    _stream()), "asyrp_faceparse_apply")
+
+
+def faceparse_labels(logits, ncls, labels):
+    """labels uint8 [N][Ho][Wo] = argmax over classes 0..ncls-1 (the first wins a tie) of the bilinear align-corners
+    upsampling of logits fp32 NHWC [N][Hi][Wi][ld]"""
+    lib = _lib.load()
+    N, Hi, Wi, ld = logits.shape
+    _, Ho, Wo = labels.shape
+    _need_cuda(logits, labels)
+    assert logits.is_contiguous() and labels.is_contiguous() and labels.dtype == torch.uint8 and labels.shape[0] == N
+    check(lib.asyrp_faceparse_labels(_ptr(logits), _ptr(labels), N, Hi, Wi, ld, ncls, Ho, Wo, _stream()),
+          "asyrp_faceparse_labels")
+
+
+def faceparse_agreement(src_logits, edited_logits, ncls, out_hw, agree, row0=0):
+    """agree int32 [n]: pixels where the labels (faceparse_labels at out_hw) of edited row j equal those of source row
+    (row0 + j) % B; src_logits [B][Hi][Wi][ld], edited_logits [n][Hi][Wi][ld]"""
+    lib = _lib.load()
+    B, Hi, Wi, ld = src_logits.shape
+    n = edited_logits.shape[0]
+    _need_cuda(src_logits, edited_logits, agree)
+    assert src_logits.is_contiguous() and edited_logits.is_contiguous() and edited_logits.shape[1:] == src_logits.shape[1:]
+    assert agree.dtype == torch.int32 and agree.is_contiguous() and agree.numel() == n
+    check(lib.asyrp_faceparse_agreement(_ptr(src_logits), _ptr(edited_logits), _ptr(agree), n, B, int(row0), Hi, Wi, ld, ncls,
+                                        out_hw[0], out_hw[1], _stream()), "asyrp_faceparse_agreement")
+
+
 def ddpm_update(x, et, z, x_next, at, bt, logvar, learned_sigma, mask):
     lib = _lib.load()
     N, Cx, H, W = x.shape

@@ -77,6 +77,39 @@ def arcface_state_dict(seed=1234):
     return sd
 
 
+def face_parsing_state_dict(seed=1234, n_classes=19, aux=True):
+    """seeded face-parsing BiSeNet(n_classes) weights in its state-dict layout (asyrp_official_b200.face_parsing),
+    scaled so that activations stay O(1) through the 18 layers: convs U(-b, b) with b = gain * (3 / fan_in)^1/2, gain
+    2^1/2 (He's, for the ReLU) except the blocks' conv2 and the downsample convs (gain 1 / 2^1/2, so that a residual
+    sum of two O(1) terms stays O(1)) and the class layer (gain 4, so that class margins are a few units and the labels
+    follow the image rather than noise); BatchNorms weight 1 + N(0, .1^2), bias and running_mean N(0, .1^2),
+    running_var exp(N(0, .2^2)); num_batches_tracked 0.  aux: include the two auxiliary heads."""
+    from .face_parsing import aux_head_shapes, state_dict_shapes
+    shapes = {**state_dict_shapes(n_classes), **(aux_head_shapes(n_classes) if aux else {})}
+    sd = {}
+    for name, shp in shapes.items():
+        g = torch.Generator()
+        g.manual_seed((zlib.crc32(name.encode()) ^ (seed * 0x9E3779B1)) & 0x7FFFFFFF)
+        if len(shp) >= 2:
+            gain = 2 ** 0.5
+            if name.endswith("conv2.weight") and ".layer" in name or ".downsample." in name:
+                gain = 2 ** -0.5
+            elif name.endswith("conv_out.weight"):
+                gain = 4.0
+            b = gain * (3.0 / math.prod(shp[1:])) ** 0.5
+            sd[name] = (torch.rand(shp, generator=g) * 2 - 1) * b
+        elif name.endswith("running_var"):
+            sd[name] = torch.exp(0.2 * torch.randn(shp, generator=g))
+        elif name.endswith(".weight"):
+            sd[name] = 1.0 + 0.1 * torch.randn(shp, generator=g)
+        else:
+            sd[name] = 0.1 * torch.randn(shp, generator=g)
+    for name in list(sd):
+        if name.endswith("running_var"):
+            sd[name[:-len("running_var")] + "num_batches_tracked"] = torch.tensor(0, dtype=torch.long)
+    return sd
+
+
 def _draw_clip(shapes, prefix, std, width, layers, seed):
     """CLIP weights of `shapes` (names without `prefix`), each from its own generator seeded by crc32(prefix + name)"""
     std = {**std, "attn.in_proj_weight": width ** -0.5, "attn.out_proj.weight": width ** -0.5 * (2 * layers) ** -0.5,

@@ -337,6 +337,42 @@ int asyrp_arcface_se_apply(const float* res, const float* scale, const float* sh
 int asyrp_arcface_l2norm(const float* in, float* out, int rows, int dim, void* stream);
 int asyrp_arcface_dot(const float* src, const float* edited, float* id, int n, int B, int dim, void* stream);
 
+/* ---- Face-parsing BiSeNet (BiSeNet(n_classes=19), eval mode) and the segmentation consistency of an edit
+ * (asyrp_official_b200/face_parsing.py gives the network).  Activations are fp32 NHWC.
+ * asyrp_faceparse_pack: x fp32 NCHW [B][3][H][W] -> out fp32 NHWC [B][S][S][4]: clamp to [-1, 1], map to [0, 1],
+ *   bilinear resize to S x S (align_corners=False; rows blended first), normalise with ImageNet's mean (0.485, 0.456,
+ *   0.406) and std (0.229, 0.224, 0.225); channel 3 zero.
+ * asyrp_faceparse_conv: out = epilogue(conv(in) + bias), k x k, zero padding `pad`, any stride, the TF32 implicit GEMM
+ *   of asyrp_arcface_conv; relu 0: bias alone (bias may be null); relu 1 without residual: max(v, 0) (bias needed);
+ *   residual [N][Ho][Wo][Cout] (relu 1): max(residual + v, 0).  in [N][H][W][Cin] (Cin % 4 == 0), out Cout % 64 == 0,
+ *   weight fp32 [Cout][asyrp_lpips_conv_kpad(Cin, k, k)].
+ * asyrp_faceparse_maxpool: MaxPool2d(3, 2, padding 1) of [N][H][W][C] (C % 4 == 0) into [N][(H-1)/2+1][(W-1)/2+1][C].
+ * asyrp_faceparse_gate: one CTA per sample: m = mean_hw(in[n]) of in [N][HW][C] (C divides 512), h = act1(w1 m + b1)
+ *   (w1 [C1][C]), out[n] = act2(w2 h + b2) (w2 [C2][C1]) or h when w2 is null; biases may be null; act 0 identity,
+ *   1 ReLU, 2 sigmoid; C1, C2 <= 512.
+ * asyrp_faceparse_apply: out[n][y][x][c] = f[n][y/up][x/up][c] * gate[n][c] + add, out [N][H*up][W*up][C], up 1 or 2;
+ *   add = add[n][c] (add_map 0) or add[n][y/up][x/up][c] (add_map 1, a map the size of f); C % 4 == 0.
+ * asyrp_faceparse_labels: labels uint8 [N][Ho][Wo] = argmax over ncls classes (first wins a tie) of
+ *   F.interpolate(logits, (Ho, Wo), 'bilinear', align_corners=True), logits [N][Hi][Wi][ld] (classes 0 .. ncls-1 of a
+ *   row of ld floats); ncls <= 64, Wi * ncls <= 12288, N <= 65535.
+ * asyrp_faceparse_agreement: agree[j] = number of pixels where the labels of edited row j equal those of source row
+ *   (row0 + j) % B (as asyrp_faceparse_labels computes them), label maps never stored; row0 >= 0 lets a chunk of
+ *   edited rows starting at row0 keep its pairing; edited_logits [n][Hi][Wi][ld],
+ *   src_logits [B][Hi][Wi][ld]; Wi * ncls <= 6144, n <= 65535.
+ * Fixed-order reductions, no float atomics, no kernel mixes samples. */
+int asyrp_faceparse_pack(const float* x, float* out, int B, int H, int W, int S, void* stream);
+int asyrp_faceparse_conv(const float* in, const float* weight, const float* bias, const float* residual, float* out,
+                         int N, int H, int W, int Cin, int Cout, int k, int stride, int pad, int relu, void* stream);
+int asyrp_faceparse_maxpool(const float* in, float* out, int N, int H, int W, int C, void* stream);
+int asyrp_faceparse_gate(const float* in, const float* w1, const float* b1, int C1, int act1, const float* w2,
+                         const float* b2, int C2, int act2, float* out, int N, int HW, int C, void* stream);
+int asyrp_faceparse_apply(const float* f, const float* gate, const float* add, int add_map, float* out, int N, int H,
+                          int W, int C, int up, void* stream);
+int asyrp_faceparse_labels(const float* logits, unsigned char* labels, int N, int Hi, int Wi, int ld, int ncls, int Ho,
+                           int Wo, void* stream);
+int asyrp_faceparse_agreement(const float* src_logits, const float* edited_logits, unsigned int* agree, int n, int B,
+                              int row0, int Hi, int Wi, int ld, int ncls, int Ho, int Wo, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

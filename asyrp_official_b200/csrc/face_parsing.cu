@@ -30,6 +30,9 @@ constexpr int kGateThreads = 512;
 constexpr int kGateMaxC = 512;
 constexpr int kArgmaxThreads = 256;
 constexpr int kMaxClasses = 64;
+// dynamic shared memory of the upsample-argmax kernel: Wi * ncls blended floats per label map (two maps with kPair);
+// with kPair's static warp_same[] the admitted 48 KB is past the default 48 KB per block, so both launches opt in
+constexpr int kArgmaxSmemBytes = 48 * 1024;
 
 __device__ __forceinline__ float gate_warp_sum(float v) {
 #pragma unroll
@@ -362,7 +365,9 @@ ASYRP_API int asyrp_faceparse_labels(const float* logits, uint8_t* labels, int N
                 "asyrp_faceparse_labels: bad shape N=%d Hi=%d Wi=%d ld=%d ncls=%d Ho=%d Wo=%d", N, Hi, Wi, ld, ncls, Ho,
                 Wo);
   const size_t smem = static_cast<size_t>(Wi) * ncls * sizeof(float);
-  ASYRP_REQUIRE(smem <= 48 * 1024, "asyrp_faceparse_labels: Wi * ncls = %d * %d too large", Wi, ncls);
+  ASYRP_REQUIRE(smem <= kArgmaxSmemBytes, "asyrp_faceparse_labels: Wi * ncls = %d * %d too large", Wi, ncls);
+  ASYRP_CHECK_CUDA(cudaFuncSetAttribute(faceparse_upsample_argmax_kernel<false>,
+                                        cudaFuncAttributeMaxDynamicSharedMemorySize, kArgmaxSmemBytes));
   ASYRP_LAUNCH(faceparse_upsample_argmax_kernel<false>, dim3(Ho, N), dim3(kArgmaxThreads), smem,
                static_cast<cudaStream_t>(stream), logits, nullptr, labels, nullptr, 1, 0, Hi, Wi, ld, ncls, Ho, Wo,
                ac_scale(Hi, Ho), ac_scale(Wi, Wo));
@@ -378,7 +383,9 @@ ASYRP_API int asyrp_faceparse_agreement(const float* src_logits, const float* ed
                 "asyrp_faceparse_agreement: bad shape n=%d B=%d row0=%d Hi=%d Wi=%d ld=%d ncls=%d Ho=%d Wo=%d", n, B,
                 row0, Hi, Wi, ld, ncls, Ho, Wo);
   const size_t smem = 2 * static_cast<size_t>(Wi) * ncls * sizeof(float);
-  ASYRP_REQUIRE(smem <= 48 * 1024, "asyrp_faceparse_agreement: Wi * ncls = %d * %d too large", Wi, ncls);
+  ASYRP_REQUIRE(smem <= kArgmaxSmemBytes, "asyrp_faceparse_agreement: Wi * ncls = %d * %d too large", Wi, ncls);
+  ASYRP_CHECK_CUDA(cudaFuncSetAttribute(faceparse_upsample_argmax_kernel<true>,
+                                        cudaFuncAttributeMaxDynamicSharedMemorySize, kArgmaxSmemBytes));
   const cudaStream_t st = static_cast<cudaStream_t>(stream);
   ASYRP_CHECK_CUDA(cudaMemsetAsync(agree, 0, static_cast<size_t>(n) * sizeof(unsigned int), st));
   ASYRP_LAUNCH(faceparse_upsample_argmax_kernel<true>, dim3(Ho, n), dim3(kArgmaxThreads), smem, st, edited_logits,

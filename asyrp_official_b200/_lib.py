@@ -125,6 +125,14 @@ SIGNATURES = {
     "asyrp_faceparse_labels": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p]),
     "asyrp_faceparse_agreement": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_int,
                                           c_int, c_int, c_void_p]),
+    "asyrp_fid_pack": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p]),
+    "asyrp_fid_conv": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_int,
+                               c_int, c_int, c_int, c_int, c_int, c_void_p]),
+    "asyrp_fid_pool": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p]),
+    "asyrp_fid_mean": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p]),
+    "asyrp_fid_moments": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_void_p]),
+    "asyrp_fid_kernel_sum_partials": (c_int, [c_int, c_int]),
+    "asyrp_fid_kernel_sum": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p]),
 }
 
 _lib = None

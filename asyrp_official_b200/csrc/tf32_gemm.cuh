@@ -1,6 +1,6 @@
 // The fp32-in / fp32-out implicit GEMM on the tensor cores shared by the LPIPS convs (lpips.cu), the CLIP towers'
 // linear layers (clip_text.cu, a linear layer being a 1x1 conv over a 1 x M image), the ArcFace IR-SE50 convs
-// (arcface.cu) and the face-parsing BiSeNet convs (face_parsing.cu): mma.sync m16n8k8, TF32
+// (arcface.cu), the face-parsing BiSeNet convs (face_parsing.cu) and the Inception-v3 convs (fid.cu): mma.sync m16n8k8, TF32
 // operands rounded to nearest, fp32 accumulation, M = N*Ho*Wo output pixels, N = Cout, K = kh*kw*Cin tap-major /
 // channel-minor.  The epilogue is a template parameter; the main loop is the same code for every epilogue, so an
 // output element is the same fixed-order accumulation whichever layer or batch it belongs to.
@@ -28,6 +28,10 @@ enum Epilogue : int {
   kEpiResidual = 3,   // residual + v               (residual may be out: read and written by the same thread)
   kEpiPrelu = 4,      // v > 0 ? v : prelu[c] * v   (ArcFace's per-channel PReLU; bias may be null)
   kEpiResidualRelu = 5,  // max(residual + v, 0)    (BiSeNet's BasicBlock end; bias may be null)
+  // max(v, 0) stored to channels [0, cstore) of output rows of pitch ldo, the horizontal padding padw (p.pad is then
+  // the vertical one): an Inception branch of any even width writes its slice of the block output.  The other
+  // epilogues ignore padw / ldo / cstore (pad both ways, pitch and bound Cout).
+  kEpiReluSlice = 6,
 };
 
 __device__ __forceinline__ void cp_async16(uint32_t dst, const void* src, int bytes) {
@@ -59,13 +63,15 @@ struct Tf32ConvParams {
   const float* prelu;     // [Cout] PReLU slopes (kEpiPrelu only)
   float* out;             // [N][Ho][Wo][Cout]
   int N, H, W, Cin, Ho, Wo, Cout, kw, stride, pad, K, Kpad, M;
+  int padw, ldo, cstore;  // kEpiReluSlice only
 };
 
 __device__ __forceinline__ float quick_gelu(float z) { return z * (1.f / (1.f + expf(-(1.702f * z)))); }
 
 // out = epilogue(conv(in) + bias).  CTA tile 128 pixels x 64 channels, K in slices of 32 through a 3-stage cp.async
 // ring; the im2col gather is 16-byte chunks (4 channels of one tap: Cin % 4 == 0), zero-filled outside the image, so
-// the padding is zeros of the operand as stored.
+// the padding is zeros of the operand as stored.  The weight rows n0 .. n0 + 63 are read without a bound: w and bias
+// hold Cout rows (zero rows past a narrower branch's width).
 template <int kEpi>
 __global__ void __launch_bounds__(kThreads) tf32_conv_kernel(const Tf32ConvParams p) {
   pdl_trigger();
@@ -89,7 +95,7 @@ __global__ void __launch_bounds__(kThreads) tf32_conv_kernel(const Tf32ConvParam
       const int oy = r / p.Wo, ox = r - oy * p.Wo;
       a_base[i] = p.in + static_cast<size_t>(n) * p.H * p.W * p.Cin;
       a_iy[i] = oy * p.stride - p.pad;
-      a_ix[i] = ox * p.stride - p.pad;
+      a_ix[i] = ox * p.stride - (kEpi == kEpiReluSlice ? p.padw : p.pad);
     }
   }
 
@@ -176,7 +182,7 @@ __global__ void __launch_bounds__(kThreads) tf32_conv_kernel(const Tf32ConvParam
   for (int ni = 0; ni < 4; ++ni) {
     const int c = n0 + wn + ni * 8 + 2 * t;
     float b0 = 0.f, b1 = 0.f;
-    if (kEpi == kEpiRelu || p.bias != nullptr) {
+    if (kEpi == kEpiRelu || kEpi == kEpiReluSlice || p.bias != nullptr) {
       b0 = p.bias[c];
       b1 = p.bias[c + 1];
     }
@@ -185,10 +191,10 @@ __global__ void __launch_bounds__(kThreads) tf32_conv_kernel(const Tf32ConvParam
 #pragma unroll
       for (int h = 0; h < 2; ++h) {
         const int m = m0 + wm + mi * 16 + g + 8 * h;
-        if (m < p.M) {
-          const size_t o = static_cast<size_t>(m) * p.Cout + c;
+        if (m < p.M && (kEpi != kEpiReluSlice || c < p.cstore)) {
+          const size_t o = static_cast<size_t>(m) * (kEpi == kEpiReluSlice ? p.ldo : p.Cout) + c;
           float2 v = make_float2(acc[mi][ni][2 * h] + b0, acc[mi][ni][2 * h + 1] + b1);
-          if (kEpi == kEpiRelu) {
+          if (kEpi == kEpiRelu || kEpi == kEpiReluSlice) {
             v = make_float2(fmaxf(v.x, 0.f), fmaxf(v.y, 0.f));
           } else if (kEpi == kEpiQuickGelu) {
             v = make_float2(quick_gelu(v.x), quick_gelu(v.y));

@@ -19,6 +19,10 @@ Mirrors, with the same attribute / flag names:
   --seg_consistency            (none)                       run_test scores every edit with the segmentation consistency
                                                             of a face-parsing BiSeNet (face_parsing.FaceParser), written
                                                             next to the PNG; this build's definition
+  --fid                        (none)                       run_test scores each set of edits (one per hs_coeff tuple)
+                                                            against the origin pass with FID and KID on Inception-v3
+                                                            pool features (fid.FIDInception), gathered to rank 0 at the
+                                                            end of the run; this build's definition
   Asyrp.precompute_pairs_with_h :877-947                    DDIM inversion of one image keeping the bottleneck h of
                                                             every step (batched here, same cache file)
   Asyrp.run_diff_style         main.py:192-202              --diff_style (DiffStyle content injection): this build's
@@ -30,8 +34,8 @@ Differences (documented in INTEGRATION.md): the reverse loop is UNetEngine.sampl
 the CLIP text cosine that picks t_edit runs on this library's kernels (clip_text.CLIPText) from --clip_weights and
 --clip_vocab, or is given as --clip_cosine; SRC_TRG_TXT_DIC is read from --text_dic (default utils/text_dic.py).
 With torch.distributed initialised (one process per GPU) the image batches are sharded round-robin across ranks;
-the only collective is the initial weight broadcast, and each rank computes the CLIP cosine itself (the kernels are
-deterministic, so every rank picks the same t_edit).
+the collectives are the initial weight broadcast and, with --fid, the end-of-run gather of the pool features to rank
+0; each rank computes the CLIP cosine itself (the kernels are deterministic, so every rank picks the same t_edit).
 """
 import ast
 import os
@@ -74,6 +78,7 @@ class Asyrp(object):
         self.directional_clip = {}  # --DirectionalClipSmilarity: save_image's file name -> S_dir [tuples][images]
         self.id_similarity = {}  # --id_similarity: save_image's file name -> 1 - IDLoss [tuples][images]
         self.seg_consistency = {}  # --seg_consistency: save_image's file name -> SC [tuples][images]
+        self.fid = {}  # --fid (rank 0): 'train' / 'test' -> fp64 [tuples][2], (FID, KID) of each tuple's set
 
     # ------------------------------------------------------------------------------------------
     def load_pretrained_model(self):
@@ -235,6 +240,52 @@ class Asyrp(object):
             return load_state_dict(path)
         except ValueError as e:
             raise ValueError(f"--seg_consistency: {e}") from None
+
+    def fid_setup(self):
+        """--fid's requirements, checked before any model is loaded; raises ValueError with the reason.  Returns the
+        validated --fid_weights state dict (fid.load_state_dict)."""
+        from .fid import load_state_dict
+        a = self.args
+        if getattr(a, "pass_editing", False):
+            raise ValueError("--fid scores the edited images: with --pass_editing nothing is edited")
+        if getattr(a, "diff_style", False):
+            raise ValueError("--fid scores the sets of --run_test; --diff_style is not scored")
+        path = getattr(a, "fid_weights", None)
+        if not path or not os.path.isfile(path):
+            raise ValueError(f"--fid: --fid_weights {path!r} is not a file (pytorch-fid's "
+                             "pt_inception-2015-12-05-6726825d.pth)")
+        try:
+            return load_state_dict(path)
+        except ValueError as e:
+            raise ValueError(f"--fid: {e}") from None
+
+    def finish_fid(self, sets, coeffs, attrs=None):
+        """--fid at the end of a run: every rank's pool features (fid.FeatureSets) to rank 0, which sorts each set by
+        image index and scores every tuple's edited set against the origin set of the same pass: printed, kept in
+        self.fid[mode] and written to <test_image_folder>/<mode>_ngen<n_train_step>_fid.tsv.  Every rank must call it,
+        also one that ran no batch."""
+        from .fid import fid_kid, set_moments
+        a = self.args
+        dist_on = self.world > 1 and torch.distributed.is_available() and torch.distributed.is_initialized()
+        got = sets.gather(self.rank, self.world if dist_on else 1)
+        if got is None:
+            return
+        for mode in ("train", "test"):
+            if (mode, "origin") not in got:
+                continue
+            ids, ref = got[(mode, "origin")]
+            ref = ref.to(self.device).contiguous()
+            ref_moments = set_moments(ref) if ref.shape[0] >= 2 else None
+            rows = []
+            for k in range(len(coeffs)):
+                ids_k, feats = got[(mode, k)]
+                if not torch.equal(ids_k, ids):
+                    raise RuntimeError(f"--fid: tuple {k} of the {mode} pass has other images than its origin set")
+                rows.append(fid_kid(ref, feats.to(self.device).contiguous(), ref_moments))
+            self.fid[mode] = torch.tensor(rows, dtype=torch.float64)
+            os.makedirs(a.test_image_folder, exist_ok=True)
+            write_fid(os.path.join(a.test_image_folder, f"{mode}_ngen{a.n_train_step}_fid.tsv"), coeffs, rows,
+                      ref.shape[0], mode, attrs=attrs)
 
     def write_id_similarity(self, path, coeffs, ids):
         """the TSV of one batch: one row per (hs_coeff tuple, image) in grid order, ID = 1 - IDLoss(origin, edit) of
@@ -415,7 +466,7 @@ class Asyrp(object):
     def save_image(self, model, x_lat_tensor, seq_inv, seq_inv_next, save_x0=False, save_x_origin=False,
                    save_process_delta_h=False, save_process_origin=False, x0_tensor=None, delta_h_dict=None,
                    get_delta_hs=False, folder_dir="", file_name="", hs_coeff=(1.0, 1.0), directional_clip=None,
-                   id_scorer=None, seg_scorer=None):
+                   id_scorer=None, seg_scorer=None, fid=None):
         """rows of the grid: [x0] [origin DDIM] one row per hs_coeff tuple  (diffusion_latent.py:445-544).
 
         delta_h_dict: {t: None | Δh tensor}.  Entries that are tensors select the explicit-Δh branch for that step
@@ -430,7 +481,9 @@ class Asyrp(object):
         self.id_similarity[file_name].
         seg_scorer: a face_parsing.FaceParser for --seg_consistency: the same for the segmentation consistency against
         the same origin pass, written to <file_name>_ngen<n_train_step>_seg_consistency.tsv and kept in
-        self.seg_consistency[file_name]."""
+        self.seg_consistency[file_name].
+        fid: (fid.FIDInception, fid.FeatureSets, mode, image index of every row) for --fid: the pool features of the
+        origin pass and of each tuple's edits are added to their sets (finish_fid scores them at the end of the run)."""
         import torchvision.utils as tvu
         a = self.args
         time_s = time.time()
@@ -439,7 +492,8 @@ class Asyrp(object):
         x_list, edited = [], []
         if save_x0 and x0_tensor is not None:
             x_list.append(x0_tensor.cpu())
-        if save_x_origin or directional_clip is not None or id_scorer is not None or seg_scorer is not None:
+        if save_x_origin or directional_clip is not None or id_scorer is not None or seg_scorer is not None or \
+                fid is not None:
             sch = self.make_schedule(seq_inv, seq_inv_next, (1.0,), edit=False,
                                      addnoise=bool(getattr(a, "origin_process_addnoise", False)))
             if save_x_origin:
@@ -529,6 +583,8 @@ class Asyrp(object):
             self.seg_consistency[file_name] = sc
             write_scores(os.path.join(folder_dir, f'{file_name}_ngen{a.n_train_step}_seg_consistency.tsv'), coeffs, sc,
                          "SC", "segmentation consistency")
+        if fid is not None and edited:
+            add_fid_features(fid, origin, edited)
         print(f'{time.time() - time_s} seconds, {file_name}_ngen{a.n_train_step}.png is saved')
         return x_list
 
@@ -638,6 +694,7 @@ class Asyrp(object):
         sdir = self.directional_clip_setup() if getattr(a, "DirectionalClipSmilarity", False) else None
         id_sd = self.id_similarity_setup() if getattr(a, "id_similarity", False) else None
         seg_sd = self.seg_consistency_setup() if getattr(a, "seg_consistency", False) else None
+        fid_sd = self.fid_setup() if getattr(a, "fid", False) else None
         if a.multiple_attr and self.needs_clip() and self.clip_configured():
             cosine = self.choose_attribute(a.multiple_attr.split(' '))  # :640-652
             self.set_t_edit_t_addnoise(LPIPS_th=a.lpips_edit_th, LPIPS_addnoise_th=a.lpips_addnoise_th, cosine=cosine)
@@ -746,7 +803,7 @@ class Asyrp(object):
         if getattr(a, "target_image_id", None):
             target_ids = [int(i) for i in str(a.target_image_id).split(" ")]
             assert a.bs_train == 1, "target_image_id is only supported for batch_size == 1"
-        results, directional_clip, id_scorer, seg_scorer = {}, None, None, None
+        results, directional_clip, id_scorer, seg_scorer, fid_net = {}, None, None, None, None
         if sdir is not None:  # the image tower lives for this run_test only
             from .clip_image import CLIPLoss
             directional_clip = (CLIPLoss(a.clip_weights, a.clip_vocab, sdir[2], device=self.device), sdir[0], sdir[1])
@@ -759,16 +816,21 @@ class Asyrp(object):
                 from .face_parsing import FaceParser
                 seg_scorer = FaceParser(seg_sd, device=self.device)
                 seg_sd = None
+            if fid_sd is not None:  # and Inception-v3, whose features are collected over the whole run
+                from .fid import FeatureSets, FIDInception
+                fid_net, fid_sets = FIDInception(fid_sd, device=self.device), FeatureSets()
+                fid_sd = None
             for mode, do, n_img in (("train", a.do_train, a.n_train_img), ("test", a.do_test, a.n_test_img)):
                 if not do:
                     continue
-                x_lat_tensor, x0_tensor, batch_idx = None, None, 0
+                x_lat_tensor, x0_tensor, batch_idx, batch_ids = None, None, 0, []
                 for step, (x0, _, x_lat) in enumerate(pairs[mode]):
                     if target_ids is not None and step not in target_ids:
                         continue
                     if a.start_image_id > step:
                         continue
                     x_lat_tensor = x_lat if x_lat_tensor is None else torch.cat((x_lat_tensor, x_lat), dim=0)
+                    batch_ids.append(step)
                     if a.use_x0_tensor:
                         x0_tensor = x0 if x0_tensor is None else torch.cat((x0_tensor, x0), dim=0)
                     if (step + 1) % a.bs_train != 0:
@@ -781,7 +843,8 @@ class Asyrp(object):
                             save_process_origin=bool(getattr(a, "save_process_origin", False)),
                             save_process_delta_h=bool(getattr(a, "save_process_delta_h", False)),
                             folder_dir=a.test_image_folder, file_name=f'{mode}_{step}_{a.n_iter - 1}', hs_coeff=hs_coeff,
-                            directional_clip=directional_clip, id_scorer=id_scorer, seg_scorer=seg_scorer)
+                            directional_clip=directional_clip, id_scorer=id_scorer, seg_scorer=seg_scorer,
+                            fid=None if fid_net is None else (fid_net, fid_sets, mode, batch_ids))
                     batch_idx += 1
                     if step == n_img - 1:
                         break
@@ -802,11 +865,13 @@ class Asyrp(object):
                         print(f'Dict: {latent_name} is saved.')
                         num_mean = 0
                         print("now we use mean of delta_hs")
-                    x_lat_tensor, x0_tensor = None, None
+                    x_lat_tensor, x0_tensor, batch_ids = None, None, []
+            if fid_net is not None:
+                self.finish_fid(fid_sets, hs_coeff if isinstance(hs_coeff, list) else [hs_coeff])
         finally:
             a.train_delta_h = a_train_delta_h_prev
-            if directional_clip is not None or id_scorer is not None or seg_scorer is not None:
-                del directional_clip, id_scorer, seg_scorer
+            if directional_clip is not None or id_scorer is not None or seg_scorer is not None or fid_net is not None:
+                del directional_clip, id_scorer, seg_scorer, fid_net
                 torch.cuda.empty_cache()
         self.last_delta_h_dict = delta_h_dict
         return results
@@ -876,6 +941,7 @@ class Asyrp(object):
             sdir = self.directional_clip_setup(attrs)
         id_sd = self.id_similarity_setup() if getattr(a, "id_similarity", False) else None
         seg_sd = self.seg_consistency_setup() if getattr(a, "seg_consistency", False) else None
+        fid_sd = self.fid_setup() if getattr(a, "fid", False) else None
         times = self.attr_sweep_schedules(attrs)
         self.sweep_times = dict(zip(attrs, times))
         seq_test = [int(s + 1e-6) for s in list(np.linspace(0, 1, a.n_test_step) * a.t_0)]
@@ -903,7 +969,7 @@ class Asyrp(object):
             pairs = self.precompute_pairs(model)
         target_ids = [int(i) for i in str(a.target_image_id).split(" ")] if getattr(a, "target_image_id", None) \
             else None
-        results, directional_clip, id_scorer, seg_scorer = {}, None, None, None
+        results, directional_clip, id_scorer, seg_scorer, fid_net = {}, None, None, None, None
         if sdir is not None:
             from .clip_image import CLIPLoss
             directional_clip = (CLIPLoss(a.clip_weights, a.clip_vocab, sdir[1], device=self.device), sdir[0])
@@ -916,14 +982,19 @@ class Asyrp(object):
                 from .face_parsing import FaceParser
                 seg_scorer = FaceParser(seg_sd, device=self.device)
                 seg_sd = None
+            if fid_sd is not None:
+                from .fid import FeatureSets, FIDInception
+                fid_net, fid_sets = FIDInception(fid_sd, device=self.device), FeatureSets()
+                fid_sd = None
             for mode, do, n_img in (("train", a.do_train, a.n_train_img), ("test", a.do_test, a.n_test_img)):
                 if not do:
                     continue
-                x_lat_tensor, x0_tensor, batch_idx = None, None, 0
+                x_lat_tensor, x0_tensor, batch_idx, batch_ids = None, None, 0, []
                 for step, (x0, _, x_lat) in enumerate(pairs[mode]):
                     if (target_ids is not None and step not in target_ids) or a.start_image_id > step:
                         continue
                     x_lat_tensor = x_lat if x_lat_tensor is None else torch.cat((x_lat_tensor, x_lat), dim=0)
+                    batch_ids.append(step)
                     if a.use_x0_tensor:
                         x0_tensor = x0 if x0_tensor is None else torch.cat((x0_tensor, x0), dim=0)
                     if (step + 1) % a.bs_train != 0:
@@ -933,14 +1004,17 @@ class Asyrp(object):
                             model, x_lat_tensor, seq_test, seq_test_next, attrs, times, coeffs, save_x0=a.save_x0,
                             save_x_origin=a.save_x_origin, x0_tensor=x0_tensor,
                             folder_dir=a.test_image_folder, file_name=f'{mode}_{step}_{a.n_iter - 1}',
-                            directional_clip=directional_clip, id_scorer=id_scorer, seg_scorer=seg_scorer)
+                            directional_clip=directional_clip, id_scorer=id_scorer, seg_scorer=seg_scorer,
+                            fid=None if fid_net is None else (fid_net, fid_sets, mode, batch_ids))
                     batch_idx += 1
                     if step == n_img - 1:
                         break
-                    x_lat_tensor, x0_tensor = None, None
+                    x_lat_tensor, x0_tensor, batch_ids = None, None, []
+            if fid_net is not None:
+                self.finish_fid(fid_sets, coeffs, attrs=attrs)
         finally:
-            if directional_clip is not None or id_scorer is not None or seg_scorer is not None:
-                del directional_clip, id_scorer, seg_scorer
+            if directional_clip is not None or id_scorer is not None or seg_scorer is not None or fid_net is not None:
+                del directional_clip, id_scorer, seg_scorer, fid_net
                 torch.cuda.empty_cache()
         return results
 
@@ -956,7 +1030,7 @@ class Asyrp(object):
     @torch.no_grad()
     def save_image_sweep(self, model, x_lat_tensor, seq_inv, seq_inv_next, attrs, times, coeffs, save_x0=False,
                          save_x_origin=False, x0_tensor=None, folder_dir="", file_name="", directional_clip=None,
-                         id_scorer=None, seg_scorer=None):
+                         id_scorer=None, seg_scorer=None, fid=None):
         """save_image for an attribute sweep: grid rows [x0] [origin DDIM] then one row per attribute in the order
         given.  Rows of the trajectory are (attribute, image), attribute-major, run in chunks of whole attributes of
         at most --max_rows_per_replay rows (sweep_chunks).  directional_clip = (CLIPLoss, [(src_txt, trg_txt)] per
@@ -970,7 +1044,8 @@ class Asyrp(object):
         x_list, edited, origin = [], [], None
         if save_x0 and x0_tensor is not None:
             x_list.append(x0_tensor.cpu())
-        if save_x_origin or directional_clip is not None or id_scorer is not None or seg_scorer is not None:
+        if save_x_origin or directional_clip is not None or id_scorer is not None or seg_scorer is not None or \
+                fid is not None:
             sch = self.make_schedule(seq_inv, seq_inv_next, (1.0,), edit=False,
                                      addnoise=bool(getattr(a, "origin_process_addnoise", False)))
             if save_x_origin:
@@ -1009,6 +1084,8 @@ class Asyrp(object):
             self.seg_consistency[file_name] = sc
             write_scores(os.path.join(folder_dir, f'{file_name}_ngen{a.n_train_step}_seg_consistency.tsv'), coeffs,
                          sc, "SC", "segmentation consistency", attrs=attrs)
+        if fid is not None:
+            add_fid_features(fid, origin, edited)
         print(f'{time.time() - time_s} seconds, {file_name}_ngen{a.n_train_step}.png is saved')
         return x_list
 
@@ -1104,6 +1181,8 @@ class Asyrp(object):
         result per γ.  Returns {(content path, style path): results [len(γ)][3][S][S]}."""
         import torchvision.utils as tvu
         a = self.args
+        if getattr(a, "fid", False):
+            self.fid_setup()  # refuses --diff_style, before any model loads
         contents, styles, gammas = self.diff_style_setup()
         print(f"DiffStyle: hs_coeff {gammas} (slerp weight on the content h: 1 - hs_coeff)")
         model = self.load_pretrained_model().to(self.device)
@@ -1230,6 +1309,30 @@ def write_scores(path, coeffs, scores, column, label, attrs=None):
     for k, row in enumerate(scores):
         name = f"attribute {attrs[k]}" if attrs is not None else f"hs_coeff {tuple(float(c) for c in coeffs[k])}"
         print(f"{label}, {name}: mean {row.double().mean().item():.6f} over {row.numel()} images")
+
+
+def add_fid_features(fid, origin, edited):
+    """--fid: the pool features of a batch's origin rows and of each tuple's edited rows (edited[k]), added to their
+    sets with the batch's image indices; fid = (FIDInception, FeatureSets, mode, image indices)"""
+    net, sets, mode, ids = fid
+    bs = origin.shape[0]
+    feats = net.features(torch.cat([origin.cpu()] + [e.cpu() for e in edited]))
+    sets.add(mode, "origin", ids, feats[:bs])
+    for k in range(len(edited)):
+        sets.add(mode, k, ids, feats[(k + 1) * bs:(k + 2) * bs])
+
+
+def write_fid(path, coeffs, rows, n, mode, attrs=None):
+    """the FID / KID table of one pass: one row per hs_coeff tuple, columns tuple, hs_coeff, n (images per set), FID and
+    KID (`attr` appended under an attribute sweep); prints each tuple's values"""
+    with open(path, "w") as f:
+        f.write("tuple\ths_coeff\tn\tFID\tKID" + ("\tattr" if attrs is not None else "") + "\n")
+        for k, (fd, kd) in enumerate(rows):
+            tup = ",".join(f"{float(c):.6g}" for c in coeffs[k])
+            f.write(f"{k}\t{tup}\t{n}\t{fd!r}\t{kd!r}" + (f"\t{attrs[k]}" if attrs is not None else "") + "\n")
+    for k, (fd, kd) in enumerate(rows):
+        name = f"attribute {attrs[k]}" if attrs is not None else f"hs_coeff {tuple(float(c) for c in coeffs[k])}"
+        print(f"FID / KID ({mode}, {n} images), {name}: FID {fd:.6f}, KID {kd:.6f}")
 
 
 def plan_sweep(n_tuples, bs, max_rows):

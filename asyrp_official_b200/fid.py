@@ -1,0 +1,353 @@
+"""Inception-v3 pool features on the engine's kernels, and the FID and KID that `--fid` reports for each set of edits.
+
+The reference has no realism score: the network and the metric here are this project's definition, following
+pytorch-fid (FID) and torch-fidelity (KID).  The network is pytorch-fid's FID Inception-v3, whose weights file is
+pt_inception-2015-12-05-6726825d.pth (a state dict with torchvision Inception3 key names), evaluated up to the 2048-d
+global average pool:
+
+    input      the image its PNG shows, then what pytorch-fid does to a PNG: u8 = clamp((x + 1) * 0.5 * 255 + 0.5, 0,
+               255) truncated (torchvision's save_image), / 255, bilinear resize to 299 x 299 (align_corners=False),
+               2 v - 1
+    stem       Conv2d_1a_3x3 (/2), 2a_3x3, 2b_3x3 (pad 1), max-pool 3x3 / 2, 3b_1x1, 4a_3x3, max-pool 3x3 / 2
+    Mixed_5b-d FIDInceptionA (pool features 32, 64, 64)        branch_pool: avg-pool 3x3 / 1 pad 1, count_include_pad
+    Mixed_6a   InceptionB                                                   False, then a 1x1 BasicConv2d
+    Mixed_6b-e FIDInceptionC (c7 = 128, 160, 160, 192)          the same avg-pool
+    Mixed_7a   InceptionD
+    Mixed_7b   FIDInceptionE_1                                  the same avg-pool
+    Mixed_7c   FIDInceptionE_2                                  max-pool 3x3 / 1 pad 1 (padding never wins the max)
+    features   mean over the 8 x 8 pixels -> 2048; fc is not evaluated
+
+BasicConv2d is conv (no bias) -> BN (eps 1e-3) -> ReLU; the BN is folded into the conv's weight and bias at load time
+(exact algebra, fp64 on the host).  Every conv is the TF32 implicit GEMM of csrc/tf32_gemm.cuh writing its channel
+slice of the block output, so no concatenation is materialised; a branch narrower than a multiple of 64 channels runs
+with zero weight rows and stores only its own channels.
+
+Sets: every hs_coeff tuple of a run (each --delta_interpolation strength, each --multiple_attr tuple, each --attr_sweep
+attribute) is one edited set, scored against the origin DDIM pass of the same x_T; train and test passes are separate.
+
+    FID  = |mu1 - mu2|^2 + tr S1 + tr S2 - 2 sum_i sqrt(l_i), l the eigenvalues (clamped at 0) of S1^1/2 S2 S1^1/2, mu
+           and S (n - 1 denominator, as np.cov) in fp64.  This is tr sqrtm(S1 S2) for PSD matrices, and unlike
+           scipy.linalg.sqrtm it is well defined when n < 2048 makes S rank-deficient.
+    KID  = the unbiased MMD^2 with k(x, y) = (x . y / 2048 + 1)^3 over all rows of both sets, the diagonal excluded in
+           the two within-set sums: torch-fidelity's KID mean with kid_subset_size = n.
+
+A set of fewer than two images gets nan for both.  The moments and the kernel sums run on the GPU in fp64
+(csrc/fid.cu); the two 2048^2 eigendecompositions per set run on the host in fp64.  No real
+pt_inception-2015-12-05-6726825d.pth has been loaded by this project's tests: the key list below follows torchvision's
+Inception3, and the loader refuses any other layout by name.
+"""
+import math
+
+import numpy as np
+import torch
+
+from . import _lib, ops
+
+BN_EPS = 1e-3
+SIZE = 299
+DIMS = 2048
+BN_STATS = ("weight", "bias", "running_mean", "running_var")
+FC = {"fc.weight": (1008, DIMS), "fc.bias": (1008,)}  # the logits layer: accepted, checked and ignored
+# fp32 bytes of the activations live at once per image at the peak (the stem's Conv2d_2b: the packed input, 2a's
+# output and 2b's): rows run in chunks of ACTIVATION_BUDGET // ROW_BYTES images
+ROW_BYTES = 4 * (SIZE * SIZE * 4 + 147 * 147 * (32 + 64))
+ACTIVATION_BUDGET = 1 << 30
+
+# name -> (cin, cout, kh, kw, stride, pad_h, pad_w) of the stem's BasicConv2d layers
+STEM = {"Conv2d_1a_3x3": (3, 32, 3, 3, 2, 0, 0), "Conv2d_2a_3x3": (32, 32, 3, 3, 1, 0, 0),
+        "Conv2d_2b_3x3": (32, 64, 3, 3, 1, 1, 1), "Conv2d_3b_1x1": (64, 80, 1, 1, 1, 0, 0),
+        "Conv2d_4a_3x3": (80, 192, 3, 3, 1, 0, 0)}
+# (block, kind, in channels, pool features / c7)
+BLOCKS = (("Mixed_5b", "A", 192, 32), ("Mixed_5c", "A", 256, 64), ("Mixed_5d", "A", 288, 64),
+          ("Mixed_6a", "B", 288, None), ("Mixed_6b", "C", 768, 128), ("Mixed_6c", "C", 768, 160),
+          ("Mixed_6d", "C", 768, 160), ("Mixed_6e", "C", 768, 192), ("Mixed_7a", "D", 768, None),
+          ("Mixed_7b", "E1", 1280, None), ("Mixed_7c", "E2", 2048, None))
+# the branches of a block in output-channel order: (pool before the first conv or None, [conv, ...]); the last entry
+# of a branch writes the block output, a pair of convs both reading the previous one writes two adjacent slices, a
+# branch without convs is the pool alone
+BRANCHES = {
+    "A": ((None, ["branch1x1"]), (None, ["branch5x5_1", "branch5x5_2"]),
+          (None, ["branch3x3dbl_1", "branch3x3dbl_2", "branch3x3dbl_3"]), ("avg", ["branch_pool"])),
+    "B": ((None, ["branch3x3"]), (None, ["branch3x3dbl_1", "branch3x3dbl_2", "branch3x3dbl_3"]), ("max2", [])),
+    "C": ((None, ["branch1x1"]), (None, ["branch7x7_1", "branch7x7_2", "branch7x7_3"]),
+          (None, ["branch7x7dbl_1", "branch7x7dbl_2", "branch7x7dbl_3", "branch7x7dbl_4", "branch7x7dbl_5"]),
+          ("avg", ["branch_pool"])),
+    "D": ((None, ["branch3x3_1", "branch3x3_2"]),
+          (None, ["branch7x7x3_1", "branch7x7x3_2", "branch7x7x3_3", "branch7x7x3_4"]), ("max2", [])),
+    "E1": ((None, ["branch1x1"]), (None, ["branch3x3_1", ("branch3x3_2a", "branch3x3_2b")]),
+           (None, ["branch3x3dbl_1", "branch3x3dbl_2", ("branch3x3dbl_3a", "branch3x3dbl_3b")]),
+           ("avg", ["branch_pool"])),
+}
+BRANCHES["E2"] = BRANCHES["E1"][:3] + (("max1", ["branch_pool"]),)
+POOL_MODE = {"avg": ops.FID_POOL_AVG3S1, "max1": ops.FID_POOL_MAX3S1, "max2": ops.FID_POOL_MAX3S2}
+
+
+def block_convs(kind, cin, arg):
+    """conv name -> (cin, cout, kh, kw, stride, pad_h, pad_w) of one block (torchvision's Inception A-E layers)"""
+    if kind == "A":
+        return {"branch1x1": (cin, 64, 1, 1, 1, 0, 0), "branch5x5_1": (cin, 48, 1, 1, 1, 0, 0),
+                "branch5x5_2": (48, 64, 5, 5, 1, 2, 2), "branch3x3dbl_1": (cin, 64, 1, 1, 1, 0, 0),
+                "branch3x3dbl_2": (64, 96, 3, 3, 1, 1, 1), "branch3x3dbl_3": (96, 96, 3, 3, 1, 1, 1),
+                "branch_pool": (cin, arg, 1, 1, 1, 0, 0)}
+    if kind == "B":
+        return {"branch3x3": (cin, 384, 3, 3, 2, 0, 0), "branch3x3dbl_1": (cin, 64, 1, 1, 1, 0, 0),
+                "branch3x3dbl_2": (64, 96, 3, 3, 1, 1, 1), "branch3x3dbl_3": (96, 96, 3, 3, 2, 0, 0)}
+    if kind == "C":
+        c7 = arg
+        return {"branch1x1": (cin, 192, 1, 1, 1, 0, 0), "branch7x7_1": (cin, c7, 1, 1, 1, 0, 0),
+                "branch7x7_2": (c7, c7, 1, 7, 1, 0, 3), "branch7x7_3": (c7, 192, 7, 1, 1, 3, 0),
+                "branch7x7dbl_1": (cin, c7, 1, 1, 1, 0, 0), "branch7x7dbl_2": (c7, c7, 7, 1, 1, 3, 0),
+                "branch7x7dbl_3": (c7, c7, 1, 7, 1, 0, 3), "branch7x7dbl_4": (c7, c7, 7, 1, 1, 3, 0),
+                "branch7x7dbl_5": (c7, 192, 1, 7, 1, 0, 3), "branch_pool": (cin, 192, 1, 1, 1, 0, 0)}
+    if kind == "D":
+        return {"branch3x3_1": (cin, 192, 1, 1, 1, 0, 0), "branch3x3_2": (192, 320, 3, 3, 2, 0, 0),
+                "branch7x7x3_1": (cin, 192, 1, 1, 1, 0, 0), "branch7x7x3_2": (192, 192, 1, 7, 1, 0, 3),
+                "branch7x7x3_3": (192, 192, 7, 1, 1, 3, 0), "branch7x7x3_4": (192, 192, 3, 3, 2, 0, 0)}
+    return {"branch1x1": (cin, 320, 1, 1, 1, 0, 0), "branch3x3_1": (cin, 384, 1, 1, 1, 0, 0),
+            "branch3x3_2a": (384, 384, 1, 3, 1, 0, 1), "branch3x3_2b": (384, 384, 3, 1, 1, 1, 0),
+            "branch3x3dbl_1": (cin, 448, 1, 1, 1, 0, 0), "branch3x3dbl_2": (448, 384, 3, 3, 1, 1, 1),
+            "branch3x3dbl_3a": (384, 384, 1, 3, 1, 0, 1), "branch3x3dbl_3b": (384, 384, 3, 1, 1, 1, 0),
+            "branch_pool": (cin, 192, 1, 1, 1, 0, 0)}
+
+
+def block_width(kind, cin, arg):
+    """output channels of a block: the widths of its branches' last convs, plus cin for a pool-only branch"""
+    return {"A": 224 + (arg or 0), "B": 480 + cin, "C": 768, "D": 512 + cin}.get(kind, 2048)
+
+
+def conv_specs():
+    """full conv name (e.g. 'Mixed_6b.branch7x7_2') -> (cin, cout, kh, kw, stride, pad_h, pad_w), in network order"""
+    out = dict(STEM)
+    for name, kind, cin, arg in BLOCKS:
+        out.update({f"{name}.{k}": v for k, v in block_convs(kind, cin, arg).items()})
+    return out
+
+
+def state_dict_shapes():
+    """name -> shape of every tensor the network evaluates (without fc and num_batches_tracked)"""
+    shapes = {}
+    for name, (cin, cout, kh, kw, *_) in conv_specs().items():
+        shapes[f"{name}.conv.weight"] = (cout, cin, kh, kw)
+        for s in BN_STATS:
+            shapes[f"{name}.bn.{s}"] = (cout,)
+    return shapes
+
+
+def load_state_dict(sd_or_path):
+    """Validate an FID Inception-v3 state dict (or the path of its torch.save) and return the tensors the network
+    evaluates as fp32 on the host, keyed as in the state dict.  fc.weight / fc.bias and every BN's num_batches_tracked
+    are accepted and ignored.  Raises ValueError naming the key on a missing, mis-shaped or unknown key, and on a file
+    that is not a state dict."""
+    sd = sd_or_path
+    if not isinstance(sd, dict):
+        try:
+            sd = torch.load(sd_or_path, map_location="cpu", weights_only=True)
+        except Exception as e:  # a truncated file, another format, ...
+            raise ValueError(f"FID Inception weights {sd_or_path!r}: cannot be read as a torch.save'd state dict "
+                             f"({e})") from None
+        if not isinstance(sd, dict):
+            raise ValueError(f"FID Inception weights {sd_or_path!r}: not a state dict (got {type(sd).__name__})")
+    expected = state_dict_shapes()
+    tracked = {f"{n}.bn.num_batches_tracked" for n in conv_specs()}
+    unknown = sorted(k for k in sd if k not in expected and k not in FC and k not in tracked)
+    if unknown:
+        raise ValueError(f"FID Inception state dict: unexpected keys {unknown[:8]}{' ...' if len(unknown) > 8 else ''} "
+                         "(expected the layout of pytorch-fid's FID Inception-v3)")
+    for k, shape in FC.items():
+        if k in sd and tuple(torch.as_tensor(sd[k]).shape) != shape:
+            raise ValueError(f"FID Inception state dict: {k!r} has shape {tuple(torch.as_tensor(sd[k]).shape)}, "
+                             f"expected {shape}")
+    out = {}
+    for k, shape in expected.items():
+        if k not in sd:
+            raise ValueError(f"FID Inception state dict: missing key {k!r}")
+        t = torch.as_tensor(sd[k])
+        if tuple(t.shape) != shape:
+            raise ValueError(f"FID Inception state dict: {k!r} has shape {tuple(t.shape)}, expected {shape}")
+        out[k] = t.detach().float().cpu().contiguous()
+    return out
+
+
+def fold(sd):
+    """conv name -> (weight [cout][cin][kh][kw], bias [cout]) fp32 of a load_state_dict() result: the BN (eps 1e-3)
+    folded into the bias-free conv in fp64, w' = w * g / sqrt(var + eps), b' = beta - mean * g / sqrt(var + eps)"""
+    out = {}
+    for name in conv_specs():
+        g = {s: sd[f"{name}.bn.{s}"].double() for s in BN_STATS}
+        scale = g["weight"] / torch.sqrt(g["running_var"] + BN_EPS)
+        w = sd[f"{name}.conv.weight"].double() * scale[:, None, None, None]
+        out[name] = (w.float().contiguous(), (g["bias"] - g["running_mean"] * scale).float().contiguous())
+    return out
+
+
+def frechet_distance(mu1, sigma1, mu2, sigma2):
+    """|mu1 - mu2|^2 + tr S1 + tr S2 - 2 sum sqrt(eig(S1^1/2 S2 S1^1/2)), eigenvalues clamped at 0; fp64 on the host"""
+    mu1, mu2 = (np.asarray(m, dtype=np.float64) for m in (mu1, mu2))
+    s1, s2 = (np.asarray(s, dtype=np.float64) for s in (sigma1, sigma2))
+    lam, vec = np.linalg.eigh((s1 + s1.T) / 2)
+    root = (vec * np.sqrt(np.clip(lam, 0, None))) @ vec.T
+    m = root @ s2 @ root
+    ev = np.clip(np.linalg.eigvalsh((m + m.T) / 2), 0, None)
+    diff = mu1 - mu2
+    return float(diff @ diff + np.trace(s1) + np.trace(s2) - 2 * np.sqrt(ev).sum())
+
+
+def kid_from_sums(kxx, kyy, kxy, n, m):
+    """the unbiased MMD^2 from the kernel sums: kxx, kyy without their diagonals, kxy over all n * m pairs"""
+    return kxx / (n * (n - 1)) + kyy / (m * (m - 1)) - 2 * kxy / (n * m)
+
+
+def kid(f1, f2):
+    """KID of two feature sets fp32 [n][d] / [m][d] on the device (n, m >= 2): kernel sums on the GPU in fp64"""
+    n, m = f1.shape[0], f2.shape[0]
+    kxx = ops.fid_kernel_sum(f1, f1, exclude_diag=True).item()
+    kyy = ops.fid_kernel_sum(f2, f2, exclude_diag=True).item()
+    kxy = ops.fid_kernel_sum(f1, f2).item()
+    return kid_from_sums(kxx, kyy, kxy, n, m)
+
+
+def set_moments(f):
+    """(mu, sigma) of a feature set fp32 [n][d] on the device, fp64 numpy on the host"""
+    mu, sigma = ops.fid_moments(f.contiguous())
+    return mu.cpu().numpy(), sigma.cpu().numpy()
+
+
+def fid_kid(ref, edited, ref_moments=None):
+    """(FID, KID) of the feature sets ref and edited (fp32 [n][d] on the device, rows in image order); nan for both when
+    either set has fewer than two rows.  ref_moments: set_moments(ref), when several sets share the reference."""
+    if ref.shape[0] < 2 or edited.shape[0] < 2:
+        print(f"FID / KID: a set of {min(ref.shape[0], edited.shape[0])} image(s) has no covariance: nan")
+        return math.nan, math.nan
+    mu1, s1 = ref_moments if ref_moments is not None else set_moments(ref)
+    mu2, s2 = set_moments(edited)
+    return frechet_distance(mu1, s1, mu2, s2), kid(ref.contiguous(), edited.contiguous())
+
+
+class FIDInception:
+    """FIDInception(weights, device): features(x) -> fp32 [B][2048] on the device, the pool features of images
+    x [B][3][H][W] in [-1, 1] (any size; quantised as their PNG, resized to 299 x 299).  Every operation is a kernel of
+    libasyrp_b200.so; an image's features are bit-identical whatever batch it is in.  Rows run in chunks of max_rows
+    images (default: ACTIVATION_BUDGET // ROW_BYTES), which bounds the activations at max_rows * ROW_BYTES bytes."""
+
+    def __init__(self, state_dict_or_path, device=None, max_rows=None):
+        if not torch.cuda.is_available():
+            raise _lib.AsyrpError("FIDInception needs a CUDA device (sm_90a); there is no CPU path")
+        _lib.load()
+        folded = fold(load_state_dict(state_dict_or_path))
+        self.max_rows = max(1, int(max_rows) if max_rows is not None else ACTIVATION_BUDGET // ROW_BYTES)
+        self.device = torch.device(device) if device is not None else torch.device("cuda", torch.cuda.current_device())
+        self.specs = conv_specs()
+        self.params = {}
+        with torch.cuda.device(self.device):
+            for name, (w, b) in folded.items():
+                cout = w.shape[0]
+                rows = -(-cout // 64) * 64  # the GEMM's 64-channel tiles: zero rows past the layer's width
+                wp = torch.zeros(rows, *w.shape[1:])
+                wp[:cout] = w
+                bp = torch.zeros(rows)
+                bp[:cout] = b
+                packed = ops.pack_lpips_conv_weight(wp, cin_pad=4 if name == "Conv2d_1a_3x3" else None)
+                self.params[name] = (packed.to(self.device), bp.to(self.device))
+
+    def _conv(self, name, x, out=None):
+        """BasicConv2d `name` of x into out (a new tensor, or a channel slice of the block output)"""
+        _, cout, kh, kw, stride, ph, pw = self.specs[name]
+        if out is None:
+            B, H, W, _ = x.shape
+            out = torch.empty(B, (H + 2 * ph - kh) // stride + 1, (W + 2 * pw - kw) // stride + 1, cout,
+                              dtype=torch.float32, device=self.device)
+        ops.fid_conv(x, *self.params[name], out, kh, kw, stride, (ph, pw), cstore=cout)
+        return out
+
+    def _block(self, name, kind, arg, x):
+        B, H, W, cin = x.shape
+        f32 = dict(dtype=torch.float32, device=self.device)
+        Ho, Wo = ((H - 3) // 2 + 1, (W - 3) // 2 + 1) if kind in ("B", "D") else (H, W)
+        out = torch.empty(B, Ho, Wo, block_width(kind, cin, arg), **f32)
+        c0 = 0
+        for pool, convs in BRANCHES[kind]:
+            if not convs:  # the pool branch of InceptionB / D: the pooled input is the slice
+                ops.fid_pool(x, out[..., c0:c0 + cin], POOL_MODE[pool])
+                c0 += cin
+                continue
+            h = x
+            if pool is not None:
+                h = torch.empty(B, H, W, cin, **f32)
+                ops.fid_pool(x, h, POOL_MODE[pool])
+            for c in convs[:-1]:
+                h = self._conv(f"{name}.{c}", h)
+            for c in convs[-1] if isinstance(convs[-1], tuple) else (convs[-1],):
+                cout = self.specs[f"{name}.{c}"][1]
+                self._conv(f"{name}.{c}", h, out[..., c0:c0 + cout])
+                c0 += cout
+        return out
+
+    def _maxpool(self, h):
+        p = torch.empty(h.shape[0], (h.shape[1] - 3) // 2 + 1, (h.shape[2] - 3) // 2 + 1, h.shape[3],
+                        dtype=torch.float32, device=self.device)
+        ops.fid_pool(h, p, ops.FID_POOL_MAX3S2)
+        return p
+
+    def _chunk_features(self, x):
+        B = x.shape[0]
+        f32 = dict(dtype=torch.float32, device=self.device)
+        h = torch.empty(B, SIZE, SIZE, 4, **f32)
+        ops.fid_pack(x.to(**f32).contiguous(), h)
+        h = self._conv("Conv2d_2a_3x3", self._conv("Conv2d_1a_3x3", h))
+        h = self._maxpool(self._conv("Conv2d_2b_3x3", h))
+        h = self._maxpool(self._conv("Conv2d_4a_3x3", self._conv("Conv2d_3b_1x1", h)))
+        for name, kind, _, arg in BLOCKS:
+            h = self._block(name, kind, arg, h)
+        feats = torch.empty(B, DIMS, **f32)
+        ops.fid_mean(h, feats)
+        return feats
+
+    @torch.no_grad()
+    def features(self, x):
+        """pool features fp32 [B][2048] on the device"""
+        x = torch.as_tensor(x)
+        if x.dim() != 4 or x.shape[1] != 3 or x.shape[0] == 0:
+            raise ValueError(f"images must be [B][3][H][W], got {tuple(x.shape)}")
+        with torch.cuda.device(self.device):
+            return torch.cat([self._chunk_features(x[i:i + self.max_rows])
+                              for i in range(0, x.shape[0], self.max_rows)])
+
+
+class FeatureSets:
+    """The pool features of a run's sets, collected batch by batch: add(mode, key, image_ids, feats) with key 'origin'
+    or a tuple index.  gather() brings every rank's rows to rank 0 sorted by image index (every rank must call it)."""
+
+    def __init__(self):
+        self.rows = {}  # (mode, key) -> [(image ids int64 [b], feats fp32 [b][d] on the host)]
+
+    def add(self, mode, key, image_ids, feats):
+        self.rows.setdefault((mode, key), []).append(
+            (torch.as_tensor(list(image_ids), dtype=torch.int64), feats.detach().float().cpu()))
+
+    def local(self):
+        """(mode, key) -> (ids, feats) of this rank's rows, sorted by image index"""
+        return {k: _sorted_rows(v) for k, v in self.rows.items()}
+
+    def gather(self, rank=0, world=1):
+        """rank 0: (mode, key) -> (ids, feats) of all ranks' rows sorted by image index; other ranks: None"""
+        if world == 1:
+            return self.local()
+        import torch.distributed as dist
+        got = [None] * world if rank == 0 else None
+        dist.gather_object(self.rows, got, dst=0)
+        if rank != 0:
+            return None
+        merged = {}
+        for part in got:
+            for k, v in part.items():
+                merged.setdefault(k, []).extend(v)
+        return {k: _sorted_rows(v) for k, v in merged.items()}
+
+
+def _sorted_rows(parts):
+    ids = torch.cat([p[0] for p in parts])
+    feats = torch.cat([p[1] for p in parts])
+    order = torch.argsort(ids, stable=True)
+    if len(set(ids.tolist())) != ids.numel():
+        raise ValueError(f"FID: an image index occurs twice in one set: {sorted(ids.tolist())}")
+    return ids[order], feats[order]

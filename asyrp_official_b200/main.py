@@ -123,6 +123,12 @@ def build_parser():
                         'written next to the PNG')
     p.add_argument('--seg_weights', type=str, default='pretrained/79999_iter.pth',
                    help='torch.save of the face-parsing BiSeNet(n_classes=19) state dict for --seg_consistency')
+    p.add_argument('--fid', **sa,
+                   help='--run_test: score each set of edits (one per hs_coeff tuple or --attr_sweep attribute) for '
+                        'realism with FID and KID on Inception-v3 pool features against the unedited DDIM pass of '
+                        'the same x_T, written to <test_image_folder>/<mode>_ngen<n_train_step>_fid.tsv')
+    p.add_argument('--fid_weights', type=str, default='pretrained/pt_inception-2015-12-05-6726825d.pth',
+                   help="pytorch-fid's FID Inception-v3 weights for --fid")
     p.add_argument('--lpips_table_dir', type=str,
                    help='directory with <config stem>_LPIPS_distance_{x,x0_t}.tsv (read by --run_test, written by '
                         '--lpips; default utils)')

@@ -704,6 +704,92 @@ def faceparse_agreement(src_logits, edited_logits, ncls, out_hw, agree, row0=0):
                                         out_hw[0], out_hw[1], _stream()), "asyrp_faceparse_agreement")
 
 
+FID_POOL_MAX3S2, FID_POOL_AVG3S1, FID_POOL_MAX3S1 = 0, 1, 2
+
+
+def fid_pack(x, out):
+    """x fp32 [B][3][H][W] in [-1, 1] -> out fp32 NHWC [B][S][S][4]: the u8 save_image writes, / 255, bilinear resize to
+    S x S (align_corners=False), 2 v - 1; channel 3 zero"""
+    lib = _lib.load()
+    B, C, H, W = x.shape
+    S = out.shape[1]
+    _need_cuda(x, out)
+    assert C == 3 and x.dtype == torch.float32 and x.is_contiguous() and tuple(out.shape) == (B, S, S, 4)
+    assert out.dtype == torch.float32 and out.is_contiguous()
+    check(lib.asyrp_fid_pack(_ptr(x), _ptr(out), B, H, W, S, _stream()), "asyrp_fid_pack")
+
+
+def fid_conv(inp, weight, bias, out, kh, kw, stride=1, pad=(0, 0), cstore=None):
+    """out[..., :cstore] = max(conv(inp) + bias, 0), fp32 NHWC, TF32 tensor cores, zero padding pad = (rows, columns);
+    weight [Cout][Kpad] from pack_lpips_conv_weight and bias [Cout] with Cout a multiple of 64 (zero rows past cstore);
+    out may be a channel slice out_full[..., c0:c0 + cstore] of a contiguous tensor (its row pitch is kept)"""
+    lib = _lib.load()
+    N, H, W, cin = inp.shape
+    cout = weight.shape[0]
+    cstore = out.shape[-1] if cstore is None else cstore
+    _need_cuda(inp, weight, bias, out)
+    assert inp.is_contiguous() and weight.is_contiguous() and bias.is_contiguous() and out.dtype == torch.float32
+    assert tuple(weight.shape) == (cout, lpips_conv_kpad(cin, kh, kw)) and weight.dtype == torch.float32
+    assert bias.numel() == cout
+    Ho, Wo = (H + 2 * pad[0] - kh) // stride + 1, (W + 2 * pad[1] - kw) // stride + 1
+    assert tuple(out.shape) == (N, Ho, Wo, cstore) and out.stride(3) == 1
+    ldo = out.stride(2)
+    assert out.stride(1) == Wo * ldo and out.stride(0) == Ho * Wo * ldo
+    check(lib.asyrp_fid_conv(_ptr(inp), _ptr(weight), _ptr(bias), _ptr(out), N, H, W, cin, cout, kh, kw, stride,
+                             pad[0], pad[1], ldo, cstore, _stream()), "asyrp_fid_conv")
+
+
+def fid_pool(inp, out, mode):
+    """3 x 3 pooling of fp32 NHWC inp into out, which may be a channel slice of a contiguous tensor: FID_POOL_MAX3S2
+    (stride 2, no padding), FID_POOL_AVG3S1 (stride 1, pad 1, count_include_pad=False), FID_POOL_MAX3S1 (stride 1,
+    pad 1)"""
+    lib = _lib.load()
+    N, H, W, Cc = inp.shape
+    _need_cuda(inp, out)
+    Ho, Wo = ((H - 3) // 2 + 1, (W - 3) // 2 + 1) if mode == FID_POOL_MAX3S2 else (H, W)
+    assert inp.is_contiguous() and out.dtype == torch.float32 and tuple(out.shape) == (N, Ho, Wo, Cc)
+    ldo = out.stride(2)
+    assert out.stride(3) == 1 and out.stride(1) == Wo * ldo and out.stride(0) == Ho * Wo * ldo
+    check(lib.asyrp_fid_pool(_ptr(inp), _ptr(out), N, H, W, Cc, int(mode), ldo, _stream()), "asyrp_fid_pool")
+
+
+def fid_mean(inp, out):
+    """out [N][C] = mean of fp32 NHWC inp over its pixels, summed in pixel order"""
+    lib = _lib.load()
+    N, H, W, Cc = inp.shape
+    _need_cuda(inp, out)
+    assert inp.is_contiguous() and out.is_contiguous() and tuple(out.shape) == (N, Cc)
+    check(lib.asyrp_fid_mean(_ptr(inp), _ptr(out), N, H * W, Cc, _stream()), "asyrp_fid_mean")
+
+
+def fid_moments(x):
+    """(mu [d], sigma [d][d]) fp64 on the device: the column means and the n - 1 normalised centred covariance of
+    x fp32 [n][d] (n >= 2, d a multiple of 64)"""
+    lib = _lib.load()
+    n, d = x.shape
+    _need_cuda(x)
+    assert x.dtype == torch.float32 and x.is_contiguous()
+    mu = torch.empty(d, dtype=torch.float64, device=x.device)
+    sigma = torch.empty(d, d, dtype=torch.float64, device=x.device)
+    check(lib.asyrp_fid_moments(_ptr(x), _ptr(mu), _ptr(sigma), n, d, _stream()), "asyrp_fid_moments")
+    return mu, sigma
+
+
+def fid_kernel_sum(x, y, exclude_diag=False):
+    """sum over the rows x_i of x [n][d] and y_j of y [m][d] (fp32) of (x_i . y_j / d + 1)^3, fp64, without the pairs
+    i == j with exclude_diag: a 0-d fp64 tensor on the device"""
+    lib = _lib.load()
+    (n, d), m = x.shape, y.shape[0]
+    _need_cuda(x, y)
+    assert x.dtype == torch.float32 and y.dtype == torch.float32 and x.is_contiguous() and y.is_contiguous()
+    assert y.shape[1] == d
+    part = torch.empty(max(1, lib.asyrp_fid_kernel_sum_partials(n, m)), dtype=torch.float64, device=x.device)
+    out = torch.empty((), dtype=torch.float64, device=x.device)
+    check(lib.asyrp_fid_kernel_sum(_ptr(x), _ptr(y), _ptr(part), _ptr(out), n, m, d, int(bool(exclude_diag)),
+                                   _stream()), "asyrp_fid_kernel_sum")
+    return out
+
+
 def ddpm_update(x, et, z, x_next, at, bt, logvar, learned_sigma, mask):
     lib = _lib.load()
     N, Cx, H, W = x.shape

@@ -110,6 +110,32 @@ def face_parsing_state_dict(seed=1234, n_classes=19, aux=True):
     return sd
 
 
+def inception_state_dict(seed=1234, fc=True):
+    """seeded FID Inception-v3 weights in its state-dict layout (asyrp_official_b200.fid), scaled so that activations
+    stay O(1) through the 94 BasicConv2d layers and the features follow the image: convs U(-b, b) with
+    b = 2^1/2 (3 / fan_in)^1/2 (He's, for the ReLU); BatchNorms weight 1 + N(0, .1^2), bias and running_mean
+    N(0, .1^2), running_var exp(N(0, .2^2)); num_batches_tracked 0.  fc: include the (ignored) fc layer."""
+    from .fid import FC, state_dict_shapes
+    shapes = {**state_dict_shapes(), **(FC if fc else {})}
+    sd = {}
+    for name, shp in shapes.items():
+        g = torch.Generator()
+        g.manual_seed((zlib.crc32(name.encode()) ^ (seed * 0x9E3779B1)) & 0x7FFFFFFF)
+        if len(shp) >= 2:
+            b = (2 ** 0.5) * (3.0 / math.prod(shp[1:])) ** 0.5
+            sd[name] = (torch.rand(shp, generator=g) * 2 - 1) * b
+        elif name.endswith("running_var"):
+            sd[name] = torch.exp(0.2 * torch.randn(shp, generator=g))
+        elif name.endswith(".weight"):
+            sd[name] = 1.0 + 0.1 * torch.randn(shp, generator=g)
+        else:
+            sd[name] = 0.1 * torch.randn(shp, generator=g)
+    for name in list(sd):
+        if name.endswith("running_var"):
+            sd[name[:-len("running_var")] + "num_batches_tracked"] = torch.tensor(0, dtype=torch.long)
+    return sd
+
+
 def _draw_clip(shapes, prefix, std, width, layers, seed):
     """CLIP weights of `shapes` (names without `prefix`), each from its own generator seeded by crc32(prefix + name)"""
     std = {**std, "attn.in_proj_weight": width ** -0.5, "attn.out_proj.weight": width ** -0.5 * (2 * layers) ** -0.5,

@@ -373,6 +373,37 @@ int asyrp_faceparse_labels(const float* logits, unsigned char* labels, int N, in
 int asyrp_faceparse_agreement(const float* src_logits, const float* edited_logits, unsigned int* agree, int n, int B,
                               int row0, int Hi, int Wi, int ld, int ncls, int Ho, int Wo, void* stream);
 
+/* ---- Inception-v3 pool features (the FID variant of pytorch-fid) and the set statistics of FID and KID
+ * (asyrp_official_b200/fid.py gives the network and the metric).  Activations are fp32 NHWC.
+ * asyrp_fid_pack: x fp32 NCHW [B][3][H][W] -> out fp32 NHWC [B][S][S][4]: q = the u8 torchvision's save_image writes
+ *   (fp32 (x + 1) * 0.5 * 255 + 0.5, clamped to [0, 255], truncated), q / 255, bilinear resize to S x S
+ *   (align_corners=False; rows blended first), 2 v - 1; channel 3 zero.
+ * asyrp_fid_conv: out = max(conv(in) + bias, 0), kh x kw, zero padding padh rows / padw columns, any stride, the TF32
+ *   implicit GEMM of asyrp_arcface_conv; in [N][H][W][Cin] (Cin % 4 == 0); weight fp32
+ *   [Cout][asyrp_lpips_conv_kpad(Cin, kh, kw)] and bias [Cout] with Cout % 64 == 0 (zero rows past the layer's width);
+ *   channels [0, cstore) of out rows [N][Ho][Wo] of pitch ldo are written, the rest untouched: cstore even,
+ *   0 < cstore <= Cout, ldo even and >= cstore, out 8-byte aligned (a channel slice of a wider tensor).
+ * asyrp_fid_pool: mode 0 max-pool 3x3 / 2 without padding (H, W >= 3), 1 avg-pool 3x3 / 1 pad 1 without the padding
+ *   (count_include_pad=False; taps summed in row-major order, then divided by their count), 2 max-pool 3x3 / 1 pad 1
+ *   (padding never wins) of in [N][H][W][C] (C % 4 == 0) into out rows of pitch ldo (ldo % 4 == 0, ldo >= C); in and
+ *   out 16-byte aligned.
+ * asyrp_fid_mean: out[n][c] = the mean of in [N][HW][C] over the HW pixels, summed in pixel order.
+ * asyrp_fid_moments: mu [d] and sigma [d][d] (fp64) of the n rows of x fp32 [n][d]: column means and the centred
+ *   covariance with the n - 1 denominator; n >= 2, d % 64 == 0.
+ * asyrp_fid_kernel_sum: out[0] = sum over i < n, j < m of (x[i] . y[j] / d + 1)^3 in fp64, pairs i == j skipped with
+ *   exclude_diag; x fp32 [n][d], y fp32 [m][d], d % 16 == 0; partial: asyrp_fid_kernel_sum_partials(n, m) doubles of
+ *   workspace.
+ * Fixed-order reductions, no atomics, no kernel mixes samples. */
+int asyrp_fid_pack(const float* x, float* out, int B, int H, int W, int S, void* stream);
+int asyrp_fid_conv(const float* in, const float* weight, const float* bias, float* out, int N, int H, int W, int Cin,
+                   int Cout, int kh, int kw, int stride, int padh, int padw, int ldo, int cstore, void* stream);
+int asyrp_fid_pool(const float* in, float* out, int N, int H, int W, int C, int mode, int ldo, void* stream);
+int asyrp_fid_mean(const float* in, float* out, int N, int HW, int C, void* stream);
+int asyrp_fid_moments(const float* x, double* mu, double* sigma, int n, int d, void* stream);
+int asyrp_fid_kernel_sum_partials(int n, int m); /* host only */
+int asyrp_fid_kernel_sum(const float* x, const float* y, double* partial, double* out, int n, int m, int d,
+                         int exclude_diag, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

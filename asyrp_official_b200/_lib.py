@@ -133,6 +133,10 @@ SIGNATURES = {
     "asyrp_fid_moments": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_void_p]),
     "asyrp_fid_kernel_sum_partials": (c_int, [c_int, c_int]),
     "asyrp_fid_kernel_sum": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p]),
+    "asyrp_fid_pack_u8": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p]),
+    "asyrp_fid_kernel_sum_subsets_partials": (c_int, [c_int, c_int]),
+    "asyrp_fid_kernel_sum_subsets": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int,
+                                             c_int, c_int, c_int, c_int, c_void_p]),
 }
 
 _lib = None

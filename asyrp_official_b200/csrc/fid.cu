@@ -1,7 +1,8 @@
 // Inception-v3 pool features (the FID variant of pytorch-fid) and the set statistics of FID and KID.
 //
 //   x299 = 2 * bilinear_299(floor(clamp((x + 1) / 2 * 255 + 1/2, 0, 255)) / 255) - 1 as NHWC, 4 channels
-//                                                                                        fid_pack_kernel
+//                                                                                        fid_pack_kernel<SavedPng>
+//   the same from the u8 of a decoded image file (u8 NHWC), bit-identical for the same u8  fid_pack_kernel<DecodedU8>
 //   BasicConv2d = conv (1x1, 3x3, 5x5, 1x7, 7x1, 1x3, 3x1; separate vertical / horizontal padding) + folded BN + ReLU,
 //     written into a channel slice [0, cstore) of rows of pitch ldo                     tf32_gemm.cuh (kEpiReluSlice)
 //   max-pool 3x3 / 2 (stem, InceptionB / D), avg-pool 3x3 / 1 pad 1 without the padding (FIDInceptionA / C / E_1),
@@ -9,6 +10,7 @@
 //   pool features = mean over the 8 x 8 pixels of Mixed_7c                             fid_mean_kernel
 //   mu, Sigma = column means and (n - 1)-normalised centred covariance, fp64           fid_colmean_kernel, fid_gram
 //   sum_ij (x_i . y_j / d + 1)^3, fp64, optionally without i == j                      fid_gram, fid_sum_kernel
+//   the same over gathered rows, one sum per index subset (subset KID)                 fid_gram<gather>, fid_sum
 //
 // Every reduction runs in a fixed order and no kernel uses atomics or mixes samples, so an image's features are the
 // same bits whatever batch it is in, and the statistics of a set are the same bits whatever launches produced its rows.
@@ -28,16 +30,39 @@ constexpr int kSumThreads = 256;
 
 enum PoolMode : int { kPoolMax3s2 = 0, kPoolAvg3s1 = 1, kPoolMax3s1 = 2 };
 
-// out[b][Y][X] = (2 * bilinear(q / 255)(Y, X) - 1, channels 0..2; 0), q = the u8 save_image writes for x: the fp32
-// operations (x + 1) * 0.5 * 255 + 0.5, each rounded once, clamped to [0, 255] and truncated.  The resize H x W ->
-// S x S is F.interpolate(mode='bilinear', align_corners=False) as in faceparse_pack_kernel: source row
+// The pixel readers of fid_pack_kernel: px(b, c, y, x) = q / 255 (fp32, rounded once) of the u8 value q of channel c
+// at (y, x) of image b.
+// SavedPng: x fp32 NCHW [B][3][H][W]; q = the u8 save_image writes for x: the fp32 operations
+// (x + 1) * 0.5 * 255 + 0.5, each rounded once, clamped to [0, 255] and truncated.
+struct SavedPng {
+  const float* __restrict__ x;
+  int H, W;
+  __device__ float operator()(size_t b, int c, int yy, int xx) const {
+    const float* img = x + (b * 3 + c) * (static_cast<size_t>(H) * W);
+    const float t = __fadd_rn(__fmul_rn(__fmul_rn(__fadd_rn(img[static_cast<size_t>(yy) * W + xx], 1.f), 0.5f),
+                                        255.f), 0.5f);
+    return __fdiv_rn(truncf(fminf(fmaxf(t, 0.f), 255.f)), 255.f);
+  }
+};
+// DecodedU8: q read from u8 NHWC [B][H][W][3], a decoded image file
+struct DecodedU8 {
+  const uint8_t* __restrict__ x;
+  int H, W;
+  __device__ float operator()(size_t b, int c, int yy, int xx) const {
+    return __fdiv_rn(static_cast<float>(x[((b * H + yy) * W + xx) * 3 + c]), 255.f);
+  }
+};
+
+// out[b][Y][X] = (2 * bilinear(px)(Y, X) - 1, channels 0..2; 0).  The resize H x W -> S x S is
+// F.interpolate(mode='bilinear', align_corners=False) as in faceparse_pack_kernel: source row
 // (Y + .5) * H / S - .5 clamped at 0, rows y0 = floor, y1 = min(y0 + 1, H - 1) weighted 1 - l, l; rows blended first.
-__global__ void fid_pack_kernel(const float* __restrict__ x, float* __restrict__ out, int B, int H, int W, int S) {
+// The blend sees only px's values, so both readers give the same bits for the same q.
+template <class Px>
+__global__ void fid_pack_kernel(Px px, float* __restrict__ out, int B, int H, int W, int S) {
   pdl_trigger();
   pdl_wait();
   const float sh = static_cast<float>(H) / static_cast<float>(S), sw = static_cast<float>(W) / static_cast<float>(S);
   const size_t total = static_cast<size_t>(B) * S * S;
-  const size_t plane = static_cast<size_t>(H) * W;
   for (size_t i = blockIdx.x * static_cast<size_t>(blockDim.x) + threadIdx.x; i < total;
        i += static_cast<size_t>(gridDim.x) * blockDim.x) {
     const int X = static_cast<int>(i % S), Y = static_cast<int>((i / S) % S);
@@ -49,14 +74,8 @@ __global__ void fid_pack_kernel(const float* __restrict__ x, float* __restrict__
     float v[3];
 #pragma unroll
     for (int c = 0; c < 3; ++c) {
-      const float* img = x + (b * 3 + c) * plane;
-      auto px = [&](int yy, int xx) {
-        const float t = __fadd_rn(__fmul_rn(__fmul_rn(__fadd_rn(img[static_cast<size_t>(yy) * W + xx], 1.f), 0.5f),
-                                            255.f), 0.5f);
-        return __fdiv_rn(truncf(fminf(fmaxf(t, 0.f), 255.f)), 255.f);
-      };
-      const float top = (1.f - lx) * px(y0, x0) + lx * px(y0, x1);
-      const float bot = (1.f - lx) * px(y1, x0) + lx * px(y1, x1);
+      const float top = (1.f - lx) * px(b, c, y0, x0) + lx * px(b, c, y0, x1);
+      const float bot = (1.f - lx) * px(b, c, y1, x0) + lx * px(b, c, y1, x1);
       v[c] = 2.f * ((1.f - ly) * top + ly * bot) - 1.f;
     }
     reinterpret_cast<float4*>(out)[i] = make_float4(v[0], v[1], v[2], 0.f);
@@ -136,12 +155,17 @@ __global__ void fid_colmean_kernel(const float* __restrict__ x, double* __restri
 //   kKid true (kernel sum): v = (x[i] . y[j]) / d + 1 over the d features, k = v^3, i < n, j < m (rows = n, cols = m);
 //     pairs i == j are skipped when exclude_diag; the CTA's sum of its k (each thread's 16 in order, then a fixed
 //     tree) goes to partial[blockIdx.y][blockIdx.x].
-template <bool kKid>
+//   kGather (with kKid, subset z = blockIdx.z): the same with row i of x read from x[idx_x[z][i]] and row j of y from
+//     y[idx_y[z][j]], n = m = the subset size; the sum goes to partial[z][blockIdx.y][blockIdx.x].  The tile order and
+//     the tree are those of the plain kernel sum, so a subset's partials are those of the gathered matrices.
+template <bool kKid, bool kGather>
 __global__ void __launch_bounds__(kGramThreads) fid_gram_kernel(const float* __restrict__ x,
                                                                 const float* __restrict__ y,
                                                                 const double* __restrict__ mu,
                                                                 double* __restrict__ out, int n, int m, int d,
-                                                                int exclude_diag) {
+                                                                int exclude_diag, const int* __restrict__ idx_x,
+                                                                const int* __restrict__ idx_y) {
+  static_assert(kKid || !kGather, "fid_gram_kernel: the gather is a kernel-sum mode");
   pdl_trigger();
   __shared__ double xs[kGramK][kGramTile];
   __shared__ double ys[kGramK][kGramTile];
@@ -149,6 +173,18 @@ __global__ void __launch_bounds__(kGramThreads) fid_gram_kernel(const float* __r
   const int i0 = blockIdx.y * kGramTile, j0 = blockIdx.x * kGramTile;
   const int kdim = kKid ? d : n;  // contraction length
   pdl_wait();
+  // kGather: the source rows of this thread's staging loads, sample ii = t / 16 + 16 q of the tile in load q
+  int rx[kGramK * kGramTile / kGramThreads], ry[kGramK * kGramTile / kGramThreads];
+  if (kGather) {
+    const int* ix = idx_x + static_cast<size_t>(blockIdx.z) * n;
+    const int* iy = idx_y + static_cast<size_t>(blockIdx.z) * m;
+#pragma unroll
+    for (int q = 0; q < kGramK * kGramTile / kGramThreads; ++q) {
+      const int ii = (t + kGramThreads * q) / kGramK;
+      rx[q] = i0 + ii < n ? ix[i0 + ii] : 0;
+      ry[q] = j0 + ii < m ? iy[j0 + ii] : 0;
+    }
+  }
   double acc[4][4];
 #pragma unroll
   for (int a = 0; a < 4; ++a)
@@ -160,8 +196,9 @@ __global__ void __launch_bounds__(kGramThreads) fid_gram_kernel(const float* __r
       const int e = t + kGramThreads * q;
       if (kKid) {  // rows of x / y are samples: 16 consecutive features of 64 samples
         const int ii = e / kGramK, kk = e % kGramK, k = k0 + kk;
-        xs[kk][ii] = i0 + ii < n ? static_cast<double>(x[static_cast<size_t>(i0 + ii) * d + k]) : 0.0;
-        ys[kk][ii] = j0 + ii < m ? static_cast<double>(y[static_cast<size_t>(j0 + ii) * d + k]) : 0.0;
+        const int r = kGather ? rx[q] : i0 + ii, c = kGather ? ry[q] : j0 + ii;
+        xs[kk][ii] = i0 + ii < n ? static_cast<double>(x[static_cast<size_t>(r) * d + k]) : 0.0;
+        ys[kk][ii] = j0 + ii < m ? static_cast<double>(y[static_cast<size_t>(c) * d + k]) : 0.0;
       } else {  // rows of x are samples, columns features: 64 consecutive features of 16 samples, centred
         const int kk = e / kGramTile, ii = e % kGramTile, r = k0 + kk;
         const bool ok = r < n;
@@ -210,25 +247,27 @@ __global__ void __launch_bounds__(kGramThreads) fid_gram_kernel(const float* __r
     if (t < h) red[t] += red[t + h];
     __syncthreads();
   }
-  if (t == 0) out[static_cast<size_t>(blockIdx.y) * gridDim.x + blockIdx.x] = red[0];
+  if (t == 0) out[(static_cast<size_t>(blockIdx.z) * gridDim.y + blockIdx.y) * gridDim.x + blockIdx.x] = red[0];
 }
 
-// out[0] = the sum of the `count` partials: thread t adds partials t, t + 256, ... in order, then a fixed tree
+// out[z] = the sum of the `count` partials partial[z][0 .. count), z = blockIdx.x: thread t adds partials t, t + 256,
+// ... in order, then a fixed tree
 __global__ void __launch_bounds__(kSumThreads) fid_sum_kernel(const double* __restrict__ partial, int count,
                                                               double* __restrict__ out) {
   pdl_trigger();
   __shared__ double red[kSumThreads];
   pdl_wait();
   const int t = threadIdx.x;
+  const double* p = partial + static_cast<size_t>(blockIdx.x) * count;
   double s = 0.0;
-  for (int i = t; i < count; i += kSumThreads) s += partial[i];
+  for (int i = t; i < count; i += kSumThreads) s += p[i];
   red[t] = s;
   __syncthreads();
   for (int h = kSumThreads / 2; h > 0; h >>= 1) {
     if (t < h) red[t] += red[t + h];
     __syncthreads();
   }
-  if (t == 0) out[0] = red[0];
+  if (t == 0) out[blockIdx.x] = red[0];
 }
 
 inline int fid_grid(size_t total, int block) {
@@ -249,8 +288,17 @@ extern "C" {
 ASYRP_API int asyrp_fid_pack(const float* x, float* out, int B, int H, int W, int S, void* stream) {
   ASYRP_REQUIRE(B > 0 && H > 0 && W > 0 && S > 0, "asyrp_fid_pack: bad shape B=%d H=%d W=%d S=%d", B, H, W, S);
   const size_t total = static_cast<size_t>(B) * S * S;
-  ASYRP_LAUNCH(fid_pack_kernel, dim3(fid_grid(total, 256)), dim3(256), 0, static_cast<cudaStream_t>(stream), x, out,
-               B, H, W, S);
+  ASYRP_LAUNCH(fid_pack_kernel<SavedPng>, dim3(fid_grid(total, 256)), dim3(256), 0, static_cast<cudaStream_t>(stream),
+               SavedPng{x, H, W}, out, B, H, W, S);
+  ASYRP_CHECK_CUDA(cudaGetLastError());
+  return ASYRP_OK;
+}
+
+ASYRP_API int asyrp_fid_pack_u8(const uint8_t* x, float* out, int B, int H, int W, int S, void* stream) {
+  ASYRP_REQUIRE(B > 0 && H > 0 && W > 0 && S > 0, "asyrp_fid_pack_u8: bad shape B=%d H=%d W=%d S=%d", B, H, W, S);
+  const size_t total = static_cast<size_t>(B) * S * S;
+  ASYRP_LAUNCH(fid_pack_kernel<DecodedU8>, dim3(fid_grid(total, 256)), dim3(256), 0,
+               static_cast<cudaStream_t>(stream), DecodedU8{x, H, W}, out, B, H, W, S);
   ASYRP_CHECK_CUDA(cudaGetLastError());
   return ASYRP_OK;
 }
@@ -322,8 +370,9 @@ ASYRP_API int asyrp_fid_moments(const float* x, double* mu, double* sigma, int n
   ASYRP_REQUIRE(static_cast<long long>(n) * d < (1LL << 40), "asyrp_fid_moments: n * d too large");
   const cudaStream_t st = static_cast<cudaStream_t>(stream);
   ASYRP_LAUNCH(fid_colmean_kernel, dim3((d + 255) / 256), dim3(256), 0, st, x, mu, n, d);
-  ASYRP_LAUNCH(fid_gram_kernel<false>, dim3(d / kGramTile, d / kGramTile), dim3(kGramThreads), 0, st, x, x,
-               static_cast<const double*>(mu), sigma, n, d, d, 0);
+  ASYRP_LAUNCH(fid_gram_kernel<false, false>, dim3(d / kGramTile, d / kGramTile), dim3(kGramThreads), 0, st, x, x,
+               static_cast<const double*>(mu), sigma, n, d, d, 0, static_cast<const int*>(nullptr),
+               static_cast<const int*>(nullptr));
   ASYRP_CHECK_CUDA(cudaGetLastError());
   return ASYRP_OK;
 }
@@ -341,10 +390,40 @@ ASYRP_API int asyrp_fid_kernel_sum(const float* x, const float* y, double* parti
                 exclude_diag);
   const cudaStream_t st = static_cast<cudaStream_t>(stream);
   const dim3 grid((m + kGramTile - 1) / kGramTile, (n + kGramTile - 1) / kGramTile);
-  ASYRP_LAUNCH(fid_gram_kernel<true>, grid, dim3(kGramThreads), 0, st, x, y, static_cast<const double*>(nullptr),
-               partial, n, m, d, exclude_diag);
+  ASYRP_LAUNCH(fid_gram_kernel<true, false>, grid, dim3(kGramThreads), 0, st, x, y,
+               static_cast<const double*>(nullptr), partial, n, m, d, exclude_diag, static_cast<const int*>(nullptr),
+               static_cast<const int*>(nullptr));
   ASYRP_LAUNCH(fid_sum_kernel, dim3(1), dim3(kSumThreads), 0, st, static_cast<const double*>(partial),
                static_cast<int>(grid.x * grid.y), out);
+  ASYRP_CHECK_CUDA(cudaGetLastError());
+  return ASYRP_OK;
+}
+
+ASYRP_API int asyrp_fid_kernel_sum_subsets_partials(int s, int subsets) {
+  const long long tiles = (s + kGramTile - 1) / kGramTile;
+  const long long count = tiles * tiles * subsets;
+  return s > 0 && subsets > 0 && count < (1LL << 31) ? static_cast<int>(count) : -1;
+}
+
+ASYRP_API int asyrp_fid_kernel_sum_subsets(const float* x, const float* y, const int* idx_x, const int* idx_y,
+                                           double* partial, double* out, int n, int m, int s, int subsets, int d,
+                                           int exclude_diag, void* stream) {
+  ASYRP_REQUIRE(n > 0 && m > 0 && s > 0 && subsets > 0 && d > 0,
+                "asyrp_fid_kernel_sum_subsets: bad shape n=%d m=%d s=%d subsets=%d d=%d", n, m, s, subsets, d);
+  ASYRP_REQUIRE(d % kGramK == 0, "asyrp_fid_kernel_sum_subsets: d=%d must be a multiple of %d", d, kGramK);
+  ASYRP_REQUIRE(subsets <= kMaxGridYZ, "asyrp_fid_kernel_sum_subsets: subsets=%d above %d", subsets, kMaxGridYZ);
+  ASYRP_REQUIRE(exclude_diag == 0 || exclude_diag == 1,
+                "asyrp_fid_kernel_sum_subsets: exclude_diag=%d must be 0 or 1", exclude_diag);
+  ASYRP_REQUIRE(!exclude_diag || s >= 2, "asyrp_fid_kernel_sum_subsets: exclude_diag needs s >= 2 (s=%d)", s);
+  ASYRP_REQUIRE(asyrp_fid_kernel_sum_subsets_partials(s, subsets) > 0,
+                "asyrp_fid_kernel_sum_subsets: s=%d x subsets=%d too large", s, subsets);
+  ASYRP_REQUIRE(idx_x != nullptr && idx_y != nullptr, "asyrp_fid_kernel_sum_subsets: needs idx_x and idx_y");
+  const cudaStream_t st = static_cast<cudaStream_t>(stream);
+  const int tiles = (s + kGramTile - 1) / kGramTile;
+  ASYRP_LAUNCH(fid_gram_kernel<true, true>, dim3(tiles, tiles, subsets), dim3(kGramThreads), 0, st, x, y,
+               static_cast<const double*>(nullptr), partial, s, s, d, exclude_diag, idx_x, idx_y);
+  ASYRP_LAUNCH(fid_sum_kernel, dim3(subsets), dim3(kSumThreads), 0, st, static_cast<const double*>(partial),
+               tiles * tiles, out);
   ASYRP_CHECK_CUDA(cudaGetLastError());
   return ASYRP_OK;
 }

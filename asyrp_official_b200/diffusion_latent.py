@@ -22,7 +22,9 @@ Mirrors, with the same attribute / flag names:
   --fid                        (none)                       run_test scores each set of edits (one per hs_coeff tuple)
                                                             against the origin pass with FID and KID on Inception-v3
                                                             pool features (fid.FIDInception), gathered to rank 0 at the
-                                                            end of the run; this build's definition
+                                                            end of the run; this build's definition; with --fid_ref also
+                                                            the origin and each edited set against real images'
+                                                            statistics (fid.score_against_stats)
   Asyrp.precompute_pairs_with_h :877-947                    DDIM inversion of one image keeping the bottleneck h of
                                                             every step (batched here, same cache file)
   Asyrp.run_diff_style         main.py:192-202              --diff_style (DiffStyle content injection): this build's
@@ -79,6 +81,9 @@ class Asyrp(object):
         self.id_similarity = {}  # --id_similarity: save_image's file name -> 1 - IDLoss [tuples][images]
         self.seg_consistency = {}  # --seg_consistency: save_image's file name -> SC [tuples][images]
         self.fid = {}  # --fid (rank 0): 'train' / 'test' -> fp64 [tuples][2], (FID, KID) of each tuple's set
+        # --fid_ref (rank 0): 'train' / 'test' -> fp64 [1 + tuples][4], (FID, KID, KID_mean, KID_std) against the real
+        # images' statistics of the origin set (row 0) and of each tuple's set
+        self.fid_real = {}
 
     # ------------------------------------------------------------------------------------------
     def load_pretrained_model(self):
@@ -244,8 +249,17 @@ class Asyrp(object):
     def fid_setup(self):
         """--fid's requirements, checked before any model is loaded; raises ValueError with the reason.  Returns the
         validated --fid_weights state dict (fid.load_state_dict)."""
-        from .fid import load_state_dict
+        from .fid import load_state_dict, validate_stats
         a = self.args
+        ref = getattr(a, "fid_ref", None)
+        if ref is not None:  # the headers only; rank 0 reads the arrays in finish_fid
+            if a.kid_subsets < 0 or a.kid_subset_size < 2:
+                raise ValueError(f"--fid_ref: --kid_subsets must be >= 0 and --kid_subset_size >= 2, got "
+                                 f"{a.kid_subsets} and {a.kid_subset_size}")
+            try:
+                validate_stats(ref)
+            except ValueError as e:
+                raise ValueError(f"--fid_ref: {e}") from None
         if getattr(a, "pass_editing", False):
             raise ValueError("--fid scores the edited images: with --pass_editing nothing is edited")
         if getattr(a, "diff_style", False):
@@ -264,28 +278,41 @@ class Asyrp(object):
         image index and scores every tuple's edited set against the origin set of the same pass: printed, kept in
         self.fid[mode] and written to <test_image_folder>/<mode>_ngen<n_train_step>_fid.tsv.  Every rank must call it,
         also one that ran no batch."""
-        from .fid import fid_kid, set_moments
+        from .fid import fid_kid, load_stats, score_against_stats, set_moments
         a = self.args
         dist_on = self.world > 1 and torch.distributed.is_available() and torch.distributed.is_initialized()
         got = sets.gather(self.rank, self.world if dist_on else 1)
         if got is None:
             return
+        real = None
+        if getattr(a, "fid_ref", None) is not None:  # --fid_ref: the real images' statistics, read once
+            real = load_stats(a.fid_ref)
+            if "features" in real:
+                real["features"] = torch.from_numpy(real["features"]).to(self.device)
         for mode in ("train", "test"):
             if (mode, "origin") not in got:
                 continue
             ids, ref = got[(mode, "origin")]
             ref = ref.to(self.device).contiguous()
             ref_moments = set_moments(ref) if ref.shape[0] >= 2 else None
-            rows = []
+            rows, edited = [], []
             for k in range(len(coeffs)):
                 ids_k, feats = got[(mode, k)]
                 if not torch.equal(ids_k, ids):
                     raise RuntimeError(f"--fid: tuple {k} of the {mode} pass has other images than its origin set")
-                rows.append(fid_kid(ref, feats.to(self.device).contiguous(), ref_moments))
+                edited.append(feats.to(self.device).contiguous())
+                rows.append(fid_kid(ref, edited[-1], ref_moments))
             self.fid[mode] = torch.tensor(rows, dtype=torch.float64)
             os.makedirs(a.test_image_folder, exist_ok=True)
             write_fid(os.path.join(a.test_image_folder, f"{mode}_ngen{a.n_train_step}_fid.tsv"), coeffs, rows,
                       ref.shape[0], mode, attrs=attrs)
+            if real is not None:
+                real_rows = [score_against_stats(f, real, a.kid_subsets, a.kid_subset_size, m)
+                             for f, m in [(ref, ref_moments)] + [(e, None) for e in edited]]
+                self.fid_real[mode] = torch.tensor(real_rows, dtype=torch.float64)
+                n_ref = real["features"].shape[0] if "features" in real else None
+                write_fid_real(os.path.join(a.test_image_folder, f"{mode}_ngen{a.n_train_step}_fid_real.tsv"),
+                               coeffs, real_rows, ref.shape[0], n_ref, mode, attrs=attrs)
 
     def write_id_similarity(self, path, coeffs, ids):
         """the TSV of one batch: one row per (hs_coeff tuple, image) in grid order, ID = 1 - IDLoss(origin, edit) of
@@ -685,6 +712,8 @@ class Asyrp(object):
     @torch.no_grad()
     def run_test(self):
         a = self.args
+        if getattr(a, "fid_ref", None) is not None and not getattr(a, "fid", False):
+            raise ValueError("--fid_ref scores the sets that --fid collects: add --fid")
         if getattr(a, "attr_sweep", ""):
             return self.run_attr_sweep()
         print("Running Test")
@@ -1333,6 +1362,27 @@ def write_fid(path, coeffs, rows, n, mode, attrs=None):
     for k, (fd, kd) in enumerate(rows):
         name = f"attribute {attrs[k]}" if attrs is not None else f"hs_coeff {tuple(float(c) for c in coeffs[k])}"
         print(f"FID / KID ({mode}, {n} images), {name}: FID {fd:.6f}, KID {kd:.6f}")
+
+
+def write_fid_real(path, coeffs, rows, n, n_ref, mode, attrs=None):
+    """the table of one pass against real images' statistics (--fid_ref): rows[0] the origin set (tuple `origin`,
+    hs_coeff `-`), rows[1 + k] tuple k's set, each (FID, KID, KID_mean, KID_std); columns tuple, hs_coeff, n (images
+    per set), n_ref (reference images; `-` for a file without features), FID, KID, KID_mean, KID_std, and `attr` under
+    an attribute sweep; values as write_fid writes them.  Prints each row's values"""
+    names = [("origin", "-", "-")] + [(str(k), ",".join(f"{float(c):.6g}" for c in coeffs[k]),
+                                        attrs[k] if attrs is not None else None) for k in range(len(coeffs))]
+    nr = "-" if n_ref is None else str(n_ref)
+    with open(path, "w") as f:
+        f.write("tuple\ths_coeff\tn\tn_ref\tFID\tKID\tKID_mean\tKID_std" + ("\tattr" if attrs is not None else "") +
+                "\n")
+        for (key, tup, attr), vals in zip(names, rows):
+            f.write(f"{key}\t{tup}\t{n}\t{nr}\t" + "\t".join(repr(float(v)) for v in vals) +
+                    (f"\t{attr}" if attrs is not None else "") + "\n")
+    for k, (fd, kd, km, ks) in enumerate(rows):
+        name = "origin" if k == 0 else (f"attribute {attrs[k - 1]}" if attrs is not None
+                                        else f"hs_coeff {tuple(float(c) for c in coeffs[k - 1])}")
+        print(f"FID / KID against the real images ({mode}, {n} images, {nr} reference), {name}: FID {fd:.6f}, "
+              f"KID {kd:.6f}, subset KID {km:.6f} +- {ks:.6f}")
 
 
 def plan_sweep(n_tuples, bs, max_rows):

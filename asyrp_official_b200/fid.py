@@ -32,11 +32,29 @@ attribute) is one edited set, scored against the origin DDIM pass of the same x_
            the two within-set sums: torch-fidelity's KID mean with kid_subset_size = n.
 
 A set of fewer than two images gets nan for both.  The moments and the kernel sums run on the GPU in fp64
-(csrc/fid.cu); the two 2048^2 eigendecompositions per set run on the host in fp64.  No real
-pt_inception-2015-12-05-6726825d.pth has been loaded by this project's tests: the key list below follows torchvision's
-Inception3, and the loader refuses any other layout by name.
+(csrc/fid.cu); the two 2048^2 eigendecompositions per set run on the host in fp64.
+
+Real images (--fid_ref STATS.npz): `python -m asyrp_official_b200.fid --save-stats DIR OUT.npz --fid_weights W` reads
+every image directly in DIR as pytorch-fid does (Image.open(p).convert('RGB') at its own size: no resize or crop to
+the edits' size), runs the u8 through features_u8 (pytorch-fid's ToTensor path, the same bits as features of
+u8 / 127.5 - 1) and writes mu / sigma (pytorch-fid's keys, fp64), the features (fp32) and kid_kxx (their kernel sum
+without the diagonal).  A run then scores its origin set and each edited set against that file:
+
+    FID       as above against the file's mu / sigma (a pytorch-fid --save-stats file works too)
+    KID       the full-set KID, the reference's within-set sum taken from kid_kxx
+    KID_mean  torch-fidelity's KID mean / std over random subsets (kid_subsets: kid_subsets subsets of
+    KID_std   kid_subset_size rows, RandomState(2020), the edited set drawn first); nan when a set is smaller
+
+The KID columns are nan for a file without features.  Precision / recall and the Inception score are not computed.
+
+No real pt_inception-2015-12-05-6726825d.pth has been loaded by this project's tests: the key list below follows
+torchvision's Inception3, and the loader refuses any other layout by name.
 """
+import argparse
 import math
+import os
+import sys
+import time
 
 import numpy as np
 import torch
@@ -223,6 +241,157 @@ def fid_kid(ref, edited, ref_moments=None):
     return frechet_distance(mu1, s1, mu2, s2), kid(ref.contiguous(), edited.contiguous())
 
 
+def kid_subset_indices(n, m, subsets, size, seed=2020):
+    """int32 [subsets][size] row indices into the scored set (n rows) and the reference (m rows): a fresh
+    RandomState(seed), per subset in order choice(n, size, replace=False) then choice(m, size, replace=False)"""
+    rng = np.random.RandomState(seed)
+    i1, i2 = np.empty((subsets, size), np.int32), np.empty((subsets, size), np.int32)
+    for z in range(subsets):
+        i1[z] = rng.choice(n, size, replace=False)
+        i2[z] = rng.choice(m, size, replace=False)
+    return i1, i2
+
+
+def kid_subsets(f1, f2, subsets, size, seed=2020):
+    """(mean, std) of the KID over random subsets, torch-fidelity's kid_features_to_metric: f1 the set scored, f2 the
+    reference (fp32 [n][d] / [m][d] on the device).  A fresh np.random.RandomState(seed) draws, for each subset in
+    order, size rows of f1 and then size rows of f2 without replacement; each subset's MMD^2 is kid_from_sums of its
+    three kernel sums (the diagonal excluded within a set); np.mean and np.std (ddof 0) of the subsets' values.  The
+    sums of all subsets run in three launches.  (nan, nan) and a printed warning when a set has fewer than size rows
+    (torch-fidelity raises there)."""
+    if subsets < 1 or size < 2:
+        raise ValueError(f"kid_subsets: needs subsets >= 1 and size >= 2, got {subsets} and {size}")
+    n, m = f1.shape[0], f2.shape[0]
+    if n < size or m < size:
+        print(f"KID subsets: a set of {min(n, m)} rows is smaller than the subset size {size}: nan")
+        return math.nan, math.nan
+    i1, i2 = kid_subset_indices(n, m, subsets, size, seed)
+    t1, t2 = torch.from_numpy(i1).to(f1.device), torch.from_numpy(i2).to(f1.device)
+    f1, f2 = f1.contiguous(), f2.contiguous()
+    kxx = ops.fid_kernel_sum_subsets(f1, f1, t1, t1, exclude_diag=True).cpu().numpy()
+    kyy = ops.fid_kernel_sum_subsets(f2, f2, t2, t2, exclude_diag=True).cpu().numpy()
+    kxy = ops.fid_kernel_sum_subsets(f1, f2, t1, t2).cpu().numpy()
+    mmd = kid_from_sums(kxx, kyy, kxy, size, size)
+    return float(np.mean(mmd)), float(np.std(mmd))
+
+
+def score_against_stats(f, real, subsets, size, moments=None):
+    """(FID, KID, KID_mean, KID_std) of the feature set f (fp32 [n][d] on the device) against reference statistics
+    real (load_stats, its features moved to the device): FID against mu / sigma; the full-set KID from real's kid_kxx
+    and f's two kernel sums; the subset KID (kid_subsets, f first) when subsets > 0.  The KID values are nan without
+    features in real, all four are nan when f has fewer than two rows.  moments: set_moments(f) when already known."""
+    n = f.shape[0]
+    if n < 2:
+        print(f"FID / KID against the real images: a set of {n} image(s) has no covariance: nan")
+        return math.nan, math.nan, math.nan, math.nan
+    mu, sigma = moments if moments is not None else set_moments(f)
+    fd = frechet_distance(mu, sigma, real["mu"], real["sigma"])
+    if "features" not in real:
+        return fd, math.nan, math.nan, math.nan
+    ref = real["features"]
+    kxx = ops.fid_kernel_sum(f, f, exclude_diag=True).item()
+    kxy = ops.fid_kernel_sum(f, ref).item()
+    kd = kid_from_sums(kxx, real["kid_kxx"], kxy, n, ref.shape[0])
+    km, ks = kid_subsets(f, ref, subsets, size) if subsets > 0 else (math.nan, math.nan)
+    return fd, kd, km, ks
+
+
+# ---- reference statistics (.npz): pytorch-fid's keys mu / sigma, plus this project's features / kid_kxx for KID ----
+# key -> (dtype, shape); None: any length >= 2
+STATS_KEYS = {"mu": (np.float64, (DIMS,)), "sigma": (np.float64, (DIMS, DIMS)), "features": (np.float32, (None, DIMS)),
+              "kid_kxx": (np.float64, ())}
+SAVE_STATS_HINT = "make one with python -m asyrp_official_b200.fid --save-stats DIR OUT.npz --fid_weights W"
+
+
+def validate_stats(path):
+    """Check a reference statistics file's keys, dtypes and shapes from the .npy headers alone (no array is read).
+    Returns (number of reference rows or None, whether it holds features / kid_kxx for KID).  mu / sigma are required;
+    features and kid_kxx come together.  Raises ValueError naming the key or the problem."""
+    import zipfile
+    what = f"FID reference statistics {path!r}"
+    if os.path.isdir(path):
+        raise ValueError(f"{what} is a directory, not a statistics file: {SAVE_STATS_HINT}")
+    if not os.path.isfile(path):
+        raise ValueError(f"{what}: no such file ({SAVE_STATS_HINT})")
+    if not zipfile.is_zipfile(path):
+        raise ValueError(f"{what}: not an .npz file")
+    headers = {}
+    try:
+        with zipfile.ZipFile(path) as zf:
+            for name in zf.namelist():
+                key = name[:-4] if name.endswith(".npy") else name
+                with zf.open(name) as f:
+                    version = np.lib.format.read_magic(f)
+                    read = {(1, 0): np.lib.format.read_array_header_1_0,
+                            (2, 0): np.lib.format.read_array_header_2_0}.get(version)
+                    if read is None:
+                        raise ValueError(f"{key!r} has .npy format version {version}")
+                    shape, _, dtype = read(f)
+                headers[key] = (dtype, tuple(shape))
+    except (zipfile.BadZipFile, OSError, EOFError, ValueError) as e:
+        raise ValueError(f"{what}: cannot be read ({e})") from None
+    unknown = sorted(set(headers) - set(STATS_KEYS))
+    if unknown:
+        raise ValueError(f"{what}: unexpected keys {unknown} (expected mu, sigma and optionally features, kid_kxx)")
+    for key in ("mu", "sigma"):
+        if key not in headers:
+            raise ValueError(f"{what}: missing key {key!r}")
+    if ("features" in headers) != ("kid_kxx" in headers):
+        missing = "kid_kxx" if "features" in headers else "features"
+        raise ValueError(f"{what}: missing key {missing!r} (features and kid_kxx come together)")
+    for key, (dtype, shape) in headers.items():
+        want_dtype, want_shape = STATS_KEYS[key]
+        if dtype != np.dtype(want_dtype):
+            raise ValueError(f"{what}: {key!r} has dtype {dtype}, expected {np.dtype(want_dtype)}")
+        if len(shape) != len(want_shape) or any(w is not None and s != w for s, w in zip(shape, want_shape)) or \
+                (key == "features" and shape[0] < 2):
+            raise ValueError(f"{what}: {key!r} has shape {shape}, expected "
+                             f"{tuple('N >= 2' if w is None else w for w in want_shape)}")
+    has_features = "features" in headers
+    return (headers["features"][1][0] if has_features else None), has_features
+
+
+def load_stats(path, with_features=True):
+    """the validated statistics of path: {'mu', 'sigma'} fp64 numpy, plus 'features' fp32 [N][2048] and 'kid_kxx'
+    (float) when with_features and the file holds them"""
+    _, has_features = validate_stats(path)
+    with np.load(path, allow_pickle=False) as z:
+        out = {"mu": z["mu"], "sigma": z["sigma"]}
+        if with_features and has_features:
+            out["features"] = z["features"]
+            out["kid_kxx"] = float(z["kid_kxx"])
+    return out
+
+
+def stats_arrays(feats):
+    """the arrays of a statistics file for the feature set feats fp32 [N][2048] on the device (N >= 2): mu and sigma
+    (set_moments), the features and kid_kxx, their kernel sum without the diagonal (ops.fid_kernel_sum)"""
+    feats = feats.contiguous()
+    mu, sigma = set_moments(feats)
+    kxx = ops.fid_kernel_sum(feats, feats, exclude_diag=True).cpu().numpy()
+    return {"mu": mu, "sigma": sigma, "features": feats.cpu().numpy(), "kid_kxx": kxx}
+
+
+def save_stats(path, feats):
+    """write the statistics of feats (fp32 [N][2048] on the device, N >= 2) to path (write_stats)"""
+    if feats.dim() != 2 or feats.shape[0] < 2 or feats.shape[1] != DIMS:
+        raise ValueError(f"save_stats: needs features [N >= 2][{DIMS}], got {tuple(feats.shape)}")
+    write_stats(path, stats_arrays(feats))
+
+
+def write_stats(path, arrays):
+    """arrays (key -> numpy array) as an uncompressed .npz that np.load reads (pytorch-fid reads its mu / sigma).  The
+    members carry a fixed time stamp, so the same arrays give the same file bytes.  Written to a temporary file, then
+    renamed."""
+    import zipfile
+    tmp = f"{path}.tmp.{os.getpid()}"
+    with zipfile.ZipFile(tmp, "w", zipfile.ZIP_STORED, allowZip64=True) as zf:
+        for key, a in arrays.items():
+            with zf.open(zipfile.ZipInfo(f"{key}.npy", date_time=(1980, 1, 1, 0, 0, 0)), "w", force_zip64=True) as f:
+                np.lib.format.write_array(f, np.asarray(a, order="C"), allow_pickle=False)
+    os.replace(tmp, path)
+
+
 class FIDInception:
     """FIDInception(weights, device): features(x) -> fp32 [B][2048] on the device, the pool features of images
     x [B][3][H][W] in [-1, 1] (any size; quantised as their PNG, resized to 299 x 299).  Every operation is a kernel of
@@ -288,11 +457,14 @@ class FIDInception:
         ops.fid_pool(h, p, ops.FID_POOL_MAX3S2)
         return p
 
-    def _chunk_features(self, x):
+    def _chunk_features(self, x, u8=False):
         B = x.shape[0]
         f32 = dict(dtype=torch.float32, device=self.device)
         h = torch.empty(B, SIZE, SIZE, 4, **f32)
-        ops.fid_pack(x.to(**f32).contiguous(), h)
+        if u8:
+            ops.fid_pack_u8(x.to(self.device, non_blocking=True).contiguous(), h)
+        else:
+            ops.fid_pack(x.to(**f32).contiguous(), h)
         h = self._conv("Conv2d_2a_3x3", self._conv("Conv2d_1a_3x3", h))
         h = self._maxpool(self._conv("Conv2d_2b_3x3", h))
         h = self._maxpool(self._conv("Conv2d_4a_3x3", self._conv("Conv2d_3b_1x1", h)))
@@ -310,6 +482,17 @@ class FIDInception:
             raise ValueError(f"images must be [B][3][H][W], got {tuple(x.shape)}")
         with torch.cuda.device(self.device):
             return torch.cat([self._chunk_features(x[i:i + self.max_rows])
+                              for i in range(0, x.shape[0], self.max_rows)])
+
+    @torch.no_grad()
+    def features_u8(self, x):
+        """pool features fp32 [B][2048] on the device of decoded images x u8 [B][H][W][3] (as PIL gives them; pinned
+        host memory or the device), pytorch-fid's input path: bit-identical to features(x / 127.5 - 1)"""
+        x = torch.as_tensor(x)
+        if x.dim() != 4 or x.shape[3] != 3 or x.shape[0] == 0 or x.dtype != torch.uint8:
+            raise ValueError(f"images must be uint8 [B][H][W][3], got {x.dtype} {tuple(x.shape)}")
+        with torch.cuda.device(self.device):
+            return torch.cat([self._chunk_features(x[i:i + self.max_rows], u8=True)
                               for i in range(0, x.shape[0], self.max_rows)])
 
 
@@ -351,3 +534,95 @@ def _sorted_rows(parts):
     if len(set(ids.tolist())) != ids.numel():
         raise ValueError(f"FID: an image index occurs twice in one set: {sorted(ids.tolist())}")
     return ids[order], feats[order]
+
+
+# ---- python -m asyrp_official_b200.fid --save-stats DIR OUT.npz: the statistics of a folder of real images ----
+IMAGE_EXTENSIONS = ("bmp", "jpg", "jpeg", "pgm", "png", "ppm", "tif", "tiff", "webp")  # pytorch-fid's
+
+
+def image_files(folder):
+    """the image files directly in folder with one of pytorch-fid's extensions (as its glob: lower case), sorted"""
+    return sorted(os.path.join(folder, f) for f in os.listdir(folder)
+                  if f.rsplit(".", 1)[-1] in IMAGE_EXTENSIONS and "." in f and os.path.isfile(os.path.join(folder, f)))
+
+
+class ImageFiles(torch.utils.data.Dataset):
+    """(index, u8 [H][W][3]) of each file, decoded as pytorch-fid decodes it: Image.open(p).convert('RGB') at its own
+    size"""
+
+    def __init__(self, files):
+        self.files = files
+
+    def __len__(self):
+        return len(self.files)
+
+    def __getitem__(self, i):
+        from PIL import Image
+        with Image.open(self.files[i]) as im:
+            return i, torch.from_numpy(np.array(im.convert("RGB"), dtype=np.uint8))
+
+
+def collate_by_size(items):
+    """a loader batch as [(indices int64 [b], u8 [b][H][W][3])], one entry per image size in order of first occurrence"""
+    groups = {}
+    for i, a in items:
+        groups.setdefault(tuple(a.shape), []).append((i, a))
+    return [(torch.tensor([i for i, _ in g]), torch.stack([a for _, a in g])) for g in groups.values()]
+
+
+def folder_features(net, files, batch_size=50, num_workers=8):
+    """(pool features fp32 [N][2048] on the device in file order, seconds waiting on the decoding workers, seconds of
+    GPU work): each loader batch decoded in DataLoader workers into pinned u8, grouped by size, through features_u8.
+    An image's features do not depend on its batch, so neither do the result's bits."""
+    loader = torch.utils.data.DataLoader(ImageFiles(files), batch_size=batch_size, num_workers=num_workers,
+                                         collate_fn=collate_by_size, pin_memory=True)
+    feats = torch.empty(len(files), DIMS, dtype=torch.float32, device=net.device)
+    wait = gpu = 0.0
+    t0 = time.perf_counter()
+    for groups in loader:
+        t1 = time.perf_counter()
+        for ids, u8 in groups:
+            feats[ids.to(net.device)] = net.features_u8(u8)
+        torch.cuda.synchronize(net.device)
+        t2 = time.perf_counter()
+        wait, gpu, t0 = wait + t1 - t0, gpu + t2 - t1, t2
+    return feats, wait, gpu
+
+
+def main(argv=None):
+    """--save-stats DIR OUT.npz: the reference statistics (mu, sigma, features, kid_kxx) of the images in DIR; prints
+    N and where the time went.  Raises ValueError before any model load on a bad argument."""
+    ap = argparse.ArgumentParser(prog="python -m asyrp_official_b200.fid",
+                                 description="FID / KID reference statistics of a folder of real images (pytorch-fid's "
+                                             "--save-stats, on this library's kernels)")
+    ap.add_argument("--save-stats", nargs=2, metavar=("DIR", "OUT"), required=True,
+                    help="images directly in DIR (pytorch-fid's extensions, each at its own size) -> OUT (.npz)")
+    ap.add_argument("--fid_weights", required=True, help="pytorch-fid's pt_inception-2015-12-05-6726825d.pth")
+    ap.add_argument("--batch_size", type=int, default=50)
+    ap.add_argument("--num_workers", type=int, default=8)
+    a = ap.parse_args(argv)
+    folder, out = a.save_stats
+    if int(os.environ.get("WORLD_SIZE", "1")) > 1:
+        raise ValueError("--save-stats runs single-process: do not launch it under torchrun (WORLD_SIZE > 1)")
+    if a.batch_size < 1 or a.num_workers < 0:
+        raise ValueError(f"--batch_size must be >= 1 and --num_workers >= 0, got {a.batch_size}, {a.num_workers}")
+    if not os.path.isdir(folder):
+        raise ValueError(f"--save-stats: {folder!r} is not a directory")
+    files = image_files(folder)
+    if len(files) < 2:
+        raise ValueError(f"--save-stats: {folder!r} holds {len(files)} image file(s) with the extensions "
+                         f"{IMAGE_EXTENSIONS}; the statistics need at least 2")
+    if not os.path.isfile(a.fid_weights):
+        raise ValueError(f"--fid_weights {a.fid_weights!r} is not a file")
+    net = FIDInception(a.fid_weights)
+    feats, wait, gpu = folder_features(net, files, a.batch_size, a.num_workers)
+    t0 = time.perf_counter()
+    save_stats(out, feats)
+    stats = time.perf_counter() - t0
+    print(f"--save-stats: {len(files)} images of {folder} -> {out}; waiting on decoding {wait:.2f} s, features on the "
+          f"GPU {gpu:.2f} s, statistics and file {stats:.2f} s")
+    return 0
+
+
+if __name__ == "__main__":
+    sys.exit(main())

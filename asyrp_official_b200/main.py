@@ -129,6 +129,14 @@ def build_parser():
                         'the same x_T, written to <test_image_folder>/<mode>_ngen<n_train_step>_fid.tsv')
     p.add_argument('--fid_weights', type=str, default='pretrained/pt_inception-2015-12-05-6726825d.pth',
                    help="pytorch-fid's FID Inception-v3 weights for --fid")
+    p.add_argument('--fid_ref', type=str, default=None,
+                   help='--fid: also score the origin set and each set of edits against the reference statistics of '
+                        'real images in this .npz (python -m asyrp_official_b200.fid --save-stats DIR OUT.npz), '
+                        'written to <test_image_folder>/<mode>_ngen<n_train_step>_fid_real.tsv')
+    p.add_argument('--kid_subsets', type=int, default=100,
+                   help='--fid_ref: random subsets of the subset KID (KID_mean / KID_std); 0 = none')
+    p.add_argument('--kid_subset_size', type=int, default=1000,
+                   help='--fid_ref: rows per subset of the subset KID (a set smaller than this gets nan)')
     p.add_argument('--lpips_table_dir', type=str,
                    help='directory with <config stem>_LPIPS_distance_{x,x0_t}.tsv (read by --run_test, written by '
                         '--lpips; default utils)')

@@ -719,6 +719,18 @@ def fid_pack(x, out):
     check(lib.asyrp_fid_pack(_ptr(x), _ptr(out), B, H, W, S, _stream()), "asyrp_fid_pack")
 
 
+def fid_pack_u8(x, out):
+    """x u8 [B][H][W][3] (decoded image files) -> out fp32 NHWC [B][S][S][4]: u8 / 255, bilinear resize to S x S
+    (align_corners=False), 2 v - 1; channel 3 zero.  The same bits as fid_pack(x / 127.5 - 1)"""
+    lib = _lib.load()
+    B, H, W, C = x.shape
+    S = out.shape[1]
+    _need_cuda(x, out)
+    assert C == 3 and x.dtype == torch.uint8 and x.is_contiguous() and tuple(out.shape) == (B, S, S, 4)
+    assert out.dtype == torch.float32 and out.is_contiguous()
+    check(lib.asyrp_fid_pack_u8(_ptr(x), _ptr(out), B, H, W, S, _stream()), "asyrp_fid_pack_u8")
+
+
 def fid_conv(inp, weight, bias, out, kh, kw, stride=1, pad=(0, 0), cstore=None):
     """out[..., :cstore] = max(conv(inp) + bias, 0), fp32 NHWC, TF32 tensor cores, zero padding pad = (rows, columns);
     weight [Cout][Kpad] from pack_lpips_conv_weight and bias [Cout] with Cout a multiple of 64 (zero rows past cstore);
@@ -787,6 +799,34 @@ def fid_kernel_sum(x, y, exclude_diag=False):
     out = torch.empty((), dtype=torch.float64, device=x.device)
     check(lib.asyrp_fid_kernel_sum(_ptr(x), _ptr(y), _ptr(part), _ptr(out), n, m, d, int(bool(exclude_diag)),
                                    _stream()), "asyrp_fid_kernel_sum")
+    return out
+
+
+def fid_kernel_sum_subsets(x, y, idx_x, idx_y, exclude_diag=False):
+    """out[z] = fid_kernel_sum(x[idx_x[z]], y[idx_y[z]], exclude_diag) for every subset z, the same bits, all subsets in
+    one launch: x [n][d], y [m][d] fp32, idx_x / idx_y int32 [subsets][s] on the device.  The indices are checked here
+    (the kernel reads them unchecked).  fp64 [subsets] on the device"""
+    lib = _lib.load()
+    (n, d), m = x.shape, y.shape[0]
+    _need_cuda(x, y, idx_x, idx_y)
+    assert x.dtype == torch.float32 and y.dtype == torch.float32 and x.is_contiguous() and y.is_contiguous()
+    assert y.shape[1] == d
+    if idx_x.dtype != torch.int32 or idx_y.dtype != torch.int32 or idx_x.dim() != 2 or idx_x.shape != idx_y.shape:
+        raise _lib.AsyrpError(f"fid_kernel_sum_subsets: idx_x / idx_y must be int32 [subsets][s] of one shape, got "
+                              f"{idx_x.dtype} {tuple(idx_x.shape)} / {idx_y.dtype} {tuple(idx_y.shape)}")
+    idx_x, idx_y = idx_x.contiguous(), idx_y.contiguous()
+    subsets, s = idx_x.shape
+    for name, idx, rows in (("idx_x", idx_x, n), ("idx_y", idx_y, m)):
+        if idx.numel():
+            lo, hi = (int(v) for v in torch.aminmax(idx))
+            if lo < 0 or hi >= rows:
+                raise _lib.AsyrpError(f"fid_kernel_sum_subsets: {name} holds rows in [{lo}, {hi}], outside [0, {rows})")
+    count = lib.asyrp_fid_kernel_sum_subsets_partials(s, subsets)
+    part = torch.empty(max(1, count), dtype=torch.float64, device=x.device)
+    out = torch.empty(max(0, subsets), dtype=torch.float64, device=x.device)
+    check(lib.asyrp_fid_kernel_sum_subsets(_ptr(x), _ptr(y), _ptr(idx_x), _ptr(idx_y), _ptr(part), _ptr(out), n, m,
+                                           s, subsets, d, int(bool(exclude_diag)), _stream()),
+          "asyrp_fid_kernel_sum_subsets")
     return out
 
 

@@ -393,8 +393,18 @@ int asyrp_faceparse_agreement(const float* src_logits, const float* edited_logit
  * asyrp_fid_kernel_sum: out[0] = sum over i < n, j < m of (x[i] . y[j] / d + 1)^3 in fp64, pairs i == j skipped with
  *   exclude_diag; x fp32 [n][d], y fp32 [m][d], d % 16 == 0; partial: asyrp_fid_kernel_sum_partials(n, m) doubles of
  *   workspace.
+ * asyrp_fid_pack_u8: x u8 NHWC [B][H][W][3] (a decoded image file) -> out as asyrp_fid_pack: q = x, q / 255,
+ *   bilinear resize to S x S, 2 v - 1 (pytorch-fid's ToTensor path); bit-identical to asyrp_fid_pack of
+ *   x / 127.5 - 1 as fp32 NCHW (whose quantiser gives back q).
+ * asyrp_fid_kernel_sum_subsets: out[z] (z < subsets, fp64) = sum over i, j < s of
+ *   (x[idx_x[z][i]] . y[idx_y[z][j]] / d + 1)^3, pairs i == j skipped with exclude_diag: bit-identical to
+ *   asyrp_fid_kernel_sum of the gathered rows x[idx_x[z]], y[idx_y[z]].  x fp32 [n][d], y fp32 [m][d], idx_x / idx_y
+ *   int32 [subsets][s] on the device; d % 16 == 0, subsets <= 65535, s >= 2 with exclude_diag.  The indices are not
+ *   checked on the device: a row outside [0, n) / [0, m) is read out of bounds (ops.fid_kernel_sum_subsets checks
+ *   them).  partial: asyrp_fid_kernel_sum_subsets_partials(s, subsets) doubles of workspace (-1: too large).
  * Fixed-order reductions, no atomics, no kernel mixes samples. */
 int asyrp_fid_pack(const float* x, float* out, int B, int H, int W, int S, void* stream);
+int asyrp_fid_pack_u8(const unsigned char* x, float* out, int B, int H, int W, int S, void* stream);
 int asyrp_fid_conv(const float* in, const float* weight, const float* bias, float* out, int N, int H, int W, int Cin,
                    int Cout, int kh, int kw, int stride, int padh, int padw, int ldo, int cstore, void* stream);
 int asyrp_fid_pool(const float* in, float* out, int N, int H, int W, int C, int mode, int ldo, void* stream);
@@ -403,6 +413,9 @@ int asyrp_fid_moments(const float* x, double* mu, double* sigma, int n, int d, v
 int asyrp_fid_kernel_sum_partials(int n, int m); /* host only */
 int asyrp_fid_kernel_sum(const float* x, const float* y, double* partial, double* out, int n, int m, int d,
                          int exclude_diag, void* stream);
+int asyrp_fid_kernel_sum_subsets_partials(int s, int subsets); /* host only */
+int asyrp_fid_kernel_sum_subsets(const float* x, const float* y, const int* idx_x, const int* idx_y, double* partial,
+                                 double* out, int n, int m, int s, int subsets, int d, int exclude_diag, void* stream);
 
 #ifdef __cplusplus
 }

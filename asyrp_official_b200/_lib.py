@@ -137,6 +137,10 @@ SIGNATURES = {
     "asyrp_fid_kernel_sum_subsets_partials": (c_int, [c_int, c_int]),
     "asyrp_fid_kernel_sum_subsets": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int,
                                              c_int, c_int, c_int, c_int, c_void_p]),
+    "asyrp_fid_knn_radii_workspace": (C.c_longlong, [c_int, c_int]),
+    "asyrp_fid_knn_radii": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p]),
+    "asyrp_fid_knn_counts": (c_int, [c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p,
+                                     c_void_p, c_void_p]),
 }
 
 _lib = None

@@ -24,7 +24,9 @@ Mirrors, with the same attribute / flag names:
                                                             pool features (fid.FIDInception), gathered to rank 0 at the
                                                             end of the run; this build's definition; with --fid_ref also
                                                             the origin and each edited set against real images'
-                                                            statistics (fid.score_against_stats)
+                                                            statistics (fid.score_against_stats); with --prdc also
+                                                            precision / recall / density / coverage of the same sets
+                                                            from k-nearest-neighbour balls (fid.prdc)
   Asyrp.precompute_pairs_with_h :877-947                    DDIM inversion of one image keeping the bottleneck h of
                                                             every step (batched here, same cache file)
   Asyrp.run_diff_style         main.py:192-202              --diff_style (DiffStyle content injection): this build's
@@ -40,6 +42,7 @@ the collectives are the initial weight broadcast and, with --fid, the end-of-run
 0; each rank computes the CLIP cosine itself (the kernels are deterministic, so every rank picks the same t_edit).
 """
 import ast
+import math
 import os
 import time
 
@@ -84,6 +87,10 @@ class Asyrp(object):
         # --fid_ref (rank 0): 'train' / 'test' -> fp64 [1 + tuples][4], (FID, KID, KID_mean, KID_std) against the real
         # images' statistics of the origin set (row 0) and of each tuple's set
         self.fid_real = {}
+        # --prdc (rank 0): 'train' / 'test' -> fp64 [tuples][4], (precision, recall, density, coverage) of each tuple's
+        # set against the origin set; with --fid_ref, prdc_real: fp64 [1 + tuples][4] against the real images' features
+        self.prdc = {}
+        self.prdc_real = {}
 
     # ------------------------------------------------------------------------------------------
     def load_pretrained_model(self):
@@ -273,13 +280,25 @@ class Asyrp(object):
         except ValueError as e:
             raise ValueError(f"--fid: {e}") from None
 
+    def prdc_check(self):
+        """--prdc's requirements, checked before any model is loaded; raises ValueError with the reason"""
+        a = self.args
+        if not getattr(a, "prdc", False):
+            return
+        if not getattr(a, "fid", False):
+            raise ValueError("--prdc scores the pool features that --fid collects: add --fid")
+        if not 1 <= a.prdc_k <= 32:
+            raise ValueError(f"--prdc: --prdc_k must be in 1..32, got {a.prdc_k}")
+
     def finish_fid(self, sets, coeffs, attrs=None):
         """--fid at the end of a run: every rank's pool features (fid.FeatureSets) to rank 0, which sorts each set by
         image index and scores every tuple's edited set against the origin set of the same pass: printed, kept in
         self.fid[mode] and written to <test_image_folder>/<mode>_ngen<n_train_step>_fid.tsv.  Every rank must call it,
-        also one that ran no batch."""
-        from .fid import fid_kid, load_stats, score_against_stats, set_moments
+        also one that ran no batch.  With --prdc also precision / recall / density / coverage from the same features
+        (_prdc.tsv, and _prdc_real.tsv against --fid_ref's features, whose radii are computed once)."""
+        from .fid import fid_kid, knn_radii, load_stats, prdc, score_against_stats, set_moments
         a = self.args
+        pk = a.prdc_k if getattr(a, "prdc", False) else None
         dist_on = self.world > 1 and torch.distributed.is_available() and torch.distributed.is_initialized()
         got = sets.gather(self.rank, self.world if dist_on else 1)
         if got is None:
@@ -289,6 +308,9 @@ class Asyrp(object):
             real = load_stats(a.fid_ref)
             if "features" in real:
                 real["features"] = torch.from_numpy(real["features"]).to(self.device)
+        real_radii = None  # --prdc --fid_ref: the real images' k-NN radii, for every set of both passes
+        if pk is not None and real is not None and real.get("features") is not None and real["features"].shape[0] > pk:
+            real_radii = knn_radii(real["features"], pk)
         for mode in ("train", "test"):
             if (mode, "origin") not in got:
                 continue
@@ -313,6 +335,22 @@ class Asyrp(object):
                 n_ref = real["features"].shape[0] if "features" in real else None
                 write_fid_real(os.path.join(a.test_image_folder, f"{mode}_ngen{a.n_train_step}_fid_real.tsv"),
                                coeffs, real_rows, ref.shape[0], n_ref, mode, attrs=attrs)
+            if pk is None:
+                continue
+            origin_radii = knn_radii(ref, pk) if ref.shape[0] > pk else None
+            prdc_rows = [prdc(ref, e, pk, origin_radii) for e in edited]
+            self.prdc[mode] = torch.tensor(prdc_rows, dtype=torch.float64)
+            write_prdc(os.path.join(a.test_image_folder, f"{mode}_ngen{a.n_train_step}_prdc.tsv"), coeffs, prdc_rows,
+                       ref.shape[0], None, mode, attrs=attrs)
+            if real is not None:
+                if "features" in real:
+                    prdc_rows = [prdc(real["features"], f, pk, real_radii) for f in [ref] + edited]
+                    n_ref = real["features"].shape[0]
+                else:
+                    prdc_rows, n_ref = [(math.nan,) * 4] * (1 + len(edited)), None
+                self.prdc_real[mode] = torch.tensor(prdc_rows, dtype=torch.float64)
+                write_prdc(os.path.join(a.test_image_folder, f"{mode}_ngen{a.n_train_step}_prdc_real.tsv"), coeffs,
+                           prdc_rows, ref.shape[0], n_ref, mode, attrs=attrs, real=True)
 
     def write_id_similarity(self, path, coeffs, ids):
         """the TSV of one batch: one row per (hs_coeff tuple, image) in grid order, ID = 1 - IDLoss(origin, edit) of
@@ -714,6 +752,7 @@ class Asyrp(object):
         a = self.args
         if getattr(a, "fid_ref", None) is not None and not getattr(a, "fid", False):
             raise ValueError("--fid_ref scores the sets that --fid collects: add --fid")
+        self.prdc_check()
         if getattr(a, "attr_sweep", ""):
             return self.run_attr_sweep()
         print("Running Test")
@@ -1210,6 +1249,7 @@ class Asyrp(object):
         result per γ.  Returns {(content path, style path): results [len(γ)][3][S][S]}."""
         import torchvision.utils as tvu
         a = self.args
+        self.prdc_check()
         if getattr(a, "fid", False):
             self.fid_setup()  # refuses --diff_style, before any model loads
         contents, styles, gammas = self.diff_style_setup()
@@ -1383,6 +1423,29 @@ def write_fid_real(path, coeffs, rows, n, n_ref, mode, attrs=None):
                                         else f"hs_coeff {tuple(float(c) for c in coeffs[k - 1])}")
         print(f"FID / KID against the real images ({mode}, {n} images, {nr} reference), {name}: FID {fd:.6f}, "
               f"KID {kd:.6f}, subset KID {km:.6f} +- {ks:.6f}")
+
+
+def write_prdc(path, coeffs, rows, n, n_ref, mode, attrs=None, real=False):
+    """the precision / recall / density / coverage table of one pass (--prdc): one row per hs_coeff tuple, columns
+    tuple, hs_coeff, n (images per set), precision, recall, density, coverage (`attr` appended under an attribute
+    sweep), values as write_fid writes them.  real (--fid_ref): rows[0] is the origin set (tuple `origin`, hs_coeff
+    `-`) and an n_ref column (reference images; `-` for a file without features) follows n.  Prints each row"""
+    names = [(str(k), ",".join(f"{float(c):.6g}" for c in coeffs[k]), attrs[k] if attrs is not None else None)
+             for k in range(len(coeffs))]
+    if real:
+        names = [("origin", "-", "-")] + names
+    nr = "-" if n_ref is None else str(n_ref)
+    with open(path, "w") as f:
+        f.write("tuple\ths_coeff\tn" + ("\tn_ref" if real else "") + "\tprecision\trecall\tdensity\tcoverage" +
+                ("\tattr" if attrs is not None else "") + "\n")
+        for (key, tup, attr), vals in zip(names, rows):
+            f.write(f"{key}\t{tup}\t{n}" + (f"\t{nr}" if real else "") + "\t" +
+                    "\t".join(repr(float(v)) for v in vals) + (f"\t{attr}" if attrs is not None else "") + "\n")
+    against = f"against the real images ({mode}, {n} images, {nr} reference)" if real else f"({mode}, {n} images)"
+    for (key, tup, attr), (p, r, d, c) in zip(names, rows):
+        name = "origin" if key == "origin" else (f"attribute {attr}" if attrs is not None else f"hs_coeff ({tup})")
+        print(f"precision / recall / density / coverage {against}, {name}: P {p:.6f}, R {r:.6f}, D {d:.6f}, "
+              f"C {c:.6f}")
 
 
 def plan_sweep(n_tuples, bs, max_rows):

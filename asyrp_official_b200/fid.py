@@ -45,7 +45,14 @@ without the diagonal).  A run then scores its origin set and each edited set aga
     KID_mean  torch-fidelity's KID mean / std over random subsets (kid_subsets: kid_subsets subsets of
     KID_std   kid_subset_size rows, RandomState(2020), the edited set drawn first); nan when a set is smaller
 
-The KID columns are nan for a file without features.  Precision / recall and the Inception score are not computed.
+The KID columns are nan for a file without features.
+
+Precision / recall / density / coverage (--prdc, prdc): improved precision / recall (Kynkaanniemi et al. 2019) and
+density / coverage (Naeem et al. 2020, the prdc package) from k-nearest-neighbour balls of the same pool features, on
+squared distances in fp64 (csrc/prdc.cu); real = the origin set, or the file's features with --fid_ref.  With k = 3,
+precision and recall are those of guided-diffusion's ADM evaluator except that it counts ties (<=) and computes its
+distances in fp16 (fp32 fallback); here every comparison is strict and every distance fp64.  The Inception score is
+not computed.
 
 No real pt_inception-2015-12-05-6726825d.pth has been loaded by this project's tests: the key list below follows
 torchvision's Inception3, and the loader refuses any other layout by name.
@@ -55,6 +62,7 @@ import math
 import os
 import sys
 import time
+import warnings
 
 import numpy as np
 import torch
@@ -294,6 +302,35 @@ def score_against_stats(f, real, subsets, size, moments=None):
     kd = kid_from_sums(kxx, real["kid_kxx"], kxy, n, ref.shape[0])
     km, ks = kid_subsets(f, ref, subsets, size) if subsets > 0 else (math.nan, math.nan)
     return fd, kd, km, ks
+
+
+# ---- precision / recall / density / coverage (--prdc) from k-nearest-neighbour balls ----
+def knn_radii(f, k):
+    """fp64 [n] on the device: the squared distance of each row of the feature set f (fp32 [n][d] on the device) to its
+    k-th nearest other row, duplicates counted: the (k + 1)-th smallest D(f_i, f_j) over every j, j = i included
+    (prdc's compute_nearest_neighbour_distances, squared).  1 <= k <= 32 and n > k."""
+    return ops.fid_knn_radii(f.contiguous(), int(k))
+
+
+def prdc(real, fake, k, real_radii=None):
+    """(precision, recall, density, coverage) as floats (fp64) of the fake set against the real set (fp32 [n][d] /
+    [m][d] on the device), prdc.compute_prdc's definitions on squared distances with strict <:
+        precision = #{j : some i has D(r_i, f_j) < r_k(i)} / m
+        recall    = #{i : some j has D(r_i, f_j) < r_k^fake(j)} / n
+        density   = #{(i, j) : D(r_i, f_j) < r_k(i)} / (k m)
+        coverage  = #{i : some j has D(r_i, f_j) < r_k(i)} / n
+    r_k the knn_radii of the real set (real_radii, when several fake sets share it) and r_k^fake those of the fake set.
+    All four are nan, with a warning, when either set has k rows or fewer."""
+    n, m = real.shape[0], fake.shape[0]
+    if n <= k or m <= k:
+        warnings.warn(f"precision / recall / density / coverage: a set of {min(n, m)} rows has no {k}-th nearest "
+                      "neighbour: nan", RuntimeWarning, stacklevel=2)
+        return math.nan, math.nan, math.nan, math.nan
+    real, fake = real.contiguous(), fake.contiguous()
+    rr = real_radii if real_radii is not None else knn_radii(real, k)
+    b_in_a, a_in_b, a_covered = ops.fid_knn_counts(real, rr, fake, knn_radii(fake, k))
+    counts = torch.stack([(b_in_a > 0).sum(), (a_in_b > 0).sum(), b_in_a.sum(), (a_covered > 0).sum()]).tolist()
+    return counts[0] / m, counts[1] / n, counts[2] / (k * m), counts[3] / n
 
 
 # ---- reference statistics (.npz): pytorch-fid's keys mu / sigma, plus this project's features / kid_kxx for KID ----

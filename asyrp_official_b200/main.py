@@ -137,6 +137,12 @@ def build_parser():
                    help='--fid_ref: random subsets of the subset KID (KID_mean / KID_std); 0 = none')
     p.add_argument('--kid_subset_size', type=int, default=1000,
                    help='--fid_ref: rows per subset of the subset KID (a set smaller than this gets nan)')
+    p.add_argument('--prdc', **sa,
+                   help='--fid: also score each set of edits with improved precision / recall and density / coverage '
+                        'from k-nearest-neighbour balls of the pool features, against the origin set '
+                        '(<mode>_ngen<n_train_step>_prdc.tsv) and with --fid_ref against its features (_prdc_real.tsv)')
+    p.add_argument('--prdc_k', type=int, default=5,
+                   help='--prdc: the k of the k-nearest-neighbour balls, 1..32 (a set of k images or fewer gets nan)')
     p.add_argument('--lpips_table_dir', type=str,
                    help='directory with <config stem>_LPIPS_distance_{x,x0_t}.tsv (read by --run_test, written by '
                         '--lpips; default utils)')

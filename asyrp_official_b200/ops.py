@@ -830,6 +830,41 @@ def fid_kernel_sum_subsets(x, y, idx_x, idx_y, exclude_diag=False):
     return out
 
 
+def fid_knn_radii(x, k):
+    """fp64 [n] on the device: the (k + 1)-th smallest D(x_i, x_j) = sum_c (x_ic - x_jc)^2 (fp64) over every row j of
+    x fp32 [n][d], j = i included, i.e. the squared distance to the k-th nearest other row (1 <= k <= 32, n > k)"""
+    lib = _lib.load()
+    n, d = x.shape
+    _need_cuda(x)
+    assert x.dtype == torch.float32 and x.is_contiguous()
+    size = lib.asyrp_fid_knn_radii_workspace(n, int(k))
+    work = torch.empty(max(1, size), dtype=torch.float64, device=x.device)
+    radii = torch.empty(n, dtype=torch.float64, device=x.device)
+    check(lib.asyrp_fid_knn_radii(_ptr(x), _ptr(radii), _ptr(work), n, d, int(k), _stream()), "asyrp_fid_knn_radii")
+    return radii
+
+
+def fid_knn_counts(a, ra, b, rb, out=None):
+    """(b_in_a [m], a_in_b [n], a_covered [n]) int32 on the device for a fp32 [n][d], b fp32 [m][d] and their radii
+    ra fp64 [n], rb fp64 [m]: b_in_a[j] = #{i : D(a_i, b_j) < ra[i]}, a_in_b[i] = #{j : D < rb[j]},
+    a_covered[i] = #{j : D < ra[i]}, D the squared distance in fp64.  out: three int32 tensors to overwrite"""
+    lib = _lib.load()
+    (n, d), m = a.shape, b.shape[0]
+    _need_cuda(a, ra, b, rb)
+    assert a.dtype == torch.float32 and b.dtype == torch.float32 and a.is_contiguous() and b.is_contiguous()
+    assert b.shape[1] == d
+    assert ra.dtype == torch.float64 and rb.dtype == torch.float64 and ra.is_contiguous() and rb.is_contiguous()
+    assert ra.numel() == n and rb.numel() == m
+    if out is None:
+        out = tuple(torch.empty(s, dtype=torch.int32, device=a.device) for s in (m, n, n))
+    b_in_a, a_in_b, a_covered = out
+    for t, s in zip(out, (m, n, n)):
+        assert t.dtype == torch.int32 and t.is_contiguous() and t.numel() == s and t.is_cuda
+    check(lib.asyrp_fid_knn_counts(_ptr(a), _ptr(ra), n, _ptr(b), _ptr(rb), m, d, _ptr(b_in_a), _ptr(a_in_b),
+                                   _ptr(a_covered), _stream()), "asyrp_fid_knn_counts")
+    return b_in_a, a_in_b, a_covered
+
+
 def ddpm_update(x, et, z, x_next, at, bt, logvar, learned_sigma, mask):
     lib = _lib.load()
     N, Cx, H, W = x.shape

@@ -417,6 +417,22 @@ int asyrp_fid_kernel_sum_subsets_partials(int s, int subsets); /* host only */
 int asyrp_fid_kernel_sum_subsets(const float* x, const float* y, const int* idx_x, const int* idx_y, double* partial,
                                  double* out, int n, int m, int s, int subsets, int d, int exclude_diag, void* stream);
 
+/* k-nearest-neighbour balls for precision / recall / density / coverage (csrc/prdc.cu).
+ * D(u, v) = sum_c (u_c - v_c)^2, each difference and the sum in fp64, summed in feature order: identical rows give 0,
+ * and a pair's D is the same bits in every launch.  The distance matrix is never written to memory.
+ * asyrp_fid_knn_radii: radii[i] (fp64) = the (k + 1)-th smallest D(x[i], x[j]) over every j < n, j = i included (the
+ *   squared distance to the k-th nearest other row, duplicates counted), x fp32 [n][d] row-major; 1 <= k <= 32,
+ *   n >= k + 1, d >= 1.  work: asyrp_fid_knn_radii_workspace(n, k) doubles (-1: bad n or k), the per-row lists of the
+ *   CTAs a row's columns are split over; the split depends on the device, the radii do not.
+ * asyrp_fid_knn_counts: one pass over the n x m pairs of a fp32 [n][d] and b fp32 [m][d] with radii ra [n], rb [m]
+ *   (fp64): b_in_a[j] = #{i : D(a_i, b_j) < ra[i]}, a_in_b[i] = #{j : D < rb[j]}, a_covered[i] = #{j : D < ra[i]}.
+ *   The three outputs are distinct buffers and are overwritten; integer atomics keep them exact.  n, m, d >= 1,
+ *   n <= 65535 * 64. */
+long long asyrp_fid_knn_radii_workspace(int n, int k); /* host only */
+int asyrp_fid_knn_radii(const float* x, double* radii, double* work, int n, int d, int k, void* stream);
+int asyrp_fid_knn_counts(const float* a, const double* ra, int n, const float* b, const double* rb, int m, int d,
+                         unsigned* b_in_a, unsigned* a_in_b, unsigned* a_covered, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

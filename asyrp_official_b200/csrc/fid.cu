@@ -15,6 +15,7 @@
 // Every reduction runs in a fixed order and no kernel uses atomics or mixes samples, so an image's features are the
 // same bits whatever batch it is in, and the statistics of a set are the same bits whatever launches produced its rows.
 #include <cfloat>
+#include <climits>
 
 #include "common.h"
 #include "ptx.cuh"
@@ -278,6 +279,9 @@ inline int fid_grid(size_t total, int block) {
 
 inline bool aligned(const void* p, size_t bytes) { return reinterpret_cast<uintptr_t>(p) % bytes == 0; }
 
+// the 64-row gram tiles of `rows` rows, in 64 bits: rows + 63 overflows int near 2^31
+inline long long gram_tiles(int rows) { return (static_cast<long long>(rows) + kGramTile - 1) / kGramTile; }
+
 }  // namespace
 }  // namespace asyrp
 
@@ -287,6 +291,7 @@ extern "C" {
 
 ASYRP_API int asyrp_fid_pack(const float* x, float* out, int B, int H, int W, int S, void* stream) {
   ASYRP_REQUIRE(B > 0 && H > 0 && W > 0 && S > 0, "asyrp_fid_pack: bad shape B=%d H=%d W=%d S=%d", B, H, W, S);
+  ASYRP_REQUIRE(aligned(out, 16), "asyrp_fid_pack: out must be 16-byte aligned (float4 stores)");
   const size_t total = static_cast<size_t>(B) * S * S;
   ASYRP_LAUNCH(fid_pack_kernel<SavedPng>, dim3(fid_grid(total, 256)), dim3(256), 0, static_cast<cudaStream_t>(stream),
                SavedPng{x, H, W}, out, B, H, W, S);
@@ -296,6 +301,7 @@ ASYRP_API int asyrp_fid_pack(const float* x, float* out, int B, int H, int W, in
 
 ASYRP_API int asyrp_fid_pack_u8(const uint8_t* x, float* out, int B, int H, int W, int S, void* stream) {
   ASYRP_REQUIRE(B > 0 && H > 0 && W > 0 && S > 0, "asyrp_fid_pack_u8: bad shape B=%d H=%d W=%d S=%d", B, H, W, S);
+  ASYRP_REQUIRE(aligned(out, 16), "asyrp_fid_pack_u8: out must be 16-byte aligned (float4 stores)");
   const size_t total = static_cast<size_t>(B) * S * S;
   ASYRP_LAUNCH(fid_pack_kernel<DecodedU8>, dim3(fid_grid(total, 256)), dim3(256), 0,
                static_cast<cudaStream_t>(stream), DecodedU8{x, H, W}, out, B, H, W, S);
@@ -309,26 +315,36 @@ ASYRP_API int asyrp_fid_conv(const float* in, const float* weight, const float* 
   using namespace tf32gemm;
   ASYRP_REQUIRE(Cin > 0 && Cin % 4 == 0, "asyrp_fid_conv: Cin=%d must be a positive multiple of 4", Cin);
   ASYRP_REQUIRE(Cout > 0 && Cout % kBN == 0, "asyrp_fid_conv: Cout=%d must be a positive multiple of %d", Cout, kBN);
-  ASYRP_REQUIRE(N > 0 && H > 0 && W > 0 && kh > 0 && kw > 0 && stride > 0 && padh >= 0 && padw >= 0 &&
-                    H + 2 * padh >= kh && W + 2 * padw >= kw,
+  // the geometry in 64 bits: the kernel's tap coordinates (oy * stride - padh + ky < H + 2 padh, likewise x), K and the
+  // output pixel index are int, so the padded extents, Kpad and N Ho Wo must each fit in one
+  const long long Hp = H + 2LL * padh, Wp = W + 2LL * padw;
+  ASYRP_REQUIRE(N > 0 && H > 0 && W > 0 && kh > 0 && kw > 0 && stride > 0 && padh >= 0 && padw >= 0 && Hp >= kh &&
+                    Wp >= kw,
                 "asyrp_fid_conv: bad geometry N=%d H=%d W=%d kh=%d kw=%d stride=%d padh=%d padw=%d", N, H, W, kh, kw,
                 stride, padh, padw);
+  ASYRP_REQUIRE(Hp <= INT_MAX && Wp <= INT_MAX,
+                "asyrp_fid_conv: padded extent H + 2 padh=%lld or W + 2 padw=%lld above 2^31 - 1", Hp, Wp);
+  constexpr long long kMaxK = INT_MAX / kBK * kBK;  // the largest Kpad in int
+  ASYRP_REQUIRE(static_cast<long long>(kh) * kw <= kMaxK / Cin,
+                "asyrp_fid_conv: K = kh * kw * Cin = %d * %d * %d above %lld", kh, kw, Cin, kMaxK);
   ASYRP_REQUIRE(cstore > 0 && cstore % 2 == 0 && cstore <= Cout && ldo >= cstore && ldo % 2 == 0,
                 "asyrp_fid_conv: cstore=%d must be even and in (0, Cout=%d], ldo=%d even and >= cstore", cstore, Cout,
                 ldo);
   ASYRP_REQUIRE(bias != nullptr && aligned(out, 8), "asyrp_fid_conv: needs a bias and an 8-byte aligned out");
   ASYRP_REQUIRE(in != out, "asyrp_fid_conv: out must not alias in");
+  const long long Ho = (Hp - kh) / stride + 1, Wo = (Wp - kw) / stride + 1;
+  const long long NHo = N * Ho;  // below 2^62; with NHo < 2^31 the product with Wo is too
+  ASYRP_REQUIRE(NHo < (1LL << 31) / kBM * kBM && NHo * Wo < (1LL << 31) / kBM * kBM,
+                "asyrp_fid_conv: too many output pixels");
   Tf32ConvParams p;
   p.in = in; p.w = weight; p.bias = bias; p.residual = nullptr; p.prelu = nullptr; p.out = out;
   p.N = N; p.H = H; p.W = W; p.Cin = Cin; p.Cout = Cout; p.kw = kw; p.stride = stride; p.pad = padh;
   p.padw = padw; p.ldo = ldo; p.cstore = cstore;
-  p.Ho = (H + 2 * padh - kh) / stride + 1;
-  p.Wo = (W + 2 * padw - kw) / stride + 1;
+  p.Ho = static_cast<int>(Ho);
+  p.Wo = static_cast<int>(Wo);
   p.K = kh * kw * Cin;
   p.Kpad = (p.K + kBK - 1) / kBK * kBK;
-  const long long M = static_cast<long long>(N) * p.Ho * p.Wo;
-  ASYRP_REQUIRE(M < (1LL << 31) / kBM * kBM, "asyrp_fid_conv: too many output pixels");
-  p.M = static_cast<int>(M);
+  p.M = static_cast<int>(NHo * Wo);
   return launch_tf32_conv<kEpiReluSlice>(p, static_cast<cudaStream_t>(stream));
 }
 
@@ -368,6 +384,8 @@ ASYRP_API int asyrp_fid_moments(const float* x, double* mu, double* sigma, int n
   ASYRP_REQUIRE(n >= 2 && d > 0 && d % kGramTile == 0 && d / kGramTile <= kMaxGridYZ,
                 "asyrp_fid_moments: bad shape n=%d d=%d (n >= 2, d a multiple of %d)", n, d, kGramTile);
   ASYRP_REQUIRE(static_cast<long long>(n) * d < (1LL << 40), "asyrp_fid_moments: n * d too large");
+  // the gram kernel steps through the n rows 16 at a time in int
+  ASYRP_REQUIRE(n <= INT_MAX - kGramK + 1, "asyrp_fid_moments: n=%d above %d rows", n, INT_MAX - kGramK + 1);
   const cudaStream_t st = static_cast<cudaStream_t>(stream);
   ASYRP_LAUNCH(fid_colmean_kernel, dim3((d + 255) / 256), dim3(256), 0, st, x, mu, n, d);
   ASYRP_LAUNCH(fid_gram_kernel<false, false>, dim3(d / kGramTile, d / kGramTile), dim3(kGramThreads), 0, st, x, x,
@@ -378,29 +396,34 @@ ASYRP_API int asyrp_fid_moments(const float* x, double* mu, double* sigma, int n
 }
 
 ASYRP_API int asyrp_fid_kernel_sum_partials(int n, int m) {
-  return ((n + kGramTile - 1) / kGramTile) * ((m + kGramTile - 1) / kGramTile);
+  // fid_sum_kernel's threads step through the count by kSumThreads in int: count + kSumThreads - 1 must fit in one
+  const long long count = gram_tiles(n) * gram_tiles(m);
+  return n > 0 && m > 0 && count <= INT_MAX - kSumThreads + 1 ? static_cast<int>(count) : -1;
 }
 
 ASYRP_API int asyrp_fid_kernel_sum(const float* x, const float* y, double* partial, double* out, int n, int m, int d,
                                    int exclude_diag, void* stream) {
   ASYRP_REQUIRE(n > 0 && m > 0 && d > 0 && d % kGramK == 0,
                 "asyrp_fid_kernel_sum: bad shape n=%d m=%d d=%d (d a multiple of %d)", n, m, d, kGramK);
-  ASYRP_REQUIRE((n + kGramTile - 1) / kGramTile <= kMaxGridYZ, "asyrp_fid_kernel_sum: n=%d too large", n);
+  ASYRP_REQUIRE(n <= kMaxGridYZ * kGramTile, "asyrp_fid_kernel_sum: n=%d too large (above %d rows)", n,
+                kMaxGridYZ * kGramTile);
   ASYRP_REQUIRE(exclude_diag == 0 || exclude_diag == 1, "asyrp_fid_kernel_sum: exclude_diag=%d must be 0 or 1",
                 exclude_diag);
+  const int count = asyrp_fid_kernel_sum_partials(n, m);
+  ASYRP_REQUIRE(count > 0, "asyrp_fid_kernel_sum: n=%d x m=%d too large (above %d partials)", n, m,
+                INT_MAX - kSumThreads + 1);
   const cudaStream_t st = static_cast<cudaStream_t>(stream);
-  const dim3 grid((m + kGramTile - 1) / kGramTile, (n + kGramTile - 1) / kGramTile);
+  const dim3 grid(static_cast<unsigned>(gram_tiles(m)), static_cast<unsigned>(gram_tiles(n)));
   ASYRP_LAUNCH(fid_gram_kernel<true, false>, grid, dim3(kGramThreads), 0, st, x, y,
                static_cast<const double*>(nullptr), partial, n, m, d, exclude_diag, static_cast<const int*>(nullptr),
                static_cast<const int*>(nullptr));
-  ASYRP_LAUNCH(fid_sum_kernel, dim3(1), dim3(kSumThreads), 0, st, static_cast<const double*>(partial),
-               static_cast<int>(grid.x * grid.y), out);
+  ASYRP_LAUNCH(fid_sum_kernel, dim3(1), dim3(kSumThreads), 0, st, static_cast<const double*>(partial), count, out);
   ASYRP_CHECK_CUDA(cudaGetLastError());
   return ASYRP_OK;
 }
 
 ASYRP_API int asyrp_fid_kernel_sum_subsets_partials(int s, int subsets) {
-  const long long tiles = (s + kGramTile - 1) / kGramTile;
+  const long long tiles = gram_tiles(s);
   const long long count = tiles * tiles * subsets;
   return s > 0 && subsets > 0 && count < (1LL << 31) ? static_cast<int>(count) : -1;
 }

@@ -251,8 +251,7 @@ ASYRP_API int asyrp_fid_knn_radii(const float* x, double* radii, double* work, i
 ASYRP_API int asyrp_fid_knn_counts(const float* a, const double* ra, int n, const float* b, const double* rb, int m,
                                    int d, unsigned* b_in_a, unsigned* a_in_b, unsigned* a_covered, void* stream) {
   ASYRP_REQUIRE(n >= 1 && m >= 1 && d >= 1, "asyrp_fid_knn_counts: bad shape n=%d m=%d d=%d", n, m, d);
-  ASYRP_REQUIRE((n + kTile - 1) / kTile <= kMaxGridYZ, "asyrp_fid_knn_counts: n=%d above %d rows", n,
-                kMaxGridYZ * kTile);
+  ASYRP_REQUIRE(n <= kMaxGridYZ * kTile, "asyrp_fid_knn_counts: n=%d above %d rows", n, kMaxGridYZ * kTile);
   ASYRP_REQUIRE(a != nullptr && ra != nullptr && b != nullptr && rb != nullptr && b_in_a != nullptr &&
                     a_in_b != nullptr && a_covered != nullptr,
                 "asyrp_fid_knn_counts: null buffer");

@@ -213,13 +213,21 @@ __global__ void __launch_bounds__(kThreads) tf32_conv_kernel(const Tf32ConvParam
   }
 }
 
-// launch over the grid of p (p.M pixels, p.Cout channels)
+// launch over the grid of p (p.M pixels, p.Cout channels).  The channel tiles sit in grid y; in and w are read with
+// 16-byte cp.async, out and the residual with 8-byte float2 accesses.  The pixel tile count is formed in 64 bits: p.M
+// may be up to 2^31 - 1.
 template <int kEpi>
 inline int launch_tf32_conv(const Tf32ConvParams& p, cudaStream_t stream) {
+  ASYRP_REQUIRE(p.Cout / kBN <= kMaxGridYZ, "tf32 conv: Cout=%d above %d channel tiles of %d", p.Cout, kMaxGridYZ,
+                kBN);
+  ASYRP_REQUIRE(reinterpret_cast<uintptr_t>(p.in) % 16 == 0 && reinterpret_cast<uintptr_t>(p.w) % 16 == 0,
+                "tf32 conv: in and weight must be 16-byte aligned");
+  ASYRP_REQUIRE(reinterpret_cast<uintptr_t>(p.out) % 8 == 0 && reinterpret_cast<uintptr_t>(p.residual) % 8 == 0,
+                "tf32 conv: out and residual must be 8-byte aligned");
   ASYRP_CHECK_CUDA(cudaFuncSetAttribute(tf32_conv_kernel<kEpi>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                         static_cast<int>(kConvSmem)));
-  ASYRP_LAUNCH(tf32_conv_kernel<kEpi>, dim3((p.M + kBM - 1) / kBM, p.Cout / kBN), dim3(kThreads), kConvSmem, stream,
-               p);
+  const unsigned pixel_tiles = static_cast<unsigned>((static_cast<long long>(p.M) + kBM - 1) / kBM);
+  ASYRP_LAUNCH(tf32_conv_kernel<kEpi>, dim3(pixel_tiles, p.Cout / kBN), dim3(kThreads), kConvSmem, stream, p);
   ASYRP_CHECK_CUDA(cudaGetLastError());
   return ASYRP_OK;
 }

@@ -240,7 +240,9 @@ int asyrp_softmax_rows(const void* S, void* P, long long rows, int T, float scal
  * asyrp_lpips_conv: out = relu(conv(in) + bias), zero padding `pad`, any kh x kw and stride; implicit GEMM on the tensor
  *   cores with TF32 operands (round to nearest) and fp32 accumulation.  in [N][H][W][Cin] (Cin % 4 == 0), out
  *   [N][Ho][Wo][Cout] (Cout % 64 == 0), weight fp32 [Cout][asyrp_lpips_conv_kpad(Cin, kh, kw)]: K = kh*kw*Cin
- *   tap-major / channel-minor, zero columns past K.  bias [Cout] is required; out must not alias in.
+ *   tap-major / channel-minor, zero columns past K.  bias [Cout] is required; out must not alias in.  The TF32 GEMM's
+ *   launcher, shared by every conv and linear layer built on it, refuses Cout above 65535 * 64 (the channel tiles sit
+ *   in grid y), in or weight not 16-byte aligned (cp.async) and out or a residual not 8-byte aligned (float2).
  * asyrp_lpips_maxpool: MaxPool2d(3, 2), no padding, floor mode, [N][H][W][C] -> [N][(H-3)/2+1][(W-3)/2+1][C].
  * asyrp_lpips_distance: one layer term of the distance: per pixel, f/(sqrt(sum_c f^2) + 1e-10) of probe row n and of
  *   ref row n % B, squared difference, lin_w [C] (the 1x1 conv C -> 1), mean over the HW pixels; d[n] = term
@@ -377,25 +379,28 @@ int asyrp_faceparse_agreement(const float* src_logits, const float* edited_logit
  * (asyrp_official_b200/fid.py gives the network and the metric).  Activations are fp32 NHWC.
  * asyrp_fid_pack: x fp32 NCHW [B][3][H][W] -> out fp32 NHWC [B][S][S][4]: q = the u8 torchvision's save_image writes
  *   (fp32 (x + 1) * 0.5 * 255 + 0.5, clamped to [0, 255], truncated), q / 255, bilinear resize to S x S
- *   (align_corners=False; rows blended first), 2 v - 1; channel 3 zero.
+ *   (align_corners=False; rows blended first), 2 v - 1; channel 3 zero; out 16-byte aligned.
  * asyrp_fid_conv: out = max(conv(in) + bias, 0), kh x kw, zero padding padh rows / padw columns, any stride, the TF32
  *   implicit GEMM of asyrp_arcface_conv; in [N][H][W][Cin] (Cin % 4 == 0); weight fp32
  *   [Cout][asyrp_lpips_conv_kpad(Cin, kh, kw)] and bias [Cout] with Cout % 64 == 0 (zero rows past the layer's width);
  *   channels [0, cstore) of out rows [N][Ho][Wo] of pitch ldo are written, the rest untouched: cstore even,
- *   0 < cstore <= Cout, ldo even and >= cstore, out 8-byte aligned (a channel slice of a wider tensor).
+ *   0 < cstore <= Cout, ldo even and >= cstore, out 8-byte aligned (a channel slice of a wider tensor).  The geometry
+ *   is checked in 64 bits: H + 2 padh and W + 2 padw at most 2^31 - 1, kh kw Cin at most 2^31 - 32 (Kpad in int),
+ *   N Ho Wo below 2^31; the launcher's limits of asyrp_lpips_conv apply.
  * asyrp_fid_pool: mode 0 max-pool 3x3 / 2 without padding (H, W >= 3), 1 avg-pool 3x3 / 1 pad 1 without the padding
  *   (count_include_pad=False; taps summed in row-major order, then divided by their count), 2 max-pool 3x3 / 1 pad 1
  *   (padding never wins) of in [N][H][W][C] (C % 4 == 0) into out rows of pitch ldo (ldo % 4 == 0, ldo >= C); in and
  *   out 16-byte aligned.
  * asyrp_fid_mean: out[n][c] = the mean of in [N][HW][C] over the HW pixels, summed in pixel order.
  * asyrp_fid_moments: mu [d] and sigma [d][d] (fp64) of the n rows of x fp32 [n][d]: column means and the centred
- *   covariance with the n - 1 denominator; n >= 2, d % 64 == 0.
+ *   covariance with the n - 1 denominator; 2 <= n <= 2^31 - 16, d % 64 == 0, d <= 65535 * 64, n d < 2^40.
  * asyrp_fid_kernel_sum: out[0] = sum over i < n, j < m of (x[i] . y[j] / d + 1)^3 in fp64, pairs i == j skipped with
- *   exclude_diag; x fp32 [n][d], y fp32 [m][d], d % 16 == 0; partial: asyrp_fid_kernel_sum_partials(n, m) doubles of
- *   workspace.
+ *   exclude_diag; x fp32 [n][d], y fp32 [m][d], d % 16 == 0, n <= 65535 * 64; partial:
+ *   asyrp_fid_kernel_sum_partials(n, m) doubles of workspace, one per 64 x 64 tile (-1: n or m not positive, or more
+ *   than 2^31 - 256 tiles, which the call refuses).
  * asyrp_fid_pack_u8: x u8 NHWC [B][H][W][3] (a decoded image file) -> out as asyrp_fid_pack: q = x, q / 255,
  *   bilinear resize to S x S, 2 v - 1 (pytorch-fid's ToTensor path); bit-identical to asyrp_fid_pack of
- *   x / 127.5 - 1 as fp32 NCHW (whose quantiser gives back q).
+ *   x / 127.5 - 1 as fp32 NCHW (whose quantiser gives back q); out 16-byte aligned.
  * asyrp_fid_kernel_sum_subsets: out[z] (z < subsets, fp64) = sum over i, j < s of
  *   (x[idx_x[z][i]] . y[idx_y[z][j]] / d + 1)^3, pairs i == j skipped with exclude_diag: bit-identical to
  *   asyrp_fid_kernel_sum of the gathered rows x[idx_x[z]], y[idx_y[z]].  x fp32 [n][d], y fp32 [m][d], idx_x / idx_y

@@ -141,6 +141,10 @@ SIGNATURES = {
     "asyrp_fid_knn_radii": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p]),
     "asyrp_fid_knn_counts": (c_int, [c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p,
                                      c_void_p, c_void_p]),
+    "asyrp_png_quantize": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p]),
+    "asyrp_preserve_sse": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, C.c_longlong, c_void_p]),
+    "asyrp_ssim_level": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p]),
+    "asyrp_ssim_pool2": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p]),
 }
 
 _lib = None

@@ -1,4 +1,4 @@
-// Host-side helpers shared by the .cu translation units of libasyrp_b200.so.
+// Helpers shared by the .cu translation units of libasyrp_b200.so (host side, and the save_image quantiser).
 #pragma once
 #include <cuda.h>
 #include <cuda_runtime.h>
@@ -60,6 +60,23 @@ int sm_count();
 
 // largest grid y / z dimension of a launch; kernels that put the batch there refuse a larger one up front
 constexpr int kMaxGridYZ = 65535;
+
+// The u8 value q torchvision's save_image writes for a pixel of an fp32 image x in [-1, 1] (NCHW [B][3][H][W]): the
+// fp32 operations (x + 1) * 0.5 * 255 + 0.5, each rounded once, clamped to [0, 255] and truncated.  q(...) gives q as a
+// float; operator() gives q / 255 (fp32, rounded once), the pixel reader of fid_pack_kernel.
+struct SavedPng {
+  const float* __restrict__ x;
+  int H, W;
+  __device__ static float quantize(float v) {
+    const float t = __fadd_rn(__fmul_rn(__fmul_rn(__fadd_rn(v, 1.f), 0.5f), 255.f), 0.5f);
+    return truncf(fminf(fmaxf(t, 0.f), 255.f));
+  }
+  __device__ float q(size_t b, int c, int yy, int xx) const {
+    const float* img = x + (b * 3 + c) * (static_cast<size_t>(H) * W);
+    return quantize(img[static_cast<size_t>(yy) * W + xx]);
+  }
+  __device__ float operator()(size_t b, int c, int yy, int xx) const { return __fdiv_rn(q(b, c, yy, xx), 255.f); }
+};
 
 // Programmatic dependent launch (PDL).  Every kernel of the library starts with `griddepcontrol.launch_dependents`
 // and executes `griddepcontrol.wait` before its first global-memory access; launched with the

@@ -33,18 +33,7 @@ enum PoolMode : int { kPoolMax3s2 = 0, kPoolAvg3s1 = 1, kPoolMax3s1 = 2 };
 
 // The pixel readers of fid_pack_kernel: px(b, c, y, x) = q / 255 (fp32, rounded once) of the u8 value q of channel c
 // at (y, x) of image b.
-// SavedPng: x fp32 NCHW [B][3][H][W]; q = the u8 save_image writes for x: the fp32 operations
-// (x + 1) * 0.5 * 255 + 0.5, each rounded once, clamped to [0, 255] and truncated.
-struct SavedPng {
-  const float* __restrict__ x;
-  int H, W;
-  __device__ float operator()(size_t b, int c, int yy, int xx) const {
-    const float* img = x + (b * 3 + c) * (static_cast<size_t>(H) * W);
-    const float t = __fadd_rn(__fmul_rn(__fmul_rn(__fadd_rn(img[static_cast<size_t>(yy) * W + xx], 1.f), 0.5f),
-                                        255.f), 0.5f);
-    return __fdiv_rn(truncf(fminf(fmaxf(t, 0.f), 255.f)), 255.f);
-  }
-};
+// SavedPng (common.h): x fp32 NCHW [B][3][H][W]; q = the u8 save_image writes for x.
 // DecodedU8: q read from u8 NHWC [B][H][W][3], a decoded image file
 struct DecodedU8 {
   const uint8_t* __restrict__ x;

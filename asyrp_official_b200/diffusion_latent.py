@@ -27,6 +27,11 @@ Mirrors, with the same attribute / flag names:
                                                             statistics (fid.score_against_stats); with --prdc also
                                                             precision / recall / density / coverage of the same sets
                                                             from k-nearest-neighbour balls (fid.prdc)
+  --content_preservation       (none)                       run_test scores every edit with PSNR, SSIM, MS-SSIM and
+                                                            LPIPS-Alex against the origin pass of the same x_T
+                                                            (preservation.ContentPreservation), and the origin pass
+                                                            against the input image for inverted latents, written next
+                                                            to the PNG; this build's definition
   Asyrp.precompute_pairs_with_h :877-947                    DDIM inversion of one image keeping the bottleneck h of
                                                             every step (batched here, same cache file)
   Asyrp.run_diff_style         main.py:192-202              --diff_style (DiffStyle content injection): this build's
@@ -91,6 +96,11 @@ class Asyrp(object):
         # set against the origin set; with --fid_ref, prdc_real: fp64 [1 + tuples][4] against the real images' features
         self.prdc = {}
         self.prdc_real = {}
+        # --content_preservation: save_image's file name -> fp64 [tuples][images][4], (PSNR, SSIM, MS_SSIM, LPIPS) of
+        # each edit against the origin pass; reconstruction: fp64 [images][4] of the origin pass against the input
+        # image, for latents inverted from images
+        self.content_preservation = {}
+        self.reconstruction = {}
 
     # ------------------------------------------------------------------------------------------
     def load_pretrained_model(self):
@@ -252,6 +262,37 @@ class Asyrp(object):
             return load_state_dict(path)
         except ValueError as e:
             raise ValueError(f"--seg_consistency: {e}") from None
+
+    def content_preservation_setup(self):
+        """--content_preservation's requirements, checked before any model is loaded; raises ValueError with the
+        reason.  Returns what ContentPreservation takes: the validated --lpips_weights path, or seeded weights with
+        --synthetic_weights (as load_lpips)."""
+        from .lpips import load_state_dict
+        from .preservation import check_image_size
+        a = self.args
+        if not getattr(a, "run_test", False) or getattr(a, "diff_style", False):
+            raise ValueError("--content_preservation scores the edits of --run_test (not --diff_style or --lpips)")
+        if getattr(a, "pass_editing", False):
+            raise ValueError("--content_preservation scores the edited images: with --pass_editing nothing is edited")
+        size = self.config.data.image_size
+        try:
+            check_image_size(size, size)
+        except ValueError as e:
+            raise ValueError(f"--content_preservation: {e}") from None
+        path = getattr(a, "lpips_weights", None)
+        if path:
+            if not os.path.isfile(path):
+                raise ValueError(f"--content_preservation: --lpips_weights {path!r} is not a file")
+            try:
+                load_state_dict(path)
+            except Exception as e:  # a file torch.load cannot read, or the wrong keys
+                raise ValueError(f"--content_preservation: --lpips_weights {path!r}: {e}") from None
+            return path
+        if getattr(a, "synthetic_weights", False):
+            from .synthetic import lpips_state_dict
+            return lpips_state_dict(seed=getattr(a, "seed", 1234))
+        raise ValueError("--content_preservation needs --lpips_weights (a torch.save of the lpips package's "
+                         "LPIPS(net='alex').state_dict()) or --synthetic_weights")
 
     def fid_setup(self):
         """--fid's requirements, checked before any model is loaded; raises ValueError with the reason.  Returns the
@@ -531,7 +572,7 @@ class Asyrp(object):
     def save_image(self, model, x_lat_tensor, seq_inv, seq_inv_next, save_x0=False, save_x_origin=False,
                    save_process_delta_h=False, save_process_origin=False, x0_tensor=None, delta_h_dict=None,
                    get_delta_hs=False, folder_dir="", file_name="", hs_coeff=(1.0, 1.0), directional_clip=None,
-                   id_scorer=None, seg_scorer=None, fid=None):
+                   id_scorer=None, seg_scorer=None, fid=None, preservation=None, x0_source=None):
         """rows of the grid: [x0] [origin DDIM] one row per hs_coeff tuple  (diffusion_latent.py:445-544).
 
         delta_h_dict: {t: None | Δh tensor}.  Entries that are tensors select the explicit-Δh branch for that step
@@ -548,7 +589,11 @@ class Asyrp(object):
         the same origin pass, written to <file_name>_ngen<n_train_step>_seg_consistency.tsv and kept in
         self.seg_consistency[file_name].
         fid: (fid.FIDInception, fid.FeatureSets, mode, image index of every row) for --fid: the pool features of the
-        origin pass and of each tuple's edits are added to their sets (finish_fid scores them at the end of the run)."""
+        origin pass and of each tuple's edits are added to their sets (finish_fid scores them at the end of the run).
+        preservation: a preservation.ContentPreservation for --content_preservation: (PSNR, SSIM, MS_SSIM, LPIPS) of
+        every edit against the same origin pass, and with x0_source (the input images the latents were inverted from)
+        of the origin pass against them; written to <file_name>_ngen<n_train_step>_content_preservation.tsv and kept in
+        self.content_preservation[file_name] / self.reconstruction[file_name]."""
         import torchvision.utils as tvu
         a = self.args
         time_s = time.time()
@@ -558,7 +603,7 @@ class Asyrp(object):
         if save_x0 and x0_tensor is not None:
             x_list.append(x0_tensor.cpu())
         if save_x_origin or directional_clip is not None or id_scorer is not None or seg_scorer is not None or \
-                fid is not None:
+                fid is not None or preservation is not None:
             sch = self.make_schedule(seq_inv, seq_inv_next, (1.0,), edit=False,
                                      addnoise=bool(getattr(a, "origin_process_addnoise", False)))
             if save_x_origin:
@@ -650,8 +695,25 @@ class Asyrp(object):
                          "SC", "segmentation consistency")
         if fid is not None and edited:
             add_fid_features(fid, origin, edited)
+        if preservation is not None and edited:
+            self.score_preservation(preservation, origin, edited, x0_source, coeffs, os.path.join(
+                folder_dir, f'{file_name}_ngen{a.n_train_step}_content_preservation.tsv'), file_name)
         print(f'{time.time() - time_s} seconds, {file_name}_ngen{a.n_train_step}.png is saved')
         return x_list
+
+    def score_preservation(self, preservation, origin, edited, x0_source, coeffs, path, file_name, attrs=None):
+        """--content_preservation of one batch: every tuple's edits (edited[k]) against the origin pass, and the origin
+        pass against x0_source when given; kept in self.content_preservation / self.reconstruction and written to
+        `path` (write_scores, the reconstruction rows first)"""
+        from .preservation import COLUMNS
+        bs = origin.shape[0]
+        cp = preservation.scores(origin, torch.cat(edited)).view(len(edited), bs, len(COLUMNS))
+        self.content_preservation[file_name] = cp
+        rec = None
+        if x0_source is not None:
+            rec = preservation.scores(x0_source, origin)
+            self.reconstruction[file_name] = rec
+        write_scores(path, coeffs, cp, COLUMNS, "content preservation", attrs=attrs, origin=rec)
 
     # ------------------------------------------------------------------------------------------
     def load_lpips(self):
@@ -697,6 +759,8 @@ class Asyrp(object):
         the others run bs_train per replay (every row's distances equal its batch-1 run bit for bit)."""
         import torchvision.utils as tvu
         a = self.args
+        if getattr(a, "content_preservation", False):
+            self.content_preservation_setup()  # refuses --lpips
         if self.world > 1:
             raise NotImplementedError("--lpips computes statistics over every image: run single-process")
         print("Get lpips distance...")
@@ -763,6 +827,7 @@ class Asyrp(object):
         id_sd = self.id_similarity_setup() if getattr(a, "id_similarity", False) else None
         seg_sd = self.seg_consistency_setup() if getattr(a, "seg_consistency", False) else None
         fid_sd = self.fid_setup() if getattr(a, "fid", False) else None
+        cp_sd = self.content_preservation_setup() if getattr(a, "content_preservation", False) else None
         if a.multiple_attr and self.needs_clip() and self.clip_configured():
             cosine = self.choose_attribute(a.multiple_attr.split(' '))  # :640-652
             self.set_t_edit_t_addnoise(LPIPS_th=a.lpips_edit_th, LPIPS_addnoise_th=a.lpips_addnoise_th, cosine=cosine)
@@ -871,7 +936,7 @@ class Asyrp(object):
         if getattr(a, "target_image_id", None):
             target_ids = [int(i) for i in str(a.target_image_id).split(" ")]
             assert a.bs_train == 1, "target_image_id is only supported for batch_size == 1"
-        results, directional_clip, id_scorer, seg_scorer, fid_net = {}, None, None, None, None
+        results, directional_clip, id_scorer, seg_scorer, fid_net, preservation = {}, None, None, None, None, None
         if sdir is not None:  # the image tower lives for this run_test only
             from .clip_image import CLIPLoss
             directional_clip = (CLIPLoss(a.clip_weights, a.clip_vocab, sdir[2], device=self.device), sdir[0], sdir[1])
@@ -888,10 +953,14 @@ class Asyrp(object):
                 from .fid import FeatureSets, FIDInception
                 fid_net, fid_sets = FIDInception(fid_sd, device=self.device), FeatureSets()
                 fid_sd = None
+            if cp_sd is not None:  # and LPIPS-Alex
+                from .preservation import ContentPreservation
+                preservation = ContentPreservation(cp_sd, device=self.device)
+                cp_sd = None
             for mode, do, n_img in (("train", a.do_train, a.n_train_img), ("test", a.do_test, a.n_test_img)):
                 if not do:
                     continue
-                x_lat_tensor, x0_tensor, batch_idx, batch_ids = None, None, 0, []
+                x_lat_tensor, x0_tensor, batch_idx, batch_ids, x0_source = None, None, 0, [], None
                 for step, (x0, _, x_lat) in enumerate(pairs[mode]):
                     if target_ids is not None and step not in target_ids:
                         continue
@@ -901,6 +970,8 @@ class Asyrp(object):
                     batch_ids.append(step)
                     if a.use_x0_tensor:
                         x0_tensor = x0 if x0_tensor is None else torch.cat((x0_tensor, x0), dim=0)
+                    if preservation is not None and not a.load_random_noise:  # the images the latents came from
+                        x0_source = x0 if x0_source is None else torch.cat((x0_source, x0), dim=0)
                     if (step + 1) % a.bs_train != 0:
                         continue
                     if batch_idx % self.world == self.rank:  # batch-sharded across ranks, no per-step communication
@@ -912,7 +983,8 @@ class Asyrp(object):
                             save_process_delta_h=bool(getattr(a, "save_process_delta_h", False)),
                             folder_dir=a.test_image_folder, file_name=f'{mode}_{step}_{a.n_iter - 1}', hs_coeff=hs_coeff,
                             directional_clip=directional_clip, id_scorer=id_scorer, seg_scorer=seg_scorer,
-                            fid=None if fid_net is None else (fid_net, fid_sets, mode, batch_ids))
+                            fid=None if fid_net is None else (fid_net, fid_sets, mode, batch_ids),
+                            preservation=preservation, x0_source=x0_source)
                     batch_idx += 1
                     if step == n_img - 1:
                         break
@@ -933,13 +1005,14 @@ class Asyrp(object):
                         print(f'Dict: {latent_name} is saved.')
                         num_mean = 0
                         print("now we use mean of delta_hs")
-                    x_lat_tensor, x0_tensor, batch_ids = None, None, []
+                    x_lat_tensor, x0_tensor, batch_ids, x0_source = None, None, [], None
             if fid_net is not None:
                 self.finish_fid(fid_sets, hs_coeff if isinstance(hs_coeff, list) else [hs_coeff])
         finally:
             a.train_delta_h = a_train_delta_h_prev
-            if directional_clip is not None or id_scorer is not None or seg_scorer is not None or fid_net is not None:
-                del directional_clip, id_scorer, seg_scorer, fid_net
+            if directional_clip is not None or id_scorer is not None or seg_scorer is not None or fid_net is not None \
+                    or preservation is not None:
+                del directional_clip, id_scorer, seg_scorer, fid_net, preservation
                 torch.cuda.empty_cache()
         self.last_delta_h_dict = delta_h_dict
         return results
@@ -1010,6 +1083,7 @@ class Asyrp(object):
         id_sd = self.id_similarity_setup() if getattr(a, "id_similarity", False) else None
         seg_sd = self.seg_consistency_setup() if getattr(a, "seg_consistency", False) else None
         fid_sd = self.fid_setup() if getattr(a, "fid", False) else None
+        cp_sd = self.content_preservation_setup() if getattr(a, "content_preservation", False) else None
         times = self.attr_sweep_schedules(attrs)
         self.sweep_times = dict(zip(attrs, times))
         seq_test = [int(s + 1e-6) for s in list(np.linspace(0, 1, a.n_test_step) * a.t_0)]
@@ -1037,7 +1111,7 @@ class Asyrp(object):
             pairs = self.precompute_pairs(model)
         target_ids = [int(i) for i in str(a.target_image_id).split(" ")] if getattr(a, "target_image_id", None) \
             else None
-        results, directional_clip, id_scorer, seg_scorer, fid_net = {}, None, None, None, None
+        results, directional_clip, id_scorer, seg_scorer, fid_net, preservation = {}, None, None, None, None, None
         if sdir is not None:
             from .clip_image import CLIPLoss
             directional_clip = (CLIPLoss(a.clip_weights, a.clip_vocab, sdir[1], device=self.device), sdir[0])
@@ -1054,10 +1128,14 @@ class Asyrp(object):
                 from .fid import FeatureSets, FIDInception
                 fid_net, fid_sets = FIDInception(fid_sd, device=self.device), FeatureSets()
                 fid_sd = None
+            if cp_sd is not None:
+                from .preservation import ContentPreservation
+                preservation = ContentPreservation(cp_sd, device=self.device)
+                cp_sd = None
             for mode, do, n_img in (("train", a.do_train, a.n_train_img), ("test", a.do_test, a.n_test_img)):
                 if not do:
                     continue
-                x_lat_tensor, x0_tensor, batch_idx, batch_ids = None, None, 0, []
+                x_lat_tensor, x0_tensor, batch_idx, batch_ids, x0_source = None, None, 0, [], None
                 for step, (x0, _, x_lat) in enumerate(pairs[mode]):
                     if (target_ids is not None and step not in target_ids) or a.start_image_id > step:
                         continue
@@ -1065,6 +1143,8 @@ class Asyrp(object):
                     batch_ids.append(step)
                     if a.use_x0_tensor:
                         x0_tensor = x0 if x0_tensor is None else torch.cat((x0_tensor, x0), dim=0)
+                    if preservation is not None and not a.load_random_noise:
+                        x0_source = x0 if x0_source is None else torch.cat((x0_source, x0), dim=0)
                     if (step + 1) % a.bs_train != 0:
                         continue
                     if batch_idx % self.world == self.rank:  # batch-sharded across ranks, as run_test
@@ -1073,16 +1153,18 @@ class Asyrp(object):
                             save_x_origin=a.save_x_origin, x0_tensor=x0_tensor,
                             folder_dir=a.test_image_folder, file_name=f'{mode}_{step}_{a.n_iter - 1}',
                             directional_clip=directional_clip, id_scorer=id_scorer, seg_scorer=seg_scorer,
-                            fid=None if fid_net is None else (fid_net, fid_sets, mode, batch_ids))
+                            fid=None if fid_net is None else (fid_net, fid_sets, mode, batch_ids),
+                            preservation=preservation, x0_source=x0_source)
                     batch_idx += 1
                     if step == n_img - 1:
                         break
-                    x_lat_tensor, x0_tensor, batch_ids = None, None, []
+                    x_lat_tensor, x0_tensor, batch_ids, x0_source = None, None, [], None
             if fid_net is not None:
                 self.finish_fid(fid_sets, coeffs, attrs=attrs)
         finally:
-            if directional_clip is not None or id_scorer is not None or seg_scorer is not None or fid_net is not None:
-                del directional_clip, id_scorer, seg_scorer, fid_net
+            if directional_clip is not None or id_scorer is not None or seg_scorer is not None or fid_net is not None \
+                    or preservation is not None:
+                del directional_clip, id_scorer, seg_scorer, fid_net, preservation
                 torch.cuda.empty_cache()
         return results
 
@@ -1098,7 +1180,7 @@ class Asyrp(object):
     @torch.no_grad()
     def save_image_sweep(self, model, x_lat_tensor, seq_inv, seq_inv_next, attrs, times, coeffs, save_x0=False,
                          save_x_origin=False, x0_tensor=None, folder_dir="", file_name="", directional_clip=None,
-                         id_scorer=None, seg_scorer=None, fid=None):
+                         id_scorer=None, seg_scorer=None, fid=None, preservation=None, x0_source=None):
         """save_image for an attribute sweep: grid rows [x0] [origin DDIM] then one row per attribute in the order
         given.  Rows of the trajectory are (attribute, image), attribute-major, run in chunks of whole attributes of
         at most --max_rows_per_replay rows (sweep_chunks).  directional_clip = (CLIPLoss, [(src_txt, trg_txt)] per
@@ -1113,7 +1195,7 @@ class Asyrp(object):
         if save_x0 and x0_tensor is not None:
             x_list.append(x0_tensor.cpu())
         if save_x_origin or directional_clip is not None or id_scorer is not None or seg_scorer is not None or \
-                fid is not None:
+                fid is not None or preservation is not None:
             sch = self.make_schedule(seq_inv, seq_inv_next, (1.0,), edit=False,
                                      addnoise=bool(getattr(a, "origin_process_addnoise", False)))
             if save_x_origin:
@@ -1154,6 +1236,9 @@ class Asyrp(object):
                          sc, "SC", "segmentation consistency", attrs=attrs)
         if fid is not None:
             add_fid_features(fid, origin, edited)
+        if preservation is not None:
+            self.score_preservation(preservation, origin, edited, x0_source, coeffs, os.path.join(
+                folder_dir, f'{file_name}_ngen{a.n_train_step}_content_preservation.tsv'), file_name, attrs=attrs)
         print(f'{time.time() - time_s} seconds, {file_name}_ngen{a.n_train_step}.png is saved')
         return x_list
 
@@ -1250,6 +1335,8 @@ class Asyrp(object):
         import torchvision.utils as tvu
         a = self.args
         self.prdc_check()
+        if getattr(a, "content_preservation", False):
+            self.content_preservation_setup()  # refuses --diff_style
         if getattr(a, "fid", False):
             self.fid_setup()  # refuses --diff_style, before any model loads
         contents, styles, gammas = self.diff_style_setup()
@@ -1365,19 +1452,32 @@ def sweep_rows(chunk, tpc, bs):
     rows = [k for k in chunk for _ in range(bs)]
     return rows + [rows[-1]] * (tpc * bs - len(rows))
 
-def write_scores(path, coeffs, scores, column, label, attrs=None):
+def write_scores(path, coeffs, scores, column, label, attrs=None, origin=None):
     """a per-edit score table: one row per (hs_coeff tuple, image) in grid order, columns image, tuple, hs_coeff and
     `column`; prints each tuple's mean as `label`.  attrs (an attribute sweep): tuple k is attribute k, named in an
-    appended `attr` column"""
+    appended `attr` column.  Several columns: `column` a sequence of names and scores [tuples][images][columns].
+    origin ([images][columns]): rows of the origin pass first, with tuple `origin`, hs_coeff `-` (and attr `-`)"""
+    columns = [column] if isinstance(column, str) else list(column)
+    tail = (lambda a: f"\t{a}") if attrs is not None else (lambda a: "")
+
+    def cells(v):
+        return "\t".join(repr(x) for x in (v if isinstance(v, list) else [v]))
     with open(path, "w") as f:
-        f.write(f"image\ttuple\ths_coeff\t{column}" + ("\tattr" if attrs is not None else "") + "\n")
+        f.write("image\ttuple\ths_coeff\t" + "\t".join(columns) + tail("attr") + "\n")
+        if origin is not None:
+            for i, v in enumerate(origin.tolist()):
+                f.write(f"{i}\torigin\t-\t{cells(v)}" + tail("-") + "\n")
         for k, row in enumerate(scores.tolist()):
             tup = ",".join(f"{float(c):.6g}" for c in coeffs[k])
             for i, v in enumerate(row):
-                f.write(f"{i}\t{k}\t{tup}\t{v!r}" + (f"\t{attrs[k]}" if attrs is not None else "") + "\n")
-    for k, row in enumerate(scores):
-        name = f"attribute {attrs[k]}" if attrs is not None else f"hs_coeff {tuple(float(c) for c in coeffs[k])}"
-        print(f"{label}, {name}: mean {row.double().mean().item():.6f} over {row.numel()} images")
+                f.write(f"{i}\t{k}\t{tup}\t{cells(v)}" + tail(attrs[k] if attrs is not None else None) + "\n")
+    rows = ([("origin", origin)] if origin is not None else []) + [
+        (f"attribute {attrs[k]}" if attrs is not None else f"hs_coeff {tuple(float(c) for c in coeffs[k])}", row)
+        for k, row in enumerate(scores)]
+    for name, row in rows:
+        means = row.double().reshape(row.shape[0], -1).mean(0).tolist()
+        vals = f"{means[0]:.6f}" if len(columns) == 1 else ", ".join(f"{c} {m:.6f}" for c, m in zip(columns, means))
+        print(f"{label}, {name}: mean {vals} over {row.shape[0]} images")
 
 
 def add_fid_features(fid, origin, edited):

@@ -147,7 +147,13 @@ def build_parser():
                    help='directory with <config stem>_LPIPS_distance_{x,x0_t}.tsv (read by --run_test, written by '
                         '--lpips; default utils)')
     p.add_argument('--lpips_weights', type=str, default=None,
-                   help="torch.save of the lpips package's LPIPS(net='alex').state_dict() (--lpips)")
+                   help="torch.save of the lpips package's LPIPS(net='alex').state_dict() (--lpips, "
+                        "--content_preservation)")
+    p.add_argument('--content_preservation', **sa,
+                   help='--run_test: score every edit for content preservation, PSNR, SSIM, MS-SSIM and LPIPS-Alex '
+                        '(--lpips_weights, or seeded weights with --synthetic_weights) of the saved u8 image against '
+                        'the unedited DDIM pass of the same x_T, and that pass against the input image for latents '
+                        'inverted from images, written next to the PNG (images larger than 160 x 160)')
     p.add_argument('--checkpoint_dir', type=str, default='checkpoint')
     p.add_argument('--max_rows_per_replay', type=int, default=16,
                    help='rows (hs_coeff tuples x images) of one batched trajectory in save_image; bounds the memory of '

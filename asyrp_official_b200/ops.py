@@ -865,6 +865,53 @@ def fid_knn_counts(a, ra, b, rb, out=None):
     return b_in_a, a_in_b, a_covered
 
 
+def png_quantize(x, q, lvl0=None, xq=None):
+    """x fp32 [B][3][H][W] -> q u8 [B][3][H][W], the value save_image writes; lvl0 fp64 q / 255 and xq fp32
+    (2 q - 255) / 255 of the same shape, each written when given"""
+    lib = _lib.load()
+    B, C, H, W = x.shape
+    _need_cuda(x, q, lvl0, xq)
+    assert C == 3 and x.dtype == torch.float32 and x.is_contiguous()
+    assert q.dtype == torch.uint8 and q.is_contiguous() and q.shape == x.shape
+    assert lvl0 is None or (lvl0.dtype == torch.float64 and lvl0.is_contiguous() and lvl0.shape == x.shape)
+    assert xq is None or (xq.dtype == torch.float32 and xq.is_contiguous() and xq.shape == x.shape)
+    check(lib.asyrp_png_quantize(_ptr(x), _ptr(q), _ptr(lvl0), _ptr(xq), B, H, W, _stream()), "asyrp_png_quantize")
+
+
+def preserve_sse(src, edited, sse):
+    """sse int64 [n]: sum of (edited[j] - src[j % B])^2 over the u8 values of each row; src [B][...], edited [n][...]"""
+    lib = _lib.load()
+    B, n = src.shape[0], edited.shape[0]
+    _need_cuda(src, edited, sse)
+    assert src.dtype == torch.uint8 and edited.dtype == torch.uint8 and src.is_contiguous() and edited.is_contiguous()
+    assert src.shape[1:] == edited.shape[1:] and sse.dtype == torch.int64 and sse.is_contiguous() and sse.numel() == n
+    check(lib.asyrp_preserve_sse(_ptr(src), _ptr(edited), _ptr(sse), n, B, src[0].numel(), _stream()),
+          "asyrp_preserve_sse")
+
+
+def ssim_level(src, edited, stats):
+    """stats fp64 [n][3][2]: per channel of edited row j against source row j % B, the means of the SSIM and cs maps
+    over the valid pixels (11-tap Gaussian, sigma 1.5, no padding); src fp64 [B][3][H][W], edited fp64 [n][3][H][W]"""
+    lib = _lib.load()
+    B, C, H, W = src.shape
+    n = edited.shape[0]
+    _need_cuda(src, edited, stats)
+    assert C == 3 and src.dtype == torch.float64 and edited.dtype == torch.float64 and edited.shape[1:] == src.shape[1:]
+    assert src.is_contiguous() and edited.is_contiguous()
+    assert stats.dtype == torch.float64 and stats.is_contiguous() and tuple(stats.shape) == (n, 3, 2)
+    check(lib.asyrp_ssim_level(_ptr(src), _ptr(edited), _ptr(stats), n, B, H, W, _stream()), "asyrp_ssim_level")
+
+
+def ssim_pool2(inp, out):
+    """out = avg_pool2d(inp, 2, stride 2, padding (H mod 2, W mod 2)) of fp64 [rows][3][H][W], count_include_pad"""
+    lib = _lib.load()
+    rows, C, H, W = inp.shape
+    _need_cuda(inp, out)
+    assert C == 3 and inp.dtype == torch.float64 and out.dtype == torch.float64
+    assert inp.is_contiguous() and out.is_contiguous() and tuple(out.shape) == (rows, 3, (H + 1) // 2, (W + 1) // 2)
+    check(lib.asyrp_ssim_pool2(_ptr(inp), _ptr(out), rows, H, W, _stream()), "asyrp_ssim_pool2")
+
+
 def ddpm_update(x, et, z, x_next, at, bt, logvar, learned_sigma, mask):
     lib = _lib.load()
     N, Cx, H, W = x.shape

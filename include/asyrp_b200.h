@@ -438,6 +438,26 @@ int asyrp_fid_knn_radii(const float* x, double* radii, double* work, int n, int 
 int asyrp_fid_knn_counts(const float* a, const double* ra, int n, const float* b, const double* rb, int m, int d,
                          unsigned* b_in_a, unsigned* a_in_b, unsigned* a_covered, void* stream);
 
+/* ---- Content preservation: PSNR, SSIM and MS-SSIM of the u8 images save_image writes (csrc/preservation.cu;
+ * asyrp_official_b200/preservation.py combines the statistics).  Edited row j is compared with source row j % B.
+ * asyrp_png_quantize: x fp32 NCHW [B][3][H][W] -> q u8 [B][3][H][W], the value save_image writes (as asyrp_fid_pack);
+ *   lvl0 fp64 q / 255 and xq fp32 (2 q - 255) / 255 (LPIPS's input for a loaded PNG) in the same layout, each
+ *   skipped when null.  x, xq 4-byte and lvl0 8-byte aligned.
+ * asyrp_preserve_sse: sse[j] (int64) = sum over the plane = 3 H W elements of (edited[j] - src[j % B])^2, exact;
+ *   src u8 [B][plane], edited u8 [n][plane], plane <= 2^47.
+ * asyrp_ssim_level: stats[j][c] = (mean SSIM map, mean cs map) over the (H - 10) x (W - 10) valid pixels of channel c,
+ *   fp64, from an 11-tap Gaussian window (sigma 1.5, normalised) applied separably without padding, C1 = 0.01^2,
+ *   C2 = 0.03^2 (pytorch_msssim's _ssim with data_range 1); src fp64 [B][3][H][W], edited fp64 [n][3][H][W],
+ *   stats fp64 [n][3][2]; H, W >= 11, 3 n <= 2^31 - 1.  A row's statistics are the same bits for any n and B.
+ * asyrp_ssim_pool2: out = avg_pool2d(in, 2, stride 2, padding (H mod 2, W mod 2)), padding counted in the divisor,
+ *   in fp64 [rows][3][H][W] -> out fp64 [rows][3][ceil(H / 2)][ceil(W / 2)]; out must not alias in.
+ * No allocation, no synchronisation, no atomics. */
+int asyrp_png_quantize(const float* x, unsigned char* q, double* lvl0, float* xq, int B, int H, int W, void* stream);
+int asyrp_preserve_sse(const unsigned char* src, const unsigned char* edited, long long* sse, int n, int B,
+                       long long plane, void* stream);
+int asyrp_ssim_level(const double* src, const double* edited, double* stats, int n, int B, int H, int W, void* stream);
+int asyrp_ssim_pool2(const double* in, double* out, int rows, int H, int W, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

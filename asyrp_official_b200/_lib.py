@@ -145,6 +145,10 @@ SIGNATURES = {
     "asyrp_preserve_sse": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, C.c_longlong, c_void_p]),
     "asyrp_ssim_level": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p]),
     "asyrp_ssim_pool2": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p]),
+    "asyrp_add_h_rows": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p,
+                                 c_void_p]),
+    "asyrp_h_gram": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_void_p]),
+    "asyrp_h_combine": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p]),
 }
 
 _lib = None

@@ -1,6 +1,8 @@
 // HBM-bound kernels of the Asyrp path: GroupNorm finalise / apply (+SiLU, +2x resample, +concat), input
 // packing, timestep embedding + small linears, and the DDIM update.  All activations NHWC fp16; statistics,
 // affine tables, embeddings and the sampler state x_t are fp32.
+#include <climits>
+
 #include "common.h"
 #include "ptx.cuh"
 
@@ -508,6 +510,38 @@ __global__ void __launch_bounds__(256) slerp_h_rows_kernel(const __half* __restr
   slerp_h_sample(h, dh, dh_stride, h2, stats, T, C, H, W, t_rows[blockIdx.x], use_mask, sh);
 }
 
+// Additive direction (h-space directions found from the bottleneck's statistics): h2[n] = c0[n] * h[n] + alpha[n] * d
+// with one fp32 NCHW direction d [C][H][W] shared by every sample and (c0, alpha) = coef[n] (fp32 [N][2], a graph
+// input like slerp's t_rows).  Each element is v = fmaf(alpha, d, __fmul_rn(c0, h)) in fp32, stored rounded to fp16.
+// One block per sample, h2's GroupNorm partial sums written as slerp_h_sample writes them: a thread owns channel pairs,
+// sums v and v * v of the fp32 values over the pixels in order into tile slot 0, and zeroes slots 1..T-1.
+__global__ void __launch_bounds__(256) add_h_rows_kernel(const __half* __restrict__ h, const float* __restrict__ dir,
+                                                         __half* __restrict__ h2, float* __restrict__ stats, int T,
+                                                         int C, int HW, const float* __restrict__ coef) {
+  pdl_trigger();
+  pdl_wait();
+  const int n = blockIdx.x;
+  const float c0 = coef[2 * n], alpha = coef[2 * n + 1];
+  const __half* hn = h + static_cast<size_t>(n) * HW * C;
+  __half* on = h2 + static_cast<size_t>(n) * HW * C;
+  float* st = stats + static_cast<size_t>(n) * T * (C / 2) * 2;
+  for (int pr = threadIdx.x; pr < C / 2; pr += blockDim.x) {
+    float s = 0.f, ss = 0.f;
+    for (int pix = 0; pix < HW; ++pix) {
+#pragma unroll
+      for (int k = 0; k < 2; ++k) {
+        const int c = pr * 2 + k;
+        const float a = __half2float(hn[static_cast<size_t>(pix) * C + c]);
+        const float v = fmaf(alpha, dir[static_cast<size_t>(c) * HW + pix], __fmul_rn(c0, a));
+        on[static_cast<size_t>(pix) * C + c] = __float2half_rn(v);
+        s += v; ss += v * v;
+      }
+    }
+    st[pr * 2] = s; st[pr * 2 + 1] = ss;
+    for (int tt = 1; tt < T; ++tt) { st[(tt * (C / 2) + pr) * 2] = 0.f; st[(tt * (C / 2) + pr) * 2 + 1] = 0.f; }
+  }
+}
+
 }  // namespace asyrp
 
 using namespace asyrp;
@@ -673,6 +707,23 @@ ASYRP_API int asyrp_slerp_h_rows(const void* h, const float* dh, long long dh_sa
   ASYRP_LAUNCH(slerp_h_rows_kernel, dim3(N), dim3(256), 0, static_cast<cudaStream_t>(stream),
                static_cast<const __half*>(h), dh, dh_sample_stride, static_cast<__half*>(h2), stats, stats_tiles, C, H,
                W, t_rows, use_mask);
+  ASYRP_CHECK_CUDA(cudaGetLastError());
+  return ASYRP_OK;
+}
+
+ASYRP_API int asyrp_add_h_rows(const void* h, const float* dir, void* h2, float* stats, int stats_tiles, int N, int C,
+                               int H, int W, const float* coef, void* stream) {
+  ASYRP_REQUIRE(N >= 1 && C >= 2 && C % 2 == 0 && H >= 1 && W >= 1 && stats_tiles >= 1,
+                "asyrp_add_h_rows: bad arguments N=%d C=%d H=%d W=%d stats_tiles=%d", N, C, H, W, stats_tiles);
+  // per-sample offsets are size_t; the element index within a sample and the tile-slot index are int
+  ASYRP_REQUIRE(static_cast<long long>(C) * H * W <= INT_MAX && static_cast<long long>(stats_tiles) * C <= INT_MAX,
+                "asyrp_add_h_rows: C * H * W or stats_tiles * C above 2^31 - 1");
+  ASYRP_REQUIRE(h != nullptr && dir != nullptr && h2 != nullptr && stats != nullptr,
+                "asyrp_add_h_rows: h, dir, h2 and stats are required");
+  ASYRP_REQUIRE(coef != nullptr, "asyrp_add_h_rows: coef is NULL");
+  ASYRP_REQUIRE(h != h2, "asyrp_add_h_rows: h2 must not alias h");
+  ASYRP_LAUNCH(add_h_rows_kernel, dim3(N), dim3(256), 0, static_cast<cudaStream_t>(stream),
+               static_cast<const __half*>(h), dir, static_cast<__half*>(h2), stats, stats_tiles, C, H * W, coef);
   ASYRP_CHECK_CUDA(cudaGetLastError());
   return ASYRP_OK;
 }

@@ -37,6 +37,9 @@ Mirrors, with the same attribute / flag names:
   Asyrp.run_diff_style         main.py:192-202              --diff_style (DiffStyle content injection): this build's
                                                             composition of the functions above with denoising_step's
                                                             delta_h branch; the reference declares the flags only
+  Asyrp.run_h_directions       (none)                       --h_directions: editing directions from the statistics of
+                                                            the bottleneck h (hspace.py), applied by --run_test
+                                                            --h_direction as h + α d; this build's definition
 
 Differences (documented in INTEGRATION.md): the reverse loop is UNetEngine.sample() — one CUDA graph per
 (batch, schedule) instead of 40 Python iterations; pretrained weights come from --model_path (no URL download);
@@ -480,15 +483,18 @@ class Asyrp(object):
         return value
 
     @torch.no_grad()
-    def invert_batch(self, model, x0, n_inv_step=None):
+    def invert_batch(self, model, x0, n_inv_step=None, reconstruct=True):
         """DDIM inversion x_0 -> x_T followed by the reconstruction x_T -> x_rec with --sample_type, both as graph
-        replays (precompute_pairs, diffusion_latent.py:1028-1072).  Returns (x_T, x_rec) on the host."""
+        replays (precompute_pairs, diffusion_latent.py:1028-1072).  Returns (x_T, x_rec) on the host; x_rec is None
+        without reconstruct."""
         a = self.args
         n = n_inv_step or a.n_inv_step
         seq_inv = [int(s + 1e-6) for s in list(np.linspace(0, 1, n) * a.t_0)]
         seq_inv_next = [-1] + list(seq_inv[:-1])
         eng = model.engine
         x_lat = eng.sample(x0.to(eng.device), Schedule.inversion(self.betas, seq_inv, seq_inv_next))
+        if not reconstruct:
+            return x_lat.cpu(), None
         sch = Schedule(self.betas, seq_inv, seq_inv_next, t_edit=10 ** 9, t_addnoise=0, hs_coeff=(1.0,), edit=False,
                        sample_type=getattr(a, "sample_type", "ddim"), logvars=self.logvar)
         noise = torch.randn((sch.n_stochastic, *x_lat.shape), device=eng.device) if sch.n_stochastic else None
@@ -496,15 +502,18 @@ class Asyrp(object):
         return x_lat.cpu(), x_rec.cpu()
 
     @torch.no_grad()
-    def precompute_pairs(self, model, save_imgs=False):
+    def precompute_pairs(self, model, save_imgs=False, modes=("train", "test")):
         """[x0, x_rec, x_T] triples per image, cached as precomputed/<category>_<mode>_t<t_0>_nim<N>_ninv<k>_pairs.pth
         — the reference's file name and list-of-triples format (:974-982,1072,1082).  Images come from
         --custom_train_dataset_dir / --custom_test_dataset_dir (png/jpg, resized to image_size, scaled to [-1, 1]);
         the reference's LMDB dataset classes are out of scope.  Under torchrun rank 0 inverts and writes the cache
-        (temp file + rename), the other ranks load it after a barrier."""
+        (temp file + rename), the other ranks load it after a barrier.  modes: the sets to return (--h_directions
+        needs only "train")."""
         a, out = self.args, {}
         os.makedirs('precomputed', exist_ok=True)
         for mode, n in (("train", a.n_train_img), ("test", a.n_test_img)):
+            if mode not in modes:
+                continue
             p = os.path.join('precomputed/', f'{self.config.data.category}_{mode}_t{a.t_0}_nim{n}_ninv{a.n_inv_step}_pairs.pth')
             if os.path.exists(p) and not getattr(a, "re_precompute", False):
                 out[mode] = torch.load(p, map_location="cpu", weights_only=True)
@@ -572,7 +581,7 @@ class Asyrp(object):
     def save_image(self, model, x_lat_tensor, seq_inv, seq_inv_next, save_x0=False, save_x_origin=False,
                    save_process_delta_h=False, save_process_origin=False, x0_tensor=None, delta_h_dict=None,
                    get_delta_hs=False, folder_dir="", file_name="", hs_coeff=(1.0, 1.0), directional_clip=None,
-                   id_scorer=None, seg_scorer=None, fid=None, preservation=None, x0_source=None):
+                   id_scorer=None, seg_scorer=None, fid=None, preservation=None, x0_source=None, h_direction=None):
         """rows of the grid: [x0] [origin DDIM] one row per hs_coeff tuple  (diffusion_latent.py:445-544).
 
         delta_h_dict: {t: None | Δh tensor}.  Entries that are tensors select the explicit-Δh branch for that step
@@ -593,7 +602,9 @@ class Asyrp(object):
         preservation: a preservation.ContentPreservation for --content_preservation: (PSNR, SSIM, MS_SSIM, LPIPS) of
         every edit against the same origin pass, and with x0_source (the input images the latents were inverted from)
         of the origin pass against them; written to <file_name>_ngen<n_train_step>_content_preservation.tsv and kept in
-        self.content_preservation[file_name] / self.reconstruction[file_name]."""
+        self.content_preservation[file_name] / self.reconstruction[file_name].
+        h_direction: a direction file (hspace.load_direction) for --h_direction: each tuple is (c0, α) and its rows take
+        h2 = c0 h + α d_t at every edit step, every tuple a row block of one batch as for DeltaBlocks."""
         import torchvision.utils as tvu
         a = self.args
         time_s = time.time()
@@ -638,6 +649,11 @@ class Asyrp(object):
                     kw["delta_hs"] = torch.stack(rows)
             elif get_delta_hs:
                 kw["record_dh"] = True
+            if h_direction is not None:
+                from .hspace import direction_rows
+                dirs = direction_rows(h_direction, edit_ts)
+                if dirs is not None:
+                    kw["h_direction"] = dirs
             max_rows = getattr(a, "max_rows_per_replay", 16)
             if "delta_hs" in kw and len({float(tup[0]) for tup in coeffs}) > 1:
                 max_rows = 0  # explicit Δh takes one slerp weight 1 - c0 per replay: one tuple per chunk
@@ -656,6 +672,10 @@ class Asyrp(object):
                         (sch.n_stochastic, *x_lat_tensor.shape), device=eng.device))
                 if per_row:
                     table = torch.tensor([[float(c) for c in coeffs[i][:n + 1]] for i in chunk for _ in range(bs)],
+                                         dtype=torch.float32)
+                    kw["hs_coeffs"] = pad_rows(table, tpc * bs)
+                elif "h_direction" in kw:  # (c0, α) per row
+                    table = torch.tensor([[float(coeffs[i][0]), float(coeffs[i][1])] for i in chunk for _ in range(bs)],
                                          dtype=torch.float32)
                     kw["hs_coeffs"] = pad_rows(table, tpc * bs)
                 x0 = self.edit_batch(model, rows_x, sch, noise=noise, record_process=save_process_delta_h, **kw)
@@ -817,6 +837,7 @@ class Asyrp(object):
         if getattr(a, "fid_ref", None) is not None and not getattr(a, "fid", False):
             raise ValueError("--fid_ref scores the sets that --fid collects: add --fid")
         self.prdc_check()
+        h_dir_path = self.h_direction_setup()  # refuses --attr_sweep too, before it is dispatched
         if getattr(a, "attr_sweep", ""):
             return self.run_attr_sweep()
         print("Running Test")
@@ -862,7 +883,12 @@ class Asyrp(object):
                 save_name, load_dict = latent_name, True
                 delta_h_dict = {i: None for i in seq_test}
         scaling_factor = a.n_train_step / a.n_test_step * a.hs_coeff_delta_h  # :626
-        if a.multiple_attr:
+        h_direction = None
+        if h_dir_path is not None:
+            from .hspace import load_direction
+            h_direction = load_direction(h_dir_path, self.config, a, model.arch.mid_ch)
+            hs_coeff = h_direction_coeffs(a)
+        elif a.multiple_attr:
             attrs = a.multiple_attr.split(' ')
             coeffs = [float(c) for c in a.multiple_hs_coeff.split(' ')] if a.multiple_hs_coeff else []
             coeffs = coeffs + [1.0] * (len(attrs) - len(coeffs))
@@ -873,7 +899,9 @@ class Asyrp(object):
             save_name_list = [save_name]
             hs_coeff = (1.0 * a.hs_coeff_origin_h, 1.0 * scaling_factor)  # :659
         # ----------- load (:662-697)
-        if os.path.exists(save_name_list[0]):
+        if h_direction is not None:
+            pass  # the direction replaces the Δh checkpoint
+        elif os.path.exists(save_name_list[0]):
             print(f'{save_name} exists. load checkpoint')
             if train_delta_block:
                 if num_mean and load_dict:  # the cached mean Δh replaces the DeltaBlock (:669-672)
@@ -915,7 +943,7 @@ class Asyrp(object):
                     delta_h_dict.setdefault(i, None)
         a_train_delta_h_prev = getattr(a, "train_delta_h", False)
         a.train_delta_h = train_delta_h  # save_image's global-Δh rule reads it (:517)
-        if a.delta_interpolation:  # :726-755
+        if a.delta_interpolation and h_direction is None:  # :726-755
             vals = np.linspace(a.min_delta, a.max_delta, a.num_delta).tolist()
             if a.multiple_attr:
                 assert a.get_h_num == 2, "delta_multiple_attr_interpolation is only supported for get_h_num == 2"
@@ -984,7 +1012,7 @@ class Asyrp(object):
                             folder_dir=a.test_image_folder, file_name=f'{mode}_{step}_{a.n_iter - 1}', hs_coeff=hs_coeff,
                             directional_clip=directional_clip, id_scorer=id_scorer, seg_scorer=seg_scorer,
                             fid=None if fid_net is None else (fid_net, fid_sets, mode, batch_ids),
-                            preservation=preservation, x0_source=x0_source)
+                            preservation=preservation, x0_source=x0_source, h_direction=h_direction)
                     batch_idx += 1
                     if step == n_img - 1:
                         break
@@ -1017,6 +1045,118 @@ class Asyrp(object):
         self.last_delta_h_dict = delta_h_dict
         return results
 
+
+    # ------------------------------------------------------------------------------------------
+    def h_direction_setup(self):
+        """--h_direction's requirements, checked before any model loads: the path (None without the flag); ValueError
+        when it is combined with a flag that selects another source of Δh"""
+        a = self.args
+        path = getattr(a, "h_direction", None)
+        if not path:
+            return None
+        for flag, on in (("--train_delta_block", bool(getattr(a, "train_delta_block", False))),
+                         ("--train_delta_h", bool(getattr(a, "train_delta_h", False))),
+                         ("--multiple_attr", bool(getattr(a, "multiple_attr", ""))),
+                         ("--num_mean_of_delta_hs", bool(getattr(a, "num_mean_of_delta_hs", 0))),
+                         ("--attr_sweep", bool(getattr(a, "attr_sweep", "")))):
+            if on:
+                raise ValueError(f"--h_direction replaces the Δh checkpoint: it does not combine with {flag}")
+        if not os.path.isfile(path):
+            raise FileNotFoundError(f"--h_direction {path!r} is not a file")
+        return path
+
+    def h_directions_setup(self):
+        """--h_directions' requirements, checked before any model loads: ('pca', K) or ('mean_diff', (pos, neg))"""
+        a = self.args
+        K = getattr(a, "h_pca", None)
+        pos, neg = getattr(a, "h_pos_dir", None), getattr(a, "h_neg_dir", None)
+        if (K is not None) == bool(pos or neg):
+            raise ValueError("--h_directions needs exactly one mode: --h_pca K, or --h_pos_dir A --h_neg_dir B")
+        if self.world > 1:
+            raise ValueError("--h_directions computes statistics over every sample: run it single-process, not under "
+                             "torchrun")
+        if not getattr(a, "h_direction_out", None):
+            raise ValueError("--h_directions needs --h_direction_out DIR for the direction files")
+        if K is not None:
+            if K < 1 or K > a.n_train_img - 1:
+                raise ValueError(f"--h_pca {K}: between 1 and n_train_img - 1 = {a.n_train_img - 1} components "
+                                 "(n samples have at most n - 1 principal directions)")
+            return "pca", K
+        if not (pos and neg):
+            raise ValueError("--h_pos_dir and --h_neg_dir go together")
+        for flag, d in (("h_pos_dir", pos), ("h_neg_dir", neg)):
+            if not os.path.isdir(d) or not image_paths(d):
+                raise ValueError(f"--{flag} {d!r} is not a directory holding png / jpg images")
+        return "mean_diff", (pos, neg)
+
+    @torch.no_grad()
+    def run_h_directions(self, keep_h=False):
+        """--h_directions: the plain generative pass (run_test's origin pass) over the n_test_step grid from every
+        latent, with h recorded at every step, bs_train rows per replay; then per step the PCA of h over the latents
+        or the mean difference of two sets.  Writes hspace.py's direction files and h_directions.tsv into
+        --h_direction_out; returns their paths.
+          --h_pca K: the n_train_img "train" latents run_test would use: random noise with --load_random_noise, else
+            the --custom_train_dataset_dir images inverted by precompute_pairs (its cache is shared with run_test).
+          --h_pos_dir A --h_neg_dir B: the first n_train_img images of each folder (sorted by name), DDIM-inverted.
+        The device memory of the recorded h ([steps][n][d] fp32) is checked before any inversion or generation.
+        keep_h: keep that buffer as self.h_directions_x (otherwise it is released when the run ends)."""
+        from . import hspace
+        a = self.args
+        mode, arg = self.h_directions_setup()
+        seq, seq_next = make_sequences(a.t_0, a.n_test_step)
+        size = self.config.data.image_size
+        bs = max(1, a.bs_train)
+        if mode == "pca":
+            folder = None if a.load_random_noise else getattr(a, "custom_train_dataset_dir", None)
+            if not a.load_random_noise and (not folder or not os.path.isdir(folder)):
+                raise FileNotFoundError(f"--custom_train_dataset_dir {folder!r} is not a directory: nothing to invert "
+                                        "(use --load_random_noise for random latents)")
+            n = a.n_train_img if folder is None else min(a.n_train_img, len(image_paths(folder)))
+            if n < arg + 1:
+                raise ValueError(f"--h_pca {arg} needs {arg + 1} latents; {folder!r} holds {n} images")
+        else:
+            n_pos, n_neg = (min(a.n_train_img, len(image_paths(f))) for f in arg)
+            n = n_pos + n_neg
+        sch = self.make_schedule(seq, seq_next, (1.0,), edit=False, addnoise=False)
+        model = self.load_pretrained_model().to(self.device)
+        eng = model.engine
+        shape = tuple(eng.plan(bs).mid_f32.shape[1:])
+        d, steps = int(np.prod(shape)), len(sch.steps)
+        need = steps * n * d * 4
+        free, _ = torch.cuda.mem_get_info(eng.device)
+        if need > free:
+            raise MemoryError(f"--h_directions: h of {steps} steps x {n} samples x {d} features takes "
+                              f"{need / 2**30:.2f} GiB; the device has {free / 2**30:.2f} GiB free (lower --n_train_img)")
+        if mode == "pca":
+            pairs = (self.random_noise_pairs(model) if a.load_random_noise else
+                     self.precompute_pairs(model, modes=("train",)))["train"]
+            x_T = torch.cat([p[2] for p in pairs[:n]])
+            n_pos = None
+        else:
+            def invert(folder):  # only x_T is needed: no reconstruction pass
+                imgs = _load_image_folder(folder, size, a.n_train_img)
+                return torch.cat([self.invert_batch(model, torch.cat(imgs[k:k + bs]), reconstruct=False)[0]
+                                  for k in range(0, len(imgs), bs)])
+            x_T = torch.cat([invert(arg[0]), invert(arg[1])])
+        if x_T.shape[0] != n:  # a pairs cache written from another state of the folder
+            raise ValueError(f"--h_directions: {x_T.shape[0]} latents for {n} images; rerun with --re_precompute")
+        X = torch.empty((steps, n, d), dtype=torch.float32, device=eng.device)
+        for k in range(0, n, bs):  # every replay bs rows (the last one padded): one captured graph
+            m = min(bs, n - k)
+            self.edit_batch(model, pad_rows(x_T[k:k + m], bs), sch, record_h=True)
+            X[:, k:k + m].copy_(eng.last_records["h"][:, :m].reshape(steps, m, d))
+        directions, rows = hspace.discover(X, [st.t for st in sch.steps], K=arg if mode == "pca" else None,
+                                           n_pos=n_pos)
+        meta = {"category": self.config.data.category, "mid_ch": int(model.arch.mid_ch), "t_0": int(a.t_0),
+                "n_test_step": int(a.n_test_step), "n": n if mode == "pca" else {"pos": n_pos, "neg": n - n_pos}}
+        self.h_directions = directions
+        if keep_h:
+            self.h_directions_x = X
+        del X
+        paths = hspace.write_directions(a.h_direction_out, directions, rows, shape, meta)
+        for p in paths:
+            print(f"{p} is saved")
+        return paths
 
     # ------------------------------------------------------------------------------------------
     def attr_sweep_setup(self):
@@ -1403,6 +1543,16 @@ def diff_style_gammas(hs_coeff, hs_coeff_list):
     if not gammas:
         raise ValueError("--hs_coeff_list names no value")
     return gammas
+
+
+def h_direction_coeffs(a):
+    """the hs_coeff tuples of --run_test --h_direction: (--hs_coeff_origin_h, α) with α = --hs_coeff_delta_h as given
+    (no n_train_step / n_test_step scaling: a direction has no training grid); --delta_interpolation: (1, v α) for v
+    in linspace(--min_delta, --max_delta, --num_delta)"""
+    alpha = float(a.hs_coeff_delta_h)
+    if a.delta_interpolation:
+        return [(1.0, v * alpha) for v in np.linspace(a.min_delta, a.max_delta, a.num_delta).tolist()]
+    return (1.0 * a.hs_coeff_origin_h, alpha)
 
 
 def image_paths(folder):

@@ -661,6 +661,8 @@ class Plan:
                 ops.slerp_h(self.middle_h.t, self.dh_user, self.h2.t, self.h2.stats, st["slerp_t"], st["use_mask"])
 
         self._emit(slerp, "slerp")
+        # additive direction (h-space directions): h2 = c0*h + α*d with (c0, α) per sample, a graph input like slerp_w
+        self.add_coef = torch.zeros(N, 2, dtype=torch.float32, device=dev)
         # ---- decoders: (h2 -> et_mod) and (h -> et); same weights, same skip tensors.  The second pass allocates from
         # its own pool: in an edit step the two passes are independent and run CONCURRENTLY on two streams
         # (run_edit_and_decoder) — a persistent conv kernel leaves SMs idle in its last wave (512 tiles on 132 SMs =
@@ -811,9 +813,13 @@ class Plan:
         torch.cuda.synchronize(self.eng.device)
         return e0.elapsed_time(e1) / reps
 
-    def run_edit(self, explicit=False):
-        for f in (self.slerp_ops if explicit else self.delta_ops):
-            f()
+    def run_edit(self, explicit=False, inject=None):
+        """h2 (the slerp, the DeltaBlocks, or `inject()` when given) and the decoder on h2"""
+        if inject is not None:
+            inject()
+        else:
+            for f in (self.slerp_ops if explicit else self.delta_ops):
+                f()
         for f in self.dec_mod_ops:
             f()
 
@@ -842,18 +848,18 @@ class Plan:
         edit()
         cur.wait_stream(self.side_stream)
 
-    def run_edit_and_decoder(self, explicit=False):
+    def run_edit_and_decoder(self, explicit=False, inject=None):
         """edit step: Δh injection + decoder(h2) on the current stream, decoder(h) concurrently on the side stream
         (fork / join by events; inside a stream capture this becomes two parallel branches of the graph)"""
         if not DUAL_STREAM:
-            self.run_edit(explicit)
+            self.run_edit(explicit, inject)
             self.run_decoder()
             return
         cur = torch.cuda.current_stream()
         self.side_stream.wait_stream(cur)
         with torch.cuda.stream(self.side_stream):
             self.run_decoder()
-        self.run_edit(explicit)
+        self.run_edit(explicit, inject)
         cur.wait_stream(self.side_stream)
 
 
@@ -935,7 +941,7 @@ class UNetEngine:
     MAX_GRAPHS = 4  # captured trajectory graphs kept per engine (least recently used is dropped)
 
     def _build_trajectory(self, P, schedule, use_graph, explicit, record_dh, record_process, lpips=None,
-                          record_h=False):
+                          record_h=False, additive=False):
         """per-(batch, schedule) state: the timestep-embedding table, the noise buffer, the step loop and its graph"""
         steps = schedule.steps
         n_sto = schedule.n_stochastic
@@ -950,12 +956,14 @@ class UNetEngine:
         learned_sigma = self.arch.out_ch == 2 * self.arch.in_ch
 
         def is_edit(s):  # 'ddpm' steps use e_t only (utils/diffusion_utils.py:74-82): the edit pass cannot change x
-            return s.edit and s.kind == "ddim" and (explicit or self.n_delta > 0)
+            return s.edit and s.kind == "ddim" and (explicit or additive or self.n_delta > 0)
 
         n_edit = sum(1 for s in steps if is_edit(s))
         rec = {}
         if explicit:   # per-edit-step explicit delta_h rows (raw-Δh checkpoints / mean Δh), filled before each replay
             rec["dh_in"] = torch.zeros((max(n_edit, 1), *P.dh_user.shape), dtype=torch.float32, device=self.device)
+        if additive:   # one direction per edit step, read in place by add_h_rows (filled before each replay)
+            rec["dir_in"] = torch.zeros((max(n_edit, 1), *P.dh_user.shape[1:]), dtype=torch.float32, device=self.device)
         if record_dh:  # DeltaBlock outputs per edit step (get_delta_hs, diffusion_latent.py:528-532)
             rec["delta_h"] = torch.zeros((max(n_edit, 1), *P.delta_f32.shape), dtype=torch.float32, device=self.device)
         if record_process:  # x_t and x0_t after every step (save_process_*, :485-491,523-527)
@@ -984,6 +992,9 @@ class UNetEngine:
             xs[:N].copy_(P.x)
             lpips.distance(lpips.features(xs, "probe"), x_start, lp_d[k].view(-1))
 
+        def add_direction(ei):  # h2 = c0*h + α*d from edit step ei's direction, read in place
+            return lambda: ops.add_h_rows(P.middle_h.t, rec["dir_in"][ei], P.h2.t, P.h2.stats, P.add_coef)
+
         def body():
             nonlocal x_start
             if lpips is not None:
@@ -998,7 +1009,7 @@ class UNetEngine:
                 if edit:
                     if explicit:
                         P.dh_user.copy_(rec["dh_in"][ei])
-                    P.run_edit_and_decoder(explicit=explicit)
+                    P.run_edit_and_decoder(explicit=explicit, inject=add_direction(ei) if additive else None)
                     if record_dh:
                         ops.unpack_nchw(P.delta_h.t, rec["delta_h"][ei])
                     ei += 1
@@ -1019,7 +1030,8 @@ class UNetEngine:
                     lpips_step(k)
 
         n_launch = sum(len(P.launches(False, temb=False)) + 1 + int(record_h) for s in steps)
-        n_launch += n_edit * ((len(P.slerp_ops) if explicit else len(P.delta_ops)) + len(P.dec_mod_ops) + int(record_dh))
+        n_launch += n_edit * ((len(P.slerp_ops) if explicit else (1 if additive else len(P.delta_ops))) +
+                              len(P.dec_mod_ops) + int(record_dh))
         if lpips is not None:
             from .lpips import LAUNCHES_DISTANCE, LAUNCHES_FEATURES
             n_launch += LAUNCHES_FEATURES + len(steps) * (LAUNCHES_FEATURES + LAUNCHES_DISTANCE)
@@ -1033,7 +1045,9 @@ class UNetEngine:
                 # warm-up launch outside capture (lazy function attributes, first-touch)
                 P.emb_all.copy_(emb_table[0])
                 P.run_encoder()
-                if explicit or self.n_delta:
+                if additive:
+                    P.run_edit_and_decoder(inject=add_direction(0))
+                elif explicit or self.n_delta:
                     P.run_edit_and_decoder(explicit=explicit)
                 else:
                     P.run_decoder()
@@ -1165,7 +1179,7 @@ class UNetEngine:
             return out
 
     def sample(self, x_T, schedule, noise=None, use_graph=True, out=None, delta_hs=None, use_mask=False,
-               record_dh=False, record_process=False, hs_coeffs=None, lpips=None, record_h=False):
+               record_dh=False, record_process=False, hs_coeffs=None, lpips=None, record_h=False, h_direction=None):
         """Run the reverse trajectory of `schedule` (sampler.Schedule) from x_T; returns x_0 (fp32 NCHW).
 
         The step list, the edit/plain/stochastic phase of every step and all sampler coefficients are host-side
@@ -1199,13 +1213,33 @@ class UNetEngine:
         editing with one DeltaBlock.  Row n then equals, bit for bit, a run of its own Schedule on an engine with only
         its block packed, fed the noise entries of the steps at which it is stochastic (RowSchedule.noise_rows).
         noise: [n_stochastic][N][C][H][W] over the steps at which any row is stochastic.  delta_hs, record_dh, hs_coeffs,
-        lpips and record_h do not apply."""
+        lpips, record_h and h_direction do not apply.
+
+        h_direction: an additive bottleneck direction per edit step, fp32 [n_edit][C][h][w] (hspace.py): at every edit
+        step h2 = c0_n * h + α_n * h_direction[step] (ops.add_h_rows) feeds the edited decoder, with hs_coeffs the
+        per-sample (c0, α) table, fp32 [N][2], required.  Like the DeltaBlock coefficients the table and the directions
+        are graph inputs: every table replays one graph, and sample n equals a batch-1 run with row n bit for bit.
+        The engine must pack no DeltaBlocks; delta_hs, record_dh and lpips do not combine with it."""
         if isinstance(schedule, RowSchedule):
-            if delta_hs is not None or record_dh or hs_coeffs is not None or lpips is not None or record_h:
-                raise ops._lib.AsyrpError("a per-row schedule takes no delta_hs, record_dh, hs_coeffs, lpips or "
-                                          "record_h")
+            if delta_hs is not None or record_dh or hs_coeffs is not None or lpips is not None or record_h or \
+                    h_direction is not None:
+                raise ops._lib.AsyrpError("a per-row schedule takes no delta_hs, record_dh, hs_coeffs, lpips, "
+                                          "record_h or h_direction")
             return self._sample_rows(x_T, schedule, noise, use_graph, out, record_process)
         N = x_T.shape[0]
+        additive = h_direction is not None
+        add_table = None
+        if additive:
+            if delta_hs is not None or record_dh or lpips is not None:
+                raise ops._lib.AsyrpError("h_direction takes no delta_hs, record_dh or lpips")
+            if self.n_delta:
+                raise ops._lib.AsyrpError(f"h_direction needs an engine without DeltaBlocks; this one packed "
+                                          f"{self.n_delta}")
+            add_table = torch.as_tensor(hs_coeffs) if hs_coeffs is not None else None
+            if add_table is None or tuple(add_table.shape) != (N, 2) or not add_table.is_floating_point():
+                raise ops._lib.AsyrpError(f"h_direction needs hs_coeffs, a float [{N}][2] table of (c0, α) per sample, "
+                                          f"got {None if add_table is None else (add_table.dtype, tuple(add_table.shape))}")
+            hs_coeffs = None  # (c0, α) are add_h_rows' table, not DeltaBlock coefficients
         P = self.plan(N)
         explicit = delta_hs is not None
         table = coeff_table(hs_coeffs, N, self.n_delta) if hs_coeffs is not None else None
@@ -1220,7 +1254,7 @@ class UNetEngine:
             slerp_t = 0.0
         key = (N, bool(use_graph), schedule.key(), explicit, slerp_t, bool(use_mask) if explicit else False,
                bool(record_dh), bool(record_process)) + ((lpips,) if lpips is not None else ()) + \
-            (("record_h",) if record_h else ())
+            (("record_h",) if record_h else ()) + (("additive",) if additive else ())
         with torch.cuda.device(self.device):
             n_sto = schedule.n_stochastic
             if n_sto:
@@ -1236,7 +1270,7 @@ class UNetEngine:
             g = self.graphs.pop(key, None)
             if g is None:
                 g = self._build_trajectory(P, schedule, use_graph, explicit, record_dh, record_process, lpips,
-                                           record_h)
+                                           record_h, additive)
                 while len(self.graphs) >= self.MAX_GRAPHS:
                     self.graphs.pop(next(iter(self.graphs)))
             self.graphs[key] = g  # most recently used last
@@ -1250,6 +1284,15 @@ class UNetEngine:
                 dh = delta_hs.to(self.device, torch.float32)
                 assert dh.shape[0] == g["n_edit"], f"delta_hs has {dh.shape[0]} rows, schedule has {g['n_edit']} edit steps"
                 g["rec"]["dh_in"].copy_(dh if dh.dim() == 5 else dh[:, None].expand_as(g["rec"]["dh_in"]))
+            if additive:
+                d = torch.as_tensor(h_direction)
+                want = (g["n_edit"], *g["rec"]["dir_in"].shape[1:])
+                if tuple(d.shape) != want:
+                    raise ops._lib.AsyrpError(f"h_direction must be [{g['n_edit']} edit steps][C][h][w] = "
+                                              f"{list(want)}, got {tuple(d.shape)}")
+                if g["n_edit"]:
+                    g["rec"]["dir_in"].copy_(d.to(self.device, torch.float32))
+                P.add_coef.copy_(add_table.to(torch.float32))
             P.x.copy_(x_T, non_blocking=True)
             if n_sto:
                 g["zbuf"].copy_(noise, non_blocking=True)

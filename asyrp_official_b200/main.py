@@ -165,6 +165,25 @@ def build_parser():
                    help='--run_test: edit every image with each of these attributes ("smiling angry young"), one grid '
                         'row per attribute, each row what --edit_attr <attribute> gives with its own t_edit / '
                         't_addnoise; the checkpoint name\'s "attribute" is replaced by each attribute')
+    p.add_argument('--h_directions', **sa,
+                   help='find editing directions from the statistics of the bottleneck h over many samples, with '
+                        'forward passes only (per-timestep PCA with --h_pca, or a mean difference with --h_pos_dir / '
+                        '--h_neg_dir); writes pc<k>.pth or mean_diff.pth and h_directions.tsv to --h_direction_out')
+    p.add_argument('--h_pca', type=int, default=None,
+                   help='--h_directions: the top K principal components of h over the n_train_img "train" latents '
+                        'of --run_test (--load_random_noise, or --custom_train_dataset_dir images inverted and cached '
+                        'by the same precompute step); 1 <= K <= n - 1')
+    p.add_argument('--h_pos_dir', type=str, default=None,
+                   help='--h_directions: images showing the attribute, the first --n_train_img of them by name, '
+                        'DDIM-inverted; the direction is the mean h of these minus the mean h of --h_neg_dir')
+    p.add_argument('--h_neg_dir', type=str, default=None,
+                   help='--h_directions: images without the attribute, the first --n_train_img of them by name')
+    p.add_argument('--h_direction_out', type=str, default=None, help='--h_directions: output directory')
+    p.add_argument('--h_direction', type=str, default=None,
+                   help='--run_test: edit with this direction file of --h_directions instead of a Δh checkpoint: '
+                        'h2 = hs_coeff_origin_h * h + α * d_t at every edit step, α = --hs_coeff_delta_h as given '
+                        '(not scaled by n_train_step / n_test_step: a direction has no training grid); with '
+                        '--delta_interpolation the rows are (1, v * α)')
     return p
 
 
@@ -192,9 +211,10 @@ def parse_args_and_config(argv=None):
 def main(argv=None):
     args, config = parse_args_and_config(argv)
     from .diffusion_latent import Asyrp
-    if args.lpips and int(os.environ.get("WORLD_SIZE", "1")) > 1:
-        logging.error("--lpips computes statistics over every image: run it single-process, not under torchrun")
-        return 1
+    for flag in ("lpips", "h_directions"):
+        if getattr(args, flag) and int(os.environ.get("WORLD_SIZE", "1")) > 1:
+            logging.error(f"--{flag} computes statistics over every image: run it single-process, not under torchrun")
+            return 1
     if int(os.environ.get("WORLD_SIZE", "1")) > 1:
         import torch.distributed as dist
         torch.cuda.set_device(int(os.environ.get("LOCAL_RANK", "0")))
@@ -203,12 +223,14 @@ def main(argv=None):
     try:
         if args.diff_style:
             runner.run_diff_style()
+        elif args.h_directions:
+            runner.run_h_directions()
         elif args.run_test:
             runner.run_test()
         elif args.lpips:
             runner.compute_lpips_distance()
         else:
-            print('Choose one mode! (this build implements --run_test, --lpips and --diff_style)')
+            print('Choose one mode! (this build implements --run_test, --lpips, --diff_style and --h_directions)')
             raise ValueError
     except Exception:
         logging.error(traceback.format_exc())

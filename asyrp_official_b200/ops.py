@@ -325,6 +325,65 @@ def slerp_h_rows(h, dh, h2, stats, t_rows, use_mask=False):
                                  _ptr(t_rows), int(use_mask), _stream()), "asyrp_slerp_h_rows")
 
 
+def add_h_rows(h, direction, h2, stats, coef):
+    """h2[n] = c0_n * h[n] + α_n * direction, each element fmaf(α_n, direction, c0_n * h) in fp32, stored as fp16:
+    h, h2 NHWC fp16 [N][H][W][C]; direction fp32 [C][H][W] (shared); stats [N][T][C/2][2] (slot 0 the sums of the fp32
+    values, the others zeroed); coef fp32 [N][2] = (c0_n, α_n) on the device (a graph input)"""
+    lib = _lib.load()
+    N, H, W, Cc = h.shape
+    _need_cuda(h, direction, h2, stats, coef)
+    if not (h.dtype == h2.dtype == torch.float16 and h.is_contiguous() and h2.is_contiguous()
+            and tuple(h2.shape) == tuple(h.shape)):
+        raise _lib.AsyrpError(f"add_h_rows: h and h2 must be contiguous fp16 NHWC tensors of one shape, got "
+                              f"{h.dtype} {tuple(h.shape)} / {h2.dtype} {tuple(h2.shape)}")
+    if not (direction.dtype == torch.float32 and direction.is_contiguous() and tuple(direction.shape) == (Cc, H, W)):
+        raise _lib.AsyrpError(f"add_h_rows: direction must be a contiguous fp32 [{Cc}][{H}][{W}] tensor, got "
+                              f"{direction.dtype} {tuple(direction.shape)}")
+    if not (coef.dtype == torch.float32 and coef.is_contiguous() and tuple(coef.shape) == (N, 2)):
+        raise _lib.AsyrpError(f"add_h_rows: coef must be a contiguous fp32 [{N}][2] device tensor, got "
+                              f"{coef.dtype} {tuple(coef.shape)}")
+    if not (stats.dtype == torch.float32 and stats.is_contiguous() and stats.dim() == 4
+            and tuple(stats.shape[:1]) + tuple(stats.shape[2:]) == (N, Cc // 2, 2)):
+        raise _lib.AsyrpError(f"add_h_rows: stats must be a contiguous fp32 [{N}][T][{Cc // 2}][2] tensor, got "
+                              f"{stats.dtype} {tuple(stats.shape)}")
+    check(lib.asyrp_add_h_rows(_ptr(h), _ptr(direction), _ptr(h2), _ptr(stats), stats.shape[1], N, Cc, H, W,
+                               _ptr(coef), _stream()), "asyrp_add_h_rows")
+
+
+def h_gram(x, mu):
+    """G fp64 [n][n] on the device: G[i][j] = sum_k (x[i][k] - mu[k]) (x[j][k] - mu[k]), the centred sample Gram of
+    x fp32 [n][d] with mu fp64 [d], each sum in feature order with fp64 fma"""
+    lib = _lib.load()
+    _need_cuda(x, mu)
+    if not (x.dtype == torch.float32 and x.dim() == 2 and x.is_contiguous()):
+        raise _lib.AsyrpError(f"h_gram: x must be a contiguous fp32 [n][d] tensor, got {x.dtype} {tuple(x.shape)}")
+    n, d = x.shape
+    if not (mu.dtype == torch.float64 and mu.is_contiguous() and tuple(mu.shape) == (d,)):
+        raise _lib.AsyrpError(f"h_gram: mu must be a contiguous fp64 [{d}] tensor, got {mu.dtype} {tuple(mu.shape)}")
+    G = torch.empty(max(n, 0), max(n, 0), dtype=torch.float64, device=x.device)
+    check(lib.asyrp_h_gram(_ptr(x), _ptr(mu), _ptr(G), n, d, _stream()), "asyrp_h_gram")
+    return G
+
+
+def h_combine(x, w, mu=None):
+    """out fp64 [K][d] on the device: out[k][j] = sum_r w[k][r] (x[r][j] - mu[j]) (mu None: 0), the rows r in order
+    with fp64 fma; x fp32 [n][d], w fp64 [K][n], mu fp64 [d]"""
+    lib = _lib.load()
+    _need_cuda(x, w, mu)
+    if not (x.dtype == torch.float32 and x.dim() == 2 and x.is_contiguous()):
+        raise _lib.AsyrpError(f"h_combine: x must be a contiguous fp32 [n][d] tensor, got {x.dtype} {tuple(x.shape)}")
+    n, d = x.shape
+    if not (w.dtype == torch.float64 and w.dim() == 2 and w.is_contiguous() and w.shape[1] == n):
+        raise _lib.AsyrpError(f"h_combine: w must be a contiguous fp64 [K][{n}] tensor, got {w.dtype} "
+                              f"{tuple(w.shape)}")
+    if mu is not None and not (mu.dtype == torch.float64 and mu.is_contiguous() and tuple(mu.shape) == (d,)):
+        raise _lib.AsyrpError(f"h_combine: mu must be a contiguous fp64 [{d}] tensor, got {mu.dtype} "
+                              f"{tuple(mu.shape)}")
+    out = torch.empty(w.shape[0], d, dtype=torch.float64, device=x.device)
+    check(lib.asyrp_h_combine(_ptr(x), _ptr(w), _ptr(mu), _ptr(out), n, d, w.shape[0], _stream()), "asyrp_h_combine")
+    return out
+
+
 def transpose_tc(inp, out):
     """inp [N][T][C] (may be a channel slice: last-dim stride 1, row stride ld) -> out [N][C][T] fp16"""
     lib = _lib.load()

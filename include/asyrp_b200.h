@@ -218,6 +218,14 @@ int asyrp_slerp_h(const void* h, const float* dh, long long dh_sample_stride, vo
 int asyrp_slerp_h_rows(const void* h, const float* dh, long long dh_sample_stride, void* h2, float* stats,
                        int stats_tiles, int N, int C, int H, int W, const float* t_rows, int use_mask, void* stream);
 
+/* Additive direction: h2[n] = c0_n * h[n] + alpha_n * dir, each element v = fmaf(alpha_n, dir, c0_n * h) in fp32
+ * (the product rounded first), stored as fp16.  h, h2: fp16 NHWC [N][H][W][C], h2 must not alias h; dir: fp32 NCHW
+ * [C][H][W] shared by every sample; coef: fp32 [N][2] = (c0_n, alpha_n) in device memory.  stats:
+ * [N][stats_tiles][C/2][2] partial sums of the fp32 v, filled as asyrp_slerp_h fills them (slot 0, the others zeroed).
+ * N >= 1, C even, C * H * W and stats_tiles * C at most 2^31 - 1.  Sample n's result does not depend on N. */
+int asyrp_add_h_rows(const void* h, const float* dir, void* h2, float* stats, int stats_tiles, int N, int C, int H,
+                     int W, const float* coef, void* stream);
+
 /* NHWC fp16 [N][HW][C] -> NCHW fp32 (API-visible delta_h / middle_h) */
 int asyrp_unpack_nchw(const void* in, float* out, int N, int C, int HW, void* stream);
 
@@ -457,6 +465,16 @@ int asyrp_preserve_sse(const unsigned char* src, const unsigned char* edited, lo
                        long long plane, void* stream);
 int asyrp_ssim_level(const double* src, const double* edited, double* stats, int n, int B, int H, int W, void* stream);
 int asyrp_ssim_pool2(const double* in, double* out, int rows, int H, int W, void* stream);
+
+/* Bottleneck statistics for h-space directions (csrc/hspace.cu), fp64, every sum in index order from 0:
+ * asyrp_h_gram: G fp64 [n][n], G[i][j] = sum_k (x[i][k] - mu[k]) (x[j][k] - mu[k]) over the d features, the centred
+ *   sample Gram (exactly symmetric); x fp32 [n][d], mu fp64 [d].  n >= 2, d > 0, n d < 2^31.
+ * asyrp_h_combine: out fp64 [K][d], out[k][j] = sum_r w[k][r] (x[r][j] - mu[j]) over the n rows; w fp64 [K][n]; mu
+ *   fp64 [d] or NULL (then 0).  n, d, K > 0; n d, K n and K d < 2^31.  Set means (w = 1/n), mean differences and
+ *   principal directions from Gram eigenvectors (w = u_k / sqrt(lambda_k)).
+ * No allocation, no synchronisation, no atomics. */
+int asyrp_h_gram(const float* x, const double* mu, double* G, int n, int d, void* stream);
+int asyrp_h_combine(const float* x, const double* w, const double* mu, double* out, int n, int d, int K, void* stream);
 
 #ifdef __cplusplus
 }

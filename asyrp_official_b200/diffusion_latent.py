@@ -5,33 +5,32 @@ Mirrors, with the same attribute / flag names:
   Asyrp.load_pretrained_model  :76-126                      dataset -> UNet family dispatch, load_state_dict(strict=False)
   Asyrp.run_test               :547-874                     sequences, Δh checkpoint, hs_coeff (single / multi-attribute /
                                                             interpolation sweep), batching of latents
-  Asyrp.save_image             :445-544                     the reverse loops + PNG grid
+  Asyrp.save_image             :445-544                     the reverse loops + PNG grid; with --attr_sweep one row
+                                                            schedule per attribute (run_attr_sweep)
   Asyrp.random_noise_pairs     :1087-1188                   x_T = N(0,1) per image
   Asyrp.set_t_edit_t_addnoise  :1308-1416                   user-defined values or LPIPS-table lookup given a cosine
                                                             (--clip_cosine, or CLIP's text cosine on the GPU)
   Asyrp.compute_lpips_distance :1191-1303                   --lpips: the LPIPS(x_t, x0) / LPIPS(x0_t, x0) tables of an
                                                             inversion, which set_t_edit_t_addnoise reads
-  --DirectionalClipSmilarity   main.py:101, losses/clip_loss.py  run_test scores every edit with CLIPLoss's directional
-                                                            similarity (clip_image.CLIPLoss), written next to the PNG
-  --id_similarity              losses/id_loss.py            run_test scores every edit with 1 - IDLoss (ArcFace IR-SE50,
-                                                            arcface.ArcFace), written next to the PNG; the reference
-                                                            uses IDLoss only in training
-  --seg_consistency            (none)                       run_test scores every edit with the segmentation consistency
-                                                            of a face-parsing BiSeNet (face_parsing.FaceParser), written
-                                                            next to the PNG; this build's definition
-  --fid                        (none)                       run_test scores each set of edits (one per hs_coeff tuple)
-                                                            against the origin pass with FID and KID on Inception-v3
-                                                            pool features (fid.FIDInception), gathered to rank 0 at the
-                                                            end of the run; this build's definition; with --fid_ref also
-                                                            the origin and each edited set against real images'
-                                                            statistics (fid.score_against_stats); with --prdc also
-                                                            precision / recall / density / coverage of the same sets
-                                                            from k-nearest-neighbour balls (fid.prdc)
-  --content_preservation       (none)                       run_test scores every edit with PSNR, SSIM, MS-SSIM and
-                                                            LPIPS-Alex against the origin pass of the same x_T
+  scoring.Scorers              main.py:101, losses/*.py     the edit scores of run_test and run_attr_sweep: each edit
+                                                            against the origin pass of the same x_T, written next to
+                                                            the PNG, and the sets of edits at the end of the run:
+    --DirectionalClipSmilarity                              CLIPLoss's directional similarity (clip_image.CLIPLoss)
+    --id_similarity                                         1 - IDLoss (ArcFace IR-SE50, arcface.ArcFace); the
+                                                            reference uses IDLoss only in training
+    --seg_consistency                                       segmentation consistency of a face-parsing BiSeNet
+                                                            (face_parsing.FaceParser); this build's definition
+    --content_preservation                                  PSNR, SSIM, MS-SSIM and LPIPS-Alex
                                                             (preservation.ContentPreservation), and the origin pass
-                                                            against the input image for inverted latents, written next
-                                                            to the PNG; this build's definition
+                                                            against the input image for inverted latents; this
+                                                            build's definition
+    --fid                                                   FID and KID of each set of edits (one per hs_coeff tuple)
+                                                            against the origin pass on Inception-v3 pool features
+                                                            (fid.FIDInception), gathered to rank 0 at the end of the
+                                                            run; this build's definition; with --fid_ref also against
+                                                            real images' statistics (fid.score_against_stats); with
+                                                            --prdc also precision / recall / density / coverage
+                                                            (fid.prdc)
   Asyrp.precompute_pairs_with_h :877-947                    DDIM inversion of one image keeping the bottleneck h of
                                                             every step (batched here, same cache file)
   Asyrp.run_diff_style         main.py:192-202              --diff_style (DiffStyle content injection): this build's
@@ -50,15 +49,16 @@ the collectives are the initial weight broadcast and, with --fid, the end-of-run
 0; each rank computes the CLIP cosine itself (the kernels are deterministic, so every rank picks the same t_edit).
 """
 import ast
-import math
 import os
 import time
 
 import numpy as np
 import torch
 
+from . import scoring
 from .modules import DDPM, guided_Diffusion, i_DDPM
 from .schedule import RowSchedule, Schedule, make_sequences
+from .scoring import write_fid, write_fid_real, write_prdc, write_scores  # noqa: F401  (the tables' former home)
 from .utils.diffusion_utils import get_beta_schedule
 
 
@@ -196,210 +196,28 @@ class Asyrp(object):
             raise ValueError(f"attribute {attr!r} is not in SRC_TRG_TXT_DIC")
         return list(dic[attr][0]), list(dic[attr][1])
 
+    # The score checks and the end of a --fid run live in scoring.py.  The runner keeps their names, and
+    # scoring.Scorers calls them through it, so that a caller who replaces one on the runner replaces it for the run.
     def directional_clip_setup(self, attrs=None):
-        """--DirectionalClipSmilarity's requirements, checked before any model is loaded; raises ValueError with the
-        reason.  Returns (src_txt, trg_txt, templates): src_txts[0] / trg_txts[0] of edit_texts(), the pair
-        run_training scores (diffusion_latent.py:343), and imagenet_templates from --text_templates.  With attrs (an
-        attribute sweep): ([(src_txt, trg_txt)] of every attribute, templates)."""
-        from .clip_image import read_templates
-        a = self.args
-        if getattr(a, "multiple_attr", ""):
-            raise ValueError("--DirectionalClipSmilarity scores one source / target text pair: a --multiple_attr edit "
-                             "has none")
-        if getattr(a, "pass_editing", False):
-            raise ValueError("--DirectionalClipSmilarity scores the edited images: with --pass_editing nothing is "
-                             "edited")
-        if not self.clip_configured():
-            raise ValueError("--DirectionalClipSmilarity needs --clip_weights and --clip_vocab")
-        for flag, path in (("--clip_weights", a.clip_weights), ("--clip_vocab", a.clip_vocab)):
-            if not os.path.isfile(path):
-                raise ValueError(f"--DirectionalClipSmilarity: {flag} {path!r} is not a file")
-        try:
-            templates = read_templates(getattr(a, "text_templates", None)
-                                       or os.path.join("utils", "text_templates.py"))
-        except FileNotFoundError as e:
-            raise ValueError(f"--DirectionalClipSmilarity: {e}") from None
-        if attrs is not None:
-            return [tuple(t[0] for t in self.edit_texts(attr)) for attr in attrs], templates
-        src, trg = self.edit_texts()
-        return src[0], trg[0], templates
-
-    def write_directional_clip(self, path, coeffs, s_dir):
-        """the TSV of one batch: one row per (hs_coeff tuple, image) in grid order, S_dir = 1 -
-        clip_directional_loss of that row; prints each tuple's mean"""
-        write_scores(path, coeffs, s_dir, "S_dir", "directional CLIP similarity")
+        return scoring.directional_clip_setup(self, attrs)
 
     def id_similarity_setup(self):
-        """--id_similarity's requirements, checked before any model is loaded; raises ValueError with the reason.
-        Returns the validated --id_weights state dict (arcface.load_state_dict)."""
-        from .arcface import check_image_size, load_state_dict
-        a = self.args
-        if getattr(a, "pass_editing", False):
-            raise ValueError("--id_similarity scores the edited images: with --pass_editing nothing is edited")
-        size = self.config.data.image_size
-        try:
-            check_image_size(size, size)
-        except ValueError as e:
-            raise ValueError(f"--id_similarity: {e}") from None
-        path = getattr(a, "id_weights", None)
-        if not path or not os.path.isfile(path):
-            raise ValueError(f"--id_similarity: --id_weights {path!r} is not a file (the reference's "
-                             "pretrained/model_ir_se50.pth)")
-        try:
-            return load_state_dict(path)
-        except ValueError as e:
-            raise ValueError(f"--id_similarity: {e}") from None
+        return scoring.id_similarity_setup(self)
 
     def seg_consistency_setup(self):
-        """--seg_consistency's requirements, checked before any model is loaded; raises ValueError with the reason.
-        Returns the validated --seg_weights state dict (face_parsing.load_state_dict)."""
-        from .face_parsing import load_state_dict
-        a = self.args
-        if getattr(a, "pass_editing", False):
-            raise ValueError("--seg_consistency scores the edited images: with --pass_editing nothing is edited")
-        path = getattr(a, "seg_weights", None)
-        if not path or not os.path.isfile(path):
-            raise ValueError(f"--seg_consistency: --seg_weights {path!r} is not a file (a torch.save of the face-parsing "
-                             "BiSeNet(n_classes=19) state dict, e.g. 79999_iter.pth)")
-        try:
-            return load_state_dict(path)
-        except ValueError as e:
-            raise ValueError(f"--seg_consistency: {e}") from None
-
-    def content_preservation_setup(self):
-        """--content_preservation's requirements, checked before any model is loaded; raises ValueError with the
-        reason.  Returns what ContentPreservation takes: the validated --lpips_weights path, or seeded weights with
-        --synthetic_weights (as load_lpips)."""
-        from .lpips import load_state_dict
-        from .preservation import check_image_size
-        a = self.args
-        if not getattr(a, "run_test", False) or getattr(a, "diff_style", False):
-            raise ValueError("--content_preservation scores the edits of --run_test (not --diff_style or --lpips)")
-        if getattr(a, "pass_editing", False):
-            raise ValueError("--content_preservation scores the edited images: with --pass_editing nothing is edited")
-        size = self.config.data.image_size
-        try:
-            check_image_size(size, size)
-        except ValueError as e:
-            raise ValueError(f"--content_preservation: {e}") from None
-        path = getattr(a, "lpips_weights", None)
-        if path:
-            if not os.path.isfile(path):
-                raise ValueError(f"--content_preservation: --lpips_weights {path!r} is not a file")
-            try:
-                load_state_dict(path)
-            except Exception as e:  # a file torch.load cannot read, or the wrong keys
-                raise ValueError(f"--content_preservation: --lpips_weights {path!r}: {e}") from None
-            return path
-        if getattr(a, "synthetic_weights", False):
-            from .synthetic import lpips_state_dict
-            return lpips_state_dict(seed=getattr(a, "seed", 1234))
-        raise ValueError("--content_preservation needs --lpips_weights (a torch.save of the lpips package's "
-                         "LPIPS(net='alex').state_dict()) or --synthetic_weights")
+        return scoring.seg_consistency_setup(self)
 
     def fid_setup(self):
-        """--fid's requirements, checked before any model is loaded; raises ValueError with the reason.  Returns the
-        validated --fid_weights state dict (fid.load_state_dict)."""
-        from .fid import load_state_dict, validate_stats
-        a = self.args
-        ref = getattr(a, "fid_ref", None)
-        if ref is not None:  # the headers only; rank 0 reads the arrays in finish_fid
-            if a.kid_subsets < 0 or a.kid_subset_size < 2:
-                raise ValueError(f"--fid_ref: --kid_subsets must be >= 0 and --kid_subset_size >= 2, got "
-                                 f"{a.kid_subsets} and {a.kid_subset_size}")
-            try:
-                validate_stats(ref)
-            except ValueError as e:
-                raise ValueError(f"--fid_ref: {e}") from None
-        if getattr(a, "pass_editing", False):
-            raise ValueError("--fid scores the edited images: with --pass_editing nothing is edited")
-        if getattr(a, "diff_style", False):
-            raise ValueError("--fid scores the sets of --run_test; --diff_style is not scored")
-        path = getattr(a, "fid_weights", None)
-        if not path or not os.path.isfile(path):
-            raise ValueError(f"--fid: --fid_weights {path!r} is not a file (pytorch-fid's "
-                             "pt_inception-2015-12-05-6726825d.pth)")
-        try:
-            return load_state_dict(path)
-        except ValueError as e:
-            raise ValueError(f"--fid: {e}") from None
+        return scoring.fid_setup(self)
+
+    def content_preservation_setup(self):
+        return scoring.content_preservation_setup(self)
 
     def prdc_check(self):
-        """--prdc's requirements, checked before any model is loaded; raises ValueError with the reason"""
-        a = self.args
-        if not getattr(a, "prdc", False):
-            return
-        if not getattr(a, "fid", False):
-            raise ValueError("--prdc scores the pool features that --fid collects: add --fid")
-        if not 1 <= a.prdc_k <= 32:
-            raise ValueError(f"--prdc: --prdc_k must be in 1..32, got {a.prdc_k}")
+        return scoring.prdc_check(self)
 
     def finish_fid(self, sets, coeffs, attrs=None):
-        """--fid at the end of a run: every rank's pool features (fid.FeatureSets) to rank 0, which sorts each set by
-        image index and scores every tuple's edited set against the origin set of the same pass: printed, kept in
-        self.fid[mode] and written to <test_image_folder>/<mode>_ngen<n_train_step>_fid.tsv.  Every rank must call it,
-        also one that ran no batch.  With --prdc also precision / recall / density / coverage from the same features
-        (_prdc.tsv, and _prdc_real.tsv against --fid_ref's features, whose radii are computed once)."""
-        from .fid import fid_kid, knn_radii, load_stats, prdc, score_against_stats, set_moments
-        a = self.args
-        pk = a.prdc_k if getattr(a, "prdc", False) else None
-        dist_on = self.world > 1 and torch.distributed.is_available() and torch.distributed.is_initialized()
-        got = sets.gather(self.rank, self.world if dist_on else 1)
-        if got is None:
-            return
-        real = None
-        if getattr(a, "fid_ref", None) is not None:  # --fid_ref: the real images' statistics, read once
-            real = load_stats(a.fid_ref)
-            if "features" in real:
-                real["features"] = torch.from_numpy(real["features"]).to(self.device)
-        real_radii = None  # --prdc --fid_ref: the real images' k-NN radii, for every set of both passes
-        if pk is not None and real is not None and real.get("features") is not None and real["features"].shape[0] > pk:
-            real_radii = knn_radii(real["features"], pk)
-        for mode in ("train", "test"):
-            if (mode, "origin") not in got:
-                continue
-            ids, ref = got[(mode, "origin")]
-            ref = ref.to(self.device).contiguous()
-            ref_moments = set_moments(ref) if ref.shape[0] >= 2 else None
-            rows, edited = [], []
-            for k in range(len(coeffs)):
-                ids_k, feats = got[(mode, k)]
-                if not torch.equal(ids_k, ids):
-                    raise RuntimeError(f"--fid: tuple {k} of the {mode} pass has other images than its origin set")
-                edited.append(feats.to(self.device).contiguous())
-                rows.append(fid_kid(ref, edited[-1], ref_moments))
-            self.fid[mode] = torch.tensor(rows, dtype=torch.float64)
-            os.makedirs(a.test_image_folder, exist_ok=True)
-            write_fid(os.path.join(a.test_image_folder, f"{mode}_ngen{a.n_train_step}_fid.tsv"), coeffs, rows,
-                      ref.shape[0], mode, attrs=attrs)
-            if real is not None:
-                real_rows = [score_against_stats(f, real, a.kid_subsets, a.kid_subset_size, m)
-                             for f, m in [(ref, ref_moments)] + [(e, None) for e in edited]]
-                self.fid_real[mode] = torch.tensor(real_rows, dtype=torch.float64)
-                n_ref = real["features"].shape[0] if "features" in real else None
-                write_fid_real(os.path.join(a.test_image_folder, f"{mode}_ngen{a.n_train_step}_fid_real.tsv"),
-                               coeffs, real_rows, ref.shape[0], n_ref, mode, attrs=attrs)
-            if pk is None:
-                continue
-            origin_radii = knn_radii(ref, pk) if ref.shape[0] > pk else None
-            prdc_rows = [prdc(ref, e, pk, origin_radii) for e in edited]
-            self.prdc[mode] = torch.tensor(prdc_rows, dtype=torch.float64)
-            write_prdc(os.path.join(a.test_image_folder, f"{mode}_ngen{a.n_train_step}_prdc.tsv"), coeffs, prdc_rows,
-                       ref.shape[0], None, mode, attrs=attrs)
-            if real is not None:
-                if "features" in real:
-                    prdc_rows = [prdc(real["features"], f, pk, real_radii) for f in [ref] + edited]
-                    n_ref = real["features"].shape[0]
-                else:
-                    prdc_rows, n_ref = [(math.nan,) * 4] * (1 + len(edited)), None
-                self.prdc_real[mode] = torch.tensor(prdc_rows, dtype=torch.float64)
-                write_prdc(os.path.join(a.test_image_folder, f"{mode}_ngen{a.n_train_step}_prdc_real.tsv"), coeffs,
-                           prdc_rows, ref.shape[0], n_ref, mode, attrs=attrs, real=True)
-
-    def write_id_similarity(self, path, coeffs, ids):
-        """the TSV of one batch: one row per (hs_coeff tuple, image) in grid order, ID = 1 - IDLoss(origin, edit) of
-        that row; prints each tuple's mean"""
-        write_scores(path, coeffs, ids, "ID", "identity similarity")
+        return scoring.finish_fid(self, sets, coeffs, attrs)
 
     @torch.no_grad()
     def clip_cosines(self, pairs):
@@ -580,41 +398,30 @@ class Asyrp(object):
     @torch.no_grad()
     def save_image(self, model, x_lat_tensor, seq_inv, seq_inv_next, save_x0=False, save_x_origin=False,
                    save_process_delta_h=False, save_process_origin=False, x0_tensor=None, delta_h_dict=None,
-                   get_delta_hs=False, folder_dir="", file_name="", hs_coeff=(1.0, 1.0), directional_clip=None,
-                   id_scorer=None, seg_scorer=None, fid=None, preservation=None, x0_source=None, h_direction=None):
+                   get_delta_hs=False, folder_dir="", file_name="", hs_coeff=(1.0, 1.0), h_direction=None,
+                   sweep_times=None, scorers=None, mode=None, batch_ids=None, x0_source=None):
         """rows of the grid: [x0] [origin DDIM] one row per hs_coeff tuple  (diffusion_latent.py:445-544).
 
         delta_h_dict: {t: None | Δh tensor}.  Entries that are tensors select the explicit-Δh branch for that step
         (raw-Δh checkpoints, mean Δh); get_delta_hs: run the DeltaBlocks and ADD their per-step output into
         delta_h_dict (mean-Δh extraction, :528-532).
-        directional_clip: (CLIPLoss, src_txt, trg_txt) for --DirectionalClipSmilarity: every tuple's edited rows are
-        scored against the origin pass of the same x_T (run for this even without save_x_origin, then left out of the
-        grid), written to <file_name>_ngen<n_train_step>_directional_clip.tsv and kept in
-        self.directional_clip[file_name].
-        id_scorer: an arcface.ArcFace for --id_similarity: the same for 1 - IDLoss against the same origin pass (which
-        runs once for both scores), written to <file_name>_ngen<n_train_step>_id_similarity.tsv and kept in
-        self.id_similarity[file_name].
-        seg_scorer: a face_parsing.FaceParser for --seg_consistency: the same for the segmentation consistency against
-        the same origin pass, written to <file_name>_ngen<n_train_step>_seg_consistency.tsv and kept in
-        self.seg_consistency[file_name].
-        fid: (fid.FIDInception, fid.FeatureSets, mode, image index of every row) for --fid: the pool features of the
-        origin pass and of each tuple's edits are added to their sets (finish_fid scores them at the end of the run).
-        preservation: a preservation.ContentPreservation for --content_preservation: (PSNR, SSIM, MS_SSIM, LPIPS) of
-        every edit against the same origin pass, and with x0_source (the input images the latents were inverted from)
-        of the origin pass against them; written to <file_name>_ngen<n_train_step>_content_preservation.tsv and kept in
-        self.content_preservation[file_name] / self.reconstruction[file_name].
         h_direction: a direction file (hspace.load_direction) for --h_direction: each tuple is (c0, α) and its rows take
-        h2 = c0 h + α d_t at every edit step, every tuple a row block of one batch as for DeltaBlocks."""
+        h2 = c0 h + α d_t at every edit step, every tuple a row block of one batch as for DeltaBlocks.
+        sweep_times (--attr_sweep): tuple k is attribute k, its rows run with its own (t_edit, t_addnoise)
+        sweep_times[k] (sweep_schedule); rows (attribute, image), attribute-major, in chunks of whole attributes of at
+        most --max_rows_per_replay rows.
+        scorers: a scoring.Scorers, which scores every tuple's edits against the origin pass of the same x_T (run for
+        this even without save_x_origin, then left out of the grid); mode, batch_ids (the image index of every row)
+        and x0_source (the input images the latents were inverted from) are passed on to Scorers.score."""
         import torchvision.utils as tvu
         a = self.args
         time_s = time.time()
         eng = model.engine
         bs = x_lat_tensor.shape[0]
-        x_list, edited = [], []
+        x_list, origin = [], None
         if save_x0 and x0_tensor is not None:
             x_list.append(x0_tensor.cpu())
-        if save_x_origin or directional_clip is not None or id_scorer is not None or seg_scorer is not None or \
-                fid is not None or preservation is not None:
+        if save_x_origin or (scorers is not None and scorers.needs_origin):
             sch = self.make_schedule(seq_inv, seq_inv_next, (1.0,), edit=False,
                                      addnoise=bool(getattr(a, "origin_process_addnoise", False)))
             if save_x_origin:
@@ -625,8 +432,17 @@ class Asyrp(object):
             else:  # the pass only the score needs leaves the random stream as it was: the edits draw the same noise
                 with torch.random.fork_rng(devices=[eng.device]):
                     origin = self.edit_batch(model, x_lat_tensor, sch)
-        if not getattr(a, "pass_editing", False):
-            coeffs = hs_coeff if isinstance(hs_coeff, list) else [hs_coeff]
+        coeffs = hs_coeff if isinstance(hs_coeff, list) else [hs_coeff]
+        edited = []
+        if sweep_times is not None:
+            tpc, chunks = plan_sweep(len(coeffs), bs, getattr(a, "max_rows_per_replay", 16))
+            for chunk in chunks:
+                rows = sweep_rows(chunk, tpc, bs)
+                sch = self.sweep_schedule(seq_inv, seq_inv_next, [sweep_times[k] for k in rows],
+                                          [coeffs[k] for k in rows])
+                x0 = self.edit_batch(model, pad_rows(x_lat_tensor.repeat(len(chunk), 1, 1, 1), tpc * bs), sch)
+                edited += [x0[j * bs:(j + 1) * bs].clone() for j in range(len(chunk))]
+        elif not getattr(a, "pass_editing", False):
             # the reference replays the trajectory once per tuple (:495-532); the tuples share x_T and the schedule, so
             # they run as rows of one batch (tuples x images), each row with its own hs_coeff, in chunks of whole tuples
             # of at most --max_rows_per_replay rows.  A sample's result does not depend on its batch neighbours, so
@@ -679,9 +495,7 @@ class Asyrp(object):
                                          dtype=torch.float32)
                     kw["hs_coeffs"] = pad_rows(table, tpc * bs)
                 x0 = self.edit_batch(model, rows_x, sch, noise=noise, record_process=save_process_delta_h, **kw)
-                for j in range(len(chunk)):
-                    x_list.append(x0[j * bs:(j + 1) * bs].clone())
-                    edited.append(x_list[-1])
+                edited += [x0[j * bs:(j + 1) * bs].clone() for j in range(len(chunk))]
                 if save_process_delta_h and chunk is chunks[-1]:  # each tuple rewrote these files: the last one stays
                     j = len(chunk) - 1
                     self._write_process(eng, sch, os.path.join(folder_dir, file_name), "delta_h", bs,
@@ -692,48 +506,14 @@ class Asyrp(object):
                         for ei, t in enumerate(edit_ts):
                             r = rec[ei][j * bs:(j + 1) * bs]
                             delta_h_dict[int(t)] = r if delta_h_dict.get(int(t)) is None else delta_h_dict[int(t)] + r
-        x = (torch.cat(x_list, dim=0) + 1) * 0.5
-        grid = tvu.make_grid(x, nrow=a.bs_train, padding=1)
+        x_list += edited
         os.makedirs(folder_dir, exist_ok=True)
-        path = os.path.join(folder_dir, f'{file_name}_ngen{a.n_train_step}.png')
-        tvu.save_image(grid, path)
-        if directional_clip is not None and edited:
-            clip_loss, src_txt, trg_txt = directional_clip
-            s_dir = clip_loss.directional_similarity(origin, src_txt, torch.cat(edited), trg_txt).view(len(edited), bs)
-            self.directional_clip[file_name] = s_dir
-            self.write_directional_clip(
-                os.path.join(folder_dir, f'{file_name}_ngen{a.n_train_step}_directional_clip.tsv'), coeffs, s_dir)
-        if id_scorer is not None and edited:
-            ids = id_scorer.id_similarity(origin, torch.cat(edited)).view(len(edited), bs)
-            self.id_similarity[file_name] = ids
-            self.write_id_similarity(
-                os.path.join(folder_dir, f'{file_name}_ngen{a.n_train_step}_id_similarity.tsv'), coeffs, ids)
-        if seg_scorer is not None and edited:
-            sc = seg_scorer.seg_consistency(origin, torch.cat(edited)).view(len(edited), bs)
-            self.seg_consistency[file_name] = sc
-            write_scores(os.path.join(folder_dir, f'{file_name}_ngen{a.n_train_step}_seg_consistency.tsv'), coeffs, sc,
-                         "SC", "segmentation consistency")
-        if fid is not None and edited:
-            add_fid_features(fid, origin, edited)
-        if preservation is not None and edited:
-            self.score_preservation(preservation, origin, edited, x0_source, coeffs, os.path.join(
-                folder_dir, f'{file_name}_ngen{a.n_train_step}_content_preservation.tsv'), file_name)
+        tvu.save_image(tvu.make_grid((torch.cat(x_list, dim=0) + 1) * 0.5, nrow=a.bs_train, padding=1),
+                       os.path.join(folder_dir, f'{file_name}_ngen{a.n_train_step}.png'))
+        if scorers is not None:
+            scorers.score(file_name, folder_dir, mode, batch_ids, origin, edited, coeffs, x0_source)
         print(f'{time.time() - time_s} seconds, {file_name}_ngen{a.n_train_step}.png is saved')
         return x_list
-
-    def score_preservation(self, preservation, origin, edited, x0_source, coeffs, path, file_name, attrs=None):
-        """--content_preservation of one batch: every tuple's edits (edited[k]) against the origin pass, and the origin
-        pass against x0_source when given; kept in self.content_preservation / self.reconstruction and written to
-        `path` (write_scores, the reconstruction rows first)"""
-        from .preservation import COLUMNS
-        bs = origin.shape[0]
-        cp = preservation.scores(origin, torch.cat(edited)).view(len(edited), bs, len(COLUMNS))
-        self.content_preservation[file_name] = cp
-        rec = None
-        if x0_source is not None:
-            rec = preservation.scores(x0_source, origin)
-            self.reconstruction[file_name] = rec
-        write_scores(path, coeffs, cp, COLUMNS, "content preservation", attrs=attrs, origin=rec)
 
     # ------------------------------------------------------------------------------------------
     def load_lpips(self):
@@ -831,12 +611,39 @@ class Asyrp(object):
             save_name = save_name[:-4] + f'_{a.choose_checkpoint_num}.pth'
         return save_name
 
+    def _batches(self, pairs, keep_source):
+        """this rank's batches of the latents of run_test and run_attr_sweep (:779-874): (mode, step, x_T, x0, image
+        indices, x0_source) per batch of the [x0, x_rec, x_T] triples of pairs[mode], step the last image's index.
+        Images before --start_image_id or outside --target_image_id are left out but count towards the batch boundary
+        (step + 1) % bs_train; the batches go round-robin to the ranks, every batch counted; a pass ends at its last
+        image (n_train_img / n_test_img).  x0 with --use_x0_tensor, x0_source (the images the latents were inverted
+        from) with keep_source, else None."""
+        a = self.args
+        target_ids = [int(i) for i in str(a.target_image_id).split(" ")] if getattr(a, "target_image_id", None) \
+            else None
+        for mode, do, n_img in (("train", a.do_train, a.n_train_img), ("test", a.do_test, a.n_test_img)):
+            if not do:
+                continue
+            batch, batch_idx = [], 0
+            for step, (x0, _, x_lat) in enumerate(pairs[mode]):
+                if (target_ids is not None and step not in target_ids) or a.start_image_id > step:
+                    continue
+                batch.append((step, x0, x_lat))
+                if (step + 1) % a.bs_train != 0:
+                    continue
+                if batch_idx % self.world == self.rank:  # batch-sharded across ranks, no per-step communication
+                    x0s = torch.cat([x for _, x, _ in batch])
+                    yield (mode, step, torch.cat([x for _, _, x in batch]), x0s if a.use_x0_tensor else None,
+                           [i for i, _, _ in batch], x0s if keep_source else None)
+                batch_idx += 1
+                if step == n_img - 1:
+                    break
+                batch = []
+
     @torch.no_grad()
     def run_test(self):
         a = self.args
-        if getattr(a, "fid_ref", None) is not None and not getattr(a, "fid", False):
-            raise ValueError("--fid_ref scores the sets that --fid collects: add --fid")
-        self.prdc_check()
+        scoring.fid_options_check(self)
         h_dir_path = self.h_direction_setup()  # refuses --attr_sweep too, before it is dispatched
         if getattr(a, "attr_sweep", ""):
             return self.run_attr_sweep()
@@ -844,11 +651,7 @@ class Asyrp(object):
         if getattr(a, "warigari", 0.0):
             print("--warigari is accepted and has no effect (the reference's branch returns the same values, "
                   "utils/diffusion_utils.py:103-109)")
-        sdir = self.directional_clip_setup() if getattr(a, "DirectionalClipSmilarity", False) else None
-        id_sd = self.id_similarity_setup() if getattr(a, "id_similarity", False) else None
-        seg_sd = self.seg_consistency_setup() if getattr(a, "seg_consistency", False) else None
-        fid_sd = self.fid_setup() if getattr(a, "fid", False) else None
-        cp_sd = self.content_preservation_setup() if getattr(a, "content_preservation", False) else None
+        scorers = scoring.Scorers(self)
         if a.multiple_attr and self.needs_clip() and self.clip_configured():
             cosine = self.choose_attribute(a.multiple_attr.split(' '))  # :640-652
             self.set_t_edit_t_addnoise(LPIPS_th=a.lpips_edit_th, LPIPS_addnoise_th=a.lpips_addnoise_th, cosine=cosine)
@@ -960,63 +763,21 @@ class Asyrp(object):
             pairs = self.random_noise_pairs(model, saved_noise=bool(getattr(a, "saved_random_noise", False)))
         else:
             pairs = self.precompute_pairs(model)
-        target_ids = None
         if getattr(a, "target_image_id", None):
-            target_ids = [int(i) for i in str(a.target_image_id).split(" ")]
             assert a.bs_train == 1, "target_image_id is only supported for batch_size == 1"
-        results, directional_clip, id_scorer, seg_scorer, fid_net, preservation = {}, None, None, None, None, None
-        if sdir is not None:  # the image tower lives for this run_test only
-            from .clip_image import CLIPLoss
-            directional_clip = (CLIPLoss(a.clip_weights, a.clip_vocab, sdir[2], device=self.device), sdir[0], sdir[1])
+        results = {}
         try:
-            if id_sd is not None:  # so does ArcFace
-                from .arcface import ArcFace
-                id_scorer = ArcFace(id_sd, device=self.device)
-                id_sd = None
-            if seg_sd is not None:  # and the face parser
-                from .face_parsing import FaceParser
-                seg_scorer = FaceParser(seg_sd, device=self.device)
-                seg_sd = None
-            if fid_sd is not None:  # and Inception-v3, whose features are collected over the whole run
-                from .fid import FeatureSets, FIDInception
-                fid_net, fid_sets = FIDInception(fid_sd, device=self.device), FeatureSets()
-                fid_sd = None
-            if cp_sd is not None:  # and LPIPS-Alex
-                from .preservation import ContentPreservation
-                preservation = ContentPreservation(cp_sd, device=self.device)
-                cp_sd = None
-            for mode, do, n_img in (("train", a.do_train, a.n_train_img), ("test", a.do_test, a.n_test_img)):
-                if not do:
-                    continue
-                x_lat_tensor, x0_tensor, batch_idx, batch_ids, x0_source = None, None, 0, [], None
-                for step, (x0, _, x_lat) in enumerate(pairs[mode]):
-                    if target_ids is not None and step not in target_ids:
-                        continue
-                    if a.start_image_id > step:
-                        continue
-                    x_lat_tensor = x_lat if x_lat_tensor is None else torch.cat((x_lat_tensor, x_lat), dim=0)
-                    batch_ids.append(step)
-                    if a.use_x0_tensor:
-                        x0_tensor = x0 if x0_tensor is None else torch.cat((x0_tensor, x0), dim=0)
-                    if preservation is not None and not a.load_random_noise:  # the images the latents came from
-                        x0_source = x0 if x0_source is None else torch.cat((x0_source, x0), dim=0)
-                    if (step + 1) % a.bs_train != 0:
-                        continue
-                    if batch_idx % self.world == self.rank:  # batch-sharded across ranks, no per-step communication
-                        results[(mode, step)] = self.save_image(
-                            model, x_lat_tensor, seq_test, seq_test_next, save_x0=a.save_x0,
-                            save_x_origin=a.save_x_origin, x0_tensor=x0_tensor, delta_h_dict=delta_h_dict,
-                            get_delta_hs=bool(num_mean),
-                            save_process_origin=bool(getattr(a, "save_process_origin", False)),
-                            save_process_delta_h=bool(getattr(a, "save_process_delta_h", False)),
-                            folder_dir=a.test_image_folder, file_name=f'{mode}_{step}_{a.n_iter - 1}', hs_coeff=hs_coeff,
-                            directional_clip=directional_clip, id_scorer=id_scorer, seg_scorer=seg_scorer,
-                            fid=None if fid_net is None else (fid_net, fid_sets, mode, batch_ids),
-                            preservation=preservation, x0_source=x0_source, h_direction=h_direction)
-                    batch_idx += 1
-                    if step == n_img - 1:
-                        break
-                    if mode == "train" and num_mean and step == num_mean - 1:
+            with scorers:
+                for mode, step, x_lat, x0, ids, x0_source in self._batches(pairs, scorers.keeps_source):
+                    results[(mode, step)] = self.save_image(
+                        model, x_lat, seq_test, seq_test_next, save_x0=a.save_x0, save_x_origin=a.save_x_origin,
+                        x0_tensor=x0, delta_h_dict=delta_h_dict, get_delta_hs=bool(num_mean),
+                        save_process_origin=bool(getattr(a, "save_process_origin", False)),
+                        save_process_delta_h=bool(getattr(a, "save_process_delta_h", False)),
+                        folder_dir=a.test_image_folder, file_name=f'{mode}_{step}_{a.n_iter - 1}', hs_coeff=hs_coeff,
+                        h_direction=h_direction, scorers=scorers, mode=mode, batch_ids=ids, x0_source=x0_source)
+                    # the last image of the pass ends it before the mean is taken
+                    if mode == "train" and num_mean and step == num_mean - 1 and step != a.n_train_img - 1:
                         # mean over the first num_mean images per timestep, key 0 = mean over timesteps (:811-832)
                         for k in delta_h_dict:
                             if delta_h_dict[k] is not None:
@@ -1033,15 +794,9 @@ class Asyrp(object):
                         print(f'Dict: {latent_name} is saved.')
                         num_mean = 0
                         print("now we use mean of delta_hs")
-                    x_lat_tensor, x0_tensor, batch_ids, x0_source = None, None, [], None
-            if fid_net is not None:
-                self.finish_fid(fid_sets, hs_coeff if isinstance(hs_coeff, list) else [hs_coeff])
+                scorers.finish(hs_coeff if isinstance(hs_coeff, list) else [hs_coeff])
         finally:
             a.train_delta_h = a_train_delta_h_prev
-            if directional_clip is not None or id_scorer is not None or seg_scorer is not None or fid_net is not None \
-                    or preservation is not None:
-                del directional_clip, id_scorer, seg_scorer, fid_net, preservation
-                torch.cuda.empty_cache()
         self.last_delta_h_dict = delta_h_dict
         return results
 
@@ -1217,13 +972,7 @@ class Asyrp(object):
         a = self.args
         print("Running Test (attribute sweep)")
         attrs, paths = self.attr_sweep_setup()
-        sdir = None
-        if getattr(a, "DirectionalClipSmilarity", False):
-            sdir = self.directional_clip_setup(attrs)
-        id_sd = self.id_similarity_setup() if getattr(a, "id_similarity", False) else None
-        seg_sd = self.seg_consistency_setup() if getattr(a, "seg_consistency", False) else None
-        fid_sd = self.fid_setup() if getattr(a, "fid", False) else None
-        cp_sd = self.content_preservation_setup() if getattr(a, "content_preservation", False) else None
+        scorers = scoring.Scorers(self, attrs)
         times = self.attr_sweep_schedules(attrs)
         self.sweep_times = dict(zip(attrs, times))
         seq_test = [int(s + 1e-6) for s in list(np.linspace(0, 1, a.n_test_step) * a.t_0)]
@@ -1249,63 +998,14 @@ class Asyrp(object):
             pairs = self.random_noise_pairs(model, saved_noise=bool(getattr(a, "saved_random_noise", False)))
         else:
             pairs = self.precompute_pairs(model)
-        target_ids = [int(i) for i in str(a.target_image_id).split(" ")] if getattr(a, "target_image_id", None) \
-            else None
-        results, directional_clip, id_scorer, seg_scorer, fid_net, preservation = {}, None, None, None, None, None
-        if sdir is not None:
-            from .clip_image import CLIPLoss
-            directional_clip = (CLIPLoss(a.clip_weights, a.clip_vocab, sdir[1], device=self.device), sdir[0])
-        try:
-            if id_sd is not None:
-                from .arcface import ArcFace
-                id_scorer = ArcFace(id_sd, device=self.device)
-                id_sd = None
-            if seg_sd is not None:
-                from .face_parsing import FaceParser
-                seg_scorer = FaceParser(seg_sd, device=self.device)
-                seg_sd = None
-            if fid_sd is not None:
-                from .fid import FeatureSets, FIDInception
-                fid_net, fid_sets = FIDInception(fid_sd, device=self.device), FeatureSets()
-                fid_sd = None
-            if cp_sd is not None:
-                from .preservation import ContentPreservation
-                preservation = ContentPreservation(cp_sd, device=self.device)
-                cp_sd = None
-            for mode, do, n_img in (("train", a.do_train, a.n_train_img), ("test", a.do_test, a.n_test_img)):
-                if not do:
-                    continue
-                x_lat_tensor, x0_tensor, batch_idx, batch_ids, x0_source = None, None, 0, [], None
-                for step, (x0, _, x_lat) in enumerate(pairs[mode]):
-                    if (target_ids is not None and step not in target_ids) or a.start_image_id > step:
-                        continue
-                    x_lat_tensor = x_lat if x_lat_tensor is None else torch.cat((x_lat_tensor, x_lat), dim=0)
-                    batch_ids.append(step)
-                    if a.use_x0_tensor:
-                        x0_tensor = x0 if x0_tensor is None else torch.cat((x0_tensor, x0), dim=0)
-                    if preservation is not None and not a.load_random_noise:
-                        x0_source = x0 if x0_source is None else torch.cat((x0_source, x0), dim=0)
-                    if (step + 1) % a.bs_train != 0:
-                        continue
-                    if batch_idx % self.world == self.rank:  # batch-sharded across ranks, as run_test
-                        results[(mode, step)] = self.save_image_sweep(
-                            model, x_lat_tensor, seq_test, seq_test_next, attrs, times, coeffs, save_x0=a.save_x0,
-                            save_x_origin=a.save_x_origin, x0_tensor=x0_tensor,
-                            folder_dir=a.test_image_folder, file_name=f'{mode}_{step}_{a.n_iter - 1}',
-                            directional_clip=directional_clip, id_scorer=id_scorer, seg_scorer=seg_scorer,
-                            fid=None if fid_net is None else (fid_net, fid_sets, mode, batch_ids),
-                            preservation=preservation, x0_source=x0_source)
-                    batch_idx += 1
-                    if step == n_img - 1:
-                        break
-                    x_lat_tensor, x0_tensor, batch_ids, x0_source = None, None, [], None
-            if fid_net is not None:
-                self.finish_fid(fid_sets, coeffs, attrs=attrs)
-        finally:
-            if directional_clip is not None or id_scorer is not None or seg_scorer is not None or fid_net is not None \
-                    or preservation is not None:
-                del directional_clip, id_scorer, seg_scorer, fid_net, preservation
-                torch.cuda.empty_cache()
+        results = {}
+        with scorers:
+            for mode, step, x_lat, x0, ids, x0_source in self._batches(pairs, scorers.keeps_source):
+                results[(mode, step)] = self.save_image(
+                    model, x_lat, seq_test, seq_test_next, save_x0=a.save_x0, save_x_origin=a.save_x_origin,
+                    x0_tensor=x0, folder_dir=a.test_image_folder, file_name=f'{mode}_{step}_{a.n_iter - 1}',
+                    hs_coeff=coeffs, sweep_times=times, scorers=scorers, mode=mode, batch_ids=ids, x0_source=x0_source)
+            scorers.finish(coeffs)
         return results
 
     def sweep_schedule(self, seq, seq_next, times, coeffs):
@@ -1316,71 +1016,6 @@ class Asyrp(object):
                            hs_coeffs=coeffs, sample_type=getattr(a, "sample_type", "ddim"),
                            dt_lambda=getattr(a, "dt_lambda", 1.0), dt_end=999,
                            ignore_timestep=bool(getattr(a, "ignore_timesteps", False)), logvars=self.logvar)
-
-    @torch.no_grad()
-    def save_image_sweep(self, model, x_lat_tensor, seq_inv, seq_inv_next, attrs, times, coeffs, save_x0=False,
-                         save_x_origin=False, x0_tensor=None, folder_dir="", file_name="", directional_clip=None,
-                         id_scorer=None, seg_scorer=None, fid=None, preservation=None, x0_source=None):
-        """save_image for an attribute sweep: grid rows [x0] [origin DDIM] then one row per attribute in the order
-        given.  Rows of the trajectory are (attribute, image), attribute-major, run in chunks of whole attributes of
-        at most --max_rows_per_replay rows (sweep_chunks).  directional_clip = (CLIPLoss, [(src_txt, trg_txt)] per
-        attribute): each attribute's rows are scored with its own texts.  The score TSVs name the attribute of each
-        row in an appended `attr` column; `tuple` is the attribute's index."""
-        import torchvision.utils as tvu
-        a = self.args
-        time_s = time.time()
-        eng = model.engine
-        bs = x_lat_tensor.shape[0]
-        x_list, edited, origin = [], [], None
-        if save_x0 and x0_tensor is not None:
-            x_list.append(x0_tensor.cpu())
-        if save_x_origin or directional_clip is not None or id_scorer is not None or seg_scorer is not None or \
-                fid is not None or preservation is not None:
-            sch = self.make_schedule(seq_inv, seq_inv_next, (1.0,), edit=False,
-                                     addnoise=bool(getattr(a, "origin_process_addnoise", False)))
-            if save_x_origin:
-                origin = self.edit_batch(model, x_lat_tensor, sch)
-                x_list.append(origin)
-            else:
-                with torch.random.fork_rng(devices=[eng.device]):
-                    origin = self.edit_batch(model, x_lat_tensor, sch)
-        tpc, chunks = plan_sweep(len(attrs), bs, getattr(a, "max_rows_per_replay", 16))
-        for chunk in chunks:
-            rows = sweep_rows(chunk, tpc, bs)
-            sch = self.sweep_schedule(seq_inv, seq_inv_next, [times[k] for k in rows], [coeffs[k] for k in rows])
-            rows_x = pad_rows(x_lat_tensor.repeat(len(chunk), 1, 1, 1), tpc * bs)
-            x0 = self.edit_batch(model, rows_x, sch)
-            for j in range(len(chunk)):
-                x_list.append(x0[j * bs:(j + 1) * bs].clone())
-                edited.append(x_list[-1])
-        x = (torch.cat(x_list, dim=0) + 1) * 0.5
-        grid = tvu.make_grid(x, nrow=a.bs_train, padding=1)
-        os.makedirs(folder_dir, exist_ok=True)
-        tvu.save_image(grid, os.path.join(folder_dir, f'{file_name}_ngen{a.n_train_step}.png'))
-        if directional_clip is not None:
-            clip_loss, texts = directional_clip
-            s_dir = torch.stack([clip_loss.directional_similarity(origin, texts[k][0], edited[k], texts[k][1]).view(bs)
-                                 for k in range(len(attrs))])
-            self.directional_clip[file_name] = s_dir
-            write_scores(os.path.join(folder_dir, f'{file_name}_ngen{a.n_train_step}_directional_clip.tsv'), coeffs,
-                         s_dir, "S_dir", "directional CLIP similarity", attrs=attrs)
-        if id_scorer is not None:
-            ids = id_scorer.id_similarity(origin, torch.cat(edited)).view(len(edited), bs)
-            self.id_similarity[file_name] = ids
-            write_scores(os.path.join(folder_dir, f'{file_name}_ngen{a.n_train_step}_id_similarity.tsv'), coeffs,
-                         ids, "ID", "identity similarity", attrs=attrs)
-        if seg_scorer is not None:
-            sc = seg_scorer.seg_consistency(origin, torch.cat(edited)).view(len(edited), bs)
-            self.seg_consistency[file_name] = sc
-            write_scores(os.path.join(folder_dir, f'{file_name}_ngen{a.n_train_step}_seg_consistency.tsv'), coeffs,
-                         sc, "SC", "segmentation consistency", attrs=attrs)
-        if fid is not None:
-            add_fid_features(fid, origin, edited)
-        if preservation is not None:
-            self.score_preservation(preservation, origin, edited, x0_source, coeffs, os.path.join(
-                folder_dir, f'{file_name}_ngen{a.n_train_step}_content_preservation.tsv'), file_name, attrs=attrs)
-        print(f'{time.time() - time_s} seconds, {file_name}_ngen{a.n_train_step}.png is saved')
-        return x_list
 
     # ------------------------------------------------------------------------------------------
     def diff_style_setup(self):
@@ -1601,101 +1236,6 @@ def sweep_rows(chunk, tpc, bs):
     tpc * bs rows with the last attribute (padding rows are discarded)"""
     rows = [k for k in chunk for _ in range(bs)]
     return rows + [rows[-1]] * (tpc * bs - len(rows))
-
-def write_scores(path, coeffs, scores, column, label, attrs=None, origin=None):
-    """a per-edit score table: one row per (hs_coeff tuple, image) in grid order, columns image, tuple, hs_coeff and
-    `column`; prints each tuple's mean as `label`.  attrs (an attribute sweep): tuple k is attribute k, named in an
-    appended `attr` column.  Several columns: `column` a sequence of names and scores [tuples][images][columns].
-    origin ([images][columns]): rows of the origin pass first, with tuple `origin`, hs_coeff `-` (and attr `-`)"""
-    columns = [column] if isinstance(column, str) else list(column)
-    tail = (lambda a: f"\t{a}") if attrs is not None else (lambda a: "")
-
-    def cells(v):
-        return "\t".join(repr(x) for x in (v if isinstance(v, list) else [v]))
-    with open(path, "w") as f:
-        f.write("image\ttuple\ths_coeff\t" + "\t".join(columns) + tail("attr") + "\n")
-        if origin is not None:
-            for i, v in enumerate(origin.tolist()):
-                f.write(f"{i}\torigin\t-\t{cells(v)}" + tail("-") + "\n")
-        for k, row in enumerate(scores.tolist()):
-            tup = ",".join(f"{float(c):.6g}" for c in coeffs[k])
-            for i, v in enumerate(row):
-                f.write(f"{i}\t{k}\t{tup}\t{cells(v)}" + tail(attrs[k] if attrs is not None else None) + "\n")
-    rows = ([("origin", origin)] if origin is not None else []) + [
-        (f"attribute {attrs[k]}" if attrs is not None else f"hs_coeff {tuple(float(c) for c in coeffs[k])}", row)
-        for k, row in enumerate(scores)]
-    for name, row in rows:
-        means = row.double().reshape(row.shape[0], -1).mean(0).tolist()
-        vals = f"{means[0]:.6f}" if len(columns) == 1 else ", ".join(f"{c} {m:.6f}" for c, m in zip(columns, means))
-        print(f"{label}, {name}: mean {vals} over {row.shape[0]} images")
-
-
-def add_fid_features(fid, origin, edited):
-    """--fid: the pool features of a batch's origin rows and of each tuple's edited rows (edited[k]), added to their
-    sets with the batch's image indices; fid = (FIDInception, FeatureSets, mode, image indices)"""
-    net, sets, mode, ids = fid
-    bs = origin.shape[0]
-    feats = net.features(torch.cat([origin.cpu()] + [e.cpu() for e in edited]))
-    sets.add(mode, "origin", ids, feats[:bs])
-    for k in range(len(edited)):
-        sets.add(mode, k, ids, feats[(k + 1) * bs:(k + 2) * bs])
-
-
-def write_fid(path, coeffs, rows, n, mode, attrs=None):
-    """the FID / KID table of one pass: one row per hs_coeff tuple, columns tuple, hs_coeff, n (images per set), FID and
-    KID (`attr` appended under an attribute sweep); prints each tuple's values"""
-    with open(path, "w") as f:
-        f.write("tuple\ths_coeff\tn\tFID\tKID" + ("\tattr" if attrs is not None else "") + "\n")
-        for k, (fd, kd) in enumerate(rows):
-            tup = ",".join(f"{float(c):.6g}" for c in coeffs[k])
-            f.write(f"{k}\t{tup}\t{n}\t{fd!r}\t{kd!r}" + (f"\t{attrs[k]}" if attrs is not None else "") + "\n")
-    for k, (fd, kd) in enumerate(rows):
-        name = f"attribute {attrs[k]}" if attrs is not None else f"hs_coeff {tuple(float(c) for c in coeffs[k])}"
-        print(f"FID / KID ({mode}, {n} images), {name}: FID {fd:.6f}, KID {kd:.6f}")
-
-
-def write_fid_real(path, coeffs, rows, n, n_ref, mode, attrs=None):
-    """the table of one pass against real images' statistics (--fid_ref): rows[0] the origin set (tuple `origin`,
-    hs_coeff `-`), rows[1 + k] tuple k's set, each (FID, KID, KID_mean, KID_std); columns tuple, hs_coeff, n (images
-    per set), n_ref (reference images; `-` for a file without features), FID, KID, KID_mean, KID_std, and `attr` under
-    an attribute sweep; values as write_fid writes them.  Prints each row's values"""
-    names = [("origin", "-", "-")] + [(str(k), ",".join(f"{float(c):.6g}" for c in coeffs[k]),
-                                        attrs[k] if attrs is not None else None) for k in range(len(coeffs))]
-    nr = "-" if n_ref is None else str(n_ref)
-    with open(path, "w") as f:
-        f.write("tuple\ths_coeff\tn\tn_ref\tFID\tKID\tKID_mean\tKID_std" + ("\tattr" if attrs is not None else "") +
-                "\n")
-        for (key, tup, attr), vals in zip(names, rows):
-            f.write(f"{key}\t{tup}\t{n}\t{nr}\t" + "\t".join(repr(float(v)) for v in vals) +
-                    (f"\t{attr}" if attrs is not None else "") + "\n")
-    for k, (fd, kd, km, ks) in enumerate(rows):
-        name = "origin" if k == 0 else (f"attribute {attrs[k - 1]}" if attrs is not None
-                                        else f"hs_coeff {tuple(float(c) for c in coeffs[k - 1])}")
-        print(f"FID / KID against the real images ({mode}, {n} images, {nr} reference), {name}: FID {fd:.6f}, "
-              f"KID {kd:.6f}, subset KID {km:.6f} +- {ks:.6f}")
-
-
-def write_prdc(path, coeffs, rows, n, n_ref, mode, attrs=None, real=False):
-    """the precision / recall / density / coverage table of one pass (--prdc): one row per hs_coeff tuple, columns
-    tuple, hs_coeff, n (images per set), precision, recall, density, coverage (`attr` appended under an attribute
-    sweep), values as write_fid writes them.  real (--fid_ref): rows[0] is the origin set (tuple `origin`, hs_coeff
-    `-`) and an n_ref column (reference images; `-` for a file without features) follows n.  Prints each row"""
-    names = [(str(k), ",".join(f"{float(c):.6g}" for c in coeffs[k]), attrs[k] if attrs is not None else None)
-             for k in range(len(coeffs))]
-    if real:
-        names = [("origin", "-", "-")] + names
-    nr = "-" if n_ref is None else str(n_ref)
-    with open(path, "w") as f:
-        f.write("tuple\ths_coeff\tn" + ("\tn_ref" if real else "") + "\tprecision\trecall\tdensity\tcoverage" +
-                ("\tattr" if attrs is not None else "") + "\n")
-        for (key, tup, attr), vals in zip(names, rows):
-            f.write(f"{key}\t{tup}\t{n}" + (f"\t{nr}" if real else "") + "\t" +
-                    "\t".join(repr(float(v)) for v in vals) + (f"\t{attr}" if attrs is not None else "") + "\n")
-    against = f"against the real images ({mode}, {n} images, {nr} reference)" if real else f"({mode}, {n} images)"
-    for (key, tup, attr), (p, r, d, c) in zip(names, rows):
-        name = "origin" if key == "origin" else (f"attribute {attr}" if attrs is not None else f"hs_coeff ({tup})")
-        print(f"precision / recall / density / coverage {against}, {name}: P {p:.6f}, R {r:.6f}, D {d:.6f}, "
-              f"C {c:.6f}")
 
 
 def plan_sweep(n_tuples, bs, max_rows):

@@ -118,6 +118,7 @@ def test_folding_is_exact_algebra():
 
 def test_cli_rejections_come_before_any_model_load(tmp_path, monkeypatch):
     from asyrp_official_b200 import main as cli
+    from asyrp_official_b200 import scoring
     from asyrp_official_b200.diffusion_latent import Asyrp
     monkeypatch.chdir(tmp_path)
     sd = synthetic.arcface_state_dict(seed=1)
@@ -146,11 +147,11 @@ def test_cli_rejections_come_before_any_model_load(tmp_path, monkeypatch):
     assert args.id_weights == "pretrained/model_ir_se50.pth" and not args.id_similarity
     # --multiple_attr needs no text pair: accepted
     args, cfg = cli.parse_args_and_config(base + ["--id_weights", "ir_se50.pth", "--multiple_attr", "smiling old"])
-    assert set(Asyrp(args, cfg, device="cpu").id_similarity_setup()) == set(arcface.state_dict_shapes())
+    assert set(scoring.id_similarity_setup(Asyrp(args, cfg, device="cpu"))) == set(arcface.state_dict_shapes())
 
 
 def test_score_table_layout(tmp_path):
-    from asyrp_official_b200.diffusion_latent import write_scores
+    from asyrp_official_b200.scoring import write_scores
     ids = torch.tensor([[0.5, 0.25], [0.75, 1.0], [0.125, 0.0]])
     coeffs = [(1.0, 0.5), (1.0, 1.0), (1.0, 1.5)]
     write_scores(str(tmp_path / "t.tsv"), coeffs, ids, "ID", "identity similarity")

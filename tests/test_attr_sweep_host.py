@@ -8,7 +8,8 @@ import pytest
 import torch
 
 from asyrp_official_b200 import _lib, engine, main as cli
-from asyrp_official_b200.diffusion_latent import Asyrp, plan_sweep, sweep_rows, write_scores
+from asyrp_official_b200.diffusion_latent import Asyrp, plan_sweep, sweep_rows
+from asyrp_official_b200.scoring import write_scores
 from asyrp_official_b200.schedule import RowSchedule, Schedule, make_sequences
 from oracle import sampler as osmp
 

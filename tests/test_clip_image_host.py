@@ -143,6 +143,7 @@ def test_templates_are_parsed_not_executed(tmp_path):
 
 def test_cli_rejections_come_before_any_model_load(tmp_path, monkeypatch):
     from asyrp_official_b200 import main as cli
+    from asyrp_official_b200 import scoring
     from asyrp_official_b200.diffusion_latent import Asyrp
     monkeypatch.chdir(tmp_path)
     os.makedirs("utils")
@@ -173,7 +174,8 @@ def test_cli_rejections_come_before_any_model_load(tmp_path, monkeypatch):
             Asyrp(args, cfg, device="cpu").run_test()
     args, cfg = cli.parse_args_and_config(base + clip)
     assert args.DirectionalClipSmilarity and args.text_templates is None
-    assert Asyrp(args, cfg, device="cpu").directional_clip_setup() == ("face", "smiling face", ["a photo of a {}."])
+    assert scoring.directional_clip_setup(Asyrp(args, cfg, device="cpu")) == ("face", "smiling face",
+                                                                           ["a photo of a {}."])
 
 
 def test_oracle_text_direction_uses_every_template(tmp_path):

@@ -180,7 +180,7 @@ def test_cli_rejections_come_before_any_model_load(tmp_path, monkeypatch):
 
 
 def test_fid_table_layout(tmp_path, capsys):
-    from asyrp_official_b200.diffusion_latent import write_fid
+    from asyrp_official_b200.scoring import write_fid
     rows = [(12.5, 0.25), (float("nan"), float("nan")), (0.1 + 0.2, 1e-17)]
     coeffs = [(1.0, 0.5), (1.0, 1.0), (1.0, 1.5)]
     write_fid(str(tmp_path / "t.tsv"), coeffs, rows, 40, "test")

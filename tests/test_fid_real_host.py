@@ -186,7 +186,7 @@ def test_image_files_are_pytorch_fids(tmp_path):
 
 
 def test_fid_real_table_layout(tmp_path, capsys):
-    from asyrp_official_b200.diffusion_latent import write_fid_real
+    from asyrp_official_b200.scoring import write_fid_real
     nan = float("nan")
     rows = [(1.5, 0.25, 0.125, 0.01), (12.5, 0.5, nan, nan), (0.1 + 0.2, 1e-17, 2.0, 0.0)]
     write_fid_real(str(tmp_path / "t.tsv"), [(1.0, 0.5), (1.0, 1.5)], rows, 40, 30000, "test")

@@ -121,7 +121,7 @@ def test_nan_and_a_warning_for_sets_of_k_rows_or_fewer():
 
 
 def test_cli_refusals_come_before_any_model_load(tmp_path, monkeypatch):
-    from asyrp_official_b200 import main as cli
+    from asyrp_official_b200 import main as cli, scoring
     from asyrp_official_b200.diffusion_latent import Asyrp
     monkeypatch.chdir(tmp_path)
 
@@ -129,7 +129,7 @@ def test_cli_refusals_come_before_any_model_load(tmp_path, monkeypatch):
         raise AssertionError("a model was loaded before the requirements were checked")
     monkeypatch.setattr(Asyrp, "load_pretrained_model", fail_load)
     monkeypatch.setattr(Asyrp, "set_t_edit_t_addnoise", fail_load)
-    monkeypatch.setattr(Asyrp, "fid_setup", fail_load)  # --prdc is checked before --fid's own requirements
+    monkeypatch.setattr(scoring, "fid_setup", fail_load)  # --prdc is checked before --fid's own requirements
     base = ["--run_test", "--config", "celeba.yml"]
     fid_argv = ["--fid", "--fid_weights", "missing.pth"]
     cases = [(["--prdc"], "add --fid"),
@@ -148,11 +148,11 @@ def test_cli_refusals_come_before_any_model_load(tmp_path, monkeypatch):
     assert args.prdc is False and args.prdc_k == 5
     for k in (1, 32):  # the bounds themselves pass the check
         args, cfg = cli.parse_args_and_config(base + fid_argv + ["--prdc", "--prdc_k", str(k)])
-        Asyrp(args, cfg, device="cpu").prdc_check()
+        scoring.prdc_check(Asyrp(args, cfg, device="cpu"))
 
 
 def test_prdc_table_layout(tmp_path, capsys):
-    from asyrp_official_b200.diffusion_latent import write_prdc
+    from asyrp_official_b200.scoring import write_prdc
     nan = float("nan")
     rows = [(0.5, 1.0, 1.0, 0.5), (0.1 + 0.2, nan, 1e-17, 0.0)]
     write_prdc(str(tmp_path / "t.tsv"), [(1.0, 0.5), (1.0, 1.5)], rows, 40, None, "test")
@@ -171,7 +171,7 @@ def test_prdc_table_layout(tmp_path, capsys):
 
 
 def test_prdc_real_table_layout(tmp_path, capsys):
-    from asyrp_official_b200.diffusion_latent import write_prdc
+    from asyrp_official_b200.scoring import write_prdc
     rows = [(0.25, 0.5, 0.75, 1.0), (0.5, 1.0, 1.0, 0.5), (0.0, 0.0, 0.0, 0.0)]
     write_prdc(str(tmp_path / "r.tsv"), [(1.0, 0.5), (1.0, 1.5)], rows, 40, 30000, "test", real=True)
     lines = (tmp_path / "r.tsv").read_text().splitlines()

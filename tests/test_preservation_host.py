@@ -147,6 +147,7 @@ def test_image_size_limit():
 
 def test_cli_rejections_come_before_any_model_load(tmp_path, monkeypatch):
     from asyrp_official_b200 import main as cli
+    from asyrp_official_b200 import scoring
     from asyrp_official_b200.diffusion_latent import Asyrp
     monkeypatch.chdir(tmp_path)
     sd = synthetic.lpips_state_dict(seed=1)
@@ -175,15 +176,15 @@ def test_cli_rejections_come_before_any_model_load(tmp_path, monkeypatch):
             r.compute_lpips_distance() if args.lpips else r.run_test()
     args, cfg = cli.parse_args_and_config(base + ["--lpips_weights", "alex.pth"])  # no --run_test
     with pytest.raises(ValueError, match="scores the edits of --run_test"):
-        Asyrp(args, cfg, device="cpu").content_preservation_setup()
+        scoring.content_preservation_setup(Asyrp(args, cfg, device="cpu"))
     args, cfg = cli.parse_args_and_config(base + ["--run_test", "--lpips_weights", "alex.pth"])
     cfg.data.image_size = 160
     with pytest.raises(ValueError, match="larger than 160"):
-        Asyrp(args, cfg, device="cpu").content_preservation_setup()
+        scoring.content_preservation_setup(Asyrp(args, cfg, device="cpu"))
     cfg.data.image_size = 256
-    assert Asyrp(args, cfg, device="cpu").content_preservation_setup() == "alex.pth"
+    assert scoring.content_preservation_setup(Asyrp(args, cfg, device="cpu")) == "alex.pth"
     args, cfg = cli.parse_args_and_config(base + ["--run_test", "--synthetic_weights"])
-    got = Asyrp(args, cfg, device="cpu").content_preservation_setup()
+    got = scoring.content_preservation_setup(Asyrp(args, cfg, device="cpu"))
     assert set(got) == set(sd) and all(torch.equal(got[k], synthetic.lpips_state_dict(seed=1234)[k]) for k in got)
     args, _ = cli.parse_args_and_config(["--run_test", "--config", "celeba.yml"])
     assert not args.content_preservation and args.lpips_weights is None
@@ -204,7 +205,7 @@ def test_diff_style_refuses_the_flag(tmp_path, monkeypatch):
 
 
 def test_score_table_layout(tmp_path, capsys):
-    from asyrp_official_b200.diffusion_latent import write_scores
+    from asyrp_official_b200.scoring import write_scores
     g = torch.Generator().manual_seed(2)
     cp = torch.rand(3, 2, 4, generator=g, dtype=torch.float64)
     cp[0, 1, 0] = float("inf")

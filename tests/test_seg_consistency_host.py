@@ -160,6 +160,7 @@ def test_oracle_seg_consistency_pairs_rows_modulo_the_sources():
 
 def test_cli_rejections_come_before_any_model_load(tmp_path, monkeypatch):
     from asyrp_official_b200 import main as cli
+    from asyrp_official_b200 import scoring
     from asyrp_official_b200.diffusion_latent import Asyrp
     monkeypatch.chdir(tmp_path)
     sd = synthetic.face_parsing_state_dict(seed=1)
@@ -186,11 +187,11 @@ def test_cli_rejections_come_before_any_model_load(tmp_path, monkeypatch):
     args, _ = cli.parse_args_and_config(["--run_test", "--config", "celeba.yml"])
     assert args.seg_weights == "pretrained/79999_iter.pth" and not args.seg_consistency
     args, cfg = cli.parse_args_and_config(base + ["--seg_weights", "79999_iter.pth", "--multiple_attr", "smiling old"])
-    assert set(Asyrp(args, cfg, device="cpu").seg_consistency_setup()) == set(fp.state_dict_shapes())
+    assert set(scoring.seg_consistency_setup(Asyrp(args, cfg, device="cpu"))) == set(fp.state_dict_shapes())
 
 
 def test_score_table_layout(tmp_path):
-    from asyrp_official_b200.diffusion_latent import write_scores
+    from asyrp_official_b200.scoring import write_scores
     sc = torch.tensor([[0.5, 0.25], [0.75, 1.0], [0.125, 0.0]], dtype=torch.float64)
     coeffs = [(1.0, 0.5), (1.0, 1.0), (1.0, 1.5)]
     write_scores(str(tmp_path / "t.tsv"), coeffs, sc, "SC", "segmentation consistency")

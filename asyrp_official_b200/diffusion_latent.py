@@ -399,7 +399,7 @@ class Asyrp(object):
     def save_image(self, model, x_lat_tensor, seq_inv, seq_inv_next, save_x0=False, save_x_origin=False,
                    save_process_delta_h=False, save_process_origin=False, x0_tensor=None, delta_h_dict=None,
                    get_delta_hs=False, folder_dir="", file_name="", hs_coeff=(1.0, 1.0), h_direction=None,
-                   sweep_times=None, scorers=None, mode=None, batch_ids=None, x0_source=None):
+                   sweep_times=None, scorers=None, mode=None, batch_ids=None, x0_source=None, edit_region=None):
         """rows of the grid: [x0] [origin DDIM] one row per hs_coeff tuple  (diffusion_latent.py:445-544).
 
         delta_h_dict: {t: None | Δh tensor}.  Entries that are tensors select the explicit-Δh branch for that step
@@ -412,7 +412,11 @@ class Asyrp(object):
         most --max_rows_per_replay rows.
         scorers: a scoring.Scorers, which scores every tuple's edits against the origin pass of the same x_T (run for
         this even without save_x_origin, then left out of the grid); mode, batch_ids (the image index of every row)
-        and x0_source (the input images the latents were inverted from) are passed on to Scorers.score."""
+        and x0_source (the input images the latents were inverted from) are passed on to Scorers.score.
+        edit_region (--edit_region): (FaceParser, class indices, dilate r, feather sigma).  The origin pass then records
+        x_t after every step and always runs; its x0 is parsed into one soft mask per image (region.region_masks),
+        written as <file>_ngen<n>_region_mask.png, and every step of the edit pass ends with x <- m x + (1 - m) x_orig
+        (UNetEngine.sample's blend), so that outside the region the edits follow the origin pass."""
         import torchvision.utils as tvu
         a = self.args
         time_s = time.time()
@@ -421,17 +425,28 @@ class Asyrp(object):
         x_list, origin = [], None
         if save_x0 and x0_tensor is not None:
             x_list.append(x0_tensor.cpu())
-        if save_x_origin or (scorers is not None and scorers.needs_origin):
+        blend = None
+        if save_x_origin or (scorers is not None and scorers.needs_origin) or edit_region is not None:
             sch = self.make_schedule(seq_inv, seq_inv_next, (1.0,), edit=False,
                                      addnoise=bool(getattr(a, "origin_process_addnoise", False)))
             if save_x_origin:
-                origin = self.edit_batch(model, x_lat_tensor, sch, record_process=save_process_origin)
+                origin = self.edit_batch(model, x_lat_tensor, sch,
+                                         record_process=save_process_origin or edit_region is not None)
                 x_list.append(origin)
                 if save_process_origin:
                     self._write_process(eng, sch, os.path.join(folder_dir, file_name), "origin", bs)
             else:  # the pass only the score needs leaves the random stream as it was: the edits draw the same noise
                 with torch.random.fork_rng(devices=[eng.device]):
-                    origin = self.edit_batch(model, x_lat_tensor, sch)
+                    origin = self.edit_batch(model, x_lat_tensor, sch, record_process=edit_region is not None)
+            if edit_region is not None:
+                from .region import region_masks
+                ref = eng.last_records["x"].clone()  # owned by the origin graph: the edit replays would reuse it
+                parser, classes, r, sigma = edit_region
+                mask = region_masks(parser, origin, classes, r, sigma).to(eng.device)
+                blend = (mask, ref)
+                os.makedirs(folder_dir, exist_ok=True)
+                tvu.save_image(tvu.make_grid(mask[:, None].cpu(), nrow=a.bs_train, padding=1),
+                               os.path.join(folder_dir, f'{file_name}_ngen{a.n_train_step}_region_mask.png'))
         coeffs = hs_coeff if isinstance(hs_coeff, list) else [hs_coeff]
         edited = []
         if sweep_times is not None:
@@ -470,6 +485,8 @@ class Asyrp(object):
                 dirs = direction_rows(h_direction, edit_ts)
                 if dirs is not None:
                     kw["h_direction"] = dirs
+            if blend is not None:  # rows are tuple-major blocks of the bs images: row n blends with image n % bs
+                kw["blend"] = blend
             max_rows = getattr(a, "max_rows_per_replay", 16)
             if "delta_hs" in kw and len({float(tup[0]) for tup in coeffs}) > 1:
                 max_rows = 0  # explicit Δh takes one slerp weight 1 - c0 per replay: one tuple per chunk
@@ -559,6 +576,7 @@ class Asyrp(object):
         the others run bs_train per replay (every row's distances equal its batch-1 run bit for bit)."""
         import torchvision.utils as tvu
         a = self.args
+        self.edit_region_setup()  # refuses --lpips
         if getattr(a, "content_preservation", False):
             self.content_preservation_setup()  # refuses --lpips
         if self.world > 1:
@@ -644,6 +662,7 @@ class Asyrp(object):
     def run_test(self):
         a = self.args
         scoring.fid_options_check(self)
+        region_spec = self.edit_region_setup()  # refuses --attr_sweep too, before it is dispatched
         h_dir_path = self.h_direction_setup()  # refuses --attr_sweep too, before it is dispatched
         if getattr(a, "attr_sweep", ""):
             return self.run_attr_sweep()
@@ -768,6 +787,12 @@ class Asyrp(object):
         results = {}
         try:
             with scorers:
+                edit_region = None
+                if region_spec is not None:  # --seg_consistency's parser serves the masks too
+                    from .face_parsing import FaceParser
+                    classes, r, sigma, seg_sd = region_spec
+                    region_spec = None
+                    edit_region = (scorers.nets.get("seg") or FaceParser(seg_sd, device=self.device), classes, r, sigma)
                 for mode, step, x_lat, x0, ids, x0_source in self._batches(pairs, scorers.keeps_source):
                     results[(mode, step)] = self.save_image(
                         model, x_lat, seq_test, seq_test_next, save_x0=a.save_x0, save_x_origin=a.save_x_origin,
@@ -775,7 +800,8 @@ class Asyrp(object):
                         save_process_origin=bool(getattr(a, "save_process_origin", False)),
                         save_process_delta_h=bool(getattr(a, "save_process_delta_h", False)),
                         folder_dir=a.test_image_folder, file_name=f'{mode}_{step}_{a.n_iter - 1}', hs_coeff=hs_coeff,
-                        h_direction=h_direction, scorers=scorers, mode=mode, batch_ids=ids, x0_source=x0_source)
+                        h_direction=h_direction, scorers=scorers, mode=mode, batch_ids=ids, x0_source=x0_source,
+                        edit_region=edit_region)
                     # the last image of the pass ends it before the mean is taken
                     if mode == "train" and num_mean and step == num_mean - 1 and step != a.n_train_img - 1:
                         # mean over the first num_mean images per timestep, key 0 = mean over timesteps (:811-832)
@@ -795,6 +821,7 @@ class Asyrp(object):
                         num_mean = 0
                         print("now we use mean of delta_hs")
                 scorers.finish(hs_coeff if isinstance(hs_coeff, list) else [hs_coeff])
+                edit_region = None  # the parser goes with the scorers' networks, and the CUDA cache after it
         finally:
             a.train_delta_h = a_train_delta_h_prev
         self.last_delta_h_dict = delta_h_dict
@@ -802,6 +829,31 @@ class Asyrp(object):
 
 
     # ------------------------------------------------------------------------------------------
+    def edit_region_setup(self):
+        """--edit_region's requirements, checked before any model loads: None without the flag, else (class indices,
+        --edit_region_dilate, --edit_region_feather, the --seg_weights state dict).  ValueError with the reason."""
+        from . import region
+        a = self.args
+        text = getattr(a, "edit_region", None)
+        if not text:
+            return None
+        if not getattr(a, "run_test", False):
+            raise ValueError("--edit_region restricts the edits of --run_test: add --run_test")
+        for flag, on, why in (
+                ("--attr_sweep", getattr(a, "attr_sweep", ""), "its rows follow per-row schedules"),
+                ("--diff_style", getattr(a, "diff_style", False), "it is not a --run_test edit"),
+                ("--lpips", getattr(a, "lpips", False), "it edits nothing"),
+                ("--h_directions", getattr(a, "h_directions", False), "it edits nothing"),
+                ("--pass_editing", getattr(a, "pass_editing", False), "nothing is edited"),
+                ("--num_mean_of_delta_hs", getattr(a, "num_mean_of_delta_hs", 0),
+                 "the mean Δh must come from the unmasked pass")):
+            if on:
+                raise ValueError(f"--edit_region does not combine with {flag}: {why}")
+        classes = region.parse_classes(text)
+        r, sigma = getattr(a, "edit_region_dilate", 0), getattr(a, "edit_region_feather", 0.0)
+        region.check_options(r, sigma, self.config.data.image_size)
+        return classes, r, float(sigma), scoring.seg_weights(self, "--edit_region")
+
     def h_direction_setup(self):
         """--h_direction's requirements, checked before any model loads: the path (None without the flag); ValueError
         when it is combined with a flag that selects another source of Δh"""
@@ -857,6 +909,7 @@ class Asyrp(object):
         keep_h: keep that buffer as self.h_directions_x (otherwise it is released when the run ends)."""
         from . import hspace
         a = self.args
+        self.edit_region_setup()  # refuses --h_directions
         mode, arg = self.h_directions_setup()
         seq, seq_next = make_sequences(a.t_0, a.n_test_step)
         size = self.config.data.image_size
@@ -1110,6 +1163,7 @@ class Asyrp(object):
         import torchvision.utils as tvu
         a = self.args
         self.prdc_check()
+        self.edit_region_setup()  # refuses --diff_style
         if getattr(a, "content_preservation", False):
             self.content_preservation_setup()  # refuses --diff_style
         if getattr(a, "fid", False):

@@ -941,8 +941,9 @@ class UNetEngine:
     MAX_GRAPHS = 4  # captured trajectory graphs kept per engine (least recently used is dropped)
 
     def _build_trajectory(self, P, schedule, use_graph, explicit, record_dh, record_process, lpips=None,
-                          record_h=False, additive=False):
-        """per-(batch, schedule) state: the timestep-embedding table, the noise buffer, the step loop and its graph"""
+                          record_h=False, additive=False, blend_B=0):
+        """per-(batch, schedule) state: the timestep-embedding table, the noise buffer, the step loop and its graph.
+        blend_B: the images of a region blend (0: none); the graph then owns its mask and reference trajectory"""
         steps = schedule.steps
         n_sto = schedule.n_stochastic
         zbuf = torch.zeros((max(n_sto, 1), *P.x.shape), dtype=torch.float32, device=self.device)
@@ -971,6 +972,10 @@ class UNetEngine:
             rec["x0_t"] = torch.zeros((len(steps), *P.x.shape), dtype=torch.float32, device=self.device)
         if record_h:  # the bottleneck h of every step (precompute_pairs_with_h's h_dic, diffusion_latent.py:931-939)
             rec["h"] = torch.zeros((len(steps), *P.mid_f32.shape), dtype=torch.float32, device=self.device)
+        if blend_B:   # region blend: one mask per image and the origin pass's x after every step, filled before a replay
+            rec["blend_mask"] = torch.zeros((blend_B, *P.x.shape[2:]), dtype=torch.float32, device=self.device)
+            rec["blend_ref"] = torch.zeros((len(steps), blend_B, *P.x.shape[1:]), dtype=torch.float32,
+                                           device=self.device)
         N = P.x.shape[0]
         if lpips is not None:
             # LPIPS(x_t, x_start) and LPIPS(x0_t, x_start) after every step (compute_lpips_distance,
@@ -1024,12 +1029,14 @@ class UNetEngine:
                 else:
                     x0_out = rec["x0_t"][k] if record_process else (xs[N:] if lpips is not None else None)
                     ops.ddim_update(P.x, P.et, P.et_mod if edit else P.et, z, P.x, x0_out, s.at, s.an, s.c1, s.c2)
+                if blend_B:  # x <- m x + (1 - m) x_orig,k: outside the region the step ends on the origin pass
+                    ops.blend_rows(P.x, rec["blend_ref"][k], rec["blend_mask"])
                 if record_process:
                     rec["x"][k].copy_(P.x)
                 if lpips is not None:
                     lpips_step(k)
 
-        n_launch = sum(len(P.launches(False, temb=False)) + 1 + int(record_h) for s in steps)
+        n_launch = sum(len(P.launches(False, temb=False)) + 1 + int(record_h) + int(bool(blend_B)) for s in steps)
         n_launch += n_edit * ((len(P.slerp_ops) if explicit else (1 if additive else len(P.delta_ops))) +
                               len(P.dec_mod_ops) + int(record_dh))
         if lpips is not None:
@@ -1054,6 +1061,8 @@ class UNetEngine:
                 if lpips is not None:
                     x_start = lpips.features(P.x, "start")
                     lpips_step(0)
+                if blend_B:
+                    ops.blend_rows(P.x, rec["blend_ref"][0], rec["blend_mask"])
             torch.cuda.current_stream().wait_stream(s_)
             torch.cuda.synchronize(self.device)
             cg = torch.cuda.CUDAGraph()
@@ -1178,8 +1187,34 @@ class UNetEngine:
             out.copy_(P.x)
             return out
 
+    def _check_blend(self, blend, x_T, schedule, lpips):
+        """the number of images B of a blend=(mask, ref) argument; AsyrpError unless it fits the batch and the schedule"""
+        if lpips is not None:
+            raise ops._lib.AsyrpError("blend= does not combine with lpips=")
+        try:
+            mask, ref = blend
+        except (TypeError, ValueError):
+            raise ops._lib.AsyrpError("blend must be a pair (mask [B][H][W], ref [steps][B][C][H][W])") from None
+        N, Cx, H, W = x_T.shape
+        steps = len(schedule.steps)
+        if not (torch.is_tensor(mask) and torch.is_tensor(ref) and mask.dtype == ref.dtype == torch.float32):
+            raise ops._lib.AsyrpError("blend: mask and ref must be fp32 tensors")
+        B = mask.shape[0] if mask.dim() == 3 else 0
+        if not B or tuple(mask.shape) != (B, H, W) or N % B:
+            raise ops._lib.AsyrpError(f"blend: mask must be [B][{H}][{W}] with the batch of {N} rows a multiple of B, "
+                                      f"got {tuple(mask.shape)}")
+        if tuple(ref.shape) != (steps, B, Cx, H, W):
+            raise ops._lib.AsyrpError(f"blend: ref must be [{steps} steps][{B}][{Cx}][{H}][{W}], got {tuple(ref.shape)}")
+        cur = torch.cuda.current_device()
+        idx = lambda d: d.index if d.index is not None else cur  # noqa: E731
+        for name, t in (("mask", mask), ("ref", ref)):
+            if not t.is_cuda or idx(t.device) != idx(self.device):
+                raise ops._lib.AsyrpError(f"blend: {name} lives on {t.device}, the engine on {self.device}")
+        return B
+
     def sample(self, x_T, schedule, noise=None, use_graph=True, out=None, delta_hs=None, use_mask=False,
-               record_dh=False, record_process=False, hs_coeffs=None, lpips=None, record_h=False, h_direction=None):
+               record_dh=False, record_process=False, hs_coeffs=None, lpips=None, record_h=False, h_direction=None,
+               blend=None):
         """Run the reverse trajectory of `schedule` (sampler.Schedule) from x_T; returns x_0 (fp32 NCHW).
 
         The step list, the edit/plain/stochastic phase of every step and all sampler coefficients are host-side
@@ -1219,12 +1254,19 @@ class UNetEngine:
         step h2 = c0_n * h + α_n * h_direction[step] (ops.add_h_rows) feeds the edited decoder, with hs_coeffs the
         per-sample (c0, α) table, fp32 [N][2], required.  Like the DeltaBlock coefficients the table and the directions
         are graph inputs: every table replays one graph, and sample n equals a batch-1 run with row n bit for bit.
-        The engine must pack no DeltaBlocks; delta_hs, record_dh and lpips do not combine with it."""
+        The engine must pack no DeltaBlocks; delta_hs, record_dh and lpips do not combine with it.
+
+        blend: (mask fp32 [B][H][W], ref fp32 [steps][B][C][H][W]) restricts the edit to a region (region.py): after
+        every step's update, before anything is recorded, row n becomes x = fmaf(m, x, (1 - m) * ref[k][n % B]) with
+        m = mask[n % B] (ops.blend_rows), N a multiple of B.  ref is the origin pass's x after every step (its
+        record_process "x").  Mask and reference are graph inputs, copied in before every replay: every batch of B
+        images replays one graph.  A mask of ones gives the unblended trajectory and a mask of zeros ref[-1], bit for
+        bit.  It does not combine with lpips."""
         if isinstance(schedule, RowSchedule):
             if delta_hs is not None or record_dh or hs_coeffs is not None or lpips is not None or record_h or \
-                    h_direction is not None:
+                    h_direction is not None or blend is not None:
                 raise ops._lib.AsyrpError("a per-row schedule takes no delta_hs, record_dh, hs_coeffs, lpips, "
-                                          "record_h or h_direction")
+                                          "record_h, h_direction or blend")
             return self._sample_rows(x_T, schedule, noise, use_graph, out, record_process)
         N = x_T.shape[0]
         additive = h_direction is not None
@@ -1240,6 +1282,7 @@ class UNetEngine:
                 raise ops._lib.AsyrpError(f"h_direction needs hs_coeffs, a float [{N}][2] table of (c0, α) per sample, "
                                           f"got {None if add_table is None else (add_table.dtype, tuple(add_table.shape))}")
             hs_coeffs = None  # (c0, α) are add_h_rows' table, not DeltaBlock coefficients
+        blend_B = self._check_blend(blend, x_T, schedule, lpips) if blend is not None else 0
         P = self.plan(N)
         explicit = delta_hs is not None
         table = coeff_table(hs_coeffs, N, self.n_delta) if hs_coeffs is not None else None
@@ -1254,7 +1297,8 @@ class UNetEngine:
             slerp_t = 0.0
         key = (N, bool(use_graph), schedule.key(), explicit, slerp_t, bool(use_mask) if explicit else False,
                bool(record_dh), bool(record_process)) + ((lpips,) if lpips is not None else ()) + \
-            (("record_h",) if record_h else ()) + (("additive",) if additive else ())
+            (("record_h",) if record_h else ()) + (("additive",) if additive else ()) + \
+            ((("blend", blend_B),) if blend_B else ())
         with torch.cuda.device(self.device):
             n_sto = schedule.n_stochastic
             if n_sto:
@@ -1270,7 +1314,7 @@ class UNetEngine:
             g = self.graphs.pop(key, None)
             if g is None:
                 g = self._build_trajectory(P, schedule, use_graph, explicit, record_dh, record_process, lpips,
-                                           record_h, additive)
+                                           record_h, additive, blend_B)
                 while len(self.graphs) >= self.MAX_GRAPHS:
                     self.graphs.pop(next(iter(self.graphs)))
             self.graphs[key] = g  # most recently used last
@@ -1293,6 +1337,9 @@ class UNetEngine:
                 if g["n_edit"]:
                     g["rec"]["dir_in"].copy_(d.to(self.device, torch.float32))
                 P.add_coef.copy_(add_table.to(torch.float32))
+            if blend_B:
+                g["rec"]["blend_mask"].copy_(blend[0])
+                g["rec"]["blend_ref"].copy_(blend[1])
             P.x.copy_(x_T, non_blocking=True)
             if n_sto:
                 g["zbuf"].copy_(noise, non_blocking=True)

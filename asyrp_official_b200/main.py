@@ -184,6 +184,17 @@ def build_parser():
                         'h2 = hs_coeff_origin_h * h + α * d_t at every edit step, α = --hs_coeff_delta_h as given '
                         '(not scaled by n_train_step / n_test_step: a direction has no training grid); with '
                         '--delta_interpolation the rows are (1, v * α)')
+    p.add_argument('--edit_region', type=str, default=None,
+                   help='--run_test: edit only these face-parsing classes ("hair hat"; names of the 19 BiSeNet '
+                        'labels, background skin l_brow r_brow l_eye r_eye eye_g l_ear r_ear ear_r nose mouth u_lip '
+                        'l_lip neck neck_l cloth hair hat).  The origin pass is parsed with --seg_weights into one '
+                        'mask per image, and every edit step ends blended into the origin pass outside it; the masks '
+                        'are written next to the PNG as <file>_ngen<n>_region_mask.png')
+    p.add_argument('--edit_region_dilate', type=int, default=0,
+                   help='--edit_region: grow the mask by a (2r + 1)^2 square max filter, r in 0..32 pixels')
+    p.add_argument('--edit_region_feather', type=float, default=0.0,
+                   help='--edit_region: soften the mask edge with a Gaussian of this sigma in pixels, 0..16 (0: hard '
+                        'edge)')
     return p
 
 

@@ -384,6 +384,82 @@ def h_combine(x, w, mu=None):
     return out
 
 
+def blend_rows(x, ref, mask):
+    """in place, x[n] = m * x[n] + (1 - m) * ref[n % B] per pixel with m = mask[n % B], each element
+    fmaf(m, x, (1 - m) * r) in fp32: x fp32 [N][C][H][W], ref fp32 [B][C][H][W], mask fp32 [B][H][W], N a multiple of B"""
+    lib = _lib.load()
+    _need_cuda(x, ref, mask)
+    if not (x.dtype == ref.dtype == mask.dtype == torch.float32 and x.is_contiguous() and ref.is_contiguous()
+            and mask.is_contiguous()):
+        raise _lib.AsyrpError(f"blend_rows: x, ref and mask must be contiguous fp32 tensors, got {x.dtype}, {ref.dtype} "
+                              f"and {mask.dtype}")
+    if x.dim() != 4 or ref.dim() != 4 or mask.dim() != 3:
+        raise _lib.AsyrpError(f"blend_rows: x [N][C][H][W], ref [B][C][H][W] and mask [B][H][W], got "
+                              f"{tuple(x.shape)}, {tuple(ref.shape)} and {tuple(mask.shape)}")
+    N, Cc, H, W = x.shape
+    B = ref.shape[0]
+    if tuple(ref.shape[1:]) != (Cc, H, W) or tuple(mask.shape) != (B, H, W) or B == 0 or N % B:
+        raise _lib.AsyrpError(f"blend_rows: ref must be [B][{Cc}][{H}][{W}] and mask [B][{H}][{W}] with N = {N} a "
+                              f"multiple of B, got {tuple(ref.shape)} and {tuple(mask.shape)}")
+    if len({x.device, ref.device, mask.device}) != 1:
+        raise _lib.AsyrpError(f"blend_rows: x, ref and mask live on {x.device}, {ref.device} and {mask.device}")
+    check(lib.asyrp_blend_rows(_ptr(x), _ptr(ref), _ptr(mask), N, B, Cc, H * W, _stream()), "asyrp_blend_rows")
+
+
+def _mask_pair(name, inp, out):
+    _need_cuda(inp, out)
+    if not (inp.dtype == out.dtype == torch.float32 and inp.is_contiguous() and out.is_contiguous()
+            and inp.dim() == 3 and inp.shape[1] == inp.shape[2] and tuple(out.shape) == tuple(inp.shape)):
+        raise _lib.AsyrpError(f"{name}: in and out must be contiguous fp32 [N][S][S] tensors of one shape, got "
+                              f"{inp.dtype} {tuple(inp.shape)} / {out.dtype} {tuple(out.shape)}")
+    if inp.device != out.device or inp.data_ptr() == out.data_ptr():
+        raise _lib.AsyrpError(f"{name}: in and out must be distinct tensors on one device")
+    return inp.shape[0], inp.shape[1]
+
+
+def region_mask(labels, class_bits, mask):
+    """mask fp32 [N][S][S] = 1 where a label of the pixel's footprint in labels u8 [N][512][512] has its bit in
+    class_bits, else 0 (S <= 512)"""
+    lib = _lib.load()
+    _need_cuda(labels, mask)
+    if not (labels.dtype == torch.uint8 and labels.is_contiguous() and labels.dim() == 3
+            and tuple(labels.shape[1:]) == (512, 512)):
+        raise _lib.AsyrpError(f"region_mask: labels must be a contiguous u8 [N][512][512] tensor, got {labels.dtype} "
+                              f"{tuple(labels.shape)}")
+    if not (mask.dtype == torch.float32 and mask.is_contiguous() and mask.dim() == 3
+            and mask.shape[0] == labels.shape[0] and mask.shape[1] == mask.shape[2]):
+        raise _lib.AsyrpError(f"region_mask: mask must be a contiguous fp32 [{labels.shape[0]}][S][S] tensor, got "
+                              f"{mask.dtype} {tuple(mask.shape)}")
+    if labels.device != mask.device:
+        raise _lib.AsyrpError(f"region_mask: labels on {labels.device}, mask on {mask.device}")
+    if not 0 <= int(class_bits) < (1 << 32):
+        raise _lib.AsyrpError(f"region_mask: class_bits {class_bits} is not a 32-bit mask")
+    check(lib.asyrp_region_mask(_ptr(labels), C.c_uint(int(class_bits)), _ptr(mask), mask.shape[0], mask.shape[1],
+                                _stream()), "asyrp_region_mask")
+
+
+def mask_dilate(inp, out, r, axis):
+    """out = the max of inp over [i - r, i + r] along axis (0: x, 1: y) of fp32 [N][S][S], indices outside the image
+    left out"""
+    lib = _lib.load()
+    N, S = _mask_pair("mask_dilate", inp, out)
+    check(lib.asyrp_mask_dilate(_ptr(inp), _ptr(out), N, S, int(r), int(axis), _stream()), "asyrp_mask_dilate")
+
+
+def mask_blur(inp, taps, out, axis):
+    """out = sum_k taps[k + R] inp[clamp(i + k)] along axis (0: x, 1: y) of fp32 [N][S][S] in tap order; flat windows
+    return their value.  taps fp32 [2R + 1] on the device"""
+    lib = _lib.load()
+    N, S = _mask_pair("mask_blur", inp, out)
+    _need_cuda(taps)
+    if not (taps.dtype == torch.float32 and taps.is_contiguous() and taps.dim() == 1 and taps.numel() % 2 == 1
+            and taps.device == inp.device):
+        raise _lib.AsyrpError(f"mask_blur: taps must be a contiguous fp32 [2R + 1] tensor on {inp.device}, got "
+                              f"{taps.dtype} {tuple(taps.shape)} on {taps.device}")
+    check(lib.asyrp_mask_blur(_ptr(inp), _ptr(taps), _ptr(out), N, S, taps.numel() // 2, int(axis), _stream()),
+          "asyrp_mask_blur")
+
+
 def transpose_tc(inp, out):
     """inp [N][T][C] (may be a channel slice: last-dim stride 1, row stride ld) -> out [N][C][T] fp16"""
     lib = _lib.load()

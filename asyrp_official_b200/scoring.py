@@ -90,18 +90,23 @@ def id_similarity_setup(runner):
 def seg_consistency_setup(runner):
     """--seg_consistency's requirements; raises ValueError with the reason.  Returns the validated --seg_weights state
     dict (face_parsing.load_state_dict)."""
-    from .face_parsing import load_state_dict
     a = runner.args
     if getattr(a, "pass_editing", False):
         raise ValueError("--seg_consistency scores the edited images: with --pass_editing nothing is edited")
-    path = getattr(a, "seg_weights", None)
+    return seg_weights(runner, "--seg_consistency")
+
+
+def seg_weights(runner, flag):
+    """the validated --seg_weights state dict (face_parsing.load_state_dict) for `flag`; ValueError with the reason"""
+    from .face_parsing import load_state_dict
+    path = getattr(runner.args, "seg_weights", None)
     if not path or not os.path.isfile(path):
-        raise ValueError(f"--seg_consistency: --seg_weights {path!r} is not a file (a torch.save of the face-parsing "
+        raise ValueError(f"{flag}: --seg_weights {path!r} is not a file (a torch.save of the face-parsing "
                          "BiSeNet(n_classes=19) state dict, e.g. 79999_iter.pth)")
     try:
         return load_state_dict(path)
     except ValueError as e:
-        raise ValueError(f"--seg_consistency: {e}") from None
+        raise ValueError(f"{flag}: {e}") from None
 
 
 def content_preservation_setup(runner):

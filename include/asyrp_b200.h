@@ -476,6 +476,26 @@ int asyrp_ssim_pool2(const double* in, double* out, int rows, int H, int W, void
 int asyrp_h_gram(const float* x, const double* mu, double* G, int n, int d, void* stream);
 int asyrp_h_combine(const float* x, const double* w, const double* mu, double* out, int n, int d, int K, void* stream);
 
+/* Region-restricted edits (csrc/region.cu): a soft mask per image from face-parsing labels, and the blend of an edit
+ * pass back into the unedited trajectory outside it.
+ * asyrp_blend_rows: in place, x[n][c][p] = fmaf(m, x, (1 - m) * r) in fp32 with m = mask[n % B][p] and
+ *   r = ref[n % B][c][p]; x fp32 [N][C][HW], ref fp32 [B][C][HW], mask fp32 [B][HW].  m = 1 gives x and m = 0 gives r
+ *   exactly.  N % B == 0; 64-bit indexing.  With HW % 4 == 0 the three pointers must be 16-byte aligned (float4
+ *   loads), else 4-byte aligned.
+ * asyrp_region_mask: mask fp32 [N][S][S] = 1 where a label of the pixel's footprint in labels u8 [N][512][512] (rows
+ *   [ceil(y 512 / S), ceil((y + 1) 512 / S)), columns likewise) has its bit set in class_bits (labels >= 32 never),
+ *   else 0.  1 <= S <= 512, 1 <= N <= 65535.
+ * asyrp_mask_dilate: out = the max of in over [i - r, i + r] along axis (0: x, 1: y), indices outside the image left
+ *   out; 0 <= r <= 32.  Both axes give the (2r + 1)^2 square max filter.
+ * asyrp_mask_blur: out[i] = sum_{k=-R..R} taps[k + R] in[clamp(i + k, 0, S - 1)] along axis, fp32 fmaf in tap order; a
+ *   window whose inputs are all equal gives that value exactly.  taps fp32 [2R + 1] on the device, 0 <= R <= 48.
+ * The mask kernels take fp32 [N][S][S] images, 4-byte aligned; out must not be in.
+ * No allocation, no synchronisation, no atomics. */
+int asyrp_blend_rows(float* x, const float* ref, const float* mask, int N, int B, int C, int HW, void* stream);
+int asyrp_region_mask(const unsigned char* labels, unsigned class_bits, float* mask, int N, int S, void* stream);
+int asyrp_mask_dilate(const float* in, float* out, int N, int S, int r, int axis, void* stream);
+int asyrp_mask_blur(const float* in, const float* taps, float* out, int N, int S, int R, int axis, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

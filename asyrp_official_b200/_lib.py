@@ -150,6 +150,7 @@ SIGNATURES = {
     "asyrp_h_gram": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_void_p]),
     "asyrp_h_combine": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p]),
     "asyrp_blend_rows": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p]),
+    "asyrp_compose_rows": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p]),
     "asyrp_region_mask": (c_int, [c_void_p, C.c_uint, c_void_p, c_int, c_int, c_void_p]),
     "asyrp_mask_dilate": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p]),
     "asyrp_mask_blur": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p]),

@@ -2,15 +2,20 @@
 // back into the unedited trajectory outside it.
 //
 //   blend      x[n][c][p] = fmaf(m, x, (1 - m) * r),  m = mask[n % B][p], r = ref[n % B][c][p]   blend_rows_kernel{,4}
+//   compose    rows n = k B + j of K attributes x B images: s = M_1 + .. + M_K (fp32, in order); w_k = M_k and
+//              w_0 = 1 - s if s <= 1, else w_k = M_k / s and w_0 = 0; acc = w_0 r, then acc = fmaf(w_k, x[k B + j],
+//              acc) for k = 1..K; acc is written to all K rows of image j           compose_rows_kernel{,4}<K>
 //   select     mask[n][y][x] = 1 if a label of the footprint rows [ceil(y 512 / S), ceil((y + 1) 512 / S)) (columns
 //              likewise) is in class_bits, else 0                                                  region_mask_kernel
 //   dilate     out = max of in over [i - r, i + r] along one axis, indices outside the image left out  mask_dilate_kernel
 //   blur       out = sum_{k=-R..R} taps[k + R] in[clamp(i + k)] along one axis, fp32 fmaf in tap order;
 //              a window whose inputs are all equal returns that value                             mask_blur_kernel
 //
-// The blend is the hot path: it runs once per step inside the trajectory graph over N * C * HW fp32.  With HW a
-// multiple of 4 each thread moves one float4 of x, ref and mask; otherwise one element.  m = 1 gives x exactly and
-// m = 0 gives r exactly (for finite x and r).  Every kernel indexes in 64 bits where a count can pass 2^31.
+// The blend and the compose are the hot paths: each runs once per step inside the trajectory graph over N * C * HW
+// fp32.  With HW a multiple of 4 each thread moves one float4 of x, ref and mask; otherwise one element.  m = 1 gives
+// x exactly and m = 0 gives r exactly (for finite x and r).  The compose computes its weights in registers from the K
+// masks of a pixel, once for all C channels; with K = 1 it is the blend operation for operation.  Every kernel
+// indexes in 64 bits where a count can pass 2^31.
 #include <cstdint>
 
 #include "common.h"
@@ -23,6 +28,7 @@ constexpr int kRegionThreads = 256;
 constexpr int kLabelSize = 512;      // the face parser's label maps are 512 x 512
 constexpr int kMaxDilate = 32;
 constexpr int kMaxBlurRadius = 48;   // ceil(3 sigma) for sigma <= 16
+constexpr int kMaxComposeRows = 8;   // attributes of one composite: their masks stay in registers
 
 __device__ __forceinline__ float blend1(float m, float x, float r) {
   return fmaf(m, x, __fmul_rn(__fsub_rn(1.f, m), r));
@@ -64,6 +70,95 @@ __global__ void __launch_bounds__(kRegionThreads) blend_rows_kernel(float* __res
     *xp = blend1(__ldg(mask + static_cast<long long>(b) * HW + p), *xp,
                  __ldg(ref + (static_cast<long long>(b) * C + c) * HW + p));
   }
+}
+
+// compose: the K masks of one pixel -> the weights, in place (w[k] replaces m[k]); returns w0
+template <int K>
+__device__ __forceinline__ float compose_weights(float (&m)[K]) {
+  float s = m[0];
+#pragma unroll
+  for (int k = 1; k < K; ++k) s = __fadd_rn(s, m[k]);
+  if (s <= 1.f) return __fsub_rn(1.f, s);
+#pragma unroll
+  for (int k = 0; k < K; ++k) m[k] = __fdiv_rn(m[k], s);
+  return 0.f;
+}
+
+// one float4 of pixels of image j per thread: grid (ceil(HW / 4 / 256), images j strided by gridDim.y).  The K mask
+// float4s are loaded once, turned into weights, and reused for the C channels.
+template <int K>
+__global__ void __launch_bounds__(kRegionThreads) compose_rows_kernel4(float4* __restrict__ x,
+                                                                      const float4* __restrict__ ref,
+                                                                      const float4* __restrict__ masks, int B, int C,
+                                                                      int HW4) {
+  pdl_trigger();
+  pdl_wait();
+  const int p = blockIdx.x * kRegionThreads + threadIdx.x;
+  if (p >= HW4) return;
+  for (int j = blockIdx.y; j < B; j += gridDim.y) {
+    float mx[K], my[K], mz[K], mw[K];
+#pragma unroll
+    for (int k = 0; k < K; ++k) {
+      const float4 m = __ldg(masks + (static_cast<long long>(k) * B + j) * HW4 + p);
+      mx[k] = m.x;
+      my[k] = m.y;
+      mz[k] = m.z;
+      mw[k] = m.w;
+    }
+    const float w0x = compose_weights<K>(mx), w0y = compose_weights<K>(my), w0z = compose_weights<K>(mz),
+                w0w = compose_weights<K>(mw);
+    for (int c = 0; c < C; ++c) {
+      const float4 r = __ldg(ref + (static_cast<long long>(j) * C + c) * HW4 + p);
+      float4 acc = make_float4(__fmul_rn(w0x, r.x), __fmul_rn(w0y, r.y), __fmul_rn(w0z, r.z), __fmul_rn(w0w, r.w));
+#pragma unroll
+      for (int k = 0; k < K; ++k) {
+        const float4 v = x[((static_cast<long long>(k) * B + j) * C + c) * HW4 + p];
+        acc.x = fmaf(mx[k], v.x, acc.x);
+        acc.y = fmaf(my[k], v.y, acc.y);
+        acc.z = fmaf(mz[k], v.z, acc.z);
+        acc.w = fmaf(mw[k], v.w, acc.w);
+      }
+#pragma unroll
+      for (int k = 0; k < K; ++k) x[((static_cast<long long>(k) * B + j) * C + c) * HW4 + p] = acc;
+    }
+  }
+}
+
+template <int K>
+__global__ void __launch_bounds__(kRegionThreads) compose_rows_kernel(float* __restrict__ x,
+                                                                     const float* __restrict__ ref,
+                                                                     const float* __restrict__ masks, int B, int C,
+                                                                     int HW) {
+  pdl_trigger();
+  pdl_wait();
+  const int p = blockIdx.x * kRegionThreads + threadIdx.x;
+  if (p >= HW) return;
+  for (int j = blockIdx.y; j < B; j += gridDim.y) {
+    float w[K];
+#pragma unroll
+    for (int k = 0; k < K; ++k) w[k] = __ldg(masks + (static_cast<long long>(k) * B + j) * HW + p);
+    const float w0 = compose_weights<K>(w);
+    for (int c = 0; c < C; ++c) {
+      float acc = __fmul_rn(w0, __ldg(ref + (static_cast<long long>(j) * C + c) * HW + p));
+#pragma unroll
+      for (int k = 0; k < K; ++k) acc = fmaf(w[k], x[((static_cast<long long>(k) * B + j) * C + c) * HW + p], acc);
+#pragma unroll
+      for (int k = 0; k < K; ++k) x[((static_cast<long long>(k) * B + j) * C + c) * HW + p] = acc;
+    }
+  }
+}
+
+template <int K>
+int launch_compose(float* x, const float* ref, const float* masks, int B, int C, int HW, bool vec, cudaStream_t st) {
+  const int per = vec ? HW / 4 : HW;
+  const dim3 grid((per + kRegionThreads - 1) / kRegionThreads, B < kMaxGridYZ ? B : kMaxGridYZ);
+  if (vec) {
+    ASYRP_LAUNCH(compose_rows_kernel4<K>, grid, dim3(kRegionThreads), 0, st, reinterpret_cast<float4*>(x),
+                 reinterpret_cast<const float4*>(ref), reinterpret_cast<const float4*>(masks), B, C, per);
+  } else {
+    ASYRP_LAUNCH(compose_rows_kernel<K>, grid, dim3(kRegionThreads), 0, st, x, ref, masks, B, C, HW);
+  }
+  return ASYRP_OK;
 }
 
 // one output pixel per thread: grid (ceil(S^2 / 256), N)
@@ -167,6 +262,33 @@ ASYRP_API int asyrp_blend_rows(float* x, const float* ref, const float* mask, in
   } else {
     ASYRP_LAUNCH(blend_rows_kernel, grid, dim3(kRegionThreads), 0, st, x, ref, mask, N, B, C, HW);
   }
+  ASYRP_CHECK_CUDA(cudaGetLastError());
+  return ASYRP_OK;
+}
+
+ASYRP_API int asyrp_compose_rows(float* x, const float* ref, const float* masks, int K, int B, int C, int HW,
+                                 void* stream) {
+  ASYRP_REQUIRE(x != nullptr && ref != nullptr && masks != nullptr,
+                "asyrp_compose_rows: x, ref and masks are required");
+  ASYRP_REQUIRE(K >= 1 && K <= kMaxComposeRows, "asyrp_compose_rows: K=%d outside 1..%d", K, kMaxComposeRows);
+  ASYRP_REQUIRE(B > 0 && C > 0 && HW > 0, "asyrp_compose_rows: bad shape B=%d C=%d HW=%d (all positive)", B, C, HW);
+  const bool vec = HW % 4 == 0;
+  const uintptr_t a = vec ? 16 : 4;
+  ASYRP_REQUIRE(aligned(x, a) && aligned(ref, a) && aligned(masks, a),
+                "asyrp_compose_rows: x, ref and masks must be %d-byte aligned (HW=%d)", static_cast<int>(a), HW);
+  const cudaStream_t st = static_cast<cudaStream_t>(stream);
+  int rc = ASYRP_OK;
+  switch (K) {
+    case 1: rc = launch_compose<1>(x, ref, masks, B, C, HW, vec, st); break;
+    case 2: rc = launch_compose<2>(x, ref, masks, B, C, HW, vec, st); break;
+    case 3: rc = launch_compose<3>(x, ref, masks, B, C, HW, vec, st); break;
+    case 4: rc = launch_compose<4>(x, ref, masks, B, C, HW, vec, st); break;
+    case 5: rc = launch_compose<5>(x, ref, masks, B, C, HW, vec, st); break;
+    case 6: rc = launch_compose<6>(x, ref, masks, B, C, HW, vec, st); break;
+    case 7: rc = launch_compose<7>(x, ref, masks, B, C, HW, vec, st); break;
+    default: rc = launch_compose<8>(x, ref, masks, B, C, HW, vec, st); break;
+  }
+  if (rc != ASYRP_OK) return rc;
   ASYRP_CHECK_CUDA(cudaGetLastError());
   return ASYRP_OK;
 }

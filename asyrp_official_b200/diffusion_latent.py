@@ -39,6 +39,9 @@ Mirrors, with the same attribute / flag names:
   Asyrp.run_h_directions       (none)                       --h_directions: editing directions from the statistics of
                                                             the bottleneck h (hspace.py), applied by --run_test
                                                             --h_direction as h + α d; this build's definition
+  Asyrp.run_region_compose     (none)                       --region_compose: several attributes composed into one
+                                                            image, each in its own face-parsing region, inside the
+                                                            per-row trajectory; this build's definition
 
 Differences (documented in INTEGRATION.md): the reverse loop is UNetEngine.sample() — one CUDA graph per
 (batch, schedule) instead of 40 Python iterations; pretrained weights come from --model_path (no URL download);
@@ -399,7 +402,8 @@ class Asyrp(object):
     def save_image(self, model, x_lat_tensor, seq_inv, seq_inv_next, save_x0=False, save_x_origin=False,
                    save_process_delta_h=False, save_process_origin=False, x0_tensor=None, delta_h_dict=None,
                    get_delta_hs=False, folder_dir="", file_name="", hs_coeff=(1.0, 1.0), h_direction=None,
-                   sweep_times=None, scorers=None, mode=None, batch_ids=None, x0_source=None, edit_region=None):
+                   sweep_times=None, scorers=None, mode=None, batch_ids=None, x0_source=None, edit_region=None,
+                   region_compose=None):
         """rows of the grid: [x0] [origin DDIM] one row per hs_coeff tuple  (diffusion_latent.py:445-544).
 
         delta_h_dict: {t: None | Δh tensor}.  Entries that are tensors select the explicit-Δh branch for that step
@@ -416,7 +420,12 @@ class Asyrp(object):
         edit_region (--edit_region): (FaceParser, class indices, dilate r, feather sigma).  The origin pass then records
         x_t after every step and always runs; its x0 is parsed into one soft mask per image (region.region_masks),
         written as <file>_ngen<n>_region_mask.png, and every step of the edit pass ends with x <- m x + (1 - m) x_orig
-        (UNetEngine.sample's blend), so that outside the region the edits follow the origin pass."""
+        (UNetEngine.sample's blend), so that outside the region the edits follow the origin pass.
+        region_compose (--region_compose): (FaceParser, class indices per attribute, r, sigma, (t_edit, t_addnoise) per
+        attribute, coefficients per attribute).  As with edit_region the origin pass records its trajectory and always
+        runs; its x0 gives K masks per image (region.compose_masks), written as <file>_ngen<n>_region_compose.png
+        (one row per attribute), and hs_coeff is the one tuple the composite is scored as.  The grid's last row is the
+        composite of every image (compose_batch)."""
         import torchvision.utils as tvu
         a = self.args
         time_s = time.time()
@@ -426,18 +435,18 @@ class Asyrp(object):
         if save_x0 and x0_tensor is not None:
             x_list.append(x0_tensor.cpu())
         blend = None
-        if save_x_origin or (scorers is not None and scorers.needs_origin) or edit_region is not None:
+        masked = edit_region is not None or region_compose is not None  # the edits follow the recorded origin pass
+        if save_x_origin or (scorers is not None and scorers.needs_origin) or masked:
             sch = self.make_schedule(seq_inv, seq_inv_next, (1.0,), edit=False,
                                      addnoise=bool(getattr(a, "origin_process_addnoise", False)))
             if save_x_origin:
-                origin = self.edit_batch(model, x_lat_tensor, sch,
-                                         record_process=save_process_origin or edit_region is not None)
+                origin = self.edit_batch(model, x_lat_tensor, sch, record_process=save_process_origin or masked)
                 x_list.append(origin)
                 if save_process_origin:
                     self._write_process(eng, sch, os.path.join(folder_dir, file_name), "origin", bs)
             else:  # the pass only the score needs leaves the random stream as it was: the edits draw the same noise
                 with torch.random.fork_rng(devices=[eng.device]):
-                    origin = self.edit_batch(model, x_lat_tensor, sch, record_process=edit_region is not None)
+                    origin = self.edit_batch(model, x_lat_tensor, sch, record_process=masked)
             if edit_region is not None:
                 from .region import region_masks
                 ref = eng.last_records["x"].clone()  # owned by the origin graph: the edit replays would reuse it
@@ -447,9 +456,19 @@ class Asyrp(object):
                 os.makedirs(folder_dir, exist_ok=True)
                 tvu.save_image(tvu.make_grid(mask[:, None].cpu(), nrow=a.bs_train, padding=1),
                                os.path.join(folder_dir, f'{file_name}_ngen{a.n_train_step}_region_mask.png'))
+            if region_compose is not None:
+                from . import region
+                ref = eng.last_records["x"].clone()  # owned by the origin graph: the edit replays would reuse it
+                parser, classes, r, sigma, times, row_coeffs = region_compose
+                masks = region.compose_masks(parser, origin, classes, r, sigma).to(eng.device)
+                os.makedirs(folder_dir, exist_ok=True)
+                tvu.save_image(tvu.make_grid(masks.reshape(-1, 1, *masks.shape[2:]).cpu(), nrow=a.bs_train, padding=1),
+                               os.path.join(folder_dir, f'{file_name}_ngen{a.n_train_step}_region_compose.png'))
         coeffs = hs_coeff if isinstance(hs_coeff, list) else [hs_coeff]
         edited = []
-        if sweep_times is not None:
+        if region_compose is not None:
+            edited = [self.compose_batch(model, x_lat_tensor, seq_inv, seq_inv_next, masks, ref, times, row_coeffs)]
+        elif sweep_times is not None:
             tpc, chunks = plan_sweep(len(coeffs), bs, getattr(a, "max_rows_per_replay", 16))
             for chunk in chunks:
                 rows = sweep_rows(chunk, tpc, bs)
@@ -577,6 +596,7 @@ class Asyrp(object):
         import torchvision.utils as tvu
         a = self.args
         self.edit_region_setup()  # refuses --lpips
+        self.region_compose_setup()  # refuses --lpips
         if getattr(a, "content_preservation", False):
             self.content_preservation_setup()  # refuses --lpips
         if self.world > 1:
@@ -662,8 +682,11 @@ class Asyrp(object):
     def run_test(self):
         a = self.args
         scoring.fid_options_check(self)
+        compose_spec = self.region_compose_setup()  # refuses --attr_sweep, --edit_region and --h_direction too
         region_spec = self.edit_region_setup()  # refuses --attr_sweep too, before it is dispatched
         h_dir_path = self.h_direction_setup()  # refuses --attr_sweep too, before it is dispatched
+        if compose_spec is not None:
+            return self.run_region_compose(compose_spec)
         if getattr(a, "attr_sweep", ""):
             return self.run_attr_sweep()
         print("Running Test")
@@ -854,6 +877,49 @@ class Asyrp(object):
         region.check_options(r, sigma, self.config.data.image_size)
         return classes, r, float(sigma), scoring.seg_weights(self, "--edit_region")
 
+    def region_compose_setup(self):
+        """--region_compose's requirements, checked before any model loads: None without the flag, else (attributes,
+        the class indices of each, --edit_region_dilate, --edit_region_feather, the --seg_weights state dict, the
+        attributes' DeltaBlock checkpoints).  ValueError with the reason."""
+        from . import region
+        a = self.args
+        text = getattr(a, "region_compose", None)
+        if not text:
+            return None
+        if not getattr(a, "run_test", False):
+            raise ValueError("--region_compose composes the edits of --run_test: add --run_test")
+        each = "every attribute edits with its own DeltaBlock"
+        for flag, on, why in (
+                ("--attr_sweep", getattr(a, "attr_sweep", ""), "it gives every attribute an image of its own"),
+                ("--edit_region", getattr(a, "edit_region", None), "every attribute takes its region from "
+                                                                  "--region_compose"),
+                ("--multiple_attr", getattr(a, "multiple_attr", ""), each),
+                ("--delta_interpolation", getattr(a, "delta_interpolation", False), "a composite has one strength"),
+                ("--num_mean_of_delta_hs", getattr(a, "num_mean_of_delta_hs", 0), each),
+                ("--train_delta_h", getattr(a, "train_delta_h", False), each),
+                ("--h_direction", getattr(a, "h_direction", None), each),
+                ("--pass_editing", getattr(a, "pass_editing", False), "nothing is edited"),
+                ("--diff_style", getattr(a, "diff_style", False), "it is not a --run_test edit"),
+                ("--lpips", getattr(a, "lpips", False), "it edits nothing"),
+                ("--h_directions", getattr(a, "h_directions", False), "it edits nothing"),
+                ("--DirectionalClipSmilarity", getattr(a, "DirectionalClipSmilarity", False),
+                 "a composite has no single source / target text pair"),
+                ("--save_process_delta_h", getattr(a, "save_process_delta_h", False),
+                 "the rows of a composite are not one edit's trajectory")):
+            if on:
+                raise ValueError(f"--region_compose does not combine with {flag}: {why}")
+        spec = region.parse_compose(text)
+        attrs = [attr for attr, _ in spec]
+        max_rows = getattr(a, "max_rows_per_replay", 16)
+        if len(attrs) > max_rows:
+            raise ValueError(f"--region_compose: {len(attrs)} attributes need {len(attrs)} rows per image, above "
+                             f"--max_rows_per_replay {max_rows}")
+        paths = self.attribute_blocks_setup("--region_compose", attrs)
+        r, sigma = getattr(a, "edit_region_dilate", 0), getattr(a, "edit_region_feather", 0.0)
+        region.check_options(r, sigma, self.config.data.image_size)
+        return (attrs, [classes for _, classes in spec], r, float(sigma), scoring.seg_weights(self, "--region_compose"),
+                paths)
+
     def h_direction_setup(self):
         """--h_direction's requirements, checked before any model loads: the path (None without the flag); ValueError
         when it is combined with a flag that selects another source of Δh"""
@@ -910,6 +976,7 @@ class Asyrp(object):
         from . import hspace
         a = self.args
         self.edit_region_setup()  # refuses --h_directions
+        self.region_compose_setup()  # refuses --h_directions
         mode, arg = self.h_directions_setup()
         seq, seq_next = make_sequences(a.t_0, a.n_test_step)
         size = self.config.data.image_size
@@ -982,23 +1049,30 @@ class Asyrp(object):
                          ("--train_delta_h", bool(getattr(a, "train_delta_h", False)))):
             if on:
                 raise ValueError(f"--attr_sweep edits with one DeltaBlock per attribute: it does not combine with {flag}")
+        return attrs, self.attribute_blocks_setup("--attr_sweep", attrs)
+
+    def attribute_blocks_setup(self, flag, attrs):
+        """the requirements of a mode whose rows edit with one DeltaBlock per attribute (`flag`: --attr_sweep,
+        --region_compose): per-row DDIM schedules, one block per checkpoint, every image edited.  Returns the
+        checkpoints, the checkpoint name with 'attribute' replaced by each attribute, as --multiple_attr resolves them."""
+        a = self.args
         if getattr(a, "sample_type", "ddim") != "ddim":
-            raise ValueError(f"--attr_sweep needs --sample_type ddim (every row its own eta schedule), got "
+            raise ValueError(f"{flag} needs --sample_type ddim (every row its own eta schedule), got "
                              f"{a.sample_type!r}")
         if a.get_h_num != 1:
-            raise ValueError(f"--attr_sweep loads one DeltaBlock per attribute: --get_h_num must be 1, got {a.get_h_num}")
+            raise ValueError(f"{flag} loads one DeltaBlock per attribute: --get_h_num must be 1, got {a.get_h_num}")
         if getattr(a, "pass_editing", False):
-            raise ValueError("--attr_sweep edits every image: it does not combine with --pass_editing")
+            raise ValueError(f"{flag} edits every image: it does not combine with --pass_editing")
         name = self.checkpoint_name()
         if "attribute" not in os.path.basename(name):
-            raise ValueError(f"--attr_sweep: the checkpoint name {name!r} has no 'attribute' to replace by each "
+            raise ValueError(f"{flag}: the checkpoint name {name!r} has no 'attribute' to replace by each "
                              "attribute (e.g. --manual_checkpoint_name attribute_LC_CelebA_HQ_t999_ninv40_ngen40_0.pth)")
         dirname, base = os.path.split(name)
         paths = [os.path.join(dirname, base.replace("attribute", attr)) for attr in attrs]
         missing = [p for p in paths if not os.path.isfile(p)]
         if missing:
-            raise ValueError(f"--attr_sweep: checkpoint(s) {missing} do not exist")
-        return attrs, paths
+            raise ValueError(f"{flag}: checkpoint(s) {missing} do not exist")
+        return paths
 
     def attr_sweep_schedules(self, attrs):
         """(t_edit, t_addnoise) of every attribute: --user_defined_t_edit / --user_defined_t_addnoise for all of them,
@@ -1030,27 +1104,7 @@ class Asyrp(object):
         self.sweep_times = dict(zip(attrs, times))
         seq_test = [int(s + 1e-6) for s in list(np.linspace(0, 1, a.n_test_step) * a.t_0)]
         seq_test_next = [-1] + list(seq_test[:-1])
-        model = self.load_pretrained_model()
-        # the latents below come from the global random stream, after the model is built: advance it as run_test does
-        # (one DeltaBlock's default init), then create the K blocks, whose initial values the checkpoints replace,
-        # without touching it, so that every image gets the x_T of its --edit_attr run
-        model.setattr_layers(a.get_h_num)
-        with torch.random.fork_rng(devices=[]):
-            model.setattr_layers(len(attrs))
-        for i, path in enumerate(paths):  # packed as layer_0 .. layer_{K-1}
-            print(f"{path} exists. load checkpoint")
-            ck = torch.load(path, map_location="cpu", weights_only=True)
-            getattr(model, f"layer_{i}").load_state_dict(ck["0"])
-        scaling_factor = a.n_train_step / a.n_test_step * a.hs_coeff_delta_h  # :626
-        coeffs = [tuple([1.0 * a.hs_coeff_origin_h] + [1.0 * scaling_factor if j == k else 0.0
-                                                        for j in range(len(attrs))]) for k in range(len(attrs))]
-        model = model.to(self.device)
-        if self.world > 1 and torch.distributed.is_initialized():
-            broadcast_weights(model)
-        if a.load_random_noise:
-            pairs = self.random_noise_pairs(model, saved_noise=bool(getattr(a, "saved_random_noise", False)))
-        else:
-            pairs = self.precompute_pairs(model)
+        model, coeffs, pairs = self.attribute_run(paths)
         results = {}
         with scorers:
             for mode, step, x_lat, x0, ids, x0_source in self._batches(pairs, scorers.keeps_source):
@@ -1060,6 +1114,88 @@ class Asyrp(object):
                     hs_coeff=coeffs, sweep_times=times, scorers=scorers, mode=mode, batch_ids=ids, x0_source=x0_source)
             scorers.finish(coeffs)
         return results
+
+    def attribute_run(self, paths):
+        """what a run with one DeltaBlock per attribute (--attr_sweep, --region_compose) edits with: (the model with the
+        blocks of `paths` packed as layer_0 .. layer_{K-1} on the device, the coefficients of each attribute's rows,
+        the latents)"""
+        a = self.args
+        K = len(paths)
+        model = self.load_pretrained_model()
+        # the latents below come from the global random stream, after the model is built: advance it as run_test does
+        # (one DeltaBlock's default init), then create the K blocks, whose initial values the checkpoints replace,
+        # without touching it, so that every image gets the x_T of its --edit_attr run
+        model.setattr_layers(a.get_h_num)
+        with torch.random.fork_rng(devices=[]):
+            model.setattr_layers(K)
+        for i, path in enumerate(paths):  # packed as layer_0 .. layer_{K-1}
+            print(f"{path} exists. load checkpoint")
+            ck = torch.load(path, map_location="cpu", weights_only=True)
+            getattr(model, f"layer_{i}").load_state_dict(ck["0"])
+        scaling_factor = a.n_train_step / a.n_test_step * a.hs_coeff_delta_h  # :626
+        coeffs = [tuple([1.0 * a.hs_coeff_origin_h] + [1.0 * scaling_factor if j == k else 0.0 for j in range(K)])
+                  for k in range(K)]
+        model = model.to(self.device)
+        if self.world > 1 and torch.distributed.is_initialized():
+            broadcast_weights(model)
+        if a.load_random_noise:
+            pairs = self.random_noise_pairs(model, saved_noise=bool(getattr(a, "saved_random_noise", False)))
+        else:
+            pairs = self.precompute_pairs(model)
+        return model, coeffs, pairs
+
+    @torch.no_grad()
+    def run_region_compose(self, spec):
+        """--run_test --region_compose "a=classes b=classes ..": one image per latent in which every attribute edits
+        only its own face-parsing region.  The K attributes run as rows of one batched trajectory (attribute-major,
+        each with its own DeltaBlock, t_edit and t_addnoise, as --attr_sweep); after every step the K rows of an image
+        are replaced by the per-pixel composite of the rows and the origin pass (UNetEngine.sample's compose).
+        spec: region_compose_setup's result.  The composite is scored as one tuple (hs_coeff_origin_h, s, .., s)
+        whose `attr` column joins the attributes with '+'."""
+        from .face_parsing import FaceParser
+        a = self.args
+        print("Running Test (region composite)")
+        attrs, classes, r, sigma, seg_sd, paths = spec
+        scorers = scoring.Scorers(self, ["+".join(attrs)])
+        times = self.attr_sweep_schedules(attrs)  # prints each attribute's t_edit and t_addnoise
+        self.compose_times = dict(zip(attrs, times))
+        seq_test, seq_test_next = make_sequences(a.t_0, a.n_test_step)
+        model, coeffs, pairs = self.attribute_run(paths)
+        tuples = [tuple([coeffs[0][0]] + [coeffs[k][1 + k] for k in range(len(attrs))])]
+        results = {}
+        with scorers:  # --seg_consistency's parser serves the masks too
+            compose = (scorers.nets.get("seg") or FaceParser(seg_sd, device=self.device), classes, r, sigma, times,
+                       coeffs)
+            for mode, step, x_lat, x0, ids, x0_source in self._batches(pairs, scorers.keeps_source):
+                results[(mode, step)] = self.save_image(
+                    model, x_lat, seq_test, seq_test_next, save_x0=a.save_x0, save_x_origin=a.save_x_origin,
+                    x0_tensor=x0, folder_dir=a.test_image_folder, file_name=f'{mode}_{step}_{a.n_iter - 1}',
+                    hs_coeff=tuples, scorers=scorers, mode=mode, batch_ids=ids, x0_source=x0_source,
+                    region_compose=compose)
+            scorers.finish(tuples)
+            compose = None  # the parser goes with the scorers' networks, and the CUDA cache after it
+        return results
+
+    def compose_batch(self, model, x_lat, seq, seq_next, masks, ref, times, coeffs):
+        """--region_compose's edit pass of one batch of B images: x_lat [B][C][S][S], masks [K][B][S][S] and the origin
+        pass's trajectory ref [steps][B][C][S][S] on the device, times / coeffs per attribute.  Images run in chunks of
+        b = --max_rows_per_replay // K (plan_compose) as K b rows, attribute-major, the last chunk padded, so that every
+        chunk replays one graph.  The noise is one draw [n_stochastic][B][..] for the batch, each chunk's images
+        repeated over its K rows (compose_noise).  Returns the composites [B][C][S][S] on the host."""
+        eng = model.engine
+        K, bs = masks.shape[0], x_lat.shape[0]
+        b, chunks = plan_compose(bs, K, getattr(self.args, "max_rows_per_replay", 16))
+        sch = self.sweep_schedule(seq, seq_next, [times[k] for k in range(K) for _ in range(b)],
+                                  [coeffs[k] for k in range(K) for _ in range(b)])
+        z = torch.randn((sch.n_stochastic, *x_lat.shape), device=eng.device) if sch.n_stochastic else None
+        per_image = lambda t, j0, j1: pad_rows(t[:, j0:j1].transpose(0, 1), b).transpose(0, 1)  # noqa: E731
+        out = []
+        for j0, j1 in chunks:
+            x0 = self.edit_batch(model, pad_rows(x_lat[j0:j1], b).repeat(K, 1, 1, 1), sch,
+                                 noise=compose_noise(z[:, j0:j1], b, K) if z is not None else None,
+                                 compose=(per_image(masks, j0, j1), per_image(ref, j0, j1)))
+            out.append(x0[:j1 - j0].clone())  # every attribute's row of an image holds its composite
+        return torch.cat(out)
 
     def sweep_schedule(self, seq, seq_next, times, coeffs):
         """the RowSchedule of sweep rows: row r has t_edit / t_addnoise times[r] and coefficients coeffs[r], with the
@@ -1164,6 +1300,7 @@ class Asyrp(object):
         a = self.args
         self.prdc_check()
         self.edit_region_setup()  # refuses --diff_style
+        self.region_compose_setup()  # refuses --diff_style
         if getattr(a, "content_preservation", False):
             self.content_preservation_setup()  # refuses --diff_style
         if getattr(a, "fid", False):
@@ -1339,6 +1476,23 @@ def lpips_tables(seq_inv, seq_inv_next, per_image):
         out["x0_t"] += f"{seq}\t{lx0[seq]}\n"
         out["x0_t_std"] += f"{seq}\t{sx0[seq]}\n"
     return out
+
+
+def plan_compose(bs, K, max_rows):
+    """Chunks of a --region_compose batch of bs images with K attributes: (b, [(first, end) image range of each
+    chunk]).  A chunk holds b = min(bs, max_rows // K) images (at least one) and runs as K b rows; the last one is
+    padded (pad_rows), so that every chunk replays one graph."""
+    b = min(bs, max(1, max_rows // K))
+    return b, [(j, min(j + b, bs)) for j in range(0, bs, b)]
+
+
+def compose_noise(z, b, K):
+    """the noise of one --region_compose chunk, [n_stochastic][K b][...], from the batch's draw of its images z
+    [n_stochastic][m <= b][...]: padded to b images (padding copies the last image), then repeated over the K
+    attribute rows, so that the K rows of an image share its noise"""
+    if z.shape[1] < b:
+        z = torch.cat([z, z[:, -1:].expand(z.shape[0], b - z.shape[1], *z.shape[2:])], dim=1)
+    return z.repeat(1, K, *([1] * (z.dim() - 2)))
 
 
 def pad_rows(t, n):

@@ -43,6 +43,7 @@ GN_FOLD_PRODUCERS_ONLY = os.environ.get("ASYRP_GN_FOLD", "0") == "2"  # diagnost
 # ResBlock identity skips x + h ride conv2's K loop as an identity weight block (C extra MACs per output, exact: fp16 x
 # times 1.0 into the fp32 accumulator).  ASYRP_SKIP_AS_K=0 reads x in the epilogue instead.
 SKIP_AS_K = os.environ.get("ASYRP_SKIP_AS_K", "1") != "0"
+MAX_COMPOSE = 8  # attributes of one region composite (sample(compose=), asyrp_compose_rows)
 
 
 class Act:
@@ -1071,11 +1072,13 @@ class UNetEngine:
             g["graph"] = cg
         return g
 
-    def _build_row_trajectory(self, P, schedule, use_graph, own, record_process):
+    def _build_row_trajectory(self, P, schedule, use_graph, own, record_process, compose_kb=None):
         """the trajectory of a per-row schedule (schedule.RowSchedule): per step the step's rows of the DeltaBlock pair
         table and of the (c1, c2) table are copied into the buffers the kernels read, as the timestep-embedding row is;
         on edit steps every DeltaBlock runs from middle_h, each editing row's output is copied into h2, and the rows
-        that do not edit take et as et_mod; the update is ddim_update_rows"""
+        that do not edit take et as et_mod; the update is ddim_update_rows.
+        compose_kb: (K attributes, b images) of a region composite (None: none); the graph then owns its masks and
+        reference trajectory, and every update is followed by compose_rows"""
         steps = schedule.steps
         N, dev = P.x.shape[0], self.device
         n_sto = schedule.n_stochastic
@@ -1093,6 +1096,10 @@ class UNetEngine:
         if record_process:
             rec["x"] = torch.zeros((len(steps), *P.x.shape), dtype=torch.float32, device=dev)
             rec["x0_t"] = torch.zeros((len(steps), *P.x.shape), dtype=torch.float32, device=dev)
+        if compose_kb:  # region composite: K masks per image and the origin pass's x after every step
+            Kc, bc = compose_kb
+            rec["compose_masks"] = torch.zeros((Kc, bc, *P.x.shape[2:]), dtype=torch.float32, device=dev)
+            rec["compose_ref"] = torch.zeros((len(steps), bc, *P.x.shape[1:]), dtype=torch.float32, device=dev)
         h2 = P.h2
 
         def selector(s):
@@ -1124,11 +1131,13 @@ class UNetEngine:
                     zi += 1
                 ops.ddim_update_rows(P.x, P.et, P.et_mod if s.edit else P.et, z, P.x,
                                      rec["x0_t"][k] if record_process else None, s.at, s.an, c12)
+                if compose_kb:  # the K rows of every image continue from their composite against the origin pass
+                    ops.compose_rows(P.x, rec["compose_ref"][k], rec["compose_masks"])
                 if record_process:
                     rec["x"][k].copy_(P.x)
 
         n_edit = sum(1 for s in steps if s.edit)
-        n_launch = sum(len(P.launches(False, temb=False)) + 1 for s in steps) + \
+        n_launch = sum(len(P.launches(False, temb=False)) + 1 + int(bool(compose_kb)) for s in steps) + \
             n_edit * (len(P.sweep_ops) + len(P.dec_mod_ops))
         g = {"zbuf": zbuf, "emb_table": emb_table, "pairs": pair_table, "c": c_table, "body": body, "graph": None,
              "launches": n_launch, "rec": rec, "n_edit": n_edit}
@@ -1139,6 +1148,8 @@ class UNetEngine:
                 P.emb_all.copy_(emb_table[0])
                 P.run_encoder()
                 P.run_sweep_and_decoder(lambda: None)
+                if compose_kb:
+                    ops.compose_rows(P.x, rec["compose_ref"][0], rec["compose_masks"])
             torch.cuda.current_stream().wait_stream(s_)
             torch.cuda.synchronize(dev)
             cg = torch.cuda.CUDAGraph()
@@ -1147,10 +1158,11 @@ class UNetEngine:
             g["graph"] = cg
         return g
 
-    def _sample_rows(self, x_T, schedule, noise, use_graph, out, record_process):
+    def _sample_rows(self, x_T, schedule, noise, use_graph, out, record_process, compose=None):
         N = x_T.shape[0]
         if schedule.N != N:
             raise ops._lib.AsyrpError(f"per-row schedule has {schedule.N} rows, x_T {N}")
+        compose_kb = self._check_compose(compose, x_T, schedule) if compose is not None else None
         if schedule.n_delta != self.n_delta or self.n_delta == 0:
             raise ops._lib.AsyrpError(f"per-row schedule carries coefficients for {schedule.n_delta} DeltaBlocks; the "
                                       f"engine packed {self.n_delta}")
@@ -1158,7 +1170,8 @@ class UNetEngine:
             raise ops._lib.AsyrpError("per-row schedules are not built with ASYRP_GN_FOLD (in-kernel GroupNorm sums)")
         own = own_blocks(schedule.hs_coeffs)
         P = self.plan(N)
-        key = (N, bool(use_graph), schedule.key(), own, bool(record_process))
+        key = (N, bool(use_graph), schedule.key(), own, bool(record_process)) + \
+            ((("compose",) + compose_kb,) if compose_kb else ())
         with torch.cuda.device(self.device):
             n_sto = schedule.n_stochastic
             if n_sto and (noise is None or noise.shape[0] != n_sto or noise.shape[1] != N):
@@ -1167,7 +1180,7 @@ class UNetEngine:
             self.state["slerp_t"], self.state["use_mask"], self.state["slerp_rows"] = 0.0, False, False
             g = self.graphs.pop(key, None)
             if g is None:
-                g = self._build_row_trajectory(P, schedule, use_graph, own, record_process)
+                g = self._build_row_trajectory(P, schedule, use_graph, own, record_process, compose_kb)
                 while len(self.graphs) >= self.MAX_GRAPHS:
                     self.graphs.pop(next(iter(self.graphs)))
             self.graphs[key] = g
@@ -1175,6 +1188,9 @@ class UNetEngine:
             self.last_records = g["rec"]
             g["pairs"].copy_(sweep_pairs(schedule.coeffs))
             g["c"].copy_(schedule.c)
+            if compose_kb:
+                g["rec"]["compose_masks"].copy_(compose[0])
+                g["rec"]["compose_ref"].copy_(compose[1])
             P.x.copy_(x_T, non_blocking=True)
             if n_sto:
                 g["zbuf"].copy_(noise, non_blocking=True)
@@ -1212,9 +1228,33 @@ class UNetEngine:
                 raise ops._lib.AsyrpError(f"blend: {name} lives on {t.device}, the engine on {self.device}")
         return B
 
+    def _check_compose(self, compose, x_T, schedule):
+        """(K, b) of a compose=(masks, ref) argument; AsyrpError unless it fits the batch of K b rows and the schedule"""
+        try:
+            masks, ref = compose
+        except (TypeError, ValueError):
+            raise ops._lib.AsyrpError("compose must be a pair (masks [K][b][H][W], ref [steps][b][C][H][W])") from None
+        N, Cx, H, W = x_T.shape
+        steps = len(schedule.steps)
+        if not (torch.is_tensor(masks) and torch.is_tensor(ref) and masks.dtype == ref.dtype == torch.float32):
+            raise ops._lib.AsyrpError("compose: masks and ref must be fp32 tensors")
+        K, b = (masks.shape[0], masks.shape[1]) if masks.dim() == 4 else (0, 0)
+        if not (1 <= K <= MAX_COMPOSE and b) or tuple(masks.shape) != (K, b, H, W) or N != K * b:
+            raise ops._lib.AsyrpError(f"compose: masks must be [K][b][{H}][{W}] with 1 <= K <= {MAX_COMPOSE} and the "
+                                      f"batch of {N} rows = K b, got {tuple(masks.shape)}")
+        if tuple(ref.shape) != (steps, b, Cx, H, W):
+            raise ops._lib.AsyrpError(f"compose: ref must be [{steps} steps][{b}][{Cx}][{H}][{W}], got "
+                                      f"{tuple(ref.shape)}")
+        cur = torch.cuda.current_device()
+        idx = lambda d: d.index if d.index is not None else cur  # noqa: E731
+        for name, t in (("masks", masks), ("ref", ref)):
+            if not t.is_cuda or idx(t.device) != idx(self.device):
+                raise ops._lib.AsyrpError(f"compose: {name} lives on {t.device}, the engine on {self.device}")
+        return K, b
+
     def sample(self, x_T, schedule, noise=None, use_graph=True, out=None, delta_hs=None, use_mask=False,
                record_dh=False, record_process=False, hs_coeffs=None, lpips=None, record_h=False, h_direction=None,
-               blend=None):
+               blend=None, compose=None):
         """Run the reverse trajectory of `schedule` (sampler.Schedule) from x_T; returns x_0 (fp32 NCHW).
 
         The step list, the edit/plain/stochastic phase of every step and all sampler coefficients are host-side
@@ -1261,13 +1301,22 @@ class UNetEngine:
         m = mask[n % B] (ops.blend_rows), N a multiple of B.  ref is the origin pass's x after every step (its
         record_process "x").  Mask and reference are graph inputs, copied in before every replay: every batch of B
         images replays one graph.  A mask of ones gives the unblended trajectory and a mask of zeros ref[-1], bit for
-        bit.  It does not combine with lpips."""
+        bit.  It does not combine with lpips.
+
+        compose: (masks fp32 [K][b][H][W], ref fp32 [steps][b][C][H][W]) composes K attribute edits into one image
+        per region (region.py), with a per-row schedule of N = K b rows, attribute-major (row k b + j: attribute k,
+        image j), 1 <= K <= 8.  After every step's update, before anything is recorded, the K rows of image j are all
+        replaced by w_0 ref[k][j] + sum_k w_k x[k b + j] (ops.compose_rows), with w_k = M_k and w_0 = 1 - sum M, or
+        M_k / sum M and 0 where the masks sum above 1.  Masks and reference are graph inputs, copied in before every
+        replay: every batch replays one graph.  With K = 1 it is blend= on the same rows, bit for bit."""
         if isinstance(schedule, RowSchedule):
             if delta_hs is not None or record_dh or hs_coeffs is not None or lpips is not None or record_h or \
                     h_direction is not None or blend is not None:
                 raise ops._lib.AsyrpError("a per-row schedule takes no delta_hs, record_dh, hs_coeffs, lpips, "
                                           "record_h, h_direction or blend")
-            return self._sample_rows(x_T, schedule, noise, use_graph, out, record_process)
+            return self._sample_rows(x_T, schedule, noise, use_graph, out, record_process, compose)
+        if compose is not None:
+            raise ops._lib.AsyrpError("compose= needs a per-row schedule (schedule.RowSchedule)")
         N = x_T.shape[0]
         additive = h_direction is not None
         add_table = None

@@ -195,6 +195,14 @@ def build_parser():
     p.add_argument('--edit_region_feather', type=float, default=0.0,
                    help='--edit_region: soften the mask edge with a Gaussian of this sigma in pixels, 0..16 (0: hard '
                         'edge)')
+    p.add_argument('--region_compose', type=str, default=None,
+                   help='--run_test: compose several attribute edits into one image, each in its own face-parsing '
+                        'region ("smiling=mouth,u_lip,l_lip grey_hair=hair"; at most 8 attributes, no class shared).  '
+                        'Each attribute runs with its own DeltaBlock (the checkpoint name\'s "attribute" replaced), '
+                        't_edit and t_addnoise, as --attr_sweep; after every step its rows are replaced by a per-pixel '
+                        'mix of the attributes and the origin pass, weighted by the --seg_weights masks of the origin '
+                        'pass (--edit_region_dilate / --edit_region_feather apply to every mask, overlaps are '
+                        'normalised).  The masks are written as <file>_ngen<n>_region_compose.png')
     return p
 
 

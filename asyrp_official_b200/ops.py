@@ -406,6 +406,30 @@ def blend_rows(x, ref, mask):
     check(lib.asyrp_blend_rows(_ptr(x), _ptr(ref), _ptr(mask), N, B, Cc, H * W, _stream()), "asyrp_blend_rows")
 
 
+def compose_rows(x, ref, masks):
+    """in place, the K attribute rows of every image replaced by their per-pixel composite against ref: x fp32
+    [K B][C][H][W] attribute-major (row k B + j), ref fp32 [B][C][H][W], masks fp32 [K][B][H][W], 1 <= K <= 8.  Weights
+    w_k = M_k, w_0 = 1 - sum M (or M_k / sum M and 0 where the masks sum above 1); every row of image j becomes
+    w_0 r + sum_k w_k x[k B + j], each step rounded in fp32 in that order (asyrp_compose_rows)"""
+    lib = _lib.load()
+    _need_cuda(x, ref, masks)
+    if not (x.dtype == ref.dtype == masks.dtype == torch.float32 and x.is_contiguous() and ref.is_contiguous()
+            and masks.is_contiguous()):
+        raise _lib.AsyrpError(f"compose_rows: x, ref and masks must be contiguous fp32 tensors, got {x.dtype}, "
+                              f"{ref.dtype} and {masks.dtype}")
+    if x.dim() != 4 or ref.dim() != 4 or masks.dim() != 4:
+        raise _lib.AsyrpError(f"compose_rows: x [K B][C][H][W], ref [B][C][H][W] and masks [K][B][H][W], got "
+                              f"{tuple(x.shape)}, {tuple(ref.shape)} and {tuple(masks.shape)}")
+    N, Cc, H, W = x.shape
+    K, B = masks.shape[0], ref.shape[0]
+    if tuple(ref.shape[1:]) != (Cc, H, W) or tuple(masks.shape) != (K, B, H, W) or N != K * B:
+        raise _lib.AsyrpError(f"compose_rows: ref must be [B][{Cc}][{H}][{W}] and masks [K][B][{H}][{W}] with N = {N} "
+                              f"= K B, got {tuple(ref.shape)} and {tuple(masks.shape)}")
+    if len({x.device, ref.device, masks.device}) != 1:
+        raise _lib.AsyrpError(f"compose_rows: x, ref and masks live on {x.device}, {ref.device} and {masks.device}")
+    check(lib.asyrp_compose_rows(_ptr(x), _ptr(ref), _ptr(masks), K, B, Cc, H * W, _stream()), "asyrp_compose_rows")
+
+
 def _mask_pair(name, inp, out):
     _need_cuda(inp, out)
     if not (inp.dtype == out.dtype == torch.float32 and inp.is_contiguous() and out.is_contiguous()

@@ -1,5 +1,6 @@
 """Region-restricted edits (`--edit_region`): a soft mask per image from the face parser's labels of the origin pass,
-and what the edit pass blends with it.
+and what the edit pass blends with it.  `--region_compose` builds one such mask per attribute and composes the
+attributes' edit passes into one image (UNetEngine.sample's compose).
 
 Asyrp edits the 8x8 bottleneck h, and the decoder spreads the change over the whole image.  With a region, every step
 of the edit pass ends with x <- m x + (1 - m) x_orig, where x_orig is the origin pass (the unedited trajectory of the
@@ -31,20 +32,50 @@ CLASSES = ("background", "skin", "l_brow", "r_brow", "l_eye", "r_eye", "eye_g", 
 MAX_DILATE = 32
 MAX_FEATHER = 16.0
 MAX_SIZE = 512  # the parser's label maps
+MAX_COMPOSE = 8  # attributes of one --region_compose composite (asyrp_compose_rows)
 
 
-def parse_classes(text):
-    """'hair hat' -> the class indices in the order given; ValueError for an unknown, repeated or missing name"""
+def parse_classes(text, flag="--edit_region"):
+    """'hair hat' -> the class indices in the order given; ValueError for an unknown, repeated or missing name, naming
+    `flag`"""
     names = str(text).split()
     if not names:
-        raise ValueError(f"--edit_region names no class; valid names: {' '.join(CLASSES)}")
+        raise ValueError(f"{flag} names no class; valid names: {' '.join(CLASSES)}")
     out = []
     for name in names:
         if name not in CLASSES:
-            raise ValueError(f"--edit_region: unknown class {name!r}; valid names: {' '.join(CLASSES)}")
+            raise ValueError(f"{flag}: unknown class {name!r}; valid names: {' '.join(CLASSES)}")
         if CLASSES.index(name) in out:
-            raise ValueError(f"--edit_region: class {name!r} given twice; valid names: {' '.join(CLASSES)}")
+            raise ValueError(f"{flag}: class {name!r} given twice; valid names: {' '.join(CLASSES)}")
         out.append(CLASSES.index(name))
+    return out
+
+
+def parse_compose(text):
+    """--region_compose 'smiling=mouth,u_lip,l_lip grey_hair=hair' -> [(attribute, class indices)] in the order
+    given; ValueError for a malformed item, an attribute named twice, an empty, unknown or repeated class, a class
+    given to two attributes, or more than MAX_COMPOSE attributes"""
+    flag = "--region_compose"
+    out = []
+    for item in str(text).split():
+        attr, sep, names = item.partition("=")
+        if not sep or not attr or "=" in names:
+            raise ValueError(f"{flag}: {item!r} is not attribute=class,class,..")
+        if attr in [a for a, _ in out]:
+            raise ValueError(f"{flag} names attribute {attr!r} twice")
+        if not names or "" in names.split(","):
+            raise ValueError(f"{flag}: attribute {attr!r} has an empty class list or an empty class name "
+                             f"({names!r}); valid names: {' '.join(CLASSES)}")
+        classes = parse_classes(names.replace(",", " "), f"{flag} ({attr})")
+        for a, other in out:
+            shared = [CLASSES[c] for c in classes if c in other]
+            if shared:
+                raise ValueError(f"{flag}: class(es) {' '.join(shared)} given to both {a!r} and {attr!r}")
+        out.append((attr, classes))
+    if not out:
+        raise ValueError(f"{flag} names no attribute")
+    if len(out) > MAX_COMPOSE:
+        raise ValueError(f"{flag} composes at most {MAX_COMPOSE} attributes, got {len(out)}")
     return out
 
 
@@ -102,3 +133,14 @@ def region_masks(parser, origin, classes, r=0, sigma=0.0):
     S = origin.shape[-1]
     check_options(r, sigma, S)
     return masks_from_labels(parser.labels(origin), classes, S, r, sigma)
+
+
+@torch.no_grad()
+def compose_masks(parser, origin, class_lists, r=0, sigma=0.0):
+    """--region_compose's masks of a batch: the origin pass's x0 (fp32 [B][3][S][S]) parsed once, then one soft mask
+    per attribute and image from that attribute's classes, fp32 [K][B][S][S] on the parser's device.  Attribute k's
+    masks are region_masks(parser, origin, class_lists[k], r, sigma)."""
+    S = origin.shape[-1]
+    check_options(r, sigma, S)
+    labels = parser.labels(origin)
+    return torch.stack([masks_from_labels(labels, classes, S, r, sigma) for classes in class_lists])

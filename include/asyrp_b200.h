@@ -490,8 +490,15 @@ int asyrp_h_combine(const float* x, const double* w, const double* mu, double* o
  * asyrp_mask_blur: out[i] = sum_{k=-R..R} taps[k + R] in[clamp(i + k, 0, S - 1)] along axis, fp32 fmaf in tap order; a
  *   window whose inputs are all equal gives that value exactly.  taps fp32 [2R + 1] on the device, 0 <= R <= 48.
  * The mask kernels take fp32 [N][S][S] images, 4-byte aligned; out must not be in.
+ * asyrp_compose_rows: in place, the K attribute rows of every image replaced by one composite against the origin
+ *   pass: x fp32 [K B][C][HW] attribute-major (row k B + j), ref fp32 [B][C][HW], masks fp32 [K][B][HW].  Per pixel,
+ *   in fp32: s = M_1 + .. + M_K in order; w_k = M_k, w_0 = 1 - s if s <= 1, else w_k = M_k / s, w_0 = 0; then
+ *   acc = w_0 r and acc = fmaf(w_k, x[k B + j], acc) for k = 1..K, written to all K rows of image j.  With K = 1 this
+ *   is asyrp_blend_rows bit for bit.  1 <= K <= 8, B, C, HW > 0; 64-bit indexing.  With HW % 4 == 0 the three
+ *   pointers must be 16-byte aligned (float4 loads), else 4-byte aligned.
  * No allocation, no synchronisation, no atomics. */
 int asyrp_blend_rows(float* x, const float* ref, const float* mask, int N, int B, int C, int HW, void* stream);
+int asyrp_compose_rows(float* x, const float* ref, const float* masks, int K, int B, int C, int HW, void* stream);
 int asyrp_region_mask(const unsigned char* labels, unsigned class_bits, float* mask, int N, int S, void* stream);
 int asyrp_mask_dilate(const float* in, float* out, int N, int S, int r, int axis, void* stream);
 int asyrp_mask_blur(const float* in, const float* taps, float* out, int N, int S, int R, int axis, void* stream);

@@ -73,6 +73,9 @@ SIGNATURES = {
                                   c_int, c_float, c_float, c_float, c_float, c_void_p]),
     "asyrp_ddim_update_rows": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int,
                                        c_int, c_int, c_float, c_float, c_void_p, c_void_p]),
+    "asyrp_ddim_update_anchored": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
+                                           c_void_p, c_int, c_int, c_int, c_int, c_int, c_float, c_float, c_float,
+                                           c_void_p, c_void_p]),
     "asyrp_ddpm_update": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_float, c_float,
                                   c_float, c_int, c_float, c_void_p]),
     "asyrp_axpby": (c_int, [c_void_p, c_void_p, c_void_p, c_float, c_float, C.c_longlong, c_void_p]),

@@ -378,7 +378,7 @@ class Asyrp(object):
         can mix attributes or edit strengths."""
         eng = model.engine
         dev = eng.device
-        if schedule.n_stochastic and noise is None:
+        if schedule.n_stochastic and noise is None and sample_kw.get("anchors") is None:  # anchored: no noise
             noise = torch.randn((schedule.n_stochastic, *x_lat.shape), device=dev)
         elif noise is not None:
             noise = noise.to(dev, non_blocking=True)
@@ -403,7 +403,7 @@ class Asyrp(object):
                    save_process_delta_h=False, save_process_origin=False, x0_tensor=None, delta_h_dict=None,
                    get_delta_hs=False, folder_dir="", file_name="", hs_coeff=(1.0, 1.0), h_direction=None,
                    sweep_times=None, scorers=None, mode=None, batch_ids=None, x0_source=None, edit_region=None,
-                   region_compose=None):
+                   region_compose=None, anchors=None):
         """rows of the grid: [x0] [origin DDIM] one row per hs_coeff tuple  (diffusion_latent.py:445-544).
 
         delta_h_dict: {t: None | Δh tensor}.  Entries that are tensors select the explicit-Δh branch for that step
@@ -425,7 +425,11 @@ class Asyrp(object):
         attribute, coefficients per attribute).  As with edit_region the origin pass records its trajectory and always
         runs; its x0 gives K masks per image (region.compose_masks), written as <file>_ngen<n>_region_compose.png
         (one row per attribute), and hs_coeff is the one tuple the composite is scored as.  The grid's last row is the
-        composite of every image (compose_batch)."""
+        composite of every image (compose_batch).
+        anchors (--exact_inversion): the inversion.Anchors of the batch's input images (anchor_batch), x_lat_tensor
+        their x_T.  No origin pass runs: the origin is the input image, which an unedited anchored pass returns bit for
+        bit.  Every edit pass is anchored (UNetEngine.sample's anchors, no noise drawn), and the region masks parse the
+        input image and blend against the anchors' trajectory A[1:]."""
         import torchvision.utils as tvu
         a = self.args
         time_s = time.time()
@@ -436,7 +440,12 @@ class Asyrp(object):
             x_list.append(x0_tensor.cpu())
         blend = None
         masked = edit_region is not None or region_compose is not None  # the edits follow the recorded origin pass
-        if save_x_origin or (scorers is not None and scorers.needs_origin) or masked:
+        kw_a = {"anchors": anchors} if anchors is not None else {}
+        if anchors is not None and (save_x_origin or (scorers is not None and scorers.needs_origin) or masked):
+            origin = anchors.x0.cpu()  # the anchored origin pass: the input image, exactly
+            if save_x_origin:
+                x_list.append(origin)
+        elif save_x_origin or (scorers is not None and scorers.needs_origin) or masked:
             sch = self.make_schedule(seq_inv, seq_inv_next, (1.0,), edit=False,
                                      addnoise=bool(getattr(a, "origin_process_addnoise", False)))
             if save_x_origin:
@@ -447,9 +456,11 @@ class Asyrp(object):
             else:  # the pass only the score needs leaves the random stream as it was: the edits draw the same noise
                 with torch.random.fork_rng(devices=[eng.device]):
                     origin = self.edit_batch(model, x_lat_tensor, sch, record_process=masked)
+        if masked:
+            # the origin pass's trajectory; anchored, the inversion's (the anchors are copies the replays do not reuse)
+            ref = anchors.ref if anchors is not None else eng.last_records["x"].clone()
             if edit_region is not None:
                 from .region import region_masks
-                ref = eng.last_records["x"].clone()  # owned by the origin graph: the edit replays would reuse it
                 parser, classes, r, sigma = edit_region
                 mask = region_masks(parser, origin, classes, r, sigma).to(eng.device)
                 blend = (mask, ref)
@@ -458,7 +469,6 @@ class Asyrp(object):
                                os.path.join(folder_dir, f'{file_name}_ngen{a.n_train_step}_region_mask.png'))
             if region_compose is not None:
                 from . import region
-                ref = eng.last_records["x"].clone()  # owned by the origin graph: the edit replays would reuse it
                 parser, classes, r, sigma, times, row_coeffs = region_compose
                 masks = region.compose_masks(parser, origin, classes, r, sigma).to(eng.device)
                 os.makedirs(folder_dir, exist_ok=True)
@@ -467,14 +477,15 @@ class Asyrp(object):
         coeffs = hs_coeff if isinstance(hs_coeff, list) else [hs_coeff]
         edited = []
         if region_compose is not None:
-            edited = [self.compose_batch(model, x_lat_tensor, seq_inv, seq_inv_next, masks, ref, times, row_coeffs)]
+            edited = [self.compose_batch(model, x_lat_tensor, seq_inv, seq_inv_next, masks, ref, times, row_coeffs,
+                                         **kw_a)]
         elif sweep_times is not None:
             tpc, chunks = plan_sweep(len(coeffs), bs, getattr(a, "max_rows_per_replay", 16))
             for chunk in chunks:
                 rows = sweep_rows(chunk, tpc, bs)
                 sch = self.sweep_schedule(seq_inv, seq_inv_next, [sweep_times[k] for k in rows],
                                           [coeffs[k] for k in rows])
-                x0 = self.edit_batch(model, pad_rows(x_lat_tensor.repeat(len(chunk), 1, 1, 1), tpc * bs), sch)
+                x0 = self.edit_batch(model, pad_rows(x_lat_tensor.repeat(len(chunk), 1, 1, 1), tpc * bs), sch, **kw_a)
                 edited += [x0[j * bs:(j + 1) * bs].clone() for j in range(len(chunk))]
         elif not getattr(a, "pass_editing", False):
             # the reference replays the trajectory once per tuple (:495-532); the tuples share x_T and the schedule, so
@@ -506,6 +517,7 @@ class Asyrp(object):
                     kw["h_direction"] = dirs
             if blend is not None:  # rows are tuple-major blocks of the bs images: row n blends with image n % bs
                 kw["blend"] = blend
+            kw.update(kw_a)  # anchored rows, like the blend, take image n % bs
             max_rows = getattr(a, "max_rows_per_replay", 16)
             if "delta_hs" in kw and len({float(tup[0]) for tup in coeffs}) > 1:
                 max_rows = 0  # explicit Δh takes one slerp weight 1 - c0 per replay: one tuple per chunk
@@ -519,7 +531,7 @@ class Asyrp(object):
                 sch = self.make_schedule(seq_inv, seq_inv_next, coeffs[chunk[0]])
                 rows_x = pad_rows(x_lat_tensor.repeat(len(chunk), 1, 1, 1), tpc * bs)
                 noise = None
-                if sch.n_stochastic:  # the per-tuple draws of the sequential loop, in tuple order
+                if sch.n_stochastic and anchors is None:  # the per-tuple draws of the sequential loop, in tuple order
                     noise = chunk_noise(len(chunk), tpc, bs, lambda: torch.randn(
                         (sch.n_stochastic, *x_lat_tensor.shape), device=eng.device))
                 if per_row:
@@ -597,6 +609,7 @@ class Asyrp(object):
         a = self.args
         self.edit_region_setup()  # refuses --lpips
         self.region_compose_setup()  # refuses --lpips
+        self.exact_inversion_setup()  # refuses --lpips
         if getattr(a, "content_preservation", False):
             self.content_preservation_setup()  # refuses --lpips
         if self.world > 1:
@@ -679,8 +692,29 @@ class Asyrp(object):
                 batch = []
 
     @torch.no_grad()
+    def anchor_batch(self, model, x0):
+        """--exact_inversion: the inversion.Anchors of the input images x0 [B][C][S][S] (UNetEngine.anchors on the
+        --n_inv_step DDIM inversion grid), on the device"""
+        a = self.args
+        seq, seq_next = make_sequences(a.t_0, a.n_inv_step)
+        eng = model.engine
+        return eng.anchors(x0.to(eng.device), Schedule.inversion(self.betas, seq, seq_next))
+
+    def _edit_batches(self, model, pairs, scorers, exact):
+        """_batches, with the batch's anchors appended (None without --exact_inversion).  Anchored, x_T is the
+        anchors' A[0], inverted here from the batch's input images; the cached x_T of the pairs is not used."""
+        for mode, step, x_lat, x0, ids, x0_source in self._batches(pairs, scorers.keeps_source or exact):
+            anchors = None
+            if exact:
+                anchors = self.anchor_batch(model, x0_source)
+                x_lat = anchors.x_T
+                x0_source = x0_source if scorers.keeps_source else None
+            yield mode, step, x_lat, x0, ids, x0_source, anchors
+
+    @torch.no_grad()
     def run_test(self):
         a = self.args
+        exact = self.exact_inversion_setup()
         scoring.fid_options_check(self)
         compose_spec = self.region_compose_setup()  # refuses --attr_sweep, --edit_region and --h_direction too
         region_spec = self.edit_region_setup()  # refuses --attr_sweep too, before it is dispatched
@@ -816,7 +850,7 @@ class Asyrp(object):
                     classes, r, sigma, seg_sd = region_spec
                     region_spec = None
                     edit_region = (scorers.nets.get("seg") or FaceParser(seg_sd, device=self.device), classes, r, sigma)
-                for mode, step, x_lat, x0, ids, x0_source in self._batches(pairs, scorers.keeps_source):
+                for mode, step, x_lat, x0, ids, x0_source, anchors in self._edit_batches(model, pairs, scorers, exact):
                     results[(mode, step)] = self.save_image(
                         model, x_lat, seq_test, seq_test_next, save_x0=a.save_x0, save_x_origin=a.save_x_origin,
                         x0_tensor=x0, delta_h_dict=delta_h_dict, get_delta_hs=bool(num_mean),
@@ -824,7 +858,7 @@ class Asyrp(object):
                         save_process_delta_h=bool(getattr(a, "save_process_delta_h", False)),
                         folder_dir=a.test_image_folder, file_name=f'{mode}_{step}_{a.n_iter - 1}', hs_coeff=hs_coeff,
                         h_direction=h_direction, scorers=scorers, mode=mode, batch_ids=ids, x0_source=x0_source,
-                        edit_region=edit_region)
+                        edit_region=edit_region, **({"anchors": anchors} if exact else {}))
                     # the last image of the pass ends it before the mean is taken
                     if mode == "train" and num_mean and step == num_mean - 1 and step != a.n_train_img - 1:
                         # mean over the first num_mean images per timestep, key 0 = mean over timesteps (:811-832)
@@ -852,6 +886,35 @@ class Asyrp(object):
 
 
     # ------------------------------------------------------------------------------------------
+    def exact_inversion_setup(self):
+        """--exact_inversion's requirements, checked before any model loads: False without the flag, else True.
+        ValueError with the reason."""
+        a = self.args
+        if not getattr(a, "exact_inversion", False):
+            return False
+        if not getattr(a, "run_test", False):
+            raise ValueError("--exact_inversion anchors the edits of --run_test to their input images: add --run_test")
+        for flag, on, why in (
+                ("--load_random_noise", getattr(a, "load_random_noise", False), "a random latent has no input image"),
+                ("--saved_random_noise", getattr(a, "saved_random_noise", False), "a random latent has no input image"),
+                ("--sample_type ddpm", getattr(a, "sample_type", "ddim") == "ddpm",
+                 "the ancestral step has no anchored form"),
+                ("--origin_process_addnoise", getattr(a, "origin_process_addnoise", False),
+                 "there is no origin pass: the origin is the input image"),
+                ("--save_process_origin", getattr(a, "save_process_origin", False),
+                 "there is no origin pass: the origin is the input image"),
+                ("--lpips", getattr(a, "lpips", False), "it edits nothing"),
+                ("--diff_style", getattr(a, "diff_style", False), "it is not a --run_test edit"),
+                ("--h_directions", getattr(a, "h_directions", False), "it edits nothing"),
+                ("--num_mean_of_delta_hs", getattr(a, "num_mean_of_delta_hs", 0),
+                 "the mean Δh must come from the unanchored pass")):
+            if on:
+                raise ValueError(f"--exact_inversion does not combine with {flag}: {why}")
+        if a.n_test_step != a.n_inv_step:
+            raise ValueError(f"--exact_inversion needs --n_test_step equal to --n_inv_step: the edit steps run on the "
+                             f"inversion's grid, got {a.n_test_step} and {a.n_inv_step}")
+        return True
+
     def edit_region_setup(self):
         """--edit_region's requirements, checked before any model loads: None without the flag, else (class indices,
         --edit_region_dilate, --edit_region_feather, the --seg_weights state dict).  ValueError with the reason."""
@@ -977,6 +1040,7 @@ class Asyrp(object):
         a = self.args
         self.edit_region_setup()  # refuses --h_directions
         self.region_compose_setup()  # refuses --h_directions
+        self.exact_inversion_setup()  # refuses --h_directions
         mode, arg = self.h_directions_setup()
         seq, seq_next = make_sequences(a.t_0, a.n_test_step)
         size = self.config.data.image_size
@@ -1099,6 +1163,7 @@ class Asyrp(object):
         a = self.args
         print("Running Test (attribute sweep)")
         attrs, paths = self.attr_sweep_setup()
+        exact = self.exact_inversion_setup()
         scorers = scoring.Scorers(self, attrs)
         times = self.attr_sweep_schedules(attrs)
         self.sweep_times = dict(zip(attrs, times))
@@ -1107,11 +1172,12 @@ class Asyrp(object):
         model, coeffs, pairs = self.attribute_run(paths)
         results = {}
         with scorers:
-            for mode, step, x_lat, x0, ids, x0_source in self._batches(pairs, scorers.keeps_source):
+            for mode, step, x_lat, x0, ids, x0_source, anchors in self._edit_batches(model, pairs, scorers, exact):
                 results[(mode, step)] = self.save_image(
                     model, x_lat, seq_test, seq_test_next, save_x0=a.save_x0, save_x_origin=a.save_x_origin,
                     x0_tensor=x0, folder_dir=a.test_image_folder, file_name=f'{mode}_{step}_{a.n_iter - 1}',
-                    hs_coeff=coeffs, sweep_times=times, scorers=scorers, mode=mode, batch_ids=ids, x0_source=x0_source)
+                    hs_coeff=coeffs, sweep_times=times, scorers=scorers, mode=mode, batch_ids=ids, x0_source=x0_source,
+                    **({"anchors": anchors} if exact else {}))
             scorers.finish(coeffs)
         return results
 
@@ -1156,6 +1222,7 @@ class Asyrp(object):
         a = self.args
         print("Running Test (region composite)")
         attrs, classes, r, sigma, seg_sd, paths = spec
+        exact = self.exact_inversion_setup()
         scorers = scoring.Scorers(self, ["+".join(attrs)])
         times = self.attr_sweep_schedules(attrs)  # prints each attribute's t_edit and t_addnoise
         self.compose_times = dict(zip(attrs, times))
@@ -1166,34 +1233,38 @@ class Asyrp(object):
         with scorers:  # --seg_consistency's parser serves the masks too
             compose = (scorers.nets.get("seg") or FaceParser(seg_sd, device=self.device), classes, r, sigma, times,
                        coeffs)
-            for mode, step, x_lat, x0, ids, x0_source in self._batches(pairs, scorers.keeps_source):
+            for mode, step, x_lat, x0, ids, x0_source, anchors in self._edit_batches(model, pairs, scorers, exact):
                 results[(mode, step)] = self.save_image(
                     model, x_lat, seq_test, seq_test_next, save_x0=a.save_x0, save_x_origin=a.save_x_origin,
                     x0_tensor=x0, folder_dir=a.test_image_folder, file_name=f'{mode}_{step}_{a.n_iter - 1}',
                     hs_coeff=tuples, scorers=scorers, mode=mode, batch_ids=ids, x0_source=x0_source,
-                    region_compose=compose)
+                    region_compose=compose, **({"anchors": anchors} if exact else {}))
             scorers.finish(tuples)
             compose = None  # the parser goes with the scorers' networks, and the CUDA cache after it
         return results
 
-    def compose_batch(self, model, x_lat, seq, seq_next, masks, ref, times, coeffs):
+    def compose_batch(self, model, x_lat, seq, seq_next, masks, ref, times, coeffs, anchors=None):
         """--region_compose's edit pass of one batch of B images: x_lat [B][C][S][S], masks [K][B][S][S] and the origin
         pass's trajectory ref [steps][B][C][S][S] on the device, times / coeffs per attribute.  Images run in chunks of
         b = --max_rows_per_replay // K (plan_compose) as K b rows, attribute-major, the last chunk padded, so that every
         chunk replays one graph.  The noise is one draw [n_stochastic][B][..] for the batch, each chunk's images
-        repeated over its K rows (compose_noise).  Returns the composites [B][C][S][S] on the host."""
+        repeated over its K rows (compose_noise).  anchors (--exact_inversion): the batch's inversion.Anchors; each chunk
+        takes its images' anchors, padded as its latents are, and draws no noise.  Returns the composites [B][C][S][S]
+        on the host."""
         eng = model.engine
         K, bs = masks.shape[0], x_lat.shape[0]
         b, chunks = plan_compose(bs, K, getattr(self.args, "max_rows_per_replay", 16))
         sch = self.sweep_schedule(seq, seq_next, [times[k] for k in range(K) for _ in range(b)],
                                   [coeffs[k] for k in range(K) for _ in range(b)])
-        z = torch.randn((sch.n_stochastic, *x_lat.shape), device=eng.device) if sch.n_stochastic else None
+        z = torch.randn((sch.n_stochastic, *x_lat.shape), device=eng.device) \
+            if sch.n_stochastic and anchors is None else None
         per_image = lambda t, j0, j1: pad_rows(t[:, j0:j1].transpose(0, 1), b).transpose(0, 1)  # noqa: E731
         out = []
         for j0, j1 in chunks:
+            kw = {"anchors": anchors.images(j0, j1, b)} if anchors is not None else {}
             x0 = self.edit_batch(model, pad_rows(x_lat[j0:j1], b).repeat(K, 1, 1, 1), sch,
                                  noise=compose_noise(z[:, j0:j1], b, K) if z is not None else None,
-                                 compose=(per_image(masks, j0, j1), per_image(ref, j0, j1)))
+                                 compose=(per_image(masks, j0, j1), per_image(ref, j0, j1)), **kw)
             out.append(x0[:j1 - j0].clone())  # every attribute's row of an image holds its composite
         return torch.cat(out)
 
@@ -1301,6 +1372,7 @@ class Asyrp(object):
         self.prdc_check()
         self.edit_region_setup()  # refuses --diff_style
         self.region_compose_setup()  # refuses --diff_style
+        self.exact_inversion_setup()  # refuses --diff_style
         if getattr(a, "content_preservation", False):
             self.content_preservation_setup()  # refuses --diff_style
         if getattr(a, "fid", False):

@@ -942,11 +942,13 @@ class UNetEngine:
     MAX_GRAPHS = 4  # captured trajectory graphs kept per engine (least recently used is dropped)
 
     def _build_trajectory(self, P, schedule, use_graph, explicit, record_dh, record_process, lpips=None,
-                          record_h=False, additive=False, blend_B=0):
+                          record_h=False, additive=False, blend_B=0, anchor_B=0):
         """per-(batch, schedule) state: the timestep-embedding table, the noise buffer, the step loop and its graph.
-        blend_B: the images of a region blend (0: none); the graph then owns its mask and reference trajectory"""
+        blend_B: the images of a region blend (0: none); the graph then owns its mask and reference trajectory.
+        anchor_B: the images of an anchored trajectory (0: none); the graph then owns its anchor tables and every
+        update is ddim_update_anchored"""
         steps = schedule.steps
-        n_sto = schedule.n_stochastic
+        n_sto = 0 if anchor_B else schedule.n_stochastic  # an anchored trajectory draws no noise
         zbuf = torch.zeros((max(n_sto, 1), *P.x.shape), dtype=torch.float32, device=self.device)
         # timestep MLP + every per-block projection depend on t only: evaluate them once per step here (4 launches
         # each, outside the graph); inside the graph a step just copies its row into the buffer the convs read
@@ -977,6 +979,8 @@ class UNetEngine:
             rec["blend_mask"] = torch.zeros((blend_B, *P.x.shape[2:]), dtype=torch.float32, device=self.device)
             rec["blend_ref"] = torch.zeros((len(steps), blend_B, *P.x.shape[1:]), dtype=torch.float32,
                                            device=self.device)
+        if anchor_B:
+            rec["anchor_x"], rec["anchor_eps"] = self._anchor_tables(len(steps), anchor_B, P)
         N = P.x.shape[0]
         if lpips is not None:
             # LPIPS(x_t, x_start) and LPIPS(x0_t, x_start) after every step (compute_lpips_distance,
@@ -1022,11 +1026,15 @@ class UNetEngine:
                 else:
                     P.run_decoder()
                 z = None
-                if s.stochastic:
+                if s.stochastic and not anchor_B:
                     z = zbuf[zi]
                     zi += 1
                 if s.kind == "ddpm":
                     ops.ddpm_update(P.x, P.et, z, P.x, s.at, s.bt, s.logvar, learned_sigma, s.mask)
+                elif anchor_B:  # no noise: the same c1 z in the row's and the anchor's update would cancel
+                    ops.ddim_update_anchored(P.x, P.et, P.et_mod if edit else P.et, P.x,
+                                             rec["x0_t"][k] if record_process else None, rec["anchor_x"][k],
+                                             rec["anchor_x"][k + 1], rec["anchor_eps"][k], s.at, s.an, s.c2)
                 else:
                     x0_out = rec["x0_t"][k] if record_process else (xs[N:] if lpips is not None else None)
                     ops.ddim_update(P.x, P.et, P.et_mod if edit else P.et, z, P.x, x0_out, s.at, s.an, s.c1, s.c2)
@@ -1064,6 +1072,8 @@ class UNetEngine:
                     lpips_step(0)
                 if blend_B:
                     ops.blend_rows(P.x, rec["blend_ref"][0], rec["blend_mask"])
+                if anchor_B:
+                    self._warm_anchored(P, steps[0], rec)
             torch.cuda.current_stream().wait_stream(s_)
             torch.cuda.synchronize(self.device)
             cg = torch.cuda.CUDAGraph()
@@ -1072,16 +1082,18 @@ class UNetEngine:
             g["graph"] = cg
         return g
 
-    def _build_row_trajectory(self, P, schedule, use_graph, own, record_process, compose_kb=None):
+    def _build_row_trajectory(self, P, schedule, use_graph, own, record_process, compose_kb=None, anchor_B=0):
         """the trajectory of a per-row schedule (schedule.RowSchedule): per step the step's rows of the DeltaBlock pair
         table and of the (c1, c2) table are copied into the buffers the kernels read, as the timestep-embedding row is;
         on edit steps every DeltaBlock runs from middle_h, each editing row's output is copied into h2, and the rows
         that do not edit take et as et_mod; the update is ddim_update_rows.
         compose_kb: (K attributes, b images) of a region composite (None: none); the graph then owns its masks and
-        reference trajectory, and every update is followed by compose_rows"""
+        reference trajectory, and every update is followed by compose_rows.
+        anchor_B: the images of an anchored trajectory (0: none); every update is then ddim_update_anchored with the
+        rows' c2 from the (c1, c2) table"""
         steps = schedule.steps
         N, dev = P.x.shape[0], self.device
-        n_sto = schedule.n_stochastic
+        n_sto = 0 if anchor_B else schedule.n_stochastic  # an anchored trajectory draws no noise
         P.build_sweep()
         zbuf = torch.zeros((max(n_sto, 1), *P.x.shape), dtype=torch.float32, device=dev)
         emb_table = torch.empty((len(steps), *P.emb_all.shape), dtype=torch.float32, device=dev)
@@ -1100,6 +1112,8 @@ class UNetEngine:
             Kc, bc = compose_kb
             rec["compose_masks"] = torch.zeros((Kc, bc, *P.x.shape[2:]), dtype=torch.float32, device=dev)
             rec["compose_ref"] = torch.zeros((len(steps), bc, *P.x.shape[1:]), dtype=torch.float32, device=dev)
+        if anchor_B:
+            rec["anchor_x"], rec["anchor_eps"] = self._anchor_tables(len(steps), anchor_B, P)
         h2 = P.h2
 
         def selector(s):
@@ -1126,11 +1140,16 @@ class UNetEngine:
                 else:
                     P.run_decoder()
                 z = None
-                if s.stochastic:
+                if s.stochastic and not anchor_B:
                     z = zbuf[zi]
                     zi += 1
-                ops.ddim_update_rows(P.x, P.et, P.et_mod if s.edit else P.et, z, P.x,
-                                     rec["x0_t"][k] if record_process else None, s.at, s.an, c12)
+                if anchor_B:  # no noise: the same c1 z in the row's and the anchor's update would cancel
+                    ops.ddim_update_anchored(P.x, P.et, P.et_mod if s.edit else P.et, P.x,
+                                             rec["x0_t"][k] if record_process else None, rec["anchor_x"][k],
+                                             rec["anchor_x"][k + 1], rec["anchor_eps"][k], s.at, s.an, c12=c12)
+                else:
+                    ops.ddim_update_rows(P.x, P.et, P.et_mod if s.edit else P.et, z, P.x,
+                                         rec["x0_t"][k] if record_process else None, s.at, s.an, c12)
                 if compose_kb:  # the K rows of every image continue from their composite against the origin pass
                     ops.compose_rows(P.x, rec["compose_ref"][k], rec["compose_masks"])
                 if record_process:
@@ -1150,6 +1169,8 @@ class UNetEngine:
                 P.run_sweep_and_decoder(lambda: None)
                 if compose_kb:
                     ops.compose_rows(P.x, rec["compose_ref"][0], rec["compose_masks"])
+                if anchor_B:
+                    self._warm_anchored(P, steps[0], rec, c12)
             torch.cuda.current_stream().wait_stream(s_)
             torch.cuda.synchronize(dev)
             cg = torch.cuda.CUDAGraph()
@@ -1158,11 +1179,12 @@ class UNetEngine:
             g["graph"] = cg
         return g
 
-    def _sample_rows(self, x_T, schedule, noise, use_graph, out, record_process, compose=None):
+    def _sample_rows(self, x_T, schedule, noise, use_graph, out, record_process, compose=None, anchors=None):
         N = x_T.shape[0]
         if schedule.N != N:
             raise ops._lib.AsyrpError(f"per-row schedule has {schedule.N} rows, x_T {N}")
         compose_kb = self._check_compose(compose, x_T, schedule) if compose is not None else None
+        anchor_B = self._check_anchors(anchors, x_T, schedule, noise, None)
         if schedule.n_delta != self.n_delta or self.n_delta == 0:
             raise ops._lib.AsyrpError(f"per-row schedule carries coefficients for {schedule.n_delta} DeltaBlocks; the "
                                       f"engine packed {self.n_delta}")
@@ -1171,16 +1193,16 @@ class UNetEngine:
         own = own_blocks(schedule.hs_coeffs)
         P = self.plan(N)
         key = (N, bool(use_graph), schedule.key(), own, bool(record_process)) + \
-            ((("compose",) + compose_kb,) if compose_kb else ())
+            ((("compose",) + compose_kb,) if compose_kb else ()) + ((("anchored", anchor_B),) if anchor_B else ())
         with torch.cuda.device(self.device):
-            n_sto = schedule.n_stochastic
+            n_sto = 0 if anchor_B else schedule.n_stochastic
             if n_sto and (noise is None or noise.shape[0] != n_sto or noise.shape[1] != N):
                 raise ops._lib.AsyrpError(f"pre-drawn noise [{n_sto}][{N}][..] required for the stochastic steps")
             self.state["ignore_timestep"] = schedule.ignore_timestep
             self.state["slerp_t"], self.state["use_mask"], self.state["slerp_rows"] = 0.0, False, False
             g = self.graphs.pop(key, None)
             if g is None:
-                g = self._build_row_trajectory(P, schedule, use_graph, own, record_process, compose_kb)
+                g = self._build_row_trajectory(P, schedule, use_graph, own, record_process, compose_kb, anchor_B)
                 while len(self.graphs) >= self.MAX_GRAPHS:
                     self.graphs.pop(next(iter(self.graphs)))
             self.graphs[key] = g
@@ -1191,6 +1213,9 @@ class UNetEngine:
             if compose_kb:
                 g["rec"]["compose_masks"].copy_(compose[0])
                 g["rec"]["compose_ref"].copy_(compose[1])
+            if anchor_B:
+                g["rec"]["anchor_x"].copy_(anchors.x)
+                g["rec"]["anchor_eps"].copy_(anchors.eps)
             P.x.copy_(x_T, non_blocking=True)
             if n_sto:
                 g["zbuf"].copy_(noise, non_blocking=True)
@@ -1202,6 +1227,119 @@ class UNetEngine:
                 return P.x.clone()
             out.copy_(P.x)
             return out
+
+    def _check_anchors(self, anchors, x_T, schedule, noise, lpips):
+        """the number of images B of an anchors= argument (0 without one); AsyrpError unless it fits the batch and the
+        schedule"""
+        if anchors is None:
+            return 0
+        if noise is not None:
+            raise ops._lib.AsyrpError("anchors= draws no noise: the same c1 z in a row's and its anchor's update cancels; "
+                                      "pass noise=None")
+        if lpips is not None:
+            raise ops._lib.AsyrpError("anchors= does not combine with lpips=")
+        anchors.check(schedule, x_T.shape[0])
+        if tuple(anchors.x.shape[2:]) != tuple(x_T.shape[1:]):
+            raise ops._lib.AsyrpError(f"anchors: images are {tuple(anchors.x.shape[2:])}, x_T rows "
+                                      f"{tuple(x_T.shape[1:])}")
+        cur = torch.cuda.current_device()
+        idx = lambda d: d.index if d.index is not None else cur  # noqa: E731
+        for name, t in (("x", anchors.x), ("eps", anchors.eps)):
+            if not (torch.is_tensor(t) and t.dtype == torch.float32 and t.is_cuda and idx(t.device) == idx(self.device)):
+                raise ops._lib.AsyrpError(f"anchors: {name} must be an fp32 tensor on {self.device}")
+        return anchors.B
+
+    def _anchor_tables(self, n, B, P):
+        """the graph-owned A [n + 1][B][C][S][S] and E [n][B][C][S][S] of an anchored trajectory of n steps"""
+        shape = (B, *P.x.shape[1:])
+        return (torch.zeros((n + 1, *shape), dtype=torch.float32, device=self.device),
+                torch.zeros((n, *shape), dtype=torch.float32, device=self.device))
+
+    @staticmethod
+    def _warm_anchored(P, s, rec, c12=None):
+        """one anchored update outside the capture (the warm-up of a trajectory graph; P.x is refilled before a
+        replay)"""
+        ops.ddim_update_anchored(P.x, P.et, P.et, P.x, None, rec["anchor_x"][0], rec["anchor_x"][1],
+                                 rec["anchor_eps"][0], s.at, s.an, getattr(s, "c2", 0.0), c12=c12)
+
+    def anchors(self, x0, inv_schedule, use_graph=True):
+        """The anchors of exact inversion (inversion.Anchors) for the B images x0 (fp32 [B][C][S][S]): the DDIM
+        inversion of inv_schedule (Schedule.inversion of make_sequences(t_0, n)), recording its state and its eps as it
+        runs, plus one UNet evaluation at (x_T, t_0) for E[0].  That is n evaluations, as many as an unedited reverse
+        pass.  Recording does not change the inversion: A[0] is sample(x0, inv_schedule) bit for bit.  One captured
+        graph per (B, inv_schedule), cached with the trajectories; the returned tensors are copies."""
+        from .inversion import Anchors
+        steps = inv_schedule.steps
+        if not steps or any(s.kind != "ddim" or s.edit or s.stochastic or s.t >= s.t_next for s in steps):
+            raise ops._lib.AsyrpError("anchors() needs a DDIM inversion schedule of at least one step "
+                                      "(Schedule.inversion)")
+        seq = [steps[0].t] + [s.t_next for s in steps]  # the forward grid, t ascending
+        n = len(seq)
+        grid = tuple((seq[m], seq[m - 1] if m else -1) for m in reversed(range(n)))
+        B = x0.shape[0]
+        P = self.plan(B)
+        key = ("anchors", B, bool(use_graph), tuple(steps))
+        with torch.cuda.device(self.device):
+            g = self.graphs.pop(key, None)
+            if g is None:
+                g = self._build_anchors(P, steps, use_graph)
+                while len(self.graphs) >= self.MAX_GRAPHS:
+                    self.graphs.pop(next(iter(self.graphs)))
+            self.graphs[key] = g
+            self.last_launches = g["launches"]
+            self.last_records = g["rec"]
+            P.x.copy_(x0, non_blocking=True)
+            if g["graph"] is not None:
+                g["graph"].replay()
+            else:
+                g["body"]()
+            return Anchors(g["rec"]["x"].clone(), g["rec"]["eps"].clone(), grid)
+
+    def _build_anchors(self, P, steps, use_graph):
+        """the recording inversion: the loop of _build_trajectory for an inversion schedule (encoder, decoder,
+        ddim_update per step), each step's eps copied into E and its state into A in reverse order, then the encoder
+        and decoder at (x_T, t_0)"""
+        n, C = len(steps) + 1, self.arch.in_ch
+        ts = [s.t for s in steps] + [steps[-1].t_next]
+        emb_table = torch.empty((n, *P.emb_all.shape), dtype=torch.float32, device=self.device)
+        for k, t in enumerate(ts):
+            P.t.fill_(float(t))
+            P.run_temb()
+            emb_table[k].copy_(P.emb_all)
+        A, E = self._anchor_tables(n, P.x.shape[0], P)
+        rec = {"x": A, "eps": E}
+
+        def body():
+            A[n].copy_(P.x)
+            A[n - 1].copy_(P.x)
+            for m, s in enumerate(steps):
+                P.emb_all.copy_(emb_table[m])
+                P.run_encoder()
+                P.run_decoder()
+                E[n - 1 - m].copy_(P.et[:, :C])
+                ops.ddim_update(P.x, P.et, P.et, None, P.x, None, s.at, s.an, s.c1, s.c2)
+                A[n - 2 - m].copy_(P.x)
+            P.emb_all.copy_(emb_table[n - 1])
+            P.run_encoder()
+            P.run_decoder()
+            E[0].copy_(P.et[:, :C])
+
+        g = {"emb_table": emb_table, "body": body, "graph": None, "rec": rec,
+             "launches": n * len(P.launches(False, temb=False)) + len(steps)}
+        if use_graph:
+            s_ = torch.cuda.Stream(device=self.device)
+            s_.wait_stream(torch.cuda.current_stream())
+            with torch.cuda.stream(s_):  # warm-up outside capture
+                P.emb_all.copy_(emb_table[0])
+                P.run_encoder()
+                P.run_decoder()
+            torch.cuda.current_stream().wait_stream(s_)
+            torch.cuda.synchronize(self.device)
+            cg = torch.cuda.CUDAGraph()
+            with torch.cuda.graph(cg):
+                body()
+            g["graph"] = cg
+        return g
 
     def _check_blend(self, blend, x_T, schedule, lpips):
         """the number of images B of a blend=(mask, ref) argument; AsyrpError unless it fits the batch and the schedule"""
@@ -1254,7 +1392,7 @@ class UNetEngine:
 
     def sample(self, x_T, schedule, noise=None, use_graph=True, out=None, delta_hs=None, use_mask=False,
                record_dh=False, record_process=False, hs_coeffs=None, lpips=None, record_h=False, h_direction=None,
-               blend=None, compose=None):
+               blend=None, compose=None, anchors=None):
         """Run the reverse trajectory of `schedule` (sampler.Schedule) from x_T; returns x_0 (fp32 NCHW).
 
         The step list, the edit/plain/stochastic phase of every step and all sampler coefficients are host-side
@@ -1308,13 +1446,22 @@ class UNetEngine:
         image j), 1 <= K <= 8.  After every step's update, before anything is recorded, the K rows of image j are all
         replaced by w_0 ref[k][j] + sum_k w_k x[k b + j] (ops.compose_rows), with w_k = M_k and w_0 = 1 - sum M, or
         M_k / sum M and 0 where the masks sum above 1.  Masks and reference are graph inputs, copied in before every
-        replay: every batch replays one graph.  With K = 1 it is blend= on the same rows, bit for bit."""
+        replay: every batch replays one graph.  With K = 1 it is blend= on the same rows, bit for bit.
+
+        anchors: an inversion.Anchors of B images (UNetEngine.anchors) anchors the trajectory to their recorded DDIM
+        inversion (exact inversion): every update is ops.ddim_update_anchored, x_{k+1} = A[k+1][b] +
+        (Phi_k(x, eps_mod, eps) - Phi_k(A[k][b], E[k][b], E[k][b])) for row n, b = n % B, N a multiple of B.  The step
+        grid must be the anchors' and every step DDIM; stochastic steps keep their c2 and draw no noise (noise must be
+        None), since the same c1 z in both updates would cancel.  A row that does not edit, started from A[0], records
+        A[1:] and ends on x0 bit for bit.  blend= and compose= still apply after the update, with A[1:]
+        (Anchors.ref) the natural reference.  The tables are graph inputs, copied in before every replay; the launch
+        count is unchanged.  It does not combine with lpips."""
         if isinstance(schedule, RowSchedule):
             if delta_hs is not None or record_dh or hs_coeffs is not None or lpips is not None or record_h or \
                     h_direction is not None or blend is not None:
                 raise ops._lib.AsyrpError("a per-row schedule takes no delta_hs, record_dh, hs_coeffs, lpips, "
                                           "record_h, h_direction or blend")
-            return self._sample_rows(x_T, schedule, noise, use_graph, out, record_process, compose)
+            return self._sample_rows(x_T, schedule, noise, use_graph, out, record_process, compose, anchors)
         if compose is not None:
             raise ops._lib.AsyrpError("compose= needs a per-row schedule (schedule.RowSchedule)")
         N = x_T.shape[0]
@@ -1332,6 +1479,7 @@ class UNetEngine:
                                           f"got {None if add_table is None else (add_table.dtype, tuple(add_table.shape))}")
             hs_coeffs = None  # (c0, α) are add_h_rows' table, not DeltaBlock coefficients
         blend_B = self._check_blend(blend, x_T, schedule, lpips) if blend is not None else 0
+        anchor_B = self._check_anchors(anchors, x_T, schedule, noise, lpips)
         P = self.plan(N)
         explicit = delta_hs is not None
         table = coeff_table(hs_coeffs, N, self.n_delta) if hs_coeffs is not None else None
@@ -1347,9 +1495,9 @@ class UNetEngine:
         key = (N, bool(use_graph), schedule.key(), explicit, slerp_t, bool(use_mask) if explicit else False,
                bool(record_dh), bool(record_process)) + ((lpips,) if lpips is not None else ()) + \
             (("record_h",) if record_h else ()) + (("additive",) if additive else ()) + \
-            ((("blend", blend_B),) if blend_B else ())
+            ((("blend", blend_B),) if blend_B else ()) + ((("anchored", anchor_B),) if anchor_B else ())
         with torch.cuda.device(self.device):
-            n_sto = schedule.n_stochastic
+            n_sto = 0 if anchor_B else schedule.n_stochastic
             if n_sto:
                 assert noise is not None and noise.shape[0] == n_sto, "pre-drawn noise required for stochastic steps"
             # kernel variants / parameters baked at capture time (all part of `key`)
@@ -1363,7 +1511,7 @@ class UNetEngine:
             g = self.graphs.pop(key, None)
             if g is None:
                 g = self._build_trajectory(P, schedule, use_graph, explicit, record_dh, record_process, lpips,
-                                           record_h, additive, blend_B)
+                                           record_h, additive, blend_B, anchor_B)
                 while len(self.graphs) >= self.MAX_GRAPHS:
                     self.graphs.pop(next(iter(self.graphs)))
             self.graphs[key] = g  # most recently used last
@@ -1389,6 +1537,9 @@ class UNetEngine:
             if blend_B:
                 g["rec"]["blend_mask"].copy_(blend[0])
                 g["rec"]["blend_ref"].copy_(blend[1])
+            if anchor_B:
+                g["rec"]["anchor_x"].copy_(anchors.x)
+                g["rec"]["anchor_eps"].copy_(anchors.eps)
             P.x.copy_(x_T, non_blocking=True)
             if n_sto:
                 g["zbuf"].copy_(noise, non_blocking=True)

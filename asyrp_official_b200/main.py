@@ -203,6 +203,13 @@ def build_parser():
                         'mix of the attributes and the origin pass, weighted by the --seg_weights masks of the origin '
                         'pass (--edit_region_dilate / --edit_region_feather apply to every mask, overlaps are '
                         'normalised).  The masks are written as <file>_ngen<n>_region_compose.png')
+    p.add_argument('--exact_inversion', **sa,
+                   help='--run_test: edit real images without inversion drift.  Each batch\'s input images are '
+                        'inverted with DDIM (the cached x_T is not used) and every edit step is anchored to that '
+                        'inversion, so that an unedited pass returns the input image exactly and the origin row is '
+                        'the input.  --edit_region / --region_compose parse the input image.  Needs --n_test_step '
+                        '== --n_inv_step and DDIM sampling; the stochastic steps of --user_defined_t_addnoise draw '
+                        'no noise')
     return p
 
 

@@ -283,6 +283,41 @@ def ddim_update_rows(x, et, em, z, x_next, x0_out, at, an, c12):
                                      H * W, at, an, _ptr(c12), _stream()), "asyrp_ddim_update_rows")
 
 
+def ddim_update_anchored(x, et, em, x_next, x0_out, a_cur, a_next, e_cur, at, an, c2=0.0, c12=None):
+    """the DDIM update anchored to a recorded inversion (exact inversion): row n with image b = n % B becomes
+    A_next[b] + (y - yr), y = ddim_update's result without noise, yr the same operations on (A_cur[b], E_cur[b],
+    E_cur[b]).  x, x_next, x0_out fp32 [N][Cx][H][W] (x_next may be x, x0_out None); et, em fp32 [N][Ce][H][W], Ce >= Cx;
+    a_cur, a_next, e_cur fp32 [B][Cx][H][W], N a multiple of B.  c12 fp32 [N][2] on the device gives row n its c2 from
+    column 1 (column 0, c1, is not read); without it every row takes c2."""
+    lib = _lib.load()
+    _need_cuda(x, et, em, x_next, x0_out, a_cur, a_next, e_cur, c12)
+    req = (("x", x), ("et", et), ("em", em), ("x_next", x_next), ("A_cur", a_cur), ("A_next", a_next),
+           ("E_cur", e_cur)) + ((("x0_out", x0_out),) if x0_out is not None else ())
+    for name, t in req:
+        if not (t.dtype == torch.float32 and t.is_contiguous() and t.dim() == 4):
+            raise _lib.AsyrpError(f"ddim_update_anchored: {name} must be a contiguous fp32 [rows][C][H][W] tensor, got "
+                                  f"{t.dtype} {tuple(t.shape)}")
+    N, Cx, H, W = x.shape
+    B, Ce = a_cur.shape[0], et.shape[1]
+    if tuple(x_next.shape) != (N, Cx, H, W) or (x0_out is not None and tuple(x0_out.shape) != (N, Cx, H, W)):
+        raise _lib.AsyrpError(f"ddim_update_anchored: x_next and x0_out must be [{N}][{Cx}][{H}][{W}]")
+    if tuple(et.shape) != (N, Ce, H, W) or tuple(em.shape) != (N, Ce, H, W) or Ce < Cx:
+        raise _lib.AsyrpError(f"ddim_update_anchored: et and em must be [{N}][Ce >= {Cx}][{H}][{W}], got "
+                              f"{tuple(et.shape)} and {tuple(em.shape)}")
+    for name, t in (("A_cur", a_cur), ("A_next", a_next), ("E_cur", e_cur)):
+        if tuple(t.shape) != (B, Cx, H, W) or B == 0 or N % B:
+            raise _lib.AsyrpError(f"ddim_update_anchored: {name} must be [B][{Cx}][{H}][{W}] with N = {N} a multiple "
+                                  f"of B = {B}, got {tuple(t.shape)}")
+    if c12 is not None and not (c12.dtype == torch.float32 and tuple(c12.shape) == (N, 2) and c12.is_contiguous()):
+        raise _lib.AsyrpError(f"ddim_update_anchored: c12 must be a contiguous fp32 [{N}][2] device tensor, got "
+                              f"{c12.dtype} {tuple(c12.shape)}")
+    if len({t.device for _, t in req} | ({c12.device} if c12 is not None else set())) != 1:
+        raise _lib.AsyrpError("ddim_update_anchored: every tensor must live on one device")
+    check(lib.asyrp_ddim_update_anchored(_ptr(x), _ptr(et), _ptr(em), _ptr(a_cur), _ptr(a_next), _ptr(e_cur),
+                                         _ptr(x_next), _ptr(x0_out), N, B, Cx, Ce, H * W, at, an, c2, _ptr(c12),
+                                         _stream()), "asyrp_ddim_update_anchored")
+
+
 def attention(qkv, out, heads, head_dim, scale):
     lib = _lib.load()
     N, T, _ = qkv.shape

@@ -198,6 +198,20 @@ int asyrp_ddim_update_rows(const float* x, const float* et, const float* em, con
                            float* x0_out, int N, int Cx, int Ce, int HW, float at, float an, const float* c12,
                            void* stream);
 
+/* Exact inversion (csrc/inversion.cu): the DDIM update of an edit pass anchored to the recorded DDIM inversion of its
+ * B input images.  Row n, image b = n % B, in fp32 with the operations of asyrp_ddim_update:
+ *   y  = sqrt(an) x0 + c2 et,  x0 = (x - em sqrt(1 - at)) / sqrt(at)
+ *   yr = the same operations on (A_cur[b], E_cur[b], E_cur[b])
+ *   x_next = A_next[b] + (y - yr)            (subtraction, then addition; never contracted)
+ * x, et, em as asyrp_ddim_update ([N][Cx][HW], [N][Ce][HW], Ce >= Cx); A_cur, A_next, E_cur fp32 [B][Cx][HW]; N % B
+ * == 0.  x_next may alias x; x0_out (may be NULL) receives the edit's x0.  c12 NULL: c2 for every row; else a DEVICE
+ * array [N][2] whose column 1 is row n's c2 (column 0, c1, is not read: no noise is drawn, it would cancel).  A row with
+ * x = A_cur and et = em = E_cur gives A_next bit for bit.  With HW % 4 == 0 every pointer must be 16-byte aligned
+ * (float4 loads), else 4-byte aligned.  64-bit indexing. */
+int asyrp_ddim_update_anchored(const float* x, const float* et, const float* em, const float* a_cur,
+                               const float* a_next, const float* e_cur, float* x_next, float* x0_out, int N, int B,
+                               int Cx, int Ce, int HW, float at, float an, float c2, const float* c12, void* stream);
+
 /* DDPM ancestral update (utils/diffusion_utils.py:74-82, sampling_type 'ddpm'):
  *   x_next = (x - bt/sqrt(1-at)*et)/sqrt(1-bt) + mask*exp(0.5*logvar)*z;  learned_sigma: logvar = et channels [Cx, 2Cx) */
 int asyrp_ddpm_update(const float* x, const float* et, const float* z, float* x_next, int N, int Cx, int Ce, int HW,

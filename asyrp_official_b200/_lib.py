@@ -157,6 +157,13 @@ SIGNATURES = {
     "asyrp_region_mask": (c_int, [c_void_p, C.c_uint, c_void_p, c_int, c_int, c_void_p]),
     "asyrp_mask_dilate": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p]),
     "asyrp_mask_blur": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p]),
+    "asyrp_dino_pack": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p]),
+    "asyrp_dino_layernorm": (c_int, [c_void_p, C.c_longlong, c_void_p, c_void_p, c_void_p, c_int, c_int, c_float,
+                                     c_void_p]),
+    "asyrp_dino_attention": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p]),
+    "asyrp_dino_selfsim_partials": (c_int, [c_int]),
+    "asyrp_dino_selfsim_distance": (c_int, [c_void_p, C.c_longlong, c_void_p, c_void_p, c_int, c_int, c_int, c_float,
+                                            c_void_p, c_void_p, c_void_p]),
 }
 
 _lib = None

@@ -14,7 +14,7 @@ SUFFIX = os.environ.get("ASYRP_LIB_SUFFIX", "")
 LIB = os.path.join(HERE, f"libasyrp_b200{SUFFIX}.so")
 SOURCES = ["common.cu", "conv_gemm.cu", "pointwise.cu", "attention.cu", "lpips.cu", "clip_text.cu", "clip_image.cu",
            "arcface.cu", "face_parsing.cu", "fid.cu", "prdc.cu", "preservation.cu",
-           "hspace.cu", "region.cu", "inversion.cu"]
+           "hspace.cu", "region.cu", "inversion.cu", "dino.cu"]
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
     "-Xcompiler", "-fPIC", "-Xcompiler", "-fvisibility=hidden", "-cudart", "static",

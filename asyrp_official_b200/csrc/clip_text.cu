@@ -266,7 +266,8 @@ ASYRP_API int asyrp_clip_linear(const float* in, const float* weight, const floa
   ASYRP_REQUIRE(M > 0 && M < (1 << 30), "asyrp_clip_linear: bad row count M=%d", M);
   ASYRP_REQUIRE(K > 0 && K % kBK == 0, "asyrp_clip_linear: K=%d must be a positive multiple of %d", K, kBK);
   ASYRP_REQUIRE(N > 0 && N % kBN == 0, "asyrp_clip_linear: N=%d must be a positive multiple of %d", N, kBN);
-  ASYRP_REQUIRE(epilogue >= kEpiBias && epilogue <= kEpiResidual, "asyrp_clip_linear: unknown epilogue %d", epilogue);
+  ASYRP_REQUIRE((epilogue >= kEpiBias && epilogue <= kEpiResidual) || epilogue == kEpiGelu,
+                "asyrp_clip_linear: unknown epilogue %d", epilogue);
   ASYRP_REQUIRE((epilogue == kEpiResidual) == (residual != nullptr),
                 "asyrp_clip_linear: a residual is required by, and only by, the residual epilogue");
   ASYRP_REQUIRE(in != out && (residual == nullptr || residual == out || residual + static_cast<size_t>(M) * N <= out ||
@@ -280,6 +281,7 @@ ASYRP_API int asyrp_clip_linear(const float* in, const float* weight, const floa
   switch (epilogue) {
     case kEpiBias: return launch_tf32_conv<kEpiBias>(p, st);
     case kEpiQuickGelu: return launch_tf32_conv<kEpiQuickGelu>(p, st);
+    case kEpiGelu: return launch_tf32_conv<kEpiGelu>(p, st);
     default: return launch_tf32_conv<kEpiResidual>(p, st);
   }
 }

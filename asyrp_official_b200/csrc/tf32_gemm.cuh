@@ -32,6 +32,7 @@ enum Epilogue : int {
   // the vertical one): an Inception branch of any even width writes its slice of the block output.  The other
   // epilogues ignore padw / ldo / cstore (pad both ways, pitch and bound Cout).
   kEpiReluSlice = 6,
+  kEpiGelu = 7,       // 0.5 v (1 + erf(v / sqrt(2)))  (DINO's exact GELU)
 };
 
 __device__ __forceinline__ void cp_async16(uint32_t dst, const void* src, int bytes) {
@@ -67,6 +68,7 @@ struct Tf32ConvParams {
 };
 
 __device__ __forceinline__ float quick_gelu(float z) { return z * (1.f / (1.f + expf(-(1.702f * z)))); }
+__device__ __forceinline__ float gelu_erf(float z) { return 0.5f * z * (1.f + erff(z * 0.70710678118654752f)); }
 
 // out = epilogue(conv(in) + bias).  CTA tile 128 pixels x 64 channels, K in slices of 32 through a 3-stage cp.async
 // ring; the im2col gather is 16-byte chunks (4 channels of one tap: Cin % 4 == 0), zero-filled outside the image, so
@@ -198,6 +200,8 @@ __global__ void __launch_bounds__(kThreads) tf32_conv_kernel(const Tf32ConvParam
             v = make_float2(fmaxf(v.x, 0.f), fmaxf(v.y, 0.f));
           } else if (kEpi == kEpiQuickGelu) {
             v = make_float2(quick_gelu(v.x), quick_gelu(v.y));
+          } else if (kEpi == kEpiGelu) {
+            v = make_float2(gelu_erf(v.x), gelu_erf(v.y));
           } else if (kEpi == kEpiResidual) {
             const float2 r = *reinterpret_cast<const float2*>(p.residual + o);
             v = make_float2(r.x + v.x, r.y + v.y);

@@ -24,6 +24,9 @@ Mirrors, with the same attribute / flag names:
                                                             (preservation.ContentPreservation), and the origin pass
                                                             against the input image for inverted latents; this
                                                             build's definition
+    --dino_structure                                        DINO-ViT key self-similarity structure distance and CLS
+                                                            cosine (dino.DINO), with the same origin rows; also each
+                                                            --diff_style result against its content and its style
     --fid                                                   FID and KID of each set of edits (one per hs_coeff tuple)
                                                             against the origin pass on Inception-v3 pool features
                                                             (fid.FIDInception), gathered to rank 0 at the end of the
@@ -107,6 +110,12 @@ class Asyrp(object):
         # image, for latents inverted from images
         self.content_preservation = {}
         self.reconstruction = {}
+        # --dino_structure: save_image's file name -> fp64 [tuples][images][2], (structure distance, CLS cosine) of each
+        # edit against the origin pass; dino_origin: fp64 [images][2] of the origin pass against the input image, for
+        # latents inverted from images; diff_style_dino (rank 0): the sorted rows of --diff_style's table
+        self.dino = {}
+        self.dino_origin = {}
+        self.diff_style_dino = None
 
     # ------------------------------------------------------------------------------------------
     def load_pretrained_model(self):
@@ -215,6 +224,9 @@ class Asyrp(object):
 
     def content_preservation_setup(self):
         return scoring.content_preservation_setup(self)
+
+    def dino_structure_setup(self):
+        return scoring.dino_structure_setup(self)
 
     def prdc_check(self):
         return scoring.prdc_check(self)
@@ -612,6 +624,8 @@ class Asyrp(object):
         self.exact_inversion_setup()  # refuses --lpips
         if getattr(a, "content_preservation", False):
             self.content_preservation_setup()  # refuses --lpips
+        if getattr(a, "dino_structure", False):
+            self.dino_structure_setup()  # refuses --lpips
         if self.world > 1:
             raise NotImplementedError("--lpips computes statistics over every image: run single-process")
         print("Get lpips distance...")
@@ -1041,6 +1055,8 @@ class Asyrp(object):
         self.edit_region_setup()  # refuses --h_directions
         self.region_compose_setup()  # refuses --h_directions
         self.exact_inversion_setup()  # refuses --h_directions
+        if getattr(self.args, "dino_structure", False):
+            self.dino_structure_setup()  # refuses --h_directions
         mode, arg = self.h_directions_setup()
         seq, seq_next = make_sequences(a.t_0, a.n_test_step)
         size = self.config.data.image_size
@@ -1366,7 +1382,7 @@ class Asyrp(object):
         The content h at t_0, which the inversion never evaluates, is the bottleneck h of the content's x_T at t_0.
         Rows are (pair, γ), whole pairs per replay of at most --max_rows_per_replay rows; each row draws its own
         noise for the eta = 1 steps.  Writes <save_dir>/<content stem>__<style stem>.png: content x0, style x0, one
-        result per γ.  Returns {(content path, style path): results [len(γ)][3][S][S]}."""
+        result per γ; with --dino_structure also <save_dir>/diff_style_dino.tsv (scoring.write_diff_style_dino).  Returns {(content path, style path): results [len(γ)][3][S][S]}."""
         import torchvision.utils as tvu
         a = self.args
         self.prdc_check()
@@ -1377,6 +1393,7 @@ class Asyrp(object):
             self.content_preservation_setup()  # refuses --diff_style
         if getattr(a, "fid", False):
             self.fid_setup()  # refuses --diff_style, before any model loads
+        dino_sd = self.dino_structure_setup() if getattr(a, "dino_structure", False) else None
         contents, styles, gammas = self.diff_style_setup()
         print(f"DiffStyle: hs_coeff {gammas} (slerp weight on the content h: 1 - hs_coeff)")
         model = self.load_pretrained_model().to(self.device)
@@ -1403,6 +1420,11 @@ class Asyrp(object):
         print(f"DiffStyle: {len(pairs)} pairs, {len(pairs) * len(gammas)} rows, {len(chunks)} replays of {R} rows")
         os.makedirs(a.save_dir, exist_ok=True)
         results = {}
+        dino, dino_rows = None, []
+        if dino_sd is not None:
+            from .dino import DINO
+            dino = DINO(dino_sd, device=self.device)
+            dino_sd = None
         for ci, chunk in enumerate(chunks):
             if ci % self.world != self.rank:  # chunks sharded round-robin across ranks
                 continue
@@ -1425,6 +1447,17 @@ class Asyrp(object):
                 grid = (torch.cat([cached[c][0].cpu(), cached[s_][0].cpu(), res]) + 1) * 0.5
                 tvu.save_image(tvu.make_grid(grid, nrow=grid.shape[0], padding=1),
                                os.path.join(a.save_dir, f"{_stem(c)}__{_stem(s_)}.png"))
+                if dino is not None:  # each result against the content and the style x0
+                    sc, ss = dino.scores(cached[c][0], res)[:, 0], dino.scores(cached[s_][0], res)[:, 0]
+                    dino_rows += [(c, s_, g, *sc[k, 0:1].tolist(), *ss[k, 0:1].tolist(), *sc[k, 1:].tolist(),
+                                   *ss[k, 1:].tolist()) for k, g in enumerate(gammas)]
+        if dino is not None:
+            dino = None
+            torch.cuda.empty_cache()
+            rows = scoring.gather_rows(self, dino_rows)
+            if rows is not None:
+                self.diff_style_dino = scoring.write_diff_style_dino(os.path.join(a.save_dir, "diff_style_dino.tsv"),
+                                                                     rows)
         return results
 
 

@@ -154,6 +154,15 @@ def build_parser():
                         '(--lpips_weights, or seeded weights with --synthetic_weights) of the saved u8 image against '
                         'the unedited DDIM pass of the same x_T, and that pass against the input image for latents '
                         'inverted from images, written next to the PNG (images larger than 160 x 160)')
+    p.add_argument('--dino_structure', **sa,
+                   help='--run_test: score every edit against the unedited DDIM pass of the same x_T (and that pass '
+                        'against the input image for latents inverted from images) with DINO-ViT: the key '
+                        'self-similarity structure distance and the CLS cosine, written next to the PNG; '
+                        '--diff_style: score every result against its content and its style image, written to '
+                        '<save_dir>/diff_style_dino.tsv')
+    p.add_argument('--dino_weights', type=str, default='pretrained/dino_vitbase8_pretrain.pth',
+                   help="torch.save of DINO's VisionTransformer state dict (ViT-S/8, S/16, B/8 or B/16) for "
+                        "--dino_structure")
     p.add_argument('--checkpoint_dir', type=str, default='checkpoint')
     p.add_argument('--max_rows_per_replay', type=int, default=16,
                    help='rows (hs_coeff tuples x images) of one batched trajectory in save_image; bounds the memory of '

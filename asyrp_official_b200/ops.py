@@ -722,6 +722,96 @@ def clip_cosine(a, b, out, eps=1e-6):
     check(lib.asyrp_clip_cosine(_ptr(a), _ptr(b), _ptr(out), n, dim, float(eps), _stream()), "asyrp_clip_cosine")
 
 
+CLIP_EPI_GELU = 7  # asyrp_clip_linear's exact-GELU epilogue (DINO's MLP)
+DINO_LN_EPS = 1e-6  # DINO's LayerNorm eps
+
+
+def _dino_f32(name, *ts):
+    for t in ts:
+        if t.dtype != torch.float32:
+            raise _lib.AsyrpError(f"{name}: fp32 tensors expected, got {t.dtype}")
+    if len({t.device for t in ts}) != 1:
+        raise _lib.AsyrpError(f"{name}: tensors live on {sorted(str(t.device) for t in ts)}")
+
+
+def dino_pack(x, out, grid, patch):
+    """DINO's input transform and patch matrix: x fp32 [B][3][S][S] in [-1, 1] -> (x+1)/2, antialiased bilinear resize
+    to grid*patch, ImageNet Normalize -> out [B*grid^2][clip_image_kpad(patch)] in (c, ky, kx) column order"""
+    lib = _lib.load()
+    _need_cuda(x, out)
+    _dino_f32("dino_pack", x, out)
+    if x.dim() != 4 or x.shape[1] != 3 or x.shape[2] != x.shape[3] or not x.is_contiguous():
+        raise _lib.AsyrpError(f"dino_pack: x must be contiguous [B][3][S][S], got {tuple(x.shape)}")
+    B, S = x.shape[0], x.shape[2]
+    kpad = clip_image_kpad(patch)
+    if tuple(out.shape) != (B * grid * grid, kpad) or not out.is_contiguous():
+        raise _lib.AsyrpError(f"dino_pack: out must be contiguous [{B * grid * grid}][{kpad}], got {tuple(out.shape)}")
+    check(lib.asyrp_dino_pack(_ptr(x), _ptr(out), B, S, grid, patch, kpad, _stream()), "asyrp_dino_pack")
+
+
+def dino_layernorm(x, gamma, beta, out, eps=DINO_LN_EPS):
+    """out [rows][w] = LayerNorm(eps)(rows of x): x a 2-D view [rows][w] whose rows may be strided (x.stride(0) >= w,
+    x.stride(1) == 1) or a contiguous tensor [..][w]; out dense, which may be x only when x is dense"""
+    lib = _lib.load()
+    _need_cuda(x, gamma, beta, out)
+    _dino_f32("dino_layernorm", x, gamma, beta, out)
+    w = x.shape[-1]
+    if x.dim() != 2:
+        if not x.is_contiguous():
+            raise _lib.AsyrpError("dino_layernorm: an x of other than 2 dims must be contiguous")
+        x = x.view(-1, w)
+    rows, ld = x.shape[0], x.stride(0)
+    if x.stride(1) != 1 or out.numel() != rows * w or out.shape[-1] != w or not out.is_contiguous():
+        raise _lib.AsyrpError(f"dino_layernorm: x rows of unit column stride and a dense out [{rows}][{w}], got x "
+                              f"strides {x.stride()} and out {tuple(out.shape)}")
+    if gamma.numel() != w or beta.numel() != w:
+        raise _lib.AsyrpError(f"dino_layernorm: gamma and beta must have {w} elements")
+    check(lib.asyrp_dino_layernorm(_ptr(x), ld, _ptr(gamma), _ptr(beta), _ptr(out), rows, w, float(eps), _stream()),
+          "asyrp_dino_layernorm")
+
+
+def dino_attention(qkv, out, heads):
+    """non-causal multi-head attention (head size 64, T <= 1025): qkv fp32 [B][T][3D] (q | k | v), out [B][T][D]"""
+    lib = _lib.load()
+    _need_cuda(qkv, out)
+    _dino_f32("dino_attention", qkv, out)
+    if qkv.dim() != 3 or not qkv.is_contiguous() or not out.is_contiguous():
+        raise _lib.AsyrpError(f"dino_attention: contiguous qkv [B][T][3D] and out [B][T][D], got {tuple(qkv.shape)}")
+    B, T, w3 = qkv.shape
+    if w3 != 3 * 64 * heads or tuple(out.shape) != (B, T, 64 * heads):
+        raise _lib.AsyrpError(f"dino_attention: qkv [B][T][{3 * 64 * heads}] and out [B][T][{64 * heads}] for {heads} "
+                              f"heads, got {tuple(qkv.shape)} and {tuple(out.shape)}")
+    check(lib.asyrp_dino_attention(_ptr(qkv), _ptr(out), B, T, heads, _stream()), "asyrp_dino_attention")
+
+
+def dino_selfsim_distance(keys, ia, ib, T, out, eps=1e-8):
+    """out fp64 [P]: the structure distance (1/T^2) sum_ij (Sa_ij - Sb_ij)^2 of each pair p, S the cosine
+    self-similarity of the T key rows starting at row ia[p] (image a) and ib[p] (image b) of keys, a 2-D fp32 view
+    [rows][D] of unit column stride whose rows may be strided (the key columns of a qkv buffer); ia, ib int64 [P] on
+    the device"""
+    lib = _lib.load()
+    _need_cuda(keys, ia, ib, out)
+    _dino_f32("dino_selfsim_distance", keys)
+    if keys.dim() != 2 or keys.stride(1) != 1 or keys.stride(0) < keys.shape[1]:
+        raise _lib.AsyrpError(f"dino_selfsim_distance: keys must be a 2-D view [rows][D] of unit column stride, got "
+                              f"shape {tuple(keys.shape)} strides {keys.stride()}")
+    if ia.dtype != torch.int64 or ib.dtype != torch.int64 or ia.dim() != 1 or ib.shape != ia.shape:
+        raise _lib.AsyrpError("dino_selfsim_distance: ia and ib must be int64 [P]")
+    if not (ia.is_contiguous() and ib.is_contiguous() and out.is_contiguous()) or out.dtype != torch.float64 or \
+            out.shape != ia.shape:
+        raise _lib.AsyrpError("dino_selfsim_distance: out must be a contiguous fp64 [P]")
+    P, D = ia.shape[0], keys.shape[1]
+    ntp = lib.asyrp_dino_selfsim_partials(int(T))
+    if ntp < 0:
+        raise _lib.AsyrpError(f"dino_selfsim_distance: T={T} outside 1..1025")
+    if P and (int(ia.min()) < 0 or int(ib.min()) < 0 or max(int(ia.max()), int(ib.max())) + T > keys.shape[0]):
+        raise _lib.AsyrpError(f"dino_selfsim_distance: the rows ia[p] .. ia[p] + {T} and ib[p] .. ib[p] + {T} must lie "
+                              f"in the {keys.shape[0]} key rows")
+    partial = torch.empty(max(P, 1) * ntp, dtype=torch.float64, device=out.device)
+    check(lib.asyrp_dino_selfsim_distance(_ptr(keys), keys.stride(0), _ptr(ia), _ptr(ib), P, int(T), D, float(eps),
+                                          _ptr(partial), _ptr(out), _stream()), "asyrp_dino_selfsim_distance")
+
+
 def arcface_preprocess(x, out):
     """IDLoss's crop x[:, :, 35:223, 32:220] and AdaptiveAvgPool2d(112): x fp32 [B][3][H][W] -> out fp32 NHWC
     [B][112][112][4], channel 3 zero"""

@@ -5,6 +5,7 @@ one run, and the score tables they write.
             --id_similarity             arcface.ArcFace               <file>_ngen<n>_id_similarity.tsv
             --seg_consistency           face_parsing.FaceParser       <file>_ngen<n>_seg_consistency.tsv
             --content_preservation      preservation.ContentPreservation  <file>_ngen<n>_content_preservation.tsv
+            --dino_structure            dino.DINO                     <file>_ngen<n>_dino.tsv
   per set   --fid (--fid_ref, --prdc)   fid.FIDInception, FeatureSets <mode>_ngen<n>_{fid,fid_real,prdc,prdc_real}.tsv
 
 Every per-edit score compares each edit against the origin pass (the unedited DDIM pass of the same x_T), which
@@ -140,6 +141,27 @@ def content_preservation_setup(runner):
                      "LPIPS(net='alex').state_dict()) or --synthetic_weights")
 
 
+def dino_structure_setup(runner):
+    """--dino_structure's requirements; raises ValueError with the reason.  Returns the validated --dino_weights state
+    dict (the tensors of dino.load_state_dict).  It scores the edits of --run_test and the results of --diff_style."""
+    from .dino import load_state_dict
+    a = runner.args
+    if getattr(a, "pass_editing", False):
+        raise ValueError("--dino_structure scores the edited images: with --pass_editing nothing is edited")
+    if not (getattr(a, "run_test", False) or getattr(a, "diff_style", False)) or getattr(a, "lpips", False) or \
+            getattr(a, "h_directions", False):
+        raise ValueError("--dino_structure scores the edits of --run_test and the results of --diff_style (not --lpips "
+                         "or --h_directions)")
+    path = getattr(a, "dino_weights", None)
+    if not path or not os.path.isfile(path):
+        raise ValueError(f"--dino_structure: --dino_weights {path!r} is not a file (a torch.save of DINO's "
+                         "VisionTransformer state dict, e.g. dino_vitbase8_pretrain.pth)")
+    try:
+        return load_state_dict(path)[1]
+    except ValueError as e:
+        raise ValueError(f"--dino_structure: {e}") from None
+
+
 def fid_setup(runner):
     """--fid's requirements; raises ValueError with the reason.  Returns the validated --fid_weights state dict
     (fid.load_state_dict)."""
@@ -184,11 +206,13 @@ class Scorers:
                  "id": runner.id_similarity_setup() if getattr(a, "id_similarity", False) else None,
                  "seg": runner.seg_consistency_setup() if getattr(a, "seg_consistency", False) else None,
                  "fid": runner.fid_setup() if getattr(a, "fid", False) else None,
-                 "cp": runner.content_preservation_setup() if getattr(a, "content_preservation", False) else None}
+                 "cp": runner.content_preservation_setup() if getattr(a, "content_preservation", False) else None,
+                 "dino": runner.dino_structure_setup() if getattr(a, "dino_structure", False) else None}
         self.specs = {name: spec for name, spec in specs.items() if spec is not None}
         self.needs_origin = bool(self.specs)  # every score compares against the origin pass
-        # --content_preservation of latents inverted from images also scores the origin pass against those images
-        self.keeps_source = "cp" in self.specs and not a.load_random_noise
+        # --content_preservation and --dino_structure of latents inverted from images also score the origin pass
+        # against those images
+        self.keeps_source = ("cp" in self.specs or "dino" in self.specs) and not a.load_random_noise
         self.nets = {}
 
     def __enter__(self):
@@ -196,11 +220,13 @@ class Scorers:
         from .clip_image import CLIPLoss
         from .face_parsing import FaceParser
         from .fid import FeatureSets, FIDInception
+        from .dino import DINO
         from .preservation import ContentPreservation
         a, dev = self.runner.args, self.runner.device
         build = {"clip": lambda s: CLIPLoss(a.clip_weights, a.clip_vocab, s, device=dev),
                  "id": lambda s: ArcFace(s, device=dev), "seg": lambda s: FaceParser(s, device=dev),
-                 "fid": lambda s: FIDInception(s, device=dev), "cp": lambda s: ContentPreservation(s, device=dev)}
+                 "fid": lambda s: FIDInception(s, device=dev), "cp": lambda s: ContentPreservation(s, device=dev),
+                 "dino": lambda s: DINO(s, device=dev)}
         try:
             for name in list(self.specs):  # the host copies of the weights go once their network is built
                 self.nets[name] = build[name](self.specs.pop(name))
@@ -256,6 +282,12 @@ class Scorers:
             if x0_source is not None:
                 rec = r.reconstruction[file_name] = nets["cp"].scores(x0_source, origin)
             keep("content_preservation", cp, COLUMNS, "content preservation", rec)
+        if "dino" in nets:
+            sc = nets["dino"].scores(origin, torch.cat(edited))
+            rec = None
+            if x0_source is not None:
+                rec = r.dino_origin[file_name] = nets["dino"].scores(x0_source, origin)[0]
+            keep("dino", sc, DINO_COLUMNS, "DINO structure distance / CLS cosine", rec)
 
     def finish(self, coeffs):
         """--fid at the end of a run (finish_fid, through Asyrp.finish_fid).  Every rank must call it, also one that
@@ -337,6 +369,37 @@ def _coeff_text(tup):
 def _tuple_name(coeffs, attrs, k):
     """tuple k as the printed lines name it: attribute <attr> under a sweep, else hs_coeff (1.0, 0.5)"""
     return f"attribute {attrs[k]}" if attrs is not None else f"hs_coeff {tuple(float(c) for c in coeffs[k])}"
+
+
+DINO_COLUMNS = ("structure", "cls_cos")
+DIFF_STYLE_DINO_COLUMNS = ("content", "style", "hs_coeff", "structure_content", "structure_style", "cls_cos_content",
+                           "cls_cos_style")
+
+
+def write_diff_style_dino(path, rows):
+    """--diff_style --dino_structure's table: rows (content path, style path, γ, structure_content, structure_style,
+    cls_cos_content, cls_cos_style), sorted by (content, style, γ), so that the file does not depend on how the rows
+    were chunked or sharded; prints each row"""
+    rows = sorted(rows, key=lambda r: (r[0], r[1], float(r[2])))
+    with open(path, "w") as f:
+        f.write("\t".join(DIFF_STYLE_DINO_COLUMNS) + "\n")
+        for c, s_, g, *vals in rows:
+            f.write("\t".join([c, s_, f"{float(g):.6g}"] + [repr(float(v)) for v in vals]) + "\n")
+    for c, s_, g, sc, ss, cc, cs in rows:
+        print(f"DINO, content {c}, style {s_}, hs_coeff {float(g):.6g}: structure against the content {sc:.6f}, "
+              f"against the style {ss:.6f}; CLS cosine with the content {cc:.6f}, with the style {cs:.6f}")
+    return rows
+
+
+def gather_rows(runner, rows):
+    """every rank's list of rows to rank 0 (torch.distributed.gather_object, as fid.FeatureSets.gather does): the
+    concatenation on rank 0, None on the other ranks; the list itself without a process group"""
+    dist_on = runner.world > 1 and torch.distributed.is_available() and torch.distributed.is_initialized()
+    if not dist_on:
+        return list(rows)
+    got = [None] * runner.world if runner.rank == 0 else None
+    torch.distributed.gather_object(list(rows), got, dst=0)
+    return None if runner.rank != 0 else [r for part in got for r in part]
 
 
 def write_scores(path, coeffs, scores, column, label, attrs=None, origin=None):

@@ -136,6 +136,28 @@ def inception_state_dict(seed=1234, fc=True):
     return sd
 
 
+def dino_state_dict(seed=1234, dim=384, depth=12, patch=8, grid=28):
+    """seeded DINO VisionTransformer weights in its state-dict layout (asyrp_official_b200.dino; default ViT-S/8 at
+    224^2): linear and conv weights U(-b, b) with b = fan_in^-1/2 (torch's default), biases N(0, .02^2), LayerNorm
+    weights 1 + N(0, .1^2) and biases N(0, .1^2), cls_token and pos_embed N(0, .02^2) (DINO's trunc_normal_ std)"""
+    from .dino import key_shapes
+    sd = {}
+    for name, shp in key_shapes(dim, depth, patch, grid).items():
+        g = torch.Generator()
+        g.manual_seed((zlib.crc32(name.encode()) ^ (seed * 0x9E3779B1)) & 0x7FFFFFFF)
+        if name in ("cls_token", "pos_embed"):
+            sd[name] = 0.02 * torch.randn(shp, generator=g)
+        elif len(shp) >= 2:
+            sd[name] = (torch.rand(shp, generator=g) * 2 - 1) * math.prod(shp[1:]) ** -0.5
+        elif "norm" in name and name.endswith(".weight"):
+            sd[name] = 1.0 + 0.1 * torch.randn(shp, generator=g)
+        elif "norm" in name:
+            sd[name] = 0.1 * torch.randn(shp, generator=g)
+        else:
+            sd[name] = 0.02 * torch.randn(shp, generator=g)
+    return sd
+
+
 def _draw_clip(shapes, prefix, std, width, layers, seed):
     """CLIP weights of `shapes` (names without `prefix`), each from its own generator seeded by crc32(prefix + name)"""
     std = {**std, "attn.in_proj_weight": width ** -0.5, "attn.out_proj.weight": width ** -0.5 * (2 * layers) ** -0.5,

@@ -288,7 +288,8 @@ int asyrp_lpips_distance(const float* probe, const float* ref, int N, int B, int
  * asyrp_clip_layernorm: LayerNorm over width, eps 1e-5, per row of [rows][width]; out may be in.
  * asyrp_clip_linear: out[M][N] = epilogue(in[M][K] @ weight[N][K]^T + bias) (nn.Linear's weight layout), TF32
  *   operands rounded to nearest, fp32 accumulation, the LPIPS conv's GEMM.  K % 32 == 0, N % 64 == 0.  epilogue 1:
- *   identity (bias may be null), 2: QuickGELU z*sigmoid(1.702z), 3: residual + z (residual [M][N], may be out).
+ *   identity (bias may be null), 2: QuickGELU z*sigmoid(1.702z), 3: residual + z (residual [M][N], may be out),
+ *   7: GELU 0.5 z (1 + erf(z / sqrt 2)) (DINO's MLP).
  * asyrp_clip_attention: causal multi-head attention, head size 64, scale 1/8; qkv [P*T][3*64*heads] as
  *   nn.MultiheadAttention's in_proj packs q | k | v, out [P*T][64*heads] (T <= 128).
  * asyrp_clip_pool: out [P][width] = LayerNorm(x[p][eot]) with eot the first argmax of ids[p].
@@ -516,6 +517,36 @@ int asyrp_compose_rows(float* x, const float* ref, const float* masks, int K, in
 int asyrp_region_mask(const unsigned char* labels, unsigned class_bits, float* mask, int N, int S, void* stream);
 int asyrp_mask_dilate(const float* in, float* out, int N, int S, int r, int axis, void* stream);
 int asyrp_mask_blur(const float* in, const float* taps, float* out, int N, int S, int R, int axis, void* stream);
+
+/* DINO ViT and the self-similarity structure distance (csrc/dino.cu): facebookresearch/dino's VisionTransformer
+ * (backbone, eval mode) and Splice's key self-similarity loss.  Activations are fp32 [B][T][D], T = 1 + grid^2 <= 1025,
+ * D = 64 * heads.  The patch embedding and every linear layer run on asyrp_clip_linear (epilogue 7: the exact GELU
+ * 0.5 v (1 + erf(v / sqrt 2)) of fc1), cls + pos on asyrp_clip_image_tokens, the CLS cosine on asyrp_clip_cosine.
+ * asyrp_dino_pack: x fp32 [B][3][S][S] in [-1, 1] (square) -> (x+1)/2 -> F.interpolate(R x R, bilinear,
+ *   align_corners=False, antialias=True), R = grid*patch, with the taps of PyTorch's _upsample_bilinear2d_aa (support
+ *   max(1, S/R), triangle weights normalised per output pixel; rows of taps summed first) -> (v - mean_c) / std_c with
+ *   ImageNet's mean and std -> out [B*grid^2][kpad] in conv-weight column order (c, ky, kx), columns 3*patch^2 ..
+ *   kpad-1 zero; kpad = 3*patch^2 rounded up to a multiple of 32.  S == R gives (x+1)/2 exactly; S, R <= 4096.
+ * asyrp_dino_layernorm: LayerNorm (eps > 0) of rows in + r*ld, r < rows, into dense out [rows][width]; out may be in
+ *   only when ld == width, and must not overlap it otherwise.
+ * asyrp_dino_attention: non-causal softmax attention, head size 64, scale 1/8; qkv [B*T][3D] packs q | k | v, out
+ *   [B*T][D].  Flash-style: key tiles of 64 in a fixed order, QK^T and PV on TF32 mma.sync m16n8k8, online softmax in
+ *   fp32.  T <= 1025, B and heads <= 65535; qkv 16-byte and out 8-byte aligned; out must not overlap qkv.
+ * asyrp_dino_selfsim_distance: out fp64 [P], out[p] = (1/T^2) sum_ij (Sa_ij - Sb_ij)^2 with S_ij = k^_i . k^_j,
+ *   k^ = k / max(|k|, eps), the key of token i of pair p's image a at keys + (ia[p] + i) * ld (D floats) and of b at
+ *   ia -> ib.  ia, ib int64 [P] on the device; ld >= D (the qkv buffer with ld = 3D at offset D gives the keys without a
+ *   copy).  64 x 64 tiles over i <= j (off-diagonal tiles twice), fp32 fmaf dot products in column order, per-tile fp64
+ *   partials in partial [P][asyrp_dino_selfsim_partials(T)] summed in tile order: equal rows give exactly 0.
+ *   T <= 1025, P <= 65535; keys 4-byte and ia, ib, partial, out 8-byte aligned.
+ * asyrp_dino_selfsim_partials: the tile pairs of T tokens (the partial columns), -1 for T outside 1..1025.
+ * Fixed-order reductions, no float atomics, no kernel mixes images. */
+int asyrp_dino_pack(const float* x, float* out, int B, int S, int grid, int patch, int kpad, void* stream);
+int asyrp_dino_layernorm(const float* in, long long ld, const float* gamma, const float* beta, float* out, int rows,
+                         int width, float eps, void* stream);
+int asyrp_dino_attention(const float* qkv, float* out, int B, int T, int heads, void* stream);
+int asyrp_dino_selfsim_partials(int T);
+int asyrp_dino_selfsim_distance(const float* keys, long long ld, const long long* ia, const long long* ib, int P, int T,
+                                int D, float eps, double* partial, double* out, void* stream);
 
 #ifdef __cplusplus
 }
